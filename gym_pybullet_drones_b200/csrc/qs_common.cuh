@@ -46,7 +46,7 @@ struct StepArgs {
     int log2D;           // log2(D) when D is a power of two, else -1
     int sc_limit;        // smallest step counter with (double)sc / pyb_freq > episode_len_sec (HoverAviary.py:113)
     int flags_late_tma;  // experiments (QS_LATE_TMA): 1 = issue the bulk copy only after the state loads have landed
-    int prefetch;        // experiments (QS_PREFETCH): 1 = L2 prefetch of the warp's inputs ahead of griddepcontrol.wait
+    int prefetch;        // QS_PREFETCH: 1 (default) = L2 prefetch of the warp's state and action ahead of griddepcontrol.wait, 2 = + its history
     int early_store;     // experiments (QS_EARLY_STORE): 1 = history written back as soon as it has landed (A = 4)
     int dbg_slot;        // QS_TIMELINE builds: which timeline buffer this launch stamps
     int row_loads;       // experiments (QS_ROW_LOADS): 1 = A = 4 fetches only the 16(B-1) history bytes of every row (one bulk copy per lane)
@@ -149,6 +149,15 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// the same copy for data read once and dead afterwards: its L2 lines are marked evict-first, so they leave the cache ahead of
+// lines that will still be read (what this launch stores, what the next launch prefetches)
+__device__ __forceinline__ void tma_bulk_g2s_read_once(void* dst_smem, const void* src_gmem, unsigned bytes, unsigned long long* bar) {
+    unsigned long long pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");

@@ -359,7 +359,7 @@ static int prepare_step(const QsParams* p, const QsState* st, const QsStepIO* io
     a.effects = effects; a.flags = flags;
     {
         static const int late = getenv("QS_LATE_TMA") ? atoi(getenv("QS_LATE_TMA")) : 1;
-        static const int pre = getenv("QS_PREFETCH") ? atoi(getenv("QS_PREFETCH")) : 2;
+        static const int pre = getenv("QS_PREFETCH") ? atoi(getenv("QS_PREFETCH")) : 1;      // 1: state + action (DESIGN.md 6)
         static const int early = getenv("QS_EARLY_STORE") ? atoi(getenv("QS_EARLY_STORE")) : 1;
         static const int rowl = getenv("QS_ROW_LOADS") ? atoi(getenv("QS_ROW_LOADS")) : 0;
         a.flags_late_tma = late; a.prefetch = pre; a.early_store = early; a.row_loads = rowl;

@@ -91,9 +91,10 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
             pf(a.st.planes + 4 * w0, nb); pf(a.st.planes + 4 * (N + w0), nb); pf(a.st.planes + 4 * (2 * N + w0), nb);
             if (((rows * 8) & 15) == 0) pf(a.st.planes + 12 * N + w0, (unsigned)rows * 8u);
             if (((rows * A * 4) & 15) == 0) pf(a.io.action + w0 * A, (unsigned)(rows * A * 4));
-            // the history too: back-to-back launches then find it in L2 and write it back during the FP64 loop (-0.5 us per step);
-            // a launch on an idle GPU has no window and would pay ~2 us because its state loads queue behind it (measured), so
-            // the previous launch on these buffers says whether it saw a window (pdl_hint)
+            // QS_PREFETCH=2 (not the default): the history too, when the previous launch on these buffers saw a window
+            // (pdl_hint; a launch on an idle GPU would pay ~2 us because its state loads queue behind it).  On the H100 the 19 MB
+            // prefetched under the previous launch compete with it for L2 and DRAM: 7 % slower per step than state and action
+            // only (DESIGN.md 6)
             if (a.prefetch > 1 && (a.io.pdl_hint == nullptr || *reinterpret_cast<const volatile unsigned*>(a.io.pdl_hint) != 0u)) pf(span_src, span_bytes);
         }
     }
@@ -135,7 +136,9 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
             __syncwarp();
             if (live) bulk_g2s(xs + (size_t)lane * od + 16, span_src + (size_t)lane * od + 16, hb, bar);
         } else if (lane == 0) {
-            tma_bulk_g2s(xs, span_src, span_bytes, bar);
+            // the old span is dead once copied (the next launch on these buffers overwrites it): evict-first in L2, so its 19 MB
+            // make room for this launch's stores and the next launch's state instead of pushing them out (+3 % per step, DESIGN.md 6)
+            tma_bulk_g2s_read_once(xs, span_src, span_bytes, bar);
         }
     };
     bool issued = false;

@@ -175,7 +175,8 @@ typedef struct QsStepIO {
                                            whether its launch found a programmatic-dependent-launch window (it was resident while its
                                            predecessor still ran); the next launch on the same buffers then prefetches its observation
                                            history into L2 during that window, and an isolated launch does not (the prefetch would only
-                                           delay its state loads).  NULL = always prefetch. */
+                                           delay its state loads).  NULL = always prefetch.  Read only when the history prefetch is
+                                           enabled (QS_PREFETCH=2; off by default: on the H100 it slows back-to-back launches). */
 } QsStepIO;
 
 /* Spins (bounded, ~2 s, then *err_flag = 1) until flags[r] - seq >= 0 for every r < world: the learner side of obs_gather. */
