@@ -36,8 +36,8 @@ struct RolloutArgs {
 //    ~160 KB of the SM's 256 KB as shared memory, the actor's 55 KB of weights stay in the rest).
 //  * First layer: the observation rows are read from the shared-memory window as 128-bit loads -- lane t supplies elements
 //    4t .. 4t+3 of each 16-wide k-step instead of the canonical {2t, 2t+1, 2t+8, 2t+9}; W1 is packed with the same permutation of
-//    k, so the product is unchanged -- and split per fragment (conversions saturate to +-65504: an observation beyond that range
-//    acts like a clipped one).
+//    k, so the product is unchanged -- and split per fragment (both conversions saturate to +-65504, so an observation acts
+//    like one clipped to +-(65504 + 65504 / 2048) = +-65535.984375).
 //  * Hidden layers never leave the registers: the accumulator fragment of n-tiles (2j, 2j+1) IS the A fragment of k-step j of the
 //    next layer (tanh, split, pack) -- no shared-memory round trip, no barrier between layers.
 // K = 144 / 64 and M = 32 rows per CTA are below a wgmma tile (M = 64 per warpgroup, B operand through shared-memory descriptors)

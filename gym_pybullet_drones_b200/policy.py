@@ -7,7 +7,8 @@ the layout the rollout kernel reads: every matrix split once into two float16 pa
 the tensor-core products hi*hi + 2^-11 (hi*lo + lo*hi) with fp32 accumulation then reproduce fp32), stored in the order of the
 mma B fragments (one 16-byte load per lane, k-step and 8 outputs), rows zero-padded to a multiple of 16 and last-layer columns to 8.  `rollout(policy=...)` then evaluates it inside the kernel every tick, from the observation
 window in shared memory: no policy launch, no action tensor round trip.  `forward_torch` is the same network in plain PyTorch
-fp32 (what a learner would run for the gradient step, and what the tests compare the kernel with)."""
+fp32 (what a learner would run for the gradient step); the tests hold the kernel to a float64 restatement of it."""
+import copy
 import ctypes as C
 
 import torch
@@ -109,14 +110,22 @@ class MlpPolicy:
         return h @ net[2][0] + net[2][1]
 
     def forward_torch(self, obs, noise=None):
-        """obs [E, D, obs_dim] (or [E, in_dim]) -> (raw action [E, out_dim], log-prob [E], value [E] or None)."""
-        x = obs.reshape(obs.shape[0], -1).to(torch.float32)
+        """obs [E, D, obs_dim] (or [E, in_dim]) -> (raw action [E, out_dim], log-prob [E], value [E] or None), in the dtype of
+        the weights (float32; `double()` gives a float64 copy)."""
+        x = obs.reshape(obs.shape[0], -1).to(self.log_std.dtype)
         mean = self._mlp(self.actor, x)
-        eps = torch.zeros_like(mean) if noise is None else noise.reshape(mean.shape)
+        eps = torch.zeros_like(mean) if noise is None else noise.reshape(mean.shape).to(mean.dtype)
         raw = mean + torch.exp(self.log_std) * eps
         logp = (-0.5 * eps * eps - self.log_std - 0.91893853320467274).sum(dim=1)
         val = None if self.critic is None else self._mlp(self.critic, x)[:, 0]
         return raw, logp, val
+
+    def double(self):
+        """A copy whose `forward_torch` runs in float64 on the same (fp32-valued) weights; the packed kernel layout is shared."""
+        c = copy.copy(self)
+        f64 = lambda net: None if net is None else [(w.double(), b.double()) for w, b in net]   # noqa: E731
+        c.actor, c.critic, c.log_std = f64(self.actor), f64(self.critic), self.log_std.double()
+        return c
 
     # ---- C struct -------------------------------------------------------------------------------------------------------
     def c_struct(self, noise=None, logprob=None, values=None):

@@ -187,7 +187,8 @@ int qs_wait_flags(const unsigned* flags, unsigned seq, int world, unsigned* err_
  * independent log_std, Gaussian sample, clip to [-1, 1] for the env -- and optionally the critic (same shape, 1 output),
  * evaluated inside the rollout kernel from the observation window in shared memory on the tensor cores (mma m16n8k16 F16) with
  * a two-term split of both operands (fp32-level accuracy: x w ~ x_hi w_hi + 2^-11 (x_hi w_lo' + x_lo' w_hi), fp32 accumulation;
- * w_hi = fp16(w), w_lo' = fp16(2048 (w - w_hi))).  Observations beyond +-65504 saturate.
+ * w_hi = fp16(w), w_lo' = fp16(2048 (w - w_hi))).  Observations saturate at +-(65504 + 65504 / 2048) = +-65535.984375: both
+ * fp16 conversions clamp to 65504, so x_hi + x_lo' / 2048 stops growing there (not at fp16's 65504).
  * Every weight matrix W[in][out] is given in FRAGMENT ORDER: rows padded with zeros to a multiple of 16, columns to a multiple
  * of 8 (the last layer's to 8 * nt3, the critic's to 8), then [k-step ks][n-tile n][lane l] x 4 words, lane l = 4 g + t:
  *     word 0 = {w_hi[16 ks + ka][8 n + g], w_hi[16 ks + ka + 1][8 n + g]}   (low half, high half)

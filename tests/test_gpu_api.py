@@ -347,45 +347,6 @@ def test_fused_observation_gather_in_process(act, world):
         assert torch.equal(go, o) and torch.equal(gr, r) and torch.equal(gte, te) and torch.equal(gtr, tr), t
 
 
-@pytest.mark.parametrize("cls,act,D,critic", [("MultiHoverAviary", "RPM", 2, True), ("HoverAviary", "ONE_D_RPM", 1, True), ("MultiHoverAviary", "RPM", 4, False)])
-def test_rollout_with_on_device_policy_matches_torch_mlp(cls, act, D, critic):
-    """SURVEY 8f rank 1: the SB3-MlpPolicy-shaped actor/critic evaluated INSIDE qs_rollout (tensor cores, F16 two-term operand
-    split, from the observation window in shared memory) against the same network in PyTorch fp32 driving a twin env step by step with the same noise: sampled
-    (unclipped) actions, log-probabilities and values within 1e-5, observations / rewards / flags of every tick equal to 1e-5."""
-    import gym_pybullet_drones_b200.envs as envs
-    from gym_pybullet_drones_b200.policy import MlpPolicy
-    from gym_pybullet_drones_b200.utils.enums import ActionType, Physics
-    E, T = 200, 10
-    kw = dict(physics=Physics.DYN, act=ActionType[act], num_envs=E, autoreset="same_step")
-    if cls == "MultiHoverAviary":
-        kw["num_drones"] = D
-    e1, e2 = getattr(envs, cls)(**kw), getattr(envs, cls)(**kw)
-    A, od = e1._A, e1._obs_dim
-    pol = MlpPolicy.random(D * od, D * A, seed=5, critic=critic, log_std=-1.0)
-    g = torch.Generator(device="cuda").manual_seed(9)
-    noise = torch.randn((T, E, D * A), device="cuda", generator=g)
-    obs, _ = e1.reset()
-    obs = obs.clone()
-    e2.reset()
-    out = e2.rollout(policy=pol, noise=noise)
-    assert out["actions"].shape == (T, E, D, A) and out["log_probs"].shape == (T, E) and (("values" in out) == critic)
-    for t in range(T):
-        raw, logp, val = pol.forward_torch(obs, noise[t])
-        assert float((out["actions"][t].reshape(E, -1) - raw).abs().max()) < 1e-5, t
-        assert float((out["log_probs"][t] - logp).abs().max()) < 1e-4, t
-        if critic:
-            assert float((out["values"][t] - val).abs().max()) < 1e-5, t
-        obs, r, te, tr, _ = e1.step(raw.clamp(-1, 1).reshape(E, D, A).contiguous())
-        obs = obs.clone()
-        assert float((out["obs"][t] - obs).abs().max()) < 1e-5 and float((out["rewards"][t] - r).abs().max()) < 1e-5, t
-        assert torch.equal(out["terminated"][t], te) and torch.equal(out["truncated"][t], tr), t
-    # deterministic mode: no noise, action = mean
-    e1.reset(); e2.reset()
-    out = e2.rollout(policy=pol, num_steps=3)
-    raw, logp, _ = pol.forward_torch(e1.reset()[0])
-    assert float((out["actions"][0].reshape(E, -1) - raw).abs().max()) < 1e-5 and float((out["log_probs"][0] - logp).abs().max()) < 1e-4
-
-
 def test_numpy_api_head_only_transfer_mode():
     """host_obs='head': the NumPy vector API moves only the kinematic head of every observation (the action-history part is
     what the caller itself supplied); it equals the first 12 columns of the full observation, flags and terminal
