@@ -30,7 +30,7 @@ FLAG_AUTORESET_SAME_STEP, FLAG_AUTORESET_NEXT_STEP, FLAG_RPY_F32 = 1, 2, 4
 FLAG_AUTORESET_CLEARS_PID, FLAG_AUTORESET_CLEARS_HISTORY = 8, 16
 FLAG_OBS_STATE20 = 32
 FLAG_SKIP_EPILOGUE, FLAG_RPM_FROM_LAST, FLAG_ACTION_F64 = 0x100, 0x200, 0x400
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 _d = C.c_double
 
@@ -68,7 +68,7 @@ class QsStepIO(C.Structure):
         ("act_buffer_size", C.c_int), ("tick_substeps", C.c_int),
         ("obs_gather", C.c_void_p), ("reward_gather", C.c_void_p), ("terminated_gather", C.c_void_p), ("truncated_gather", C.c_void_p),
         ("gather_flag", C.c_void_p), ("gather_counter", C.c_void_p), ("gather_seq", C.c_uint), ("pad_", C.c_uint),
-        ("pdl_hint", C.c_void_p),
+        ("warp_ticket", C.c_void_p), ("warp_done", C.c_void_p), ("ready_err", C.c_void_p),
     ]
 
 

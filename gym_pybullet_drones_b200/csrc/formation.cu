@@ -601,6 +601,7 @@ int qs_dw_publish(const float* pos, int n, int offset, float* const* gathered, i
     }
     a.pos = pos; a.counter = counter; a.n = n; a.offset = offset; a.n_total = n_total; a.world = world; a.rank = rank; a.seq = seq;
     dw_publish_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(a);
+    pdl_note((cudaStream_t)stream, kPdlOther);                          // triggers its successor at its first instruction
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_dw_publish launch");
 }

@@ -46,7 +46,7 @@ struct StepArgs {
     int log2D;           // log2(D) when D is a power of two, else -1
     int sc_limit;        // smallest step counter with (double)sc / pyb_freq > episode_len_sec (HoverAviary.py:113)
     int flags_late_tma;  // experiments (QS_LATE_TMA): 1 = issue the bulk copy only after the state loads have landed
-    int prefetch;        // QS_PREFETCH: 1 (default) = L2 prefetch of the warp's state and action ahead of griddepcontrol.wait, 2 = + its history
+    int grid_wait;       // fast kernels: 1 = griddepcontrol.wait for the whole previous grid (quadsim.cu launch_step_tracked, DESIGN.md 4.1)
     int early_store;     // experiments (QS_EARLY_STORE): 1 = history written back as soon as it has landed (A = 4)
     int dbg_slot;        // QS_TIMELINE builds: which timeline buffer this launch stamps
     int row_loads;       // experiments (QS_ROW_LOADS): 1 = A = 4 fetches only the 16(B-1) history bytes of every row (one bulk copy per lane)
@@ -186,6 +186,36 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     return t;
 }
 
+// ---- per-warp readiness between consecutive fast steps on the same buffers (QsStepIO.warp_ticket / warp_done, DESIGN.md 4.1)
+// One thread per warp.  Spins until *done == ticket (acquire, gpu scope), backing off with __nanosleep; after ~1 s of
+// %globaltimer it raises *err and proceeds, so a protocol bug shows up as a wrong result and a non-zero error word, never as
+// a hung GPU.  The fence orders the acquire before the warp's later bulk copies, which read through the async proxy.
+__device__ __forceinline__ void warp_wait_turn(const unsigned* done, unsigned ticket, unsigned* err) {
+    unsigned v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(done) : "memory");
+    if (v != ticket) {
+        const unsigned long long t0 = globaltimer_ns();
+        unsigned ns = 32;
+        do {
+            __nanosleep(ns);
+            if (ns < 1024) ns <<= 1;
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(done) : "memory");
+            if (v != ticket && globaltimer_ns() - t0 > 1000000000ull) { if (err) atomicOr(err, 1u); break; }
+        } while (v != ticket);
+    }
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+}
+// All 32 lanes.  Every generic store of the warp (state, counters, rewards, observation patches, terminal rows) and its bulk
+// stores, which must have COMPLETED (cp.async.bulk.wait_group 0, not .read), come before the release of the next ticket.
+__device__ __forceinline__ void warp_publish(unsigned* done, unsigned next) {
+    __threadfence();
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) {
+        asm volatile("fence.proxy.async.global;" ::: "memory");
+        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(done), "r"(next) : "memory");
+    }
+}
+
 __device__ __forceinline__ void cp_async4(float* dst_smem, const float* src_gmem) {      // LDGSTS, 4-byte granule
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
 }
@@ -255,8 +285,16 @@ int cta_capacity(long long N, int D, bool rollout = false);               // qua
 inline int block_size_for(int D, int cap = kMaxTPB) { return D <= cap ? D * (cap / D) : cap; }
 
 // launchers of the kernel families (one translation unit each)
-cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, cudaStream_t s);      // step_general.cu
+// pdl_ok = false: an ordinary stream-ordered launch (not a programmatic dependent of the previous kernel)
+cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s);      // step_general.cu
 bool step_fast_eligible(const StepArgs& a);                                                       // step_fast.cu
 cudaError_t launch_step_fast(const StepArgs& a, cudaStream_t s);                                  // step_fast.cu
+
+// What the last library launch on a stream that lets its successor start early (griddepcontrol.launch_dependents) was:
+// nothing yet, a fast step, or another kernel (general step, formation publish).  Only the library's own early-triggering
+// launches are recorded; every other kernel or copy releases its successor at completion.  quadsim.cu.
+enum PdlPrev { kPdlNone = 0, kPdlFast = 1, kPdlOther = 2 };
+PdlPrev pdl_prev(cudaStream_t s);
+void pdl_note(cudaStream_t s, PdlPrev what);
 
 }  // namespace qsi

@@ -10,10 +10,59 @@
 // No tensor cores: the path is element-wise; the roofline that bounds it is HBM bandwidth (DESIGN.md).
 #include "qs_common.cuh"
 
+#include <map>
+#include <mutex>
+#include <utility>
+
 namespace qsi {
 thread_local char g_err[256] = "";
+
+// Per (device, stream): the last early-triggering library launch (PdlPrev).  Unknown streams read kPdlNone: nothing of the
+// library that triggers early ran on them.  The per-thread default stream is tracked per host thread.
+constexpr int kPdlDevices = 32;
+static std::mutex g_pdl_mu;
+static std::map<std::pair<int, cudaStream_t>, PdlPrev>* g_pdl = new std::map<std::pair<int, cudaStream_t>, PdlPrev>();   // never freed
+static thread_local PdlPrev t_pdl_per_thread[kPdlDevices] = {};
+
+PdlPrev pdl_prev(cudaStream_t s) {
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kPdlDevices) { (void)cudaGetLastError(); return kPdlOther; }
+    if (s == cudaStreamPerThread) return t_pdl_per_thread[dev];
+    std::lock_guard<std::mutex> lk(g_pdl_mu);
+    const auto it = g_pdl->find(std::make_pair(dev, s));
+    return it == g_pdl->end() ? kPdlNone : it->second;
 }
+
+void pdl_note(cudaStream_t s, PdlPrev what) {
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kPdlDevices) { (void)cudaGetLastError(); return; }
+    if (s == cudaStreamPerThread) { t_pdl_per_thread[dev] = what; return; }
+    std::lock_guard<std::mutex> lk(g_pdl_mu);
+    (*g_pdl)[std::make_pair(dev, s)] = what;
+}
+}  // namespace qsi
 using namespace qsi;
+
+namespace {
+// Launches one step kernel and records it for the ordering of the next one (include/quadsim.h, qs_step; DESIGN.md 4.1).
+// A fast step skips the whole-grid wait when its stream predecessor that may have triggered early is a fast step: a
+// fast step only touches the drones of its own warps, and the per-warp tickets order it after the previous step on the
+// same buffers.  The wait stays when that predecessor is another early-triggering kernel, without the readiness words,
+// and with obs_gather (the learner's flag counts the warps of one grid at a time).  A general step directly after a
+// fast step is launched as an ordinary dependent (full stream order): the fast step may finish before ITS predecessor.
+cudaError_t launch_step_tracked(StepArgs& a, bool fast, bool state20, bool pid_act, cudaStream_t s) {
+    const PdlPrev prev = pdl_prev(s);
+    if (fast) {
+        a.grid_wait = (prev == kPdlOther || !a.io.warp_ticket || a.io.obs_gather) ? 1 : 0;
+        const cudaError_t e = launch_step_fast(a, s);
+        if (e == cudaSuccess) pdl_note(s, kPdlFast);
+        return e;
+    }
+    const cudaError_t e = launch_step_general(a, state20, pid_act, prev != kPdlFast, s);
+    pdl_note(s, kPdlOther);
+    return e;
+}
+}  // namespace
 
 namespace {
 
@@ -359,11 +408,14 @@ static int prepare_step(const QsParams* p, const QsState* st, const QsStepIO* io
     a.effects = effects; a.flags = flags;
     {
         static const int late = getenv("QS_LATE_TMA") ? atoi(getenv("QS_LATE_TMA")) : 1;
-        static const int pre = getenv("QS_PREFETCH") ? atoi(getenv("QS_PREFETCH")) : 1;      // 1: state + action (DESIGN.md 6)
         static const int early = getenv("QS_EARLY_STORE") ? atoi(getenv("QS_EARLY_STORE")) : 1;
         static const int rowl = getenv("QS_ROW_LOADS") ? atoi(getenv("QS_ROW_LOADS")) : 0;
-        a.flags_late_tma = late; a.prefetch = pre; a.early_store = early; a.row_loads = rowl;
+        a.flags_late_tma = late; a.early_store = early; a.row_loads = rowl;
+        a.grid_wait = 1;
     }
+    if ((io->warp_ticket == nullptr) != (io->warp_done == nullptr)) return fail(QS_ERR_NULL, "qs_step: warp_ticket and warp_done go together");
+    if ((reinterpret_cast<uintptr_t>(io->warp_ticket) | reinterpret_cast<uintptr_t>(io->warp_done) | reinterpret_cast<uintptr_t>(io->ready_err)) & 3u)
+        return fail(QS_ERR_ALIGN, "qs_step: warp_ticket / warp_done / ready_err must be 4-byte aligned");
     a.log2D = -1;
     for (int k = 0; k < 6; ++k) if ((1 << k) == drones_per_env) a.log2D = k;
     {   // time-out threshold on the integer step counter, evaluated with the reference's float64 division
@@ -397,7 +449,7 @@ int qs_step(const QsParams* p, const QsState* st, const QsStepIO* io, int act_ty
     StepArgs a;
     bool state20 = false, pid_act = false, fast = false;
     if (int rc = prepare_step(p, st, io, act_type, task, n_envs, drones_per_env, substeps, effects, flags, a, state20, pid_act, fast)) return rc;
-    const cudaError_t e = fast ? launch_step_fast(a, (cudaStream_t)stream) : launch_step_general(a, state20, pid_act, (cudaStream_t)stream);
+    const cudaError_t e = launch_step_tracked(a, fast, state20, pid_act, (cudaStream_t)stream);
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_step launch");
 }
 
@@ -486,7 +538,7 @@ int qs_step_host(const QsParams* p, const QsState* st, const QsStepIO* io, const
             e = cudaMemcpyAsync(h->action_dev + d0 * A, h->action_host + d0 * A, (size_t)(d1 - d0) * A * 4, cudaMemcpyHostToDevice, s);
             if (e != cudaSuccess) return cuda_fail(e, "qs_step_host H2D action");
             sa.first_warp = (int)w0; sa.n_warps = (int)(w1 - w0);
-            e = launch_step_fast(sa, s);
+            e = launch_step_tracked(sa, true, sa_state20, sa_pid, s);
             if (e != cudaSuccess) return cuda_fail(e, "qs_step_host launch");
             cudaEventRecord(cev[c], s);
             cudaStreamWaitEvent(cs, cev[c], 0);
@@ -497,7 +549,7 @@ int qs_step_host(const QsParams* p, const QsState* st, const QsStepIO* io, const
     } else {
         e = cudaMemcpyAsync(h->action_dev, h->action_host, (size_t)N * A * 4, cudaMemcpyHostToDevice, s);
         if (e != cudaSuccess) return cuda_fail(e, "qs_step_host H2D action");
-        e = sa_fast ? launch_step_fast(sa, s) : launch_step_general(sa, sa_state20, sa_pid, s);
+        e = launch_step_tracked(sa, sa_fast, sa_state20, sa_pid, s);
         if (e != cudaSuccess) return cuda_fail(e, "qs_step_host launch");
     }
     if (want_final) {
@@ -606,7 +658,7 @@ int qs_dyn_substeps_pub(const QsParams* p, const QsState* st, const float* rpm, 
         a.pub_counter = pub->counter; a.pub_world = pub->world; a.pub_rank = pub->rank; a.pub_offset = pub->offset;
         a.pub_n_total = pub->n_total; a.pub_seq = pub->seq;
     }
-    const cudaError_t e = launch_step_general(a, true, false, (cudaStream_t)stream);
+    const cudaError_t e = launch_step_tracked(a, false, true, false, (cudaStream_t)stream);
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_dyn_substeps launch");
 }
 

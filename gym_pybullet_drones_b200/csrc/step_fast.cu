@@ -74,40 +74,33 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
     float* span_dst = a.io.obs + w0 * od;
     const unsigned span_bytes = (unsigned)(rows * od * 4);
     QS_STAMP(0);
-    const bool hint_writer = a.io.pdl_hint != nullptr && wg == 0 && lane == 0;
-    unsigned long long t_wait0 = 0;
-    if (hint_writer) t_wait0 = globaltimer_ns();
-    if (lane == 0) {
-        mbar_init(bar, 1);
-        if (a.prefetch) {
-            // Programmatic dependent launch: this CTA may be resident while the previous kernel of the stream is still in its
-            // compute / store phases with the memory system idle.  Pulling this warp's inputs into L2 now is always safe (L2 is
-            // the point of coherence: lines the previous kernel still writes are simply updated) and turns the DRAM round trips
-            // after the dependency wait into L2 hits.
-            auto pf = [](const void* p, unsigned bytes) {
-                asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-            };
-            const unsigned nb = (unsigned)rows * 32u;
-            pf(a.st.planes + 4 * w0, nb); pf(a.st.planes + 4 * (N + w0), nb); pf(a.st.planes + 4 * (2 * N + w0), nb);
-            if (((rows * 8) & 15) == 0) pf(a.st.planes + 12 * N + w0, (unsigned)rows * 8u);
-            if (((rows * A * 4) & 15) == 0) pf(a.io.action + w0 * A, (unsigned)(rows * A * 4));
-            // QS_PREFETCH=2 (not the default): the history too, when the previous launch on these buffers saw a window
-            // (pdl_hint; a launch on an idle GPU would pay ~2 us because its state loads queue behind it).  On the H100 the 19 MB
-            // prefetched under the previous launch compete with it for L2 and DRAM: 7 % slower per step than state and action
-            // only (DESIGN.md 6)
-            if (a.prefetch > 1 && (a.io.pdl_hint == nullptr || *reinterpret_cast<const volatile unsigned*>(a.io.pdl_hint) != 0u)) pf(span_src, span_bytes);
-        }
-    }
-    __syncwarp();
+    if (lane == 0) mbar_init(bar, 1);
     // read-only tables (never written by a kernel): safe ahead of the dependency wait
     double tpx = 0.0, tpy = 0.0, tpz = 0.0;
     if (TASK) { const D4 tp = ld256_nc(a.st.target_pos, tbl); tpx = tp.x; tpy = tp.y; tpz = tp.z; }
 
-    // nothing written by the previous kernel in the stream is read above this line (programmatic dependent launch)
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    // ---- readiness (DESIGN.md 4.1) ----------------------------------------------------------------------------------------
+    // This warp's ticket among the steps on these buffers: taken (the atomic has returned, hence the shuffle) BEFORE the CTA lets
+    // the next grid launch, so tickets follow launch order and a warp only ever waits for a warp that is already resident.
+    // Then, with grid_wait, the whole previous grid (it was not a fast step); then the previous step's warp of the same 32
+    // drones.  Nothing written by an earlier kernel is read above this point.
+    const bool ticketed = a.io.warp_ticket != nullptr;
+    unsigned ticket = 0;
+    if (ticketed) {
+        if (lane == 0) ticket = atomicAdd(a.io.warp_ticket + wg, 1u);
+        ticket = __shfl_sync(0xffffffffu, ticket, 0);
+    }
+    if (a.grid_wait) asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");        // let the next grid's CTAs take the free slots now
-    if (hint_writer) *a.io.pdl_hint = (globaltimer_ns() - t_wait0 > 1500ull) ? 1u : 0u;      // was I resident > 1.5 us before my dependency resolved?
+    if (ticketed && lane == 0) warp_wait_turn(a.io.warp_done + wg, ticket, a.io.ready_err);
+    __syncwarp();
     QS_STAMP(1);
+    // the end of this warp's work: its bulk stores have COMPLETED, then the next step's warp of these drones may go
+    auto publish = [&]() {
+        if (!ticketed) return;
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        warp_publish(a.io.warp_done + wg, ticket + 1u);
+    };
 
     // ---- loads: state (3 x 32 B + 8 B), action, step counter; then the bulk copy of the old observation span ------------
     qs::Drone d;
@@ -133,6 +126,7 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
         if (by_rows) {
             const unsigned hb = (unsigned)(od - 16) * 4u;
             if (lane == 0) mbar_expect_tx(bar, hb * (unsigned)rows);
+            if (ticketed) asm volatile("fence.proxy.async.global;" ::: "memory");     // every lane issues an async-proxy read
             __syncwarp();
             if (live) bulk_g2s(xs + (size_t)lane * od + 16, span_src + (size_t)lane * od + 16, hb, bar);
         } else if (lane == 0) {
@@ -303,6 +297,7 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
         }
         QS_STAMP(8);
         if (a.io.obs_gather) { patch_rows_a4(); gather(shifted); }      // (the early bulk store has completed: shared memory is free)
+        publish();
         return;
     }
     mbar_wait(bar, 0);
@@ -352,8 +347,9 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
         }
     }
     QS_STAMP(8);
-    if (a.io.obs_gather) { gather(A == 4 ? (const void*)shifted : (const void*)ys); return; }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // shared memory must outlive the bulk store's reads
+    if (a.io.obs_gather) { gather(A == 4 ? (const void*)shifted : (const void*)ys); publish(); return; }
+    if (ticketed) publish();
+    else if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // shared memory must outlive the bulk store's reads
     QS_STAMP(9);
 }
 

@@ -414,7 +414,7 @@ size_t step_smem_bytes(const StepArgs& a) {
 }
 
 template <bool RAW, bool PIDACT>
-cudaError_t launch_step(const StepArgs& a, cudaStream_t s) {
+cudaError_t launch_step(const StepArgs& a, bool pdl_ok, cudaStream_t s) {
     const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
     const int threads = ((a.tpb + 31) / 32) * 32;
     const size_t sm = step_smem_bytes(a);
@@ -424,7 +424,7 @@ cudaError_t launch_step(const StepArgs& a, cudaStream_t s) {
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = (pdl && pdl_ok) ? 1 : 0;
 #define QS_CASE(E)                                                                                               \
     case E: {                                                                                                    \
         if (sm > 48 * 1024)      /* per device and cheap: no process-wide "already set" flag */                 \
@@ -441,9 +441,9 @@ cudaError_t launch_step(const StepArgs& a, cudaStream_t s) {
 
 }  // namespace
 
-cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, cudaStream_t s) {
-    if (raw) return pid_act ? launch_step<true, true>(a, s) : launch_step<true, false>(a, s);
-    return pid_act ? launch_step<false, true>(a, s) : launch_step<false, false>(a, s);
+cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s) {
+    if (raw) return pid_act ? launch_step<true, true>(a, pdl_ok, s) : launch_step<true, false>(a, pdl_ok, s);
+    return pid_act ? launch_step<false, true>(a, pdl_ok, s) : launch_step<false, false>(a, pdl_ok, s);
 }
 
 }  // namespace qsi

@@ -329,8 +329,11 @@ class BaseAviary(Env):
         io.dw_fz = self._dw_fz.data_ptr() if self._dw_fz is not None else None
         io.act_buffer_size = self._B
         io.tick_substeps = 0
-        self._pdl_hint = torch.zeros((1,), dtype=torch.int32, device=dev)
-        io.pdl_hint = self._pdl_hint.data_ptr()
+        # per-warp readiness of the fast step kernel (include/quadsim.h): consecutive steps of this env overlap warp by warp
+        self._warp_ticket = torch.zeros(((n + 31) // 32,), dtype=torch.int32, device=dev)
+        self._warp_done = torch.zeros(((n + 31) // 32,), dtype=torch.int32, device=dev)
+        self._ready_err = torch.zeros((1,), dtype=torch.int32, device=dev)
+        io.warp_ticket, io.warp_done, io.ready_err = self._warp_ticket.data_ptr(), self._warp_done.data_ptr(), self._ready_err.data_ptr()
         self._io = io
         #### pre-resolved handles for the per-step fast path ####
         self._obs_ptr = [b.data_ptr() for b in self._obs_buf]

@@ -39,7 +39,8 @@
 extern "C" {
 #endif
 
-#define QS_ABI_VERSION 2     /* 2: the persistent state (planes, last_rpm, pid, init/target tables) is float64 */
+#define QS_ABI_VERSION 3     /* 2: the persistent state (planes, last_rpm, pid, init/target tables) is float64;
+                                3: QsStepIO.pdl_hint replaced by the per-warp readiness words */
 
 /* drone models (utils/enums.py:3-9) */
 enum { QS_MODEL_CF2X = 0, QS_MODEL_CF2P = 1, QS_MODEL_RACE = 2 };
@@ -171,12 +172,14 @@ typedef struct QsStepIO {
     unsigned* gather_counter;           /* one zeroed device word owned by the caller (arrival count); required with gather_flag */
     unsigned gather_seq;
     unsigned pad_;
-    unsigned* pdl_hint;                 /* optional device word owned by the caller (one per env, zero-initialised): the kernel records in it
-                                           whether its launch found a programmatic-dependent-launch window (it was resident while its
-                                           predecessor still ran); the next launch on the same buffers then prefetches its observation
-                                           history into L2 during that window, and an isolated launch does not (the prefetch would only
-                                           delay its state loads).  NULL = always prefetch.  Read only when the history prefetch is
-                                           enabled (QS_PREFETCH=2; off by default: on the H100 it slows back-to-back launches). */
+    /* Per-warp readiness of the fast step kernels (DESIGN.md 4.1): device words owned by the caller, zero-initialised once, and
+     * passed with EVERY qs_step / qs_step_host call on the same state and observation buffers (or never).  With them a warp of
+     * 32 drones waits only for the warp of the previous step on these buffers that owns the same 32 drones, instead of for the
+     * whole previous kernel of the stream, so consecutive steps overlap.  All NULL = the whole-grid wait.
+     * ready_err becomes non-zero if a warp ever waited longer than ~1 s for its turn (the step then went ahead unordered). */
+    unsigned* warp_ticket;              /* [ceil(N / 32)] */
+    unsigned* warp_done;                /* [ceil(N / 32)] */
+    unsigned* ready_err;                /* one word */
 } QsStepIO;
 
 /* Spins (bounded, ~2 s, then *err_flag = 1) until flags[r] - seq >= 0 for every r < world: the learner side of obs_gather. */
@@ -276,7 +279,16 @@ int qs_sizeof_rollout_io(void);
 int qs_sizeof_host_io(void);
 
 /* One control tick for n_envs aviaries of drones_per_env drones: action decode -> `substeps` x DYN ->
- * obs / reward / terminated / truncated (+ autoreset).  RL action types; task = QS_TASK_HOVER or NONE. */
+ * obs / reward / terminated / truncated (+ autoreset).  RL action types; task = QS_TASK_HOVER or NONE.
+ *
+ * Ordering with the work before it on `stream`: the step kernels are launched as programmatic dependents (they may start
+ * before the previous kernel of the stream has finished).  With QsStepIO.warp_ticket / warp_done a fast step kernel does
+ * not wait for the whole previous kernel when that kernel is a fast step of this library: it then waits per warp for the
+ * previous step on its own buffers only.  Kernels and copies that do not trigger their successor early (torch kernels,
+ * qs_reset, qs_rollout, memcpy) are complete before the step starts, and the library's other early-triggering kernels are
+ * always waited for.  The caller's side of the contract: a kernel of the caller's own that triggers programmatic launch
+ * early (griddepcontrol.launch_dependents / cudaTriggerProgrammaticLaunchCompletion) must not directly precede qs_step
+ * on the stream when it writes that step's action or state. */
 int qs_step(const QsParams* p, const QsState* st, const QsStepIO* io, int act_type, int task,
             int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 

@@ -1,6 +1,6 @@
 """Per-warp phase timeline of the fast step kernel (tools, not product): builds a -DQS_TIMELINE copy of the library
 (build/libquadsim_timeline.so, %globaltimer stamps by lane 0 of every warp), runs the bench workload and prints where a
-warp's time goes.  Stamps: 0 start, 1 after griddepcontrol.wait, 2 loads issued / bulk copy issued (= state arrived with
+warp's time goes.  Stamps: 0 start, 1 after the readiness wait (per-warp ticket, and griddepcontrol.wait when kept), 2 loads issued / bulk copy issued (= state arrived with
 QS_LATE_TMA=1), 3 physics done, 4 state stored, 5 old span arrived, 6 bulk store + terminal rows issued, 7 exit.
 
     python tools/timeline.py --build          # here (nvcc)
