@@ -97,7 +97,7 @@ class QsHostIO(C.Structure):
 
 
 class QsLogRing(C.Structure):
-    _fields_ = [("ring", C.c_void_p), ("head", C.c_void_p), ("capacity", C.c_int), ("first_drone", C.c_int), ("n_drones", C.c_int), ("pad_", C.c_int)]
+    _fields_ = [("ring", C.c_void_p), ("head", C.c_void_p), ("capacity", C.c_int), ("first_drone", C.c_int), ("n_drones", C.c_int), ("kin_rows", C.c_int)]
 
 
 class QsStepCall(C.Structure):

@@ -205,7 +205,7 @@ __global__ void log_append_kernel(QsParams P, QsState st, const float* __restric
         double roll, pitch, yaw;
         qs::quat_to_euler<false>(d.qx, d.qy, d.qz, d.qw, roll, pitch, yaw);
         const float* row = obs + i * obs_dim;
-        const int av = obs_dim == 20 ? 13 : 9;                                  // ang_v in a state vector / in a KIN row
+        const int av = (obs_dim == 20 && !rg.kin_rows) ? 13 : 9;                // ang_v in a state vector / in a KIN row
         double* o = rg.ring + ((head % rg.capacity) * rg.n_drones + j) * 32;
         o[0] = d.px; o[1] = d.py; o[2] = d.pz; o[3] = d.vx; o[4] = d.vy; o[5] = d.vz;          // Logger.py:117
         o[6] = roll; o[7] = pitch; o[8] = yaw;

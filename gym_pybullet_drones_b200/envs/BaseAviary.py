@@ -829,7 +829,7 @@ class BaseAviary(Env):
         yaw = torch.atan2(2.0 * (x * y + w * z), w * w + x * x - y * y - z * z)
         rpy = torch.stack([roll, pitch, yaw], dim=1)
         obs = self._obs_buf[self._cur]
-        ang_v = obs[:, 13:16].double() if self._obs_dim == 20 else obs[:, 9:12].double()
+        ang_v = obs[:, 13:16].double() if self._state20_obs() else obs[:, 9:12].double()      # (a KIN row can be 20 wide)
         sv = torch.cat([pos, quat, rpy, vel, ang_v, self._last_rpm], dim=1)
         return sv.view(self._E, self._D, 20).cpu().numpy()
 

@@ -144,6 +144,8 @@ class BaseRLAviary(BaseAviary):
                 out["values"] = torch.empty((T, E), dtype=torch.float32, device=dev)
         tmax = self._lib.qs_rollout_max_ticks(self._act_type(), self._B, D)
         if tmax <= 0:
+            if self._B == 0:
+                raise ValueError("rollout() needs an action buffer: ctrl_freq=%d gives ACTION_BUFFER_SIZE = 0" % self.CTRL_FREQ)
             raise ValueError("rollout() is not available for this observation width (action buffer too long for shared memory)")
         io = N.QsRolloutIO()
         io.seed, io.act_buffer_size = int(seed) & 0xFFFFFFFFFFFFFFFF, self._B

@@ -80,6 +80,7 @@ class Logger(object):
         rg = N.QsLogRing()
         rg.ring, rg.head, rg.capacity = self._ring.data_ptr(), self._head.data_ptr(), cap
         rg.first_drone, rg.n_drones = aviary * env.NUM_DRONES, self.NUM_DRONES
+        rg.kin_rows = 0 if env._state20_obs() else 1          # a KIN row can be 20 floats wide as well
         self._rg, self._env, self._flushed = rg, env, 0
         env._log = (rg, self._ctrl_dev)
         return self

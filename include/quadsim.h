@@ -405,12 +405,13 @@ int qs_reset_heads(const QsState* st, int rows, unsigned flags, float* out, void
  * ang_v3, rpm4), the 12 control targets, the simulation time of the entry and 3 pad doubles -- 32 float64 per drone and
  * entry, ring[(head % capacity)][drone][32]; the kernel then advances *head.  pos/vel/rpm come from the float64 state
  * (planes, last_rpm), rpy is re-evaluated from the quaternion in float64, ang_v is taken from the observation rows
- * (float32: obs_dim = 20 state vectors or KIN rows).  controls: [n_drones][12] float32 device array or NULL (zeros).
+ * (float32: columns 9-11 of a KIN row, 13-15 of a [20] state vector).  kin_rows = 1: the rows are KIN observations whatever
+ * obs_dim (a KIN row is 20 floats wide too, e.g. ONE_D_RPM at ctrl_freq 16); 0: state vectors iff obs_dim == 20.  controls: [n_drones][12] float32 device array or NULL (zeros).
  * Nothing crosses PCIe until the caller copies the ring (Logger.save). */
 typedef struct QsLogRing {
     double* ring;            /* [capacity][n_drones][32] */
     long long* head;         /* device counter: entries appended so far */
-    int capacity, first_drone, n_drones, pad_;
+    int capacity, first_drone, n_drones, kin_rows;
 } QsLogRing;
 int qs_sizeof_log_ring(void);
 int qs_log_append(const QsParams* p, const QsState* st, const float* obs, int obs_dim, const float* controls,

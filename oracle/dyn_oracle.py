@@ -424,7 +424,7 @@ class OracleAviary:
         action = np.asarray(action)
         if self.kind == "ctrl":
             return np.clip(action.astype(self.dtype), 0, P.MAX_RPM)
-        if self.kind != "velocity":
+        if self.kind != "velocity" and self.B > 0:                                # deque(maxlen=0) at ctrl_freq 1: no buffer
             self.action_buffer.pop(0)
             self.action_buffer.append(action.copy())                             # :187 (deque maxlen)
         # NumPy-2 promotion (reference pins numpy ^2.2, pyproject.toml:15): python scalars are weak,

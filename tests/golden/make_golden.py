@@ -1,7 +1,8 @@
 """Regenerates tests/golden/*.npz by running the UNMODIFIED reference (tier-1 oracle).
 
 Needs a checkout of the reference (oracle/ref_loader.py, QS_REFERENCE_ROOT):
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py              # every fixture
+    python tests/golden/make_golden.py rl_configs   # rl_configs.npz only
 The reference's Physics.DYN path is executed through the stand-in modules of
 oracle/standins/ (see oracle/ref_loader.py); everything recorded here is float64
 output of the reference's own code.  The tests read only the fixtures, never the
@@ -277,6 +278,57 @@ def adjacency_fixture():
     save("adjacency", **out)
 
 
+# Single-aviary RL trajectories away from the 240 Hz / CF2X defaults: other drone models, physics and control rates (the
+# substep count S and the action-buffer length B = ctrl_freq // 2 with it), initial attitudes, the episode time-out at
+# 1000 Hz, B = 0 (ctrl_freq = 1), the embedded PID at 60 Hz and actions far outside [-1, 1] (RPM is not clipped,
+# BaseRLAviary.py:192,225).  `obs_every`: observation recorded every k ticks.
+RL_CONFIG_CASES = [
+    dict(key="race_500_50_rpm", kind="hover", model="racer", pyb=500, ctrl=50, act="rpm", T=100, obs_every=10, seed=101),
+    dict(key="cf2p_240_16_one_d_rpm", kind="hover", model="cf2p", pyb=240, ctrl=16, act="one_d_rpm", T=80, obs_every=5, seed=102),
+    dict(key="multi3_race_240_80_rpm_rpys", kind="multihover", nd=3, model="racer", pyb=240, ctrl=80, act="rpm", T=150, obs_every=10,
+         seed=103, rpys=[[0.1, -0.05, 0.3], [-0.08, 0.12, -0.7], [0.03, 0.02, 1.9]]),
+    dict(key="cf2x_1000_50_one_d_rpm_timeout", kind="hover", model="cf2x", pyb=1000, ctrl=50, act="one_d_rpm", T=405, obs_every=25,
+         seed=None),
+    dict(key="cf2x_240_1_one_d_rpm_b0", kind="hover", model="cf2x", pyb=240, ctrl=1, act="one_d_rpm", T=12, obs_every=1, seed=105,
+         scale=0.02),                # small enough to stay in the box until the time-out on tick 10
+    dict(key="cf2p_240_60_pid", kind="hover", model="cf2p", pyb=240, ctrl=60, act="pid", T=240, obs_every=10, seed=106),
+    dict(key="cf2x_240_30_rpm_x30", kind="hover", model="cf2x", pyb=240, ctrl=30, act="rpm", T=40, obs_every=1, seed=107, scale=30.0),
+]
+
+
+def rl_config_actions(c):
+    """float32 actions [T, D, A] of one RL_CONFIG_CASES entry."""
+    nd = c.get("nd", 1)
+    aw = {"rpm": 4, "one_d_rpm": 1, "pid": 3}[c["act"]]
+    if c["seed"] is None:
+        return np.zeros((c["T"], nd, aw), np.float32)
+    rng = np.random.default_rng(c["seed"])
+    if c["act"] == "pid":           # piecewise-constant set-points inside the truncation box, like rl_pid_cf30
+        seg = (np.array([0, 0, 1.0], np.float32) + 0.5 * rng.uniform(-1, 1, (4, nd, aw)).astype(np.float32)).astype(np.float32)
+        return np.repeat(seg, c["T"] // 4, axis=0)
+    return (np.float32(c.get("scale", 1.0)) * rng.uniform(-1, 1, (c["T"], nd, aw)).astype(np.float32)).astype(np.float32)
+
+
+def rl_config_fixture():
+    """RL_CONFIG_CASES through the reference's HoverAviary / MultiHoverAviary -> rl_configs.npz."""
+    import json
+    A = R.ActionType
+    acts_enum = {"rpm": A.RPM, "one_d_rpm": A.ONE_D_RPM, "pid": A.PID}
+    models = {"cf2x": R.DroneModel.CF2X, "cf2p": R.DroneModel.CF2P, "racer": R.DroneModel.RACE}
+    out = {"cases": np.array(json.dumps(RL_CONFIG_CASES))}
+    for c in RL_CONFIG_CASES:
+        kw = dict(drone_model=models[c["model"]], physics=R.Physics.DYN, pyb_freq=c["pyb"], ctrl_freq=c["ctrl"], act=acts_enum[c["act"]])
+        if "rpys" in c:
+            kw["initial_rpys"] = np.array(c["rpys"])
+        with quiet():
+            env = R.HoverAviary(**kw) if c["kind"] == "hover" else R.MultiHoverAviary(num_drones=c["nd"], **kw)
+            rec = run_env(env, rl_config_actions(c), record_obs_every=c["obs_every"])
+        if c["kind"] == "multihover":
+            rec["TARGET_POS"] = np.asarray(env.TARGET_POS)
+        out.update(flat(c["key"], rec))
+    save("rl_configs", **out)
+
+
 def logger_fixture():
     """utils/Logger.log (Logger.py:83-127) of 3 drones over 7 ticks of random states and controls: the logged arrays."""
     import types
@@ -296,5 +348,9 @@ def logger_fixture():
 
 
 if __name__ == "__main__":
-    main()
-    logger_fixture()
+    if sys.argv[1:] == ["rl_configs"]:      # only rl_configs.npz; the other fixtures stay as they are
+        rl_config_fixture()
+    else:
+        main()
+        logger_fixture()
+        rl_config_fixture()

@@ -32,7 +32,7 @@ def state_of(env):
     obs = env._obs_buf[env._cur].view(env._E, env._D, env._obs_dim).double().cpu().numpy()
     assert env._planes.dtype == torch.float64
     out = dict(pos=env.pos.cpu().numpy(), quat=env.quat.cpu().numpy(), vel=env.vel.cpu().numpy(), rpy_rates=env.rpy_rates.cpu().numpy())
-    if env._obs_dim == 20:
+    if env._state20_obs():          # (not the width: a KIN row is 20 floats wide at ONE_D_RPM / ctrl_freq 16)
         out["rpy"], out["ang_v"] = obs[..., 7:10], obs[..., 13:16]
     else:
         out["rpy"], out["ang_v"] = obs[..., 3:6], obs[..., 9:12]

@@ -120,6 +120,72 @@ def test_rl_env_with_embedded_pid_teacher_forced(golden, key, kind, nd, act):
         assert bool(tr[0]) == bool(g[key + "_truncated"][t])
 
 
+def rl_config_cases(g):
+    import json
+    return {c["key"]: c for c in json.loads(str(g["cases"]))}
+
+
+def rl_config_oracle(c, num_envs=1):
+    return O.OracleAviary(c["kind"], num_envs, c.get("nd", 1), drone_model=c["model"], pyb_freq=c["pyb"], ctrl_freq=c["ctrl"],
+                          act=c["act"], initial_rpys=c.get("rpys"))
+
+
+RL_CONFIG_FREE = ["race_500_50_rpm", "cf2p_240_16_one_d_rpm", "multi3_race_240_80_rpm_rpys", "cf2x_1000_50_one_d_rpm_timeout",
+                  "cf2x_240_1_one_d_rpm_b0", "cf2x_240_30_rpm_x30"]
+
+
+@pytest.mark.parametrize("key", RL_CONFIG_FREE)
+def test_rl_configs(golden, key):
+    """Other drone models, rates, initial attitudes, B = 0 and out-of-range actions: whole trajectories at TOL."""
+    g = golden("rl_configs")
+    c = rl_config_cases(g)[key]
+    env = rl_config_oracle(c)
+    if c["kind"] == "multihover":
+        assert relerr(env.TARGET_POS[0], g[key + "_TARGET_POS"]) == 0
+    assert env.B == c["ctrl"] // 2 and env.P.S == c["pyb"] // c["ctrl"]
+    replay(env, g, key, c["obs_every"])
+    assert g[key + "_obs"].shape[-1] == 12 + env.B * env.A
+
+
+def test_rl_configs_time_out_ticks(golden):
+    """The time-out tick follows pyb_freq: step_counter / PYB_FREQ > EPISODE_LEN_SEC first holds on tick 402 at 1000/50
+    (step counter 8020 before the tick's increment) and on tick 10 at 240/1."""
+    g = golden("rl_configs")
+    for key, first in (("cf2x_1000_50_one_d_rpm_timeout", 402), ("cf2x_240_1_one_d_rpm_b0", 10)):
+        tr = g[key + "_truncated"]
+        assert int(np.argmax(tr)) + 1 == first and tr[first - 1:].all(), key
+
+
+def test_rl_configs_pid_60hz_teacher_forced(golden):
+    """CF2P 240/60 with the embedded PID: every tick from the reference's previous state and controller integrals."""
+    key = "cf2p_240_60_pid"
+    g = golden("rl_configs")
+    c = rl_config_cases(g)[key]
+    env = rl_config_oracle(c)
+    acts = g[key + "_actions"]
+    env.reset()
+    for t in range(acts.shape[0]):
+        force_state(env, g, key, t - 1)
+        obs, r, te, tr = env.step(acts[t][None])
+        for f in FIELDS:
+            assert relerr(getattr(env, f)[0], g[key + "_" + f][t]) < 1e-11, (key, f, t)
+        assert relerr(env.ctrl.integral_rpy_e, g[key + "_pid_integral_rpy_e"][t]) < 1e-11
+        assert relerr(env.ctrl.integral_pos_e, g[key + "_pid_integral_pos_e"][t]) < 1e-11
+        assert abs(r[0] - g[key + "_reward"][t]) < 1e-10
+        assert bool(tr[0]) == bool(g[key + "_truncated"][t])
+        if t % c["obs_every"] == 0:
+            assert relerr(obs[0], g[key + "_obs"][t // c["obs_every"]]) < 1e-6, t
+
+
+def test_oracle_without_action_buffer():
+    """ctrl_freq = 1: B = 0, the observation is the 12-column kinematic head and stepping keeps no buffer."""
+    env = O.OracleAviary("hover", 2, 1, ctrl_freq=1, act="one_d_rpm")
+    assert env.B == 0 and env.reset().shape == (2, 1, 12)
+    for _ in range(3):
+        obs, r, te, tr = env.step(np.zeros((2, 1, 1), np.float32))
+        assert obs.shape == (2, 1, 12) and env.action_buffer == []
+
+
 @pytest.mark.parametrize("model", ["cf2x", "cf2p"])
 def test_pid_circle(golden, model):
     """examples/pid.py workload: CtrlAviary(DYN, 240/48) x 3 drones tracked by DSLPIDControl.  Free-running for the
