@@ -30,7 +30,8 @@ FLAG_AUTORESET_SAME_STEP, FLAG_AUTORESET_NEXT_STEP, FLAG_RPY_F32 = 1, 2, 4
 FLAG_AUTORESET_CLEARS_PID, FLAG_AUTORESET_CLEARS_HISTORY = 8, 16
 FLAG_OBS_STATE20 = 32
 FLAG_SKIP_EPILOGUE, FLAG_RPM_FROM_LAST, FLAG_ACTION_F64 = 0x100, 0x200, 0x400
-ABI_VERSION = 3
+ABI_VERSION = 4
+PHYS_WIDTH = 16          # float64 columns of one QsState.phys row
 
 _d = C.c_double
 
@@ -58,6 +59,7 @@ class QsState(C.Structure):
         ("planes", C.c_void_p), ("last_rpm", C.c_void_p), ("step_counter", C.c_void_p), ("pending_reset", C.c_void_p),
         ("pid", C.c_void_p), ("init_pos", C.c_void_p), ("init_quat", C.c_void_p), ("target_pos", C.c_void_p),
         ("reset_head", C.c_void_p), ("pos_f32", C.c_void_p), ("tables_per_env", C.c_int), ("pad_", C.c_int),
+        ("phys", C.c_void_p),
     ]
 
 

@@ -253,6 +253,26 @@ __device__ __forceinline__ void init_drone(const QsState& st, long long tbl, qs:
     d.wx = d.wy = d.wz = 0.0;
 }
 
+// row e of QsState.phys (include/quadsim.h): 7 x 16 bytes of the 128-byte row through the read-only path.  The drones of one
+// aviary read the same row, so within a warp the loads are broadcasts; the padding is never read.
+__device__ __forceinline__ qs::PhysRow load_phys(const double* phys, long long e) {
+    const double2* r = reinterpret_cast<const double2*>(phys + 16 * e);
+    const double2 v0 = __ldg(r), v1 = __ldg(r + 1), v2 = __ldg(r + 2), v3 = __ldg(r + 3), v4 = __ldg(r + 4), v5 = __ldg(r + 5), v6 = __ldg(r + 6);
+    qs::PhysRow c;
+    c.inv_m = v0.x; c.gravity = v0.y; c.kf = v1.x; c.km = v1.y; c.kx = v2.x; c.ky = v2.y;
+    c.j[0] = v3.x; c.j[1] = v3.y; c.j[2] = v4.x; c.j_inv[0] = v4.y; c.j_inv[1] = v5.x; c.j_inv[2] = v5.y;
+    c.hover_rpm = v6.x; c.max_rpm = v6.y;
+    return c;
+}
+// only the two columns the action decode reads (HOVER_RPM, MAX_RPM): the embedded PID controller runs between the decode and the
+// physics, and the full row live across it would spill
+__device__ __forceinline__ qs::PhysRow load_phys_rpm(const double* phys, long long e) {
+    const double2 v6 = __ldg(reinterpret_cast<const double2*>(phys + 16 * e) + 6);
+    qs::PhysRow c;
+    c.hover_rpm = v6.x; c.max_rpm = v6.y;
+    return c;
+}
+
 __device__ __forceinline__ void load_rpm(const double* last_rpm, long long i, double rpm[4]) {
     const D4 v = ld256(last_rpm, i);
     rpm[0] = v.x; rpm[1] = v.y; rpm[2] = v.z; rpm[3] = v.w;

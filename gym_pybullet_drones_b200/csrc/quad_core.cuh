@@ -197,21 +197,26 @@ QS_HD void integrate_q(Drone& d, double dt) {
 // `between` is called after every substep with its index (the fused kernels poll an asynchronous copy there).
 struct NoHook { QS_HD void operator()(int) const {} };
 
-template <int EFF, class Hook = NoHook>
-QS_HD void dyn_tick(const QsParams& P, Drone& d, const double rpm[4], const double rpm_prev[4], double dw_fz,
-                    int substeps, double R_last[9], Hook between = Hook()) {
+// The drone's physical constants -- M (as 1/M), GRAVITY, KF, KM, the arm inside kx/ky, J, J^-1, HOVER_RPM, MAX_RPM -- come
+// from `c`: the QsParams themselves (one drone for the whole batch), or the aviary's PhysRow when QsState.phys is set.
+// Everything else (time step, mixing signs, DYN+ coefficients, task, embedded controller) always comes from P.
+struct PhysRow { double inv_m, gravity, kf, km, kx, ky, j[3], j_inv[3], hover_rpm, max_rpm; };
+
+template <int EFF, class K, class Hook = NoHook>
+QS_HD void dyn_tick_k(const QsParams& P, const K& c, Drone& d, const double rpm[4], const double rpm_prev[4], double dw_fz,
+                      int substeps, double R_last[9], Hook between = Hook()) {
     const double dt = P.dt;
-    const double dt_m = dt * P.inv_m;                                                // v += dt * (F / M)  (:858,:860)
+    const double dt_m = dt * c.inv_m;                                                // v += dt * (F / M)  (:858,:860)
     double f[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) f[i] = rpm[i] * rpm[i] * P.kf;                       // :838
+    for (int i = 0; i < 4; ++i) f[i] = rpm[i] * rpm[i] * c.kf;                       // :838
     // z torque (:842-845); sz carries the -1,+1,-1,+1 pattern (negated for RACE)
-    const double zt0 = rpm[0] * rpm[0] * P.km, zt1 = rpm[1] * rpm[1] * P.km,
-                 zt2 = rpm[2] * rpm[2] * P.km, zt3 = rpm[3] * rpm[3] * P.km;
+    const double zt0 = rpm[0] * rpm[0] * c.km, zt1 = rpm[1] * rpm[1] * c.km,
+                 zt2 = rpm[2] * rpm[2] * c.km, zt3 = rpm[3] * rpm[3] * c.km;
     const double tz = P.sz[0] * zt0 + P.sz[1] * zt1 + P.sz[2] * zt2 + P.sz[3] * zt3;
     double thrust = f[0] + f[1] + f[2] + f[3];                                       // :839
-    double tx = (P.sx[0] * f[0] + P.sx[1] * f[1] + P.sx[2] * f[2] + P.sx[3] * f[3]) * P.kx;   // :846-854
-    double ty = (P.sy[0] * f[0] + P.sy[1] * f[1] + P.sy[2] * f[2] + P.sy[3] * f[3]) * P.ky;
+    double tx = (P.sx[0] * f[0] + P.sx[1] * f[1] + P.sx[2] * f[2] + P.sx[3] * f[3]) * c.kx;   // :846-854
+    double ty = (P.sy[0] * f[0] + P.sy[1] * f[1] + P.sy[2] * f[2] + P.sy[3] * f[3]) * c.ky;
     double drag_sum = 0.0;
     if (EFF & QS_EFFECT_DRAG) {                                                      // :773
         const double k = 2.0 * 3.14159265358979323846;
@@ -231,9 +236,9 @@ QS_HD void dyn_tick(const QsParams& P, Drone& d, const double rpm[4], const doub
     }
     double q0x = d.qx, q0y = d.qy, q0z = d.qz, q0w = d.qw;                           // attitude at the start of the last substep
     // per-tick constants of the Euler step: dt*J^-1, the gyroscopic differences (w x Jw for a diagonal J), dt/M*gravity
-    const double dj0 = dt * P.j_inv[0], dj1 = dt * P.j_inv[1], dj2 = dt * P.j_inv[2];
-    const double g21 = P.j[2] - P.j[1], g02 = P.j[0] - P.j[2], g10 = P.j[1] - P.j[0];
-    const double gm = dt_m * P.gravity;
+    const double dj0 = dt * c.j_inv[0], dj1 = dt * c.j_inv[1], dj2 = dt * c.j_inv[2];
+    const double g21 = c.j[2] - c.j[1], g02 = c.j[0] - c.j[2], g10 = c.j[1] - c.j[0];
+    const double gm = dt_m * c.gravity;
     const double tm2 = 2.0 * (dt_m * thrust), tmg = dt_m * thrust - gm;             // EFF == 0: thrust is constant over the tick
     for (int s = 0; s < substeps; ++s) {
         q0x = d.qx; q0y = d.qy; q0z = d.qz; q0w = d.qw;
@@ -258,12 +263,12 @@ QS_HD void dyn_tick(const QsParams& P, Drone& d, const double rpm[4], const doub
                 const double hz = d.pz + r20 * P.prop_xyz[i][0] + r21 * P.prop_xyz[i][1] + r22 * P.prop_xyz[i][2];
                 const double h = hz < P.gnd_eff_h_clip ? P.gnd_eff_h_clip : hz;       // :739-740
                 const double rr = P.prop_radius / (4.0 * h);
-                g[i] = upright ? rpm[i] * rpm[i] * P.kf * P.gnd_eff_coeff * (rr * rr) : 0.0;   // :741
+                g[i] = upright ? rpm[i] * rpm[i] * c.kf * P.gnd_eff_coeff * (rr * rr) : 0.0;   // :741
             }
             const double f0 = f[0] + g[0], f1 = f[1] + g[1], f2 = f[2] + g[2], f3 = f[3] + g[3];
             thrust = f0 + f1 + f2 + f3;
-            tx = (P.sx[0] * f0 + P.sx[1] * f1 + P.sx[2] * f2 + P.sx[3] * f3) * P.kx;
-            ty = (P.sy[0] * f0 + P.sy[1] * f1 + P.sy[2] * f2 + P.sy[3] * f3) * P.ky;
+            tx = (P.sx[0] * f0 + P.sx[1] * f1 + P.sx[2] * f2 + P.sx[3] * f3) * c.kx;
+            ty = (P.sy[0] * f0 + P.sy[1] * f1 + P.sy[2] * f2 + P.sy[3] * f3) * c.ky;
         }
         if (EFF == 0) {
             // v += dt (R[:,2] thrust - [0,0,GRAVITY]) / M   (:840-841,:858,:860) with R[:,2] = (2(xz+wy), 2(yz-wx), 1-2(xx+yy)):
@@ -272,7 +277,7 @@ QS_HD void dyn_tick(const QsParams& P, Drone& d, const double rpm[4], const doub
             d.vy = d.vy + (y * z - w * x) * tm2;
             d.vz = (d.vz + tmg) - (x * x + y * y) * tm2;
         } else {
-            double fx = r02 * thrust, fy = r12 * thrust, fz = r22 * thrust - P.gravity;  // :840-841
+            double fx = r02 * thrust, fy = r12 * thrust, fz = r22 * thrust - c.gravity;  // :840-841
             if (EFF & QS_EFFECT_DRAG) {                                                  // world force = -DRAG_COEFF*sum (.) vel
                 fx += (-1.0 * P.drag_coeff[0] * drag_sum) * d.vx;
                 fy += (-1.0 * P.drag_coeff[1] * drag_sum) * d.vy;
@@ -301,6 +306,12 @@ QS_HD void dyn_tick(const QsParams& P, Drone& d, const double rpm[4], const doub
         between(s);
     }
     quat_to_matrix_unit(q0x, q0y, q0z, q0w, R_last);                                 // R used by :873 (ang_v = R_old w_new)
+}
+
+template <int EFF, class Hook = NoHook>
+QS_HD void dyn_tick(const QsParams& P, Drone& d, const double rpm[4], const double rpm_prev[4], double dw_fz,
+                    int substeps, double R_last[9], Hook between = Hook()) {
+    dyn_tick_k<EFF>(P, P, d, rpm, rpm_prev, dw_fz, substeps, R_last, between);
 }
 
 template <bool RPY_F32>
@@ -383,18 +394,19 @@ QS_HD void pid_control(const QsParams& P, PidState& st, double dt,
 // ---- action decoding (BaseRLAviary._preprocessAction, envs/BaseRLAviary.py:160-239) -----------------
 // `a` = this drone's float32 action; `der` = the cached kinematics the reference reads through
 // _getDroneStateVector (rpy from the end of the previous tick).  PID variants update `pst`.
-template <bool PIDACT>
-QS_HD void decode_action(const QsParams& P, int act_type, const float a[4], const Drone& d, double cur_yaw,
-                         PidState& pst, double rpm[4]) {
+// HOVER_RPM and MAX_RPM come from `c` (see dyn_tick_k); the embedded controller keeps P's constants (BaseRLAviary.py:76).
+template <bool PIDACT, class K>
+QS_HD void decode_action_k(const QsParams& P, const K& c, int act_type, const float a[4], const Drone& d, double cur_yaw,
+                           PidState& pst, double rpm[4]) {
     if (act_type == QS_ACT_RPM) {                                                    // :192
 #pragma unroll
-        for (int i = 0; i < 4; ++i) rpm[i] = P.hover_rpm * (double)f32_add(1.0f, f32_mul(0.05f, a[i]));
+        for (int i = 0; i < 4; ++i) rpm[i] = c.hover_rpm * (double)f32_add(1.0f, f32_mul(0.05f, a[i]));
     } else if (act_type == QS_ACT_ONE_D_RPM) {                                       // :225
-        const double v = P.hover_rpm * (double)f32_add(1.0f, f32_mul(0.05f, a[0]));
+        const double v = c.hover_rpm * (double)f32_add(1.0f, f32_mul(0.05f, a[0]));
         rpm[0] = rpm[1] = rpm[2] = rpm[3] = v;
     } else if (act_type == QS_ACT_RAW_RPM) {                                         // CtrlAviary.py:140
 #pragma unroll
-        for (int i = 0; i < 4; ++i) rpm[i] = clampd((double)a[i], 0.0, P.max_rpm);
+        for (int i = 0; i < 4; ++i) rpm[i] = clampd((double)a[i], 0.0, c.max_rpm);
     } else if (PIDACT) {
         double tpx, tpy, tpz, tyaw = 0.0, tvx = 0.0, tvy = 0.0, tvz = 0.0;
         if (act_type == QS_ACT_PID) {                                                // :194-207, _calculateNextStep :1108-1150
@@ -416,6 +428,12 @@ QS_HD void decode_action(const QsParams& P, int act_type, const float a[4], cons
         pid_control(P, pst, P.ctrl_dt, d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz,
                     tpx, tpy, tpz, tyaw, tvx, tvy, tvz, 0.0, 0.0, 0.0, rpm, pe, ye);
     }
+}
+
+template <bool PIDACT>
+QS_HD void decode_action(const QsParams& P, int act_type, const float a[4], const Drone& d, double cur_yaw,
+                         PidState& pst, double rpm[4]) {
+    decode_action_k<PIDACT>(P, P, act_type, a, d, cur_yaw, pst, rpm);
 }
 
 // ---- task: Hover / MultiHover per-drone terms ----------------------------------------------------

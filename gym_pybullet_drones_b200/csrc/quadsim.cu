@@ -333,6 +333,7 @@ int check_state(const QsState* st, int need_tables) {
     if (!aligned32(st->planes)) return fail(QS_ERR_ALIGN, "QsState.planes must be 32-byte aligned");
     if (st->last_rpm && !aligned32(st->last_rpm)) return fail(QS_ERR_ALIGN, "QsState.last_rpm must be 32-byte aligned");
     if (st->pos_f32 && !aligned16(st->pos_f32)) return fail(QS_ERR_ALIGN, "QsState.pos_f32 must be 16-byte aligned");
+    if (st->phys && !aligned32(st->phys)) return fail(QS_ERR_ALIGN, "QsState.phys must be 32-byte aligned");
     if (need_tables) {
         if (!st->init_pos || !st->init_quat) return fail(QS_ERR_NULL, "QsState: init_pos/init_quat is NULL");
         if (!aligned32(st->init_pos) || !aligned32(st->init_quat)) return fail(QS_ERR_ALIGN, "init tables must be 32-byte aligned");
@@ -396,6 +397,7 @@ static int prepare_step(const QsParams* p, const QsState* st, const QsStepIO* io
     if ((effects & QS_EFFECT_DW) && !io->dw_fz && drones_per_env > kMaxTPB)
         return fail(QS_ERR_UNSUPPORTED, "qs_step: in-CTA downwash needs drones_per_env <= 128 (else pass dw_fz from qs_downwash, substeps = 1)");
     if ((effects & QS_EFFECT_DW) && io->dw_fz && substeps != 1) return fail(QS_ERR_UNSUPPORTED, "qs_step: external dw_fz requires substeps == 1");
+    if (st->phys && io->dw_fz) return fail(QS_ERR_UNSUPPORTED, "qs_step: per-aviary physical constants (QsState.phys) are not supported with external downwash (dw_fz)");
     if ((flags & QS_FLAG_AUTORESET_NEXT_STEP) && !st->pending_reset) return fail(QS_ERR_NULL, "qs_step: NEXT_STEP autoreset needs pending_reset");
     memset(&a, 0, sizeof(a));
     a.P = *p; a.st = *st; a.io = *io;
@@ -632,6 +634,8 @@ int qs_dyn_substeps_pub(const QsParams* p, const QsState* st, const float* rpm, 
     if ((effects & QS_EFFECT_DW) && !dw_fz && drones_per_env > kMaxTPB)
         return fail(QS_ERR_UNSUPPORTED, "qs_dyn_substeps: in-CTA downwash needs drones_per_env <= 128 (else pass dw_fz, substeps = 1)");
     if ((effects & QS_EFFECT_DW) && dw_fz && substeps != 1) return fail(QS_ERR_UNSUPPORTED, "qs_dyn_substeps: external dw_fz requires substeps == 1");
+    if (st->phys && (dw_fz || pub))
+        return fail(QS_ERR_UNSUPPORTED, "qs_dyn_substeps: per-aviary physical constants (QsState.phys) are not supported with external downwash or a formation publish");
     StepArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.st = *st;

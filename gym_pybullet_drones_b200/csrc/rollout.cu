@@ -218,7 +218,9 @@ __device__ __forceinline__ void round_to_planes(qs::Drone& d) {
     d.qx = __dmul_rn(d.qx, inv); d.qy = __dmul_rn(d.qy, inv); d.qz = __dmul_rn(d.qz, inv); d.qw = __dmul_rn(d.qw, inv);
 }
 
-template <int EFF, bool PIDACT, bool POLICY>
+// PHYS: the physical constants come from the aviary's row of QsState.phys, re-read (L1) every tick rather than held in 28
+// registers for the whole rollout -- the POLICY variant has none to spare (128 registers, 7 CTAs per SM, DESIGN.md 4.1b).
+template <int EFF, bool PIDACT, bool POLICY, bool PHYS>
 __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout_kernel(const __grid_constant__ RolloutArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const QsParams& P = a.P;
@@ -342,10 +344,16 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
         }
         // ---- physics ---------------------------------------------------------------------------------------------
         double R_last[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+        qs::PhysRow ph;
         if (live) {
             double cur_yaw = 0.0;
             if (a.act_type == QS_ACT_VEL) { double r_, p_; qs::quat_to_euler<false>(d.qx, d.qy, d.qz, d.qw, r_, p_, cur_yaw); }
-            qs::decode_action<PIDACT>(P, a.act_type, act, d, cur_yaw, pst, rpm);
+            if constexpr (PHYS) {
+                qs::decode_action_k<PIDACT>(P, load_phys_rpm(a.st.phys, e), a.act_type, act, d, cur_yaw, pst, rpm);
+                ph = load_phys(a.st.phys, e);                 // after the decode (and its PID controller)
+            } else {
+                qs::decode_action<PIDACT>(P, a.act_type, act, d, cur_yaw, pst, rpm);
+            }
         }
         if (EFF & QS_EFFECT_DW) {
             for (int s = 0; s < a.substeps; ++s) {
@@ -360,12 +368,14 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
                         const double dxy2 = dx * dx + dy * dy;
                         if (dz > 0.0 && dxy2 < 100.0) fz += qs::downwash_pair(P, dz, dxy2);
                     }
-                    qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                    if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, ph, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                    else qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
                 }
                 __syncthreads();
             }
         } else if (live) {
-            qs::dyn_tick<EFF>(P, d, rpm, rpm_prev, 0.0, a.substeps, R_last);
+            if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, ph, d, rpm, rpm_prev, 0.0, a.substeps, R_last);
+            else qs::dyn_tick<EFF>(P, d, rpm, rpm_prev, 0.0, a.substeps, R_last);
         }
         qs::Derived o;
         if (live) { if (a.flags & QS_FLAG_RPY_F32) qs::derive<true>(d, R_last, o); else qs::derive<false>(d, R_last, o); }
@@ -458,6 +468,59 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
     }
 }
 
+// validates the policy (if any) and launches the rollout kernel family of `a` (PHYS: with the per-aviary table)
+template <bool PHYS>
+int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* stream) {
+    const int drones_per_env = a.D, A = a.A;
+    const unsigned effects = a.effects;
+    const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
+    int threads = ((a.tpb + 31) / 32) * 32;
+    size_t sm = smem_fixed(a.cap) + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (io->policy) {
+        const QsPolicy& q = *io->policy;
+        if (pid_act || (effects & 7u) || a.cap > 64) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports RPM / ONE_D_RPM actions, no DYN+ effects, drones_per_env <= 64");
+        if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: pass either actions or a policy");
+        if (!q.w1 || !q.b1 || !q.w2 || !q.b2 || !q.w3 || !q.b3 || !q.log_std) return fail(QS_ERR_NULL, "qs_rollout: policy weights are NULL");
+        if (q.nt3 != 1 && q.nt3 != 2 && q.nt3 != 4) return fail(QS_ERR_SIZE, "qs_rollout: policy nt3 (padded output tiles of 8) must be 1, 2 or 4");
+        if (q.out_dim > 8 * q.nt3) return fail(QS_ERR_SIZE, "qs_rollout: policy out_dim exceeds the padded output width");
+        if (q.in_dim != drones_per_env * a.obs_dim || q.out_dim != drones_per_env * A) return fail(QS_ERR_SIZE, "qs_rollout: policy in_dim/out_dim must be D*obs_dim / D*A");
+        if (q.vw1 && (!q.vb1 || !q.vw2 || !q.vb2 || !q.vw3 || !q.vb3)) return fail(QS_ERR_NULL, "qs_rollout: incomplete critic");
+        if (q.values && !q.vw1) return fail(QS_ERR_NULL, "qs_rollout: values requested without a critic");
+        if (!aligned16(q.w1) || !aligned16(q.w2) || !aligned16(q.w3) || (q.vw1 && (!aligned16(q.vw1) || !aligned16(q.vw2) || !aligned16(q.vw3))))
+            return fail(QS_ERR_ALIGN, "qs_rollout: policy weight arrays must be 16-byte aligned");
+        a.pol = q;
+        threads = 64;                                            // two warps: 64 drones, 32 hidden units each in the MLP
+        const int n_av_max = 64 / drones_per_env;
+        sm = 1280 + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32
+           + (size_t)(n_av_max * 8 * q.nt3 + n_av_max * 8 + 64) * 4 + 16;      // compact fixed part, window, means, values, log-prob terms
+        if (sm > 200 * 1024) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
+        if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<0, false, true, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+        {   // shared-memory carve-out: just enough for the 7 resident CTAs, so that the weights find the rest of the 256 KB as L1
+            const size_t need = 7 * (sm + 1024);
+            int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
+            cudaFuncSetAttribute(rollout_kernel<0, false, true, PHYS>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
+        }
+        rollout_kernel<0, false, true, PHYS><<<blocks, threads, sm, s>>>(a);
+        const cudaError_t e = cudaGetLastError();
+        return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout (policy) launch");
+    }
+#define QS_RCASE(E)                                                                                                   \
+    case E: {                                                                                                         \
+        if (pid_act) {                                                                                                \
+            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, true, false, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
+            rollout_kernel<E, true, false, PHYS><<<blocks, threads, sm, s>>>(a);                                            \
+        } else {                                                                                                      \
+            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, false, false, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
+            rollout_kernel<E, false, false, PHYS><<<blocks, threads, sm, s>>>(a);                                           \
+        }                                                                                                             \
+    } break;
+    switch (effects & 7u) { QS_RCASE(0) QS_RCASE(1) QS_RCASE(2) QS_RCASE(3) QS_RCASE(4) QS_RCASE(5) QS_RCASE(6) QS_RCASE(7) }
+#undef QS_RCASE
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout launch");
+}
+
 }  // namespace
 
 extern "C" {
@@ -507,52 +570,7 @@ int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int 
         const bool aligned = aligned16(io->obs_init) && (span % 16 == 0) && ((row_bytes * ((size_t)a.N % a.tpb)) % 16 == 0);
         a.stage_mode = (aligned && A == 4) ? 1 : 2;
     }
-    const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
-    int threads = ((a.tpb + 31) / 32) * 32;
-    size_t sm = smem_fixed(a.cap) + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (io->policy) {
-        const QsPolicy& q = *io->policy;
-        if (pid_act || (effects & 7u) || a.cap > 64) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports RPM / ONE_D_RPM actions, no DYN+ effects, drones_per_env <= 64");
-        if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: pass either actions or a policy");
-        if (!q.w1 || !q.b1 || !q.w2 || !q.b2 || !q.w3 || !q.b3 || !q.log_std) return fail(QS_ERR_NULL, "qs_rollout: policy weights are NULL");
-        if (q.nt3 != 1 && q.nt3 != 2 && q.nt3 != 4) return fail(QS_ERR_SIZE, "qs_rollout: policy nt3 (padded output tiles of 8) must be 1, 2 or 4");
-        if (q.out_dim > 8 * q.nt3) return fail(QS_ERR_SIZE, "qs_rollout: policy out_dim exceeds the padded output width");
-        if (q.in_dim != drones_per_env * a.obs_dim || q.out_dim != drones_per_env * A) return fail(QS_ERR_SIZE, "qs_rollout: policy in_dim/out_dim must be D*obs_dim / D*A");
-        if (q.vw1 && (!q.vb1 || !q.vw2 || !q.vb2 || !q.vw3 || !q.vb3)) return fail(QS_ERR_NULL, "qs_rollout: incomplete critic");
-        if (q.values && !q.vw1) return fail(QS_ERR_NULL, "qs_rollout: values requested without a critic");
-        if (!aligned16(q.w1) || !aligned16(q.w2) || !aligned16(q.w3) || (q.vw1 && (!aligned16(q.vw1) || !aligned16(q.vw2) || !aligned16(q.vw3))))
-            return fail(QS_ERR_ALIGN, "qs_rollout: policy weight arrays must be 16-byte aligned");
-        a.pol = q;
-        threads = 64;                                            // two warps: 64 drones, 32 hidden units each in the MLP
-        const int n_av_max = 64 / drones_per_env;
-        sm = 1280 + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32
-           + (size_t)(n_av_max * 8 * q.nt3 + n_av_max * 8 + 64) * 4 + 16;      // compact fixed part, window, means, values, log-prob terms
-        if (sm > 200 * 1024) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
-        if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<0, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        {   // shared-memory carve-out: just enough for the 7 resident CTAs, so that the weights find the rest of the 256 KB as L1
-            const size_t need = 7 * (sm + 1024);
-            int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
-            cudaFuncSetAttribute(rollout_kernel<0, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
-        }
-        rollout_kernel<0, false, true><<<blocks, threads, sm, s>>>(a);
-        const cudaError_t e = cudaGetLastError();
-        return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout (policy) launch");
-    }
-#define QS_RCASE(E)                                                                                                   \
-    case E: {                                                                                                         \
-        if (pid_act) {                                                                                                \
-            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
-            rollout_kernel<E, true, false><<<blocks, threads, sm, s>>>(a);                                            \
-        } else {                                                                                                      \
-            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
-            rollout_kernel<E, false, false><<<blocks, threads, sm, s>>>(a);                                           \
-        }                                                                                                             \
-    } break;
-    switch (effects & 7u) { QS_RCASE(0) QS_RCASE(1) QS_RCASE(2) QS_RCASE(3) QS_RCASE(4) QS_RCASE(5) QS_RCASE(6) QS_RCASE(7) }
-#undef QS_RCASE
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout launch");
+    return a.st.phys ? launch_rollout<true>(a, io, pid_act, stream) : launch_rollout<false>(a, io, pid_act, stream);
 }
 
 }  // extern "C"

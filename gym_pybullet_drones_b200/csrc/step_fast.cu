@@ -43,7 +43,8 @@ struct FastSmem {
 
 // A: action width (4 = RPM, 1 = ONE_D_RPM).  TASK: Hover/MultiHover reward + flags (else the CtrlAviary-style dummy task).
 // RESET: SAME_STEP autoreset.  RPYF: float32 atan2f/asinf for the reported rpy.  WARPS: warps per CTA (independent).
-template <int A, bool TASK, bool RESET, bool RPYF, int WARPS>
+// PHYS: the drone's physical constants come from its aviary's row of QsState.phys (else from QsParams).
+template <int A, bool TASK, bool RESET, bool RPYF, int WARPS, bool PHYS>
 __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_constant__ StepArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const QsParams& P = a.P;
@@ -114,6 +115,8 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
         act[0] = __ldg(a.io.action + il);
     }
     sc = a.st.step_counter[e];
+    qs::PhysRow ph;
+    if constexpr (PHYS) ph = load_phys(a.st.phys, e);                      // one row per aviary: aviaries never straddle warps
     // The bulk copy of the old span (9 KB per warp) is issued only once the step counter -- and with it the batch of small
     // state loads issued just before it -- has ARRIVED: warps issue in order, so the comparison below stalls until then, and
     // the memory system serves every warp's 120 bytes of state ahead of the 19 MB of history the physics does not need yet.
@@ -146,7 +149,8 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
     double rpm[4];
     {
         qs::PidState none = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-        qs::decode_action<false>(P, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
+        if constexpr (PHYS) qs::decode_action_k<false>(P, ph, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
+        else qs::decode_action<false>(P, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
     }
     // A = 4: the history part of the new rows does not depend on the physics: as soon as the old span has landed (polled between
     // substeps) the copy engine writes it back shifted by one action; the heads and the new actions follow at the end as
@@ -168,7 +172,8 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
         }
     };
     double R_last[9];
-    qs::dyn_tick<0>(P, d, rpm, rpm, 0.0, a.substeps, R_last, poll);
+    if constexpr (PHYS) qs::dyn_tick_k<0>(P, ph, d, rpm, rpm, 0.0, a.substeps, R_last, poll);
+    else qs::dyn_tick<0>(P, d, rpm, rpm, 0.0, a.substeps, R_last, poll);
     QS_STAMP(3);
     qs::Derived o;
     qs::derive<RPYF>(d, R_last, o);
@@ -353,7 +358,7 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
     QS_STAMP(9);
 }
 
-template <int A, bool TASK, bool RESET, bool RPYF, int WARPS>
+template <int A, bool TASK, bool RESET, bool RPYF, int WARPS, bool PHYS>
 cudaError_t launch_one(const StepArgs& a, cudaStream_t s) {
     const long long warps = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
     const int blocks = (int)((warps + WARPS - 1) / WARPS);
@@ -367,24 +372,36 @@ cudaError_t launch_one(const StepArgs& a, cudaStream_t s) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
     if (sm > 48 * 1024)
-        cudaFuncSetAttribute(step_fast_kernel<A, TASK, RESET, RPYF, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    return cudaLaunchKernelEx(&cfg, step_fast_kernel<A, TASK, RESET, RPYF, WARPS>, a);
+        cudaFuncSetAttribute(step_fast_kernel<A, TASK, RESET, RPYF, WARPS, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    return cudaLaunchKernelEx(&cfg, step_fast_kernel<A, TASK, RESET, RPYF, WARPS, PHYS>, a);
 }
 
-template <int A, int WARPS>
+template <int A, int WARPS, bool PHYS>
 cudaError_t launch_modes(const StepArgs& a, cudaStream_t s) {
     const bool task = a.task == QS_TASK_HOVER, reset = a.flags & QS_FLAG_AUTORESET_SAME_STEP, rpyf = a.flags & QS_FLAG_RPY_F32;
     const int key = (task ? 4 : 0) | (reset ? 2 : 0) | (rpyf ? 1 : 0);
     switch (key) {
-        case 0: return launch_one<A, false, false, false, WARPS>(a, s);
-        case 1: return launch_one<A, false, false, true, WARPS>(a, s);
-        case 2: return launch_one<A, false, true, false, WARPS>(a, s);
-        case 3: return launch_one<A, false, true, true, WARPS>(a, s);
-        case 4: return launch_one<A, true, false, false, WARPS>(a, s);
-        case 5: return launch_one<A, true, false, true, WARPS>(a, s);
-        case 6: return launch_one<A, true, true, false, WARPS>(a, s);
-        default: return launch_one<A, true, true, true, WARPS>(a, s);
+        case 0: return launch_one<A, false, false, false, WARPS, PHYS>(a, s);
+        case 1: return launch_one<A, false, false, true, WARPS, PHYS>(a, s);
+        case 2: return launch_one<A, false, true, false, WARPS, PHYS>(a, s);
+        case 3: return launch_one<A, false, true, true, WARPS, PHYS>(a, s);
+        case 4: return launch_one<A, true, false, false, WARPS, PHYS>(a, s);
+        case 5: return launch_one<A, true, false, true, WARPS, PHYS>(a, s);
+        case 6: return launch_one<A, true, true, false, WARPS, PHYS>(a, s);
+        default: return launch_one<A, true, true, true, WARPS, PHYS>(a, s);
     }
+}
+
+template <bool PHYS>
+cudaError_t launch_warps(const StepArgs& a, int warps, cudaStream_t s) {
+    if (a.A == 4) {
+        if (warps == 4) return launch_modes<4, 4, PHYS>(a, s);
+        if (warps == 2) return launch_modes<4, 2, PHYS>(a, s);
+        return launch_modes<4, 1, PHYS>(a, s);
+    }
+    if (warps == 4) return launch_modes<1, 4, PHYS>(a, s);
+    if (warps == 2) return launch_modes<1, 2, PHYS>(a, s);
+    return launch_modes<1, 1, PHYS>(a, s);
 }
 
 }  // namespace
@@ -413,14 +430,8 @@ cudaError_t launch_step_fast(const StepArgs& a_in, cudaStream_t s) {
     const StepArgs& a = a_in;
 #endif
     static const int warps = getenv("QS_FAST_WARPS") ? atoi(getenv("QS_FAST_WARPS")) : 1;      // measured default (DESIGN.md 6)
-    if (a.A == 4) {
-        if (warps == 4) return launch_modes<4, 4>(a, s);
-        if (warps == 2) return launch_modes<4, 2>(a, s);
-        return launch_modes<4, 1>(a, s);
-    }
-    if (warps == 4) return launch_modes<1, 4>(a, s);
-    if (warps == 2) return launch_modes<1, 2>(a, s);
-    return launch_modes<1, 1>(a, s);
+    if (a.st.phys) return launch_warps<true>(a, warps, s);
+    return launch_warps<false>(a, warps, s);
 }
 
 }  // namespace qsi

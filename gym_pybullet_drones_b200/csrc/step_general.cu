@@ -70,8 +70,9 @@ __device__ __forceinline__ void write_rows(const StepArgs& a, long long c0, int 
 // Block = tpb threads, tpb a multiple of D (drones of one aviary never straddle CTAs) when D <= 128.
 // ---------------------------------------------------------------------------------------------------------
 // PIDACT = the action type runs the embedded DSLPIDControl (PID / VEL / ONE_D_PID): a separate instantiation keeps
-// the controller's registers out of the plain RPM kernels.
-template <int EFF, bool RAW, bool PIDACT>
+// the controller's registers out of the plain RPM kernels.  PHYS = the physical constants come from the aviary's row of
+// QsState.phys (a separate instantiation: without the table the kernels are the ones of ABI 3).
+template <int EFF, bool RAW, bool PIDACT, bool PHYS>
 __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant__ StepArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const QsParams& P = a.P;
@@ -114,6 +115,7 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
     int sc = 0;
     bool pending = false;
     constexpr bool pid_act = PIDACT;
+    qs::PhysRow ph;
 
     // The observation rows of this CTA are one contiguous span, and the new rows are the old ones shifted left by one
     // action: new_flat[j] = old_flat[j + A] once every thread has patched its own row (head -> slots [A, A+12), new
@@ -176,11 +178,14 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
             rpm[0] = rpm_prev[0]; rpm[1] = rpm_prev[1]; rpm[2] = rpm_prev[2]; rpm[3] = rpm_prev[3];
         } else if (RAW && (a.flags & QS_FLAG_ACTION_F64)) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k) rpm[k] = qs::clampd(rpm[k], 0.0, P.max_rpm);              // CtrlAviary.py:140
+            for (int k = 0; k < 4; ++k) rpm[k] = qs::clampd(rpm[k], 0.0, PHYS ? load_phys_rpm(a.st.phys, e).max_rpm : P.max_rpm);   // CtrlAviary.py:140
+        } else if constexpr (PHYS) {
+            qs::decode_action_k<PIDACT>(P, load_phys_rpm(a.st.phys, e), a.act_type, act, d, cur_yaw, pst, rpm);
         } else {
             qs::decode_action<PIDACT>(P, a.act_type, act, d, cur_yaw, pst, rpm);
         }
     }
+    if constexpr (PHYS) { if (live && !pending) ph = load_phys(a.st.phys, e); }      // after the decode (and its PID controller)
 
     // ---- physics: S substeps ------------------------------------------------------------------------------
     if ((EFF & QS_EFFECT_DW) && a.io.dw_fz == nullptr) {
@@ -197,13 +202,15 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
                     const double dxy2 = dx * dx + dy * dy;
                     if (dz > 0.0 && dxy2 < 100.0) fz += qs::downwash_pair(P, dz, dxy2);
                 }
-                qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, ph, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                else qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
             }
             __syncthreads();
         }
     } else if (live && !pending) {
         const double fz = (EFF & QS_EFFECT_DW) ? (double)__ldg(a.io.dw_fz + i) : 0.0;
-        qs::dyn_tick<EFF>(P, d, rpm, rpm_prev, fz, a.substeps, R_last);
+        if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, ph, d, rpm, rpm_prev, fz, a.substeps, R_last);
+        else qs::dyn_tick<EFF>(P, d, rpm, rpm_prev, fz, a.substeps, R_last);
     }
 
     // ---- derived outputs, task terms --------------------------------------------------------------------
@@ -413,7 +420,7 @@ size_t step_smem_bytes(const StepArgs& a) {
     return smem_fixed(a.cap) + (a.stage_rows ? (size_t)a.tpb * a.obs_dim * 4 + 32 : 0);
 }
 
-template <bool RAW, bool PIDACT>
+template <bool RAW, bool PIDACT, bool PHYS>
 cudaError_t launch_step(const StepArgs& a, bool pdl_ok, cudaStream_t s) {
     const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
     const int threads = ((a.tpb + 31) / 32) * 32;
@@ -428,9 +435,9 @@ cudaError_t launch_step(const StepArgs& a, bool pdl_ok, cudaStream_t s) {
 #define QS_CASE(E)                                                                                               \
     case E: {                                                                                                    \
         if (sm > 48 * 1024)      /* per device and cheap: no process-wide "already set" flag */                 \
-            cudaFuncSetAttribute(step_kernel<E, RAW, PIDACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
+            cudaFuncSetAttribute(step_kernel<E, RAW, PIDACT, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                  (int)(kStepSmemFixed + kStageLimit + 32));                                      \
-        return cudaLaunchKernelEx(&cfg, step_kernel<E, RAW, PIDACT>, a);                                         \
+        return cudaLaunchKernelEx(&cfg, step_kernel<E, RAW, PIDACT, PHYS>, a);                                   \
     }
     switch (a.effects & 7u) {
         QS_CASE(0) QS_CASE(1) QS_CASE(2) QS_CASE(3) QS_CASE(4) QS_CASE(5) QS_CASE(6) QS_CASE(7)
@@ -439,11 +446,16 @@ cudaError_t launch_step(const StepArgs& a, bool pdl_ok, cudaStream_t s) {
     return cudaGetLastError();
 }
 
+template <bool PHYS>
+cudaError_t launch_families(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s) {
+    if (raw) return pid_act ? launch_step<true, true, PHYS>(a, pdl_ok, s) : launch_step<true, false, PHYS>(a, pdl_ok, s);
+    return pid_act ? launch_step<false, true, PHYS>(a, pdl_ok, s) : launch_step<false, false, PHYS>(a, pdl_ok, s);
+}
+
 }  // namespace
 
 cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s) {
-    if (raw) return pid_act ? launch_step<true, true>(a, pdl_ok, s) : launch_step<true, false>(a, pdl_ok, s);
-    return pid_act ? launch_step<false, true>(a, pdl_ok, s) : launch_step<false, false>(a, pdl_ok, s);
+    return a.st.phys ? launch_families<true>(a, raw, pid_act, pdl_ok, s) : launch_families<false>(a, raw, pid_act, pdl_ok, s);
 }
 
 }  // namespace qsi

@@ -25,7 +25,8 @@ import torch
 
 from .. import _native as N
 from .._compat import (AUTORESET_DISABLED, AUTORESET_NEXT_STEP, AUTORESET_SAME_STEP, Env, batch_box, spaces)
-from ..params import AviaryConstants, fill_params, quaternion_from_euler
+from ..params import (PHYS_KEYS, AviaryConstants, coerce_physical_args, fill_params, nominal_properties, physical_rows,
+                      quaternion_from_euler)
 from ..utils.enums import DroneModel, Physics
 
 _PHYSICS_EFFECTS = {
@@ -182,6 +183,8 @@ class BaseAviary(Env):
         self._log = None                     # (QsLogRing, controls tensor) while a utils.Logger is attached
         self._gather = None                  # sharding.ObsGather: the tick also writes its rows into the learner's tensor
         self._order = self._inv = None       # reorder_by_morton(): storage index -> drone id and back
+        self._phys = None                    # [E, 16] QsState.phys rows, allocated by the first set_physical_params()
+        self._phys_props = None              # [E, 8] the PHYS_KEYS values behind them
         #### Initial poses (BaseAviary.py:194-207); [D,3] shared by all aviaries or [E,D,3] per aviary ####
         self._tables_per_env = False
         if initial_xyzs is None:
@@ -459,6 +462,79 @@ class BaseAviary(Env):
             self._wz[:] = w[:, 2]
         if step_counter is not None:
             self._step_counter[:] = torch.as_tensor(np.broadcast_to(np.asarray(step_counter), (self._E,)).astype(np.int32), device=self.device)
+
+    ################################################################################
+    # per-aviary physical constants (domain randomisation; include/quadsim.h, QsState.phys)
+
+    def set_physical_params(self, m=None, ixx=None, iyy=None, izz=None, kf=None, km=None, arm=None, thrust2weight=None, envs=None,
+                            check=False):
+        """Gives every aviary its own drone: mass, inertia, motor constants, arm and thrust-to-weight ratio (the DRONE_PROPERTIES
+        keys).  The reference reads M, J, J_INV, KF, KM, L, GRAVITY (_dynamics), HOVER_RPM (action decode) and MAX_RPM (CtrlAviary
+        clip) from the env at every call, so a user can change them between episodes; here they live in a per-aviary table that
+        the step and rollout kernels read.  GRAVITY = G*M, HOVER_RPM, MAX_RPM, J^-1 and the torque arms are derived as
+        BaseAviary.__init__ does (params.physical_rows).  The drone model (mixing signs), propeller offsets, ground-effect, drag
+        and downwash coefficients, SPEED_LIMIT, the task and the embedded DSLPIDControl (a nominal CF2X, as in the reference) stay
+        env-wide.
+
+        Each value: a scalar, an [E] NumPy array or an [E] CUDA tensor; None keeps the current value.  `envs`: [E] bool mask
+        (NumPy or CUDA) of the aviaries to change, None = all.  Wrong shapes, and non-finite or non-positive scalars / NumPy
+        values, raise ValueError.  By default CUDA tensors are not read back (no host synchronisation, so the call can sit between
+        the steps of a training loop): an aviary whose new values are not all finite and positive keeps its previous row, and
+        `physical_params_rejected` (an int64 CUDA tensor) counts such aviaries.  `check=True` reads them back first (one
+        synchronisation) and raises ValueError like the host inputs, changing nothing.  The single-env API takes scalars.
+
+        A change takes effect at the next step() or rollout(); a rollout keeps each aviary's row for all its ticks.  With
+        same-step autoreset, `set_physical_params(..., envs=done)` after a step re-randomises exactly the aviaries that start a
+        new episode.  The first call allocates the table; it is never reallocated.  The M, KF, ... attributes keep describing
+        the constructor's model.  Not available for aviaries larger than one CTA with downwash or for FormationShard."""
+        if self._dw_fz is not None:
+            raise ValueError("set_physical_params() is not available with external downwash (num_drones > 128 with downwash, "
+                             "formations): the split-substep and formation kernels take the constants of QsParams only")
+        vals = coerce_physical_args(self._E, self.device, dict(m=m, ixx=ixx, iyy=iyy, izz=izz, kf=kf, km=km, arm=arm,
+                                                               thrust2weight=thrust2weight), single=not self.VECTORIZED)
+        if check:
+            bad = [k for k, v in vals.items() if not bool((torch.isfinite(v) & (v > 0)).all())]
+            if bad:
+                raise ValueError("%s must be finite and positive" % ", ".join(bad))
+        sel = None
+        if envs is not None:
+            if not self.VECTORIZED:
+                raise ValueError("envs= needs the vector API (num_envs=...)")
+            sel = torch.as_tensor(envs, device=self.device)
+            if sel.dtype != torch.bool or tuple(sel.shape) != (self._E,):
+                raise ValueError("envs must be a [%d] bool mask" % self._E)
+        with self._on_device():
+            if self._phys is None:
+                nom = nominal_properties(self.DRONE_MODEL)
+                self._phys_props = torch.tensor([[nom[k] for k in PHYS_KEYS]] * self._E, dtype=torch.float64, device=self.device)
+                self._phys_rejected = torch.zeros((), dtype=torch.int64, device=self.device)
+                self._phys = physical_rows(self.DRONE_MODEL, {k: self._phys_props[:, j] for j, k in enumerate(PHYS_KEYS)}, self.G)
+                self._st.phys = self._phys.data_ptr()
+            if not vals:
+                return
+            new = self._phys_props.clone()
+            ok = torch.ones((self._E,), dtype=torch.bool, device=self.device)
+            for k, v in vals.items():
+                new[:, PHYS_KEYS.index(k)] = v
+                ok &= torch.isfinite(v) & (v > 0)
+            take = ok if sel is None else ok & sel
+            self._phys_rejected += ((~ok) if sel is None else (~ok & sel)).sum()
+            rows = physical_rows(self.DRONE_MODEL, {k: new[:, j] for j, k in enumerate(PHYS_KEYS)}, self.G)
+            self._phys_props.copy_(torch.where(take[:, None], new, self._phys_props))
+            self._phys.copy_(torch.where(take[:, None], rows, self._phys))
+
+    @property
+    def physical_params_rejected(self):
+        """int64 CUDA tensor: aviaries whose CUDA-tensor values set_physical_params() refused (not finite and positive)."""
+        return self._phys_rejected if self._phys is not None else torch.zeros((), dtype=torch.int64, device=self.device)
+
+    def physical_params(self):
+        """{key: [E] float64 CUDA tensor} of the eight PHYS_KEYS values every aviary flies with (the constructor's model until
+        the first set_physical_params())."""
+        if self._phys_props is None:
+            nom = nominal_properties(self.DRONE_MODEL)
+            return {k: torch.full((self._E,), nom[k], dtype=torch.float64, device=self.device) for k in PHYS_KEYS}
+        return {k: self._phys_props[:, j].clone() for j, k in enumerate(PHYS_KEYS)}
 
     ################################################################################
 

@@ -113,24 +113,97 @@ class AviaryConstants:
                           np.ones(num_drones) * (self.COLLISION_H / 2 - self.COLLISION_Z_OFFSET + .1)]).transpose().reshape(num_drones, 3)
 
 
+# ---- per-aviary physical constants (QsState.phys, include/quadsim.h) ------------------------------------------------------
+# The properties a user may vary per aviary (names of DRONE_PROPERTIES) and the columns of one table row derived from them.
+PHYS_KEYS = ("m", "ixx", "iyy", "izz", "kf", "km", "arm", "thrust2weight")
+PHYS_COLUMNS = ("inv_m", "gravity", "kf", "km", "kx", "ky", "jx", "jy", "jz", "jx_inv", "jy_inv", "jz_inv", "hover_rpm", "max_rpm")
+
+
+def _sqrt(t):
+    # correctly rounded like np.sqrt: CUDA's float64 sqrt is; torch's vectorised CPU sqrt is not (1 ulp apart now and then)
+    if t.device.type == "cpu":
+        import torch
+        return torch.from_numpy(np.sqrt(t.numpy()))
+    return t.sqrt()
+
+
+def physical_rows(drone_model, props, g=9.8):
+    """[E, 16] float64 rows of QsState.phys from the properties `props` (dict PHYS_KEYS -> [E] float64 torch tensors, any device),
+    derived in float64 with BaseAviary.__init__'s formulas and operation order (envs/BaseAviary.py:117-119, :1000 J^-1, the
+    _dynamics arm L/sqrt(2) of :846-851).  fill_params packs its QsParams fields from the same function, so a row of nominal
+    properties has exactly their bits."""
+    import torch
+    m, kf, km, arm, t2w = props["m"], props["kf"], props["km"], props["arm"], props["thrust2weight"]
+    j = torch.stack([props["ixx"], props["iyy"], props["izz"]], dim=1)
+    gravity = g * m                                                                         # :117
+    mix = _MIXING[drone_model]
+    a = arm / math.sqrt(2) if mix["diag"] else arm                                          # np.sqrt(2) == math.sqrt(2)
+    out = torch.zeros((m.shape[0], N.PHYS_WIDTH), dtype=torch.float64, device=m.device)
+    out[:, 0] = 1.0 / m
+    out[:, 1] = gravity
+    out[:, 2], out[:, 3] = kf, km
+    out[:, 4], out[:, 5] = mix["kx_sign"] * a, a
+    out[:, 6:9] = j
+    out[:, 9:12] = 1.0 / j                                                                  # np.linalg.inv of the diagonal J
+    out[:, 12] = _sqrt(gravity / (4 * kf))                                                  # :118
+    out[:, 13] = _sqrt((t2w * gravity) / (4 * kf))                                          # :119
+    return out
+
+
+def nominal_properties(drone_model):
+    """The model's PHYS_KEYS values (DRONE_PROPERTIES)."""
+    u = DRONE_PROPERTIES[drone_model]
+    return {k: float(u[k]) for k in PHYS_KEYS}
+
+
+def coerce_physical_args(n_envs, device, values, single=False):
+    """Validates the arguments of BaseAviary.set_physical_params: `values` maps PHYS_KEYS to a scalar, an [E] NumPy array or an
+    [E] torch tensor (None = keep).  Returns {key: [E] float64 tensor on `device`}.  Wrong keys, types or shapes raise
+    ValueError, and so do non-finite or non-positive scalars and NumPy values (checked on the host).  Tensors are not read
+    back (no synchronisation): set_physical_params screens them on the device.  single = the single-env API: scalars only."""
+    import torch
+    out = {}
+    for k, v in values.items():
+        if k not in PHYS_KEYS:
+            raise ValueError("unknown physical parameter %r (expected one of %s)" % (k, ", ".join(PHYS_KEYS)))
+        if v is None:
+            continue
+        if isinstance(v, torch.Tensor):
+            if single and v.numel() != 1:
+                raise ValueError("%s: the single-env API takes scalars" % k)
+            if v.dim() > 1 or (v.dim() == 1 and v.shape[0] != n_envs) or not (v.dtype.is_floating_point or v.dtype in (torch.int32, torch.int64)):
+                raise ValueError("%s must be a scalar or a [%d] float tensor, got %s %s" % (k, n_envs, v.dtype, tuple(v.shape)))
+            out[k] = v.to(device=device, dtype=torch.float64).reshape(-1).expand(n_envs)
+            continue
+        a = np.asarray(v)
+        if a.dtype.kind not in "fiu" or (a.ndim == 1 and single) or a.ndim > 1 or (a.ndim == 1 and a.shape[0] != n_envs):
+            raise ValueError("%s must be a scalar or a [%d] array of floats, got %s %s" % (k, n_envs, a.dtype, a.shape))
+        a = a.astype(np.float64)
+        if not np.all(np.isfinite(a)) or not np.all(a > 0):
+            raise ValueError("%s must be finite and positive" % k)
+        out[k] = torch.as_tensor(np.broadcast_to(a, (n_envs,)).copy(), device=device)
+    return out
+
+
 def fill_params(c, *, episode_len_sec=8.0, xy_bound=1.5, z_bound=2.0, tilt_bound=0.4, term_dist=1e-4,
                 pid_model=DroneModel.CF2X, pid_coeffs=None, pid_g=9.8):
     """Packs an AviaryConstants (+ task and controller constants) into the C-ABI QsParams."""
+    import torch
     P = N.QsParams()
     P.dt, P.ctrl_dt, P.pyb_freq = c.PYB_TIMESTEP, c.CTRL_TIMESTEP, float(c.PYB_FREQ)
-    P.m, P.inv_m, P.gravity, P.kf, P.km = c.M, 1.0 / c.M, c.GRAVITY, c.KF, c.KM
+    props = dict(m=c.M, ixx=c.J[0, 0], iyy=c.J[1, 1], izz=c.J[2, 2], kf=c.KF, km=c.KM, arm=c.L, thrust2weight=c.THRUST2WEIGHT_RATIO)
+    row = physical_rows(c.DRONE_MODEL, {k: torch.tensor([float(v)], dtype=torch.float64) for k, v in props.items()}, c.G)[0].tolist()
+    P.m = c.M
+    P.inv_m, P.gravity, P.kf, P.km, P.kx, P.ky = row[0:6]
     for k in range(3):
-        P.j[k] = c.J[k, k]
-        P.j_inv[k] = c.J_INV[k, k]
+        P.j[k], P.j_inv[k] = row[6 + k], row[9 + k]
         P.drag_coeff[k] = c.DRAG_COEFF[k]
-    P.hover_rpm, P.max_rpm = float(c.HOVER_RPM), float(c.MAX_RPM)
+    P.hover_rpm, P.max_rpm = row[12], row[13]
     mix = _MIXING[c.DRONE_MODEL]
     for k in range(4):
         P.sx[k], P.sy[k], P.sz[k] = mix["sx"][k], mix["sy"][k], mix["sz"][k]
         for a in range(3):
             P.prop_xyz[k][a] = c.PROP_OFFSETS[k, a]
-    arm = float(c.L / np.sqrt(2)) if mix["diag"] else c.L
-    P.kx, P.ky = mix["kx_sign"] * arm, arm
     P.gnd_eff_coeff, P.prop_radius, P.gnd_eff_h_clip = c.GND_EFF_COEFF, c.PROP_RADIUS, float(c.GND_EFF_H_CLIP)
     P.dw_coeff[0], P.dw_coeff[1], P.dw_coeff[2] = c.DW_COEFF_1, c.DW_COEFF_2, c.DW_COEFF_3
     P.episode_len_sec, P.xy_bound, P.z_bound, P.tilt_bound, P.term_dist = episode_len_sec, xy_bound, z_bound, tilt_bound, term_dist

@@ -39,8 +39,9 @@
 extern "C" {
 #endif
 
-#define QS_ABI_VERSION 3     /* 2: the persistent state (planes, last_rpm, pid, init/target tables) is float64;
-                                3: QsStepIO.pdl_hint replaced by the per-warp readiness words */
+#define QS_ABI_VERSION 4     /* 2: the persistent state (planes, last_rpm, pid, init/target tables) is float64;
+                                3: QsStepIO.pdl_hint replaced by the per-warp readiness words;
+                                4: QsState.phys, per-aviary physical constants */
 
 /* drone models (utils/enums.py:3-9) */
 enum { QS_MODEL_CF2X = 0, QS_MODEL_CF2P = 1, QS_MODEL_RACE = 2 };
@@ -141,7 +142,27 @@ typedef struct QsState {
                                        qs_dw_publish); nullable otherwise */
     int tables_per_env;             /* 0: the three tables have D rows shared by all envs; 1: N rows */
     int pad_;
+    const double* phys;             /* optional [E][16] float64, 32-byte aligned: per-aviary physical constants (domain randomisation),
+                                       see "Per-aviary physical constants" below; NULL = every aviary flies the drone of QsParams */
 } QsState;
+
+/* Per-aviary physical constants (QsState.phys).  Row e, shared by the D drones of aviary e, holds the constants the reference
+ * reads from the env object at call time (envs/BaseAviary.py:838-858 _dynamics, BaseRLAviary.py:192,225 HOVER_RPM,
+ * CtrlAviary.py:140 MAX_RPM), derived as BaseAviary.__init__ does (BaseAviary.py:117-119):
+ *     [0] inv_m = 1/M   [1] gravity = G*M   [2] kf   [3] km   [4] kx   [5] ky   [6..8] diag(J)   [9..11] diag(J^-1)
+ *     [12] hover_rpm   [13] max_rpm   [14..15] pad
+ * kx / ky carry the arm and the model's torque-mixing sign exactly as in QsParams.  Everything else stays in QsParams: the
+ * mixing signs, the propeller offsets, GND_EFF_COEFF / PROP_RADIUS / GND_EFF_H_CLIP, DRAG_COEFF, DW_COEFF, SPEED_LIMIT, the
+ * task and the embedded controller's constants (the reference's embedded DSLPIDControl reads its own CF2X URDF).
+ * With the table, qs_step (both kernel families, qs_step_host), qs_rollout (with and without a policy) and qs_dyn_substeps
+ * (including the MAX_RPM clip) read row e in place of the QsParams fields; with NULL they run unchanged, same bits.
+ * qs_pid_control / qs_pid_control_state and the formation paths do not take it: a non-NULL table with external downwash
+ * (QsStepIO.dw_fz, the split-substep protocol of aviaries larger than one CTA) or with qs_dyn_substeps_pub is refused with
+ * QS_ERR_UNSUPPORTED.
+ * Ordering: the kernels only READ the table.  The caller writes it between launches with ordinary stream-ordered work (torch
+ * kernels, copies): such work never lets its successor start early, so it is complete before the next step, rollout or
+ * substep starts, whether or not that kernel is a programmatic dependent -- the argument made for the action tensor at qs_step.
+ * A change therefore takes effect at the next launch; a rollout keeps each aviary's row for all its T ticks. */
 
 /* Inputs/outputs of one control tick. */
 typedef struct QsStepIO {
