@@ -179,13 +179,25 @@ __device__ __forceinline__ void warp_net(const float* x_s, int in_dim, const uin
     }
 }
 
+// What a policy rollout hands over across policy_forward besides the drone: the embedded controller's state (PIDACT) and the
+// previous tick's RPMs (drag).  Members a variant does not carry are neither written nor read.
+struct ParkedCtl {
+    qs::Drone d;
+    qs::PidState pst;
+    double rpm_prev[4];
+};
+__device__ __forceinline__ qs::Drone& parked_drone(qs::Drone* p) { return *p; }
+__device__ __forceinline__ qs::Drone& parked_drone(ParkedCtl* p) { return p->d; }
+
 // The policy part of one tick for the whole CTA: actor (and critic) over the CTA's aviaries in tiles of 16; work item i = net x tile
 // goes to warp i & 1.  Deliberately NOT inlined: inside the tick loop its ~120 live registers made the compiler spill the drone state
 // in the middle of the physics substeps; as a call, the state is saved once per tick around it.  `parked` is not touched: the caller
-// hands over the address of its drone state so that the state demonstrably lives in local memory across the call (one store + load
-// per tick) instead of being spilled piecemeal inside the substep loop.
-__device__ __noinline__ void policy_forward(const RolloutArgs& a, const float* base, float* mean_s, float* val_s, int n_av, int t, qs::Drone* parked) {
-    if (n_av < 0) parked->px = 0.0;                          // never taken; keeps the hand-over opaque to the optimiser
+// hands over the address of its drone state (Park = qs::Drone, or ParkedCtl with the controller state and previous RPMs) so that
+// the state demonstrably lives in local memory across the call (one store + load per tick) instead of being spilled piecemeal
+// inside the substep loop.
+template <class Park>
+__device__ __noinline__ void policy_forward(const RolloutArgs& a, const float* base, float* mean_s, float* val_s, int n_av, int t, Park* parked) {
+    if (n_av < 0) parked_drone(parked).px = 0.0;             // never taken; keeps the hand-over opaque to the optimiser
     const int warp = t >> 5, lane = t & 31, ost = 8 * a.pol.nt3;
     const int tiles = (n_av + 15) >> 4, items = a.pol.vw1 ? 2 * tiles : tiles;
     for (int i = warp; i < items; i += 2) {
@@ -218,10 +230,23 @@ __device__ __forceinline__ void round_to_planes(qs::Drone& d) {
     d.qx = __dmul_rn(d.qx, inv); d.qy = __dmul_rn(d.qy, inv); d.qz = __dmul_rn(d.qz, inv); d.qw = __dmul_rn(d.qw, inv);
 }
 
+// Fixed part of a POLICY CTA's dynamic shared memory: red_s [64][2] doubles, oob [64], done [64], and with in-CTA downwash the
+// positions pos_s [64][3] doubles; the mbarrier sits in the last 16 bytes.  1280 bytes without downwash, 2816 with it.
+__host__ __device__ constexpr size_t policy_smem_fixed(int eff) {
+    return (eff & QS_EFFECT_DW) ? (size_t)(64 * 2 * 8 + 64 + 64 + 64 * 3 * 8 + 16 + 127) / 128 * 128 : (size_t)(64 * 2 * 8 + 64 + 64 + 16 + 112);
+}
+constexpr size_t kPolicyPosOffset = 64 * 2 * 8 + 64 + 64;       // pos_s of the downwash variants (8-byte aligned)
+// resident CTAs per SM a POLICY variant is compiled for (__launch_bounds__) and its shared-memory carve-out is sized for: 7 give
+// 128 registers; the in-CTA downwash substep loop (positions of the aviary's drones, barriers, all three effects) spills the drone
+// state at 128, so those variants get 6 CTAs and 168 registers (DESIGN.md 4.1b)
+__host__ __device__ constexpr int policy_ctas(int eff) { return (eff & QS_EFFECT_DW) ? 6 : 7; }
+
 // PHYS: the physical constants come from the aviary's row of QsState.phys, re-read (L1) every tick rather than held in 28
-// registers for the whole rollout -- the POLICY variant has none to spare (128 registers, 7 CTAs per SM, DESIGN.md 4.1b).
+// registers for the whole rollout -- the POLICY variants have none to spare (128 registers, 7 CTAs per SM, DESIGN.md 4.1b).
+// POLICY takes every EFF x PIDACT combination the envs produce (EFF = 0, GND, DRAG, DW, all three): the physics and the embedded
+// controller are the action rollout's code, so a policy rollout gives the bits of the action rollout fed its clipped actions.
 template <int EFF, bool PIDACT, bool POLICY, bool PHYS>
-__global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout_kernel(const __grid_constant__ RolloutArgs a) {
+__global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? policy_ctas(EFF) : 4) rollout_kernel(const __grid_constant__ RolloutArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const QsParams& P = a.P;
     const int tpb = a.tpb, D = a.D, A = a.A, od = a.obs_dim, T = a.io.T;
@@ -233,10 +258,12 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
     const int rows = (int)((N - c0) < tpb ? (N - c0) : tpb);
     double* red_s = reinterpret_cast<double*>(smem_raw);                               // [tpb][2]
     const int cap = a.cap;
-    // POLICY (no DYN+ effects, CTA of 64 drones): a compact fixed part -- red_s [64][2] doubles, oob [64], done [64], mbarrier --
-    // so that 7 CTAs per SM (924 on the H100's 132 SMs) fit into shared memory next to the window and the MLP scratch
-    const size_t fixed = POLICY ? (size_t)(64 * 2 * 8 + 64 + 64 + 16 + 112) : smem_fixed(cap);       // 1280 for POLICY
-    double* pos_s = red_s + (size_t)cap * 2;                                           // [tpb][3] (in-CTA downwash only)
+    // POLICY (CTA of 64 drones): a compact fixed part -- red_s [64][2] doubles, oob [64], done [64], with downwash pos_s [64][3]
+    // doubles, mbarrier -- so that 7 CTAs per SM (924 on the H100's 132 SMs) fit into shared memory next to the window and the
+    // MLP scratch
+    const size_t fixed = POLICY ? policy_smem_fixed(EFF) : smem_fixed(cap);           // 1280 for POLICY, 2816 with downwash
+    double* pos_s = (POLICY && (EFF & QS_EFFECT_DW)) ? reinterpret_cast<double*>(smem_raw + kPolicyPosOffset)
+                                                     : red_s + (size_t)cap * 2;         // [tpb][3] (in-CTA downwash only)
     unsigned char* oob_s = POLICY ? reinterpret_cast<unsigned char*>(red_s + 128) : reinterpret_cast<unsigned char*>(pos_s + (size_t)cap * 3);
     unsigned char* done_s = oob_s + (POLICY ? 64 : cap);
     unsigned long long* bar_s = reinterpret_cast<unsigned long long*>(smem_raw + fixed - 16);
@@ -286,7 +313,17 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
             // the aviaries of this CTA: rows [le D, le D + D) of the window = one flattened observation of in_dim floats each
             const int n_av = rows / D;
             const int ost = 8 * a.pol.nt3;                        // padded width of the output rows in mean_s
-            {
+            if constexpr (PIDACT || (EFF & QS_EFFECT_DRAG)) {
+                // the controller state and the previous RPMs are live across the call too: handed over the same way
+                ParkedCtl parked;
+                parked.d = d;
+                if constexpr (PIDACT) parked.pst = pst;
+                if constexpr ((EFF & QS_EFFECT_DRAG) != 0) for (int j = 0; j < 4; ++j) parked.rpm_prev[j] = rpm_prev[j];
+                policy_forward(a, base, mean_s, val_s, n_av, t, &parked);
+                d = parked.d;
+                if constexpr (PIDACT) pst = parked.pst;
+                if constexpr ((EFF & QS_EFFECT_DRAG) != 0) for (int j = 0; j < 4; ++j) rpm_prev[j] = parked.rpm_prev[j];
+            } else {
                 qs::Drone parked = d;
                 policy_forward(a, base, mean_s, val_s, n_av, t, &parked);
                 d = parked;
@@ -368,8 +405,19 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
                         const double dxy2 = dx * dx + dy * dy;
                         if (dz > 0.0 && dxy2 < 100.0) fz += qs::downwash_pair(P, dz, dxy2);
                     }
-                    if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, ph, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
-                    else qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                    if constexpr (POLICY) {
+                        // the same values selected element by element: a pointer chosen at run time between the two arrays
+                        // puts both in local memory, inside the substep loop (the policy variants have no registers to spare);
+                        // for the same reason the row of constants is re-read (L1) every substep, not held across the barriers
+                        double rp[4];
+                        for (int j = 0; j < 4; ++j) rp[j] = s == 0 ? rpm_prev[j] : rpm[j];
+                        if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, load_phys(a.st.phys, e), d, rpm, rp, fz, 1, R_last);
+                        else qs::dyn_tick<EFF>(P, d, rpm, rp, fz, 1, R_last);
+                    } else if constexpr (PHYS) {
+                        qs::dyn_tick_k<EFF>(P, ph, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                    } else {
+                        qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
+                    }
                 }
                 __syncthreads();
             }
@@ -468,6 +516,19 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? 7 : 4) rollout
     }
 }
 
+// one policy variant: `sm_var` = its dynamic shared memory without the fixed part
+template <int EFF, bool PIDACT, bool PHYS>
+void launch_policy(const RolloutArgs& a, size_t sm_var, int blocks, cudaStream_t s) {
+    const size_t sm = policy_smem_fixed(EFF) + sm_var;
+    if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    {   // shared-memory carve-out: just enough for the resident CTAs, so that the weights find the rest of the 256 KB as L1
+        const size_t need = (size_t)policy_ctas(EFF) * (sm + 1024);
+        int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
+        cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
+    }
+    rollout_kernel<EFF, PIDACT, true, PHYS><<<blocks, 64, sm, s>>>(a);       // two warps: 64 drones, 32 hidden units each in the MLP
+}
+
 // validates the policy (if any) and launches the rollout kernel family of `a` (PHYS: with the per-aviary table)
 template <bool PHYS>
 int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* stream) {
@@ -479,7 +540,10 @@ int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* st
     cudaStream_t s = (cudaStream_t)stream;
     if (io->policy) {
         const QsPolicy& q = *io->policy;
-        if (pid_act || (effects & 7u) || a.cap > 64) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports RPM / ONE_D_RPM actions, no DYN+ effects, drones_per_env <= 64");
+        const unsigned eff = effects & 7u;
+        if (eff != 0 && eff != QS_EFFECT_GND && eff != QS_EFFECT_DRAG && eff != QS_EFFECT_DW && eff != 7u)
+            return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports no DYN+ effect, GND, DRAG, DW or all three; not GND|DRAG, GND|DW or DRAG|DW");
+        if (a.cap > 64) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports drones_per_env <= 64");
         if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: pass either actions or a policy");
         if (!q.w1 || !q.b1 || !q.w2 || !q.b2 || !q.w3 || !q.b3 || !q.log_std) return fail(QS_ERR_NULL, "qs_rollout: policy weights are NULL");
         if (q.nt3 != 1 && q.nt3 != 2 && q.nt3 != 4) return fail(QS_ERR_SIZE, "qs_rollout: policy nt3 (padded output tiles of 8) must be 1, 2 or 4");
@@ -490,18 +554,17 @@ int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* st
         if (!aligned16(q.w1) || !aligned16(q.w2) || !aligned16(q.w3) || (q.vw1 && (!aligned16(q.vw1) || !aligned16(q.vw2) || !aligned16(q.vw3))))
             return fail(QS_ERR_ALIGN, "qs_rollout: policy weight arrays must be 16-byte aligned");
         a.pol = q;
-        threads = 64;                                            // two warps: 64 drones, 32 hidden units each in the MLP
         const int n_av_max = 64 / drones_per_env;
-        sm = 1280 + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32
-           + (size_t)(n_av_max * 8 * q.nt3 + n_av_max * 8 + 64) * 4 + 16;      // compact fixed part, window, means, values, log-prob terms
-        if (sm > 200 * 1024) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
-        if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<0, false, true, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        {   // shared-memory carve-out: just enough for the 7 resident CTAs, so that the weights find the rest of the 256 KB as L1
-            const size_t need = 7 * (sm + 1024);
-            int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
-            cudaFuncSetAttribute(rollout_kernel<0, false, true, PHYS>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
-        }
-        rollout_kernel<0, false, true, PHYS><<<blocks, threads, sm, s>>>(a);
+        const size_t sm_var = (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32
+                            + (size_t)(n_av_max * 8 * q.nt3 + n_av_max * 8 + 64) * 4 + 16;      // window, means, values, log-prob terms
+        if (policy_smem_fixed(eff) + sm_var > 200 * 1024) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
+#define QS_PCASE(E)                                                                                                   \
+    case E:                                                                                                           \
+        if (pid_act) launch_policy<E, true, PHYS>(a, sm_var, blocks, s);                                              \
+        else launch_policy<E, false, PHYS>(a, sm_var, blocks, s);                                                     \
+        break;
+        switch (eff) { QS_PCASE(0) QS_PCASE(QS_EFFECT_GND) QS_PCASE(QS_EFFECT_DRAG) QS_PCASE(QS_EFFECT_DW) QS_PCASE(7) }
+#undef QS_PCASE
         const cudaError_t e = cudaGetLastError();
         return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout (policy) launch");
     }

@@ -104,7 +104,11 @@ class BaseRLAviary(BaseAviary):
         INSIDE the kernel on the current observation -- SB3 `collect_rollouts` (examples/learn.py:93) without a policy launch
         or an action tensor per tick.  `noise` [T, E, D*A] standard-normal draws (None = act deterministically).  The result
         then also holds `log_probs` [T, E] and, with a critic, `values` [T, E]; `actions` are the UNCLIPPED samples (what PPO
-        stores), the env applied them clipped to [-1, 1]."""
+        stores), the env applied them clipped to [-1, 1].  Every action type (RPM, ONE_D_RPM, and PID, VEL, ONE_D_PID through the
+        embedded DSLPID controller), every `Physics` mode (DYN and the ground effect, drag and downwash variants) and a per-aviary
+        `set_physical_params` table are supported; the physics is bit for bit that of `rollout(actions)` fed the clipped actions.
+        Up to 64 drones per aviary and 32 action outputs (D * A) per aviary; what the kernel refuses raises ValueError with the
+        reason."""
         if not self.VECTORIZED:
             raise ValueError("rollout() needs the vector API (num_envs=...)")
         if self._flags & N.FLAG_AUTORESET_NEXT_STEP:

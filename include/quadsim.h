@@ -220,7 +220,8 @@ int qs_wait_flags(const unsigned* flags, unsigned seq, int world, unsigned* err_
  *     word 2, 3 = the same two pairs of w_lo'
  * with (ka, kb) = (2 t, 2 t + 8) for layers 2 and 3 -- the B fragment of mma.m16n8k16 -- and (ka, kb) = (4 t, 4 t + 2) for
  * layer 1 (its A operand is read as 4 consecutive observation elements per lane; any permutation of k inside a k-step is
- * allowed as long as A and B agree).  gym_pybullet_drones_b200/policy.py prepares the arrays (16-byte aligned). */
+ * allowed as long as A and B agree).  gym_pybullet_drones_b200/policy.py prepares the arrays (16-byte aligned).
+ * in_dim = drones_per_env * obs_dim and out_dim = drones_per_env * A for any action type (A = 4, 3 or 1), out_dim <= 32. */
 typedef struct QsPolicy {
     const unsigned* w1; const float* b1;      /* [ceil(in_dim / 16)][8][32][4], [64]   in_dim = D * obs_dim */
     const unsigned* w2; const float* b2;      /* [4][8][32][4], [64] */
@@ -256,7 +257,10 @@ typedef struct QsRolloutIO {
     int act_buffer_size;        /* B */
     const QsPolicy* policy;     /* optional (HOST pointer): the actions come from this policy evaluated on the current observation;
                                    `actions` must then be NULL, actions_out receives the sampled, UNCLIPPED actions (what PPO
-                                   stores), the env applies them clipped to [-1, 1].  RPM / ONE_D_RPM, no DYN+ effects, hidden 64. */
+                                   stores), the env applies them clipped to [-1, 1], through the embedded DSLPID controller
+                                   for PID / VEL / ONE_D_PID: the physics is bit for bit that of `actions` = the clipped
+                                   samples.  Every action type; effects none, GND, DRAG, DW or all three (GND|DRAG, GND|DW and
+                                   DRAG|DW return QS_ERR_UNSUPPORTED); drones_per_env <= 64; hidden 64. */
 } QsRolloutIO;
 
 /* Host-buffer variant of one control tick (what a CPU-side caller such as SB3's DummyVecEnv loop sees): pinned host
