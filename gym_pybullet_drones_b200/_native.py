@@ -79,6 +79,7 @@ class QsRolloutIO(C.Structure):
         ("actions", C.c_void_p), ("actions_out", C.c_void_p), ("obs_init", C.c_void_p), ("obs", C.c_void_p), ("obs_last", C.c_void_p),
         ("reward", C.c_void_p), ("terminated", C.c_void_p), ("truncated", C.c_void_p), ("done", C.c_void_p),
         ("seed", C.c_ulonglong), ("tick0", C.c_longlong), ("T", C.c_int), ("act_buffer_size", C.c_int), ("policy", C.c_void_p),
+        ("final_obs", C.c_void_p), ("final_values", C.c_void_p),
     ]
 
 

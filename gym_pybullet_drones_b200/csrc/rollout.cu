@@ -194,14 +194,14 @@ __device__ __forceinline__ qs::Drone& parked_drone(ParkedCtl* p) { return p->d; 
 // in the middle of the physics substeps; as a call, the state is saved once per tick around it.  `parked` is not touched: the caller
 // hands over the address of its drone state (Park = qs::Drone, or ParkedCtl with the controller state and previous RPMs) so that
 // the state demonstrably lives in local memory across the call (one store + load per tick) instead of being spilled piecemeal
-// inside the substep loop.
-template <class Park>
+// inside the substep loop.  CRITIC_ONLY: the critic alone (on the terminal rows of a same-step autoreset, for final_values).
+template <bool CRITIC_ONLY, class Park>
 __device__ __noinline__ void policy_forward(const RolloutArgs& a, const float* base, float* mean_s, float* val_s, int n_av, int t, Park* parked) {
     if (n_av < 0) parked_drone(parked).px = 0.0;             // never taken; keeps the hand-over opaque to the optimiser
     const int warp = t >> 5, lane = t & 31, ost = 8 * a.pol.nt3;
     const int tiles = (n_av + 15) >> 4, items = a.pol.vw1 ? 2 * tiles : tiles;
-    for (int i = warp; i < items; i += 2) {
-        const bool critic = i >= tiles;
+    for (int i = (CRITIC_ONLY ? tiles : 0) + warp; i < items; i += 2) {
+        const bool critic = CRITIC_ONLY || i >= tiles;
         const int r0 = 16 * (critic ? i - tiles : i);
         const float* x0 = base + (size_t)r0 * a.pol.in_dim;
         if (!critic)
@@ -212,6 +212,35 @@ __device__ __noinline__ void policy_forward(const RolloutArgs& a, const float* b
                      a.pol.vb1, a.pol.vb2, a.pol.vb3, 1, val_s + (size_t)r0 * 8, n_av - r0, lane);
     }
     __syncthreads();                                         // means / values of every aviary of the CTA are in shared memory
+}
+
+// policy_forward with the live state parked across the call: the drone, with PIDACT the controller state, with drag `rp` (the RPMs
+// the next tick's drag reads)
+template <int EFF, bool PIDACT, bool CRITIC_ONLY>
+__device__ __forceinline__ void parked_policy_forward(const RolloutArgs& a, const float* base, float* mean_s, float* val_s, int n_av, int t,
+                                                      qs::Drone& d, qs::PidState& pst, double (&rp)[4]) {
+    if constexpr (PIDACT || (EFF & QS_EFFECT_DRAG)) {
+        ParkedCtl parked;
+        parked.d = d;
+        if constexpr (PIDACT) parked.pst = pst;
+        if constexpr ((EFF & QS_EFFECT_DRAG) != 0) for (int j = 0; j < 4; ++j) parked.rpm_prev[j] = rp[j];
+        policy_forward<CRITIC_ONLY>(a, base, mean_s, val_s, n_av, t, &parked);
+        d = parked.d;
+        if constexpr (PIDACT) pst = parked.pst;
+        if constexpr ((EFF & QS_EFFECT_DRAG) != 0) for (int j = 0; j < 4; ++j) rp[j] = parked.rpm_prev[j];
+    } else {
+        qs::Drone parked = d;
+        policy_forward<CRITIC_ONLY>(a, base, mean_s, val_s, n_av, t, &parked);
+        d = parked;
+    }
+}
+
+// the kinematic head of an observation row: pos3 rpy3 vel3 ang_v3 (BaseRLAviary.py:310-315)
+__device__ __forceinline__ void store_head(float* row, const qs::Drone& d, const qs::Derived& o) {
+    row[0] = (float)d.px; row[1] = (float)d.py; row[2] = (float)d.pz;
+    row[3] = (float)o.roll; row[4] = (float)o.pitch; row[5] = (float)o.yaw;
+    row[6] = (float)d.vx; row[7] = (float)d.vy; row[8] = (float)d.vz;
+    row[9] = (float)o.ax; row[10] = (float)o.ay; row[11] = (float)o.az;
 }
 
 __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
@@ -245,7 +274,9 @@ __host__ __device__ constexpr int policy_ctas(int eff) { return (eff & QS_EFFECT
 // registers for the whole rollout -- the POLICY variants have none to spare (128 registers, 7 CTAs per SM, DESIGN.md 4.1b).
 // POLICY takes every EFF x PIDACT combination the envs produce (EFF = 0, GND, DRAG, DW, all three): the physics and the embedded
 // controller are the action rollout's code, so a policy rollout gives the bits of the action rollout fed its clipped actions.
-template <int EFF, bool PIDACT, bool POLICY, bool PHYS>
+// FIN: the terminal observations (io.final_obs) and with POLICY their critic values (io.final_values) are produced.  A template
+// parameter rather than a run-time branch: the new code moved the registers and spills of every entry that does not need it.
+template <int EFF, bool PIDACT, bool POLICY, bool PHYS, bool FIN>
 __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? policy_ctas(EFF) : 4) rollout_kernel(const __grid_constant__ RolloutArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const QsParams& P = a.P;
@@ -313,21 +344,8 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? policy_ctas(EF
             // the aviaries of this CTA: rows [le D, le D + D) of the window = one flattened observation of in_dim floats each
             const int n_av = rows / D;
             const int ost = 8 * a.pol.nt3;                        // padded width of the output rows in mean_s
-            if constexpr (PIDACT || (EFF & QS_EFFECT_DRAG)) {
-                // the controller state and the previous RPMs are live across the call too: handed over the same way
-                ParkedCtl parked;
-                parked.d = d;
-                if constexpr (PIDACT) parked.pst = pst;
-                if constexpr ((EFF & QS_EFFECT_DRAG) != 0) for (int j = 0; j < 4; ++j) parked.rpm_prev[j] = rpm_prev[j];
-                policy_forward(a, base, mean_s, val_s, n_av, t, &parked);
-                d = parked.d;
-                if constexpr (PIDACT) pst = parked.pst;
-                if constexpr ((EFF & QS_EFFECT_DRAG) != 0) for (int j = 0; j < 4; ++j) rpm_prev[j] = parked.rpm_prev[j];
-            } else {
-                qs::Drone parked = d;
-                policy_forward(a, base, mean_s, val_s, n_av, t, &parked);
-                d = parked;
-            }
+            // the controller state and the previous RPMs are live across the call too: handed over the same way
+            parked_policy_forward<EFF, PIDACT, false>(a, base, mean_s, val_s, n_av, t, d, pst, rpm_prev);
             float lp = 0.f;
             if (live) {
                 const int od_out = a.pol.out_dim;
@@ -454,6 +472,28 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? policy_ctas(EF
             if (a.io.done) a.io.done[oe] = 0;
         }
         // ---- autoreset, head, bookkeeping ----------------------------------------------------------------------------
+        if constexpr (FIN) {
+            const bool fin = live && (a.flags & QS_FLAG_AUTORESET_SAME_STEP) && env_done;
+            if (fin) {
+                // the terminal observation in my row of the next window: the head of the state before the reset, the history before
+                // CLEARS_HISTORY zeroes it -- the row qs_step writes to final_obs (rare path: strided stores are fine)
+                float* row = base + A + (size_t)t * od;
+                store_head(row, d, o);
+                if (a.io.final_obs) {
+                    float* f = a.io.final_obs + ((long long)k * N + i) * od;
+                    for (int q = 0; q < od; ++q) f[q] = row[q];
+                }
+            }
+            if constexpr (POLICY) {
+                // the critic on the terminal rows, which exist only between the task and the reset: one pass of the critic alone,
+                // on the ticks where an aviary of this CTA finished (CTA-uniform branch); the other aviaries' rows are evaluated
+                // too and dropped.  The pass ends with a barrier, so the reset below overwrites rows nobody reads any more.
+                if (a.io.final_values && __syncthreads_or(fin)) {
+                    parked_policy_forward<EFF, PIDACT, true>(a, base + A, mean_s, val_s, rows / D, t, d, pst, rpm);
+                    if (fin && dslot == 0) a.io.final_values[(long long)k * E + e] = val_s[le * 8];
+                }
+            }
+        }
         if (live) {
             float* row = base + A + (size_t)t * od;              // my row in the NEXT window
             if ((a.flags & QS_FLAG_AUTORESET_SAME_STEP) && env_done) {
@@ -465,10 +505,7 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? policy_ctas(EF
                 rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;
                 sc = -a.substeps;
             }
-            row[0] = (float)d.px; row[1] = (float)d.py; row[2] = (float)d.pz;
-            row[3] = (float)o.roll; row[4] = (float)o.pitch; row[5] = (float)o.yaw;
-            row[6] = (float)d.vx; row[7] = (float)d.vy; row[8] = (float)d.vz;
-            row[9] = (float)o.ax; row[10] = (float)o.ay; row[11] = (float)o.az;
+            store_head(row, d, o);
             sc += a.substeps;
             if (k < T - 1) round_to_planes(d);                // (the final store_drone applies the same rounding once)
             rpm_prev[0] = rpm[0]; rpm_prev[1] = rpm[1]; rpm_prev[2] = rpm[2]; rpm_prev[3] = rpm[3];
@@ -517,20 +554,21 @@ __global__ void __launch_bounds__(POLICY ? 64 : kMaxTPB, POLICY ? policy_ctas(EF
 }
 
 // one policy variant: `sm_var` = its dynamic shared memory without the fixed part
-template <int EFF, bool PIDACT, bool PHYS>
+template <int EFF, bool PIDACT, bool PHYS, bool FIN>
 void launch_policy(const RolloutArgs& a, size_t sm_var, int blocks, cudaStream_t s) {
     const size_t sm = policy_smem_fixed(EFF) + sm_var;
-    if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS, FIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     {   // shared-memory carve-out: just enough for the resident CTAs, so that the weights find the rest of the 256 KB as L1
         const size_t need = (size_t)policy_ctas(EFF) * (sm + 1024);
         int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
-        cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
+        cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS, FIN>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
     }
-    rollout_kernel<EFF, PIDACT, true, PHYS><<<blocks, 64, sm, s>>>(a);       // two warps: 64 drones, 32 hidden units each in the MLP
+    rollout_kernel<EFF, PIDACT, true, PHYS, FIN><<<blocks, 64, sm, s>>>(a);       // two warps: 64 drones, 32 hidden units each in the MLP
 }
 
-// validates the policy (if any) and launches the rollout kernel family of `a` (PHYS: with the per-aviary table)
-template <bool PHYS>
+// validates the policy (if any) and launches the rollout kernel family of `a` (PHYS: with the per-aviary table; FIN: with the
+// terminal observations and values)
+template <bool PHYS, bool FIN>
 int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* stream) {
     const int drones_per_env = a.D, A = a.A;
     const unsigned effects = a.effects;
@@ -560,8 +598,8 @@ int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* st
         if (policy_smem_fixed(eff) + sm_var > 200 * 1024) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
 #define QS_PCASE(E)                                                                                                   \
     case E:                                                                                                           \
-        if (pid_act) launch_policy<E, true, PHYS>(a, sm_var, blocks, s);                                              \
-        else launch_policy<E, false, PHYS>(a, sm_var, blocks, s);                                                     \
+        if (pid_act) launch_policy<E, true, PHYS, FIN>(a, sm_var, blocks, s);                                              \
+        else launch_policy<E, false, PHYS, FIN>(a, sm_var, blocks, s);                                                     \
         break;
         switch (eff) { QS_PCASE(0) QS_PCASE(QS_EFFECT_GND) QS_PCASE(QS_EFFECT_DRAG) QS_PCASE(QS_EFFECT_DW) QS_PCASE(7) }
 #undef QS_PCASE
@@ -571,11 +609,11 @@ int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* st
 #define QS_RCASE(E)                                                                                                   \
     case E: {                                                                                                         \
         if (pid_act) {                                                                                                \
-            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, true, false, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
-            rollout_kernel<E, true, false, PHYS><<<blocks, threads, sm, s>>>(a);                                            \
+            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, true, false, PHYS, FIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
+            rollout_kernel<E, true, false, PHYS, FIN><<<blocks, threads, sm, s>>>(a);                                            \
         } else {                                                                                                      \
-            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, false, false, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
-            rollout_kernel<E, false, false, PHYS><<<blocks, threads, sm, s>>>(a);                                           \
+            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, false, false, PHYS, FIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
+            rollout_kernel<E, false, false, PHYS, FIN><<<blocks, threads, sm, s>>>(a);                                           \
         }                                                                                                             \
     } break;
     switch (effects & 7u) { QS_RCASE(0) QS_RCASE(1) QS_RCASE(2) QS_RCASE(3) QS_RCASE(4) QS_RCASE(5) QS_RCASE(6) QS_RCASE(7) }
@@ -611,6 +649,9 @@ int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int 
         return fail(QS_ERR_UNSUPPORTED, "qs_rollout: only SAME_STEP autoreset (or none) is supported");
     if (drones_per_env > kMaxTPB) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: drones_per_env <= 128");
     if (!io->obs_init || !io->obs || !io->reward || !io->terminated || !io->truncated) return fail(QS_ERR_NULL, "qs_rollout: NULL buffer");
+    if ((io->final_obs || io->final_values) && !(flags & QS_FLAG_AUTORESET_SAME_STEP))
+        return fail(QS_ERR_UNSUPPORTED, "qs_rollout: final_obs / final_values need QS_FLAG_AUTORESET_SAME_STEP");
+    if (io->final_values && !(io->policy && io->policy->vw1)) return fail(QS_ERR_NULL, "qs_rollout: final_values requested without a policy critic");
     if (io->act_buffer_size <= 0) return fail(QS_ERR_SIZE, "qs_rollout: act_buffer_size must be > 0");
     if (io->T > qs_rollout_max_ticks(act_type, io->act_buffer_size, drones_per_env)) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: T exceeds qs_rollout_max_ticks (split the rollout)");
     if (task == QS_TASK_HOVER && (!st->target_pos || !aligned32(st->target_pos))) return fail(QS_ERR_NULL, "qs_rollout: target_pos NULL/misaligned");
@@ -633,7 +674,9 @@ int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int 
         const bool aligned = aligned16(io->obs_init) && (span % 16 == 0) && ((row_bytes * ((size_t)a.N % a.tpb)) % 16 == 0);
         a.stage_mode = (aligned && A == 4) ? 1 : 2;
     }
-    return a.st.phys ? launch_rollout<true>(a, io, pid_act, stream) : launch_rollout<false>(a, io, pid_act, stream);
+    if (io->final_obs || io->final_values)
+        return a.st.phys ? launch_rollout<true, true>(a, io, pid_act, stream) : launch_rollout<false, true>(a, io, pid_act, stream);
+    return a.st.phys ? launch_rollout<true, false>(a, io, pid_act, stream) : launch_rollout<false, false>(a, io, pid_act, stream);
 }
 
 }  // extern "C"

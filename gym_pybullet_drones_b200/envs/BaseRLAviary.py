@@ -90,15 +90,21 @@ class BaseRLAviary(BaseAviary):
 
     ################################################################################
 
-    def rollout(self, actions=None, num_steps=None, seed=0, out=None, policy=None, noise=None):
+    def rollout(self, actions=None, num_steps=None, seed=0, out=None, policy=None, noise=None, final_obs=False, final_values=False):
         """T control ticks in one kernel launch (qs_rollout): exactly `num_steps` calls of `step()` with the same
         actions, but the drone state stays in registers and the action history in shared memory between ticks.
 
         Vector API only.  `actions`: float32 CUDA tensor [T, E, D, A], or None for uniform[-1, 1) actions generated on the
         device from (`seed`, tick, drone) -- the synthetic random-action workload.  Autoreset must be "same_step" or
-        disabled; `info["final_obs"]` is not produced.  Returns a dict of CUDA tensors in rollout-buffer layout:
+        disabled.  Returns a dict of CUDA tensors in rollout-buffer layout:
         obs [T, E, D, obs_dim] (observation AFTER each tick), actions [T, E, D, A], rewards / terminated / truncated [T, E].
         `out` may pass a previous result dict to reuse its buffers.
+
+        `final_obs=True` (same-step autoreset only) adds `final_obs` [T, E, D, obs_dim]: the terminal observation of every
+        aviary that finished at tick k, bit for bit `step()`'s `info["final_obs"]`; `final_values=True` (with a policy that has
+        a critic) adds `final_values` [T, E]: the critic on those terminal observations.  Both are valid where
+        `terminated | truncated` and unspecified elsewhere.  SB3's `collect_rollouts` bootstraps a time-out with them:
+        `rewards[k] += gamma * final_values[k]` where `truncated[k]`.
 
         `policy` (a `gym_pybullet_drones_b200.policy.MlpPolicy`): the actions of every tick come from the policy evaluated
         INSIDE the kernel on the current observation -- SB3 `collect_rollouts` (examples/learn.py:93) without a policy launch
@@ -115,6 +121,10 @@ class BaseRLAviary(BaseAviary):
             raise ValueError("rollout() supports autoreset='same_step' or disabled")
         if self._dw_fz is not None:
             raise ValueError("rollout() needs drones_per_env <= 128")
+        if (final_obs or final_values) and not (self._flags & N.FLAG_AUTORESET_SAME_STEP):
+            raise ValueError("rollout(final_obs=..., final_values=...) needs autoreset='same_step'")
+        if final_values and (policy is None or policy.critic is None):
+            raise ValueError("rollout(final_values=True) needs a policy with a critic")
         E, D, A, od, dev = self._E, self._D, self._A, self._obs_dim, self.device
         if policy is not None:
             if actions is not None:
@@ -146,6 +156,10 @@ class BaseRLAviary(BaseAviary):
                 out["log_probs"] = torch.empty((T, E), dtype=torch.float32, device=dev)
             if policy.critic is not None and "values" not in out:
                 out["values"] = torch.empty((T, E), dtype=torch.float32, device=dev)
+        if final_obs and "final_obs" not in out:
+            out["final_obs"] = torch.empty((T, E, D, od), dtype=torch.float32, device=dev)
+        if final_values and "final_values" not in out:
+            out["final_values"] = torch.empty((T, E), dtype=torch.float32, device=dev)
         tmax = self._lib.qs_rollout_max_ticks(self._act_type(), self._B, D)
         if tmax <= 0:
             if self._B == 0:
@@ -167,6 +181,8 @@ class BaseRLAviary(BaseAviary):
                 io.obs_last = self._obs_ptr[1 - cur]
                 io.reward, io.terminated, io.truncated = out["rewards"][k0].data_ptr(), out["terminated"][k0].data_ptr(), out["truncated"][k0].data_ptr()
                 io.done = None
+                io.final_obs = out["final_obs"][k0].data_ptr() if final_obs else None
+                io.final_values = out["final_values"][k0].data_ptr() if final_values else None
                 io.tick0, io.T = int(getattr(self, "_rollout_tick", 0)) + k0, tt
                 if policy is not None:
                     qp = policy.c_struct(None if noise is None else noise.view(T, -1)[k0], out["log_probs"][k0],

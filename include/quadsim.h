@@ -240,7 +240,11 @@ typedef struct QsPolicy {
 /* Multi-tick rollout: T control ticks in ONE launch (SURVEY.md 8f rank 1; the caller is SB3's collect_rollouts,
  * examples/learn.py:93).  Exactly T calls of qs_step with SAME_STEP (or no) autoreset, but the drone state stays in
  * registers and the action history in shared memory between ticks: per tick only the action is read and the observation
- * row, reward and flags are written. */
+ * row, reward and flags are written.
+ * Terminal observations (SAME_STEP autoreset): at tick k the kernel writes final_obs[k][i] for every drone i of an aviary that
+ * finished at k, bit for bit the row qs_step writes to QsStepIO.final_obs, and with a policy critic final_values[k][e] = the
+ * critic on that aviary's terminal rows (the value SB3 bootstraps a truncated episode with).  Entries of the aviaries that did
+ * not finish at k are not written.  The critic pass runs only in CTAs that hold a finished aviary at that tick. */
 typedef struct QsRolloutIO {
     const float* actions;       /* [T][N][A] float32, or NULL: uniform[-1,1) actions generated on the device from (seed, tick, drone) */
     float* actions_out;         /* out [T][N][A] the actions that were applied; nullable */
@@ -261,6 +265,10 @@ typedef struct QsRolloutIO {
                                    for PID / VEL / ONE_D_PID: the physics is bit for bit that of `actions` = the clipped
                                    samples.  Every action type; effects none, GND, DRAG, DW or all three (GND|DRAG, GND|DW and
                                    DRAG|DW return QS_ERR_UNSUPPORTED); drones_per_env <= 64; hidden 64. */
+    float* final_obs;           /* out [T][N][12+B*A] terminal observations (see above); nullable.  Needs QS_FLAG_AUTORESET_SAME_STEP
+                                   (QS_ERR_UNSUPPORTED otherwise) */
+    float* final_values;        /* out [T][E] critic on the terminal observations; nullable.  Needs SAME_STEP autoreset
+                                   (QS_ERR_UNSUPPORTED) and a policy with a critic (QS_ERR_NULL) */
 } QsRolloutIO;
 
 /* Host-buffer variant of one control tick (what a CPU-side caller such as SB3's DummyVecEnv loop sees): pinned host
@@ -335,7 +343,8 @@ int qs_step_host(const QsParams* p, const QsState* st, const QsStepIO* io, const
                  int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 
 /* T fused control ticks (see QsRolloutIO).  RL action types, KIN observations, drones_per_env <= 128, autoreset SAME_STEP or
- * none (flags as qs_step; final_obs is not produced).  qs_rollout_max_ticks gives the largest T for an observation width. */
+ * none (flags as qs_step; the terminal observations go to QsRolloutIO.final_obs, their critic values to final_values).
+ * qs_rollout_max_ticks gives the largest T for an observation width. */
 int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int act_type, int task,
                int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 int qs_rollout_max_ticks(int act_type, int act_buffer_size, int drones_per_env);
