@@ -219,6 +219,7 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
         if (pending) {                       // NEXT_STEP autoreset: this call only resets the env
             init_drone(a.st, tbl, d);
             if (a.flags & QS_FLAG_AUTORESET_CLEARS_PID) pst = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+            rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                               // last_clipped_action = 0 (BaseAviary.py:468)
         }
         if (a.flags & QS_FLAG_RPY_F32) qs::derive<true>(d, R_last, o); else qs::derive<false>(d, R_last, o);
         if (pending) { o.ax = o.ay = o.az = 0.0; }
@@ -293,7 +294,7 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
         }
         mode_s[t] = mode;
         store_drone(a.st, N, i, d);
-        if (a.st.last_rpm && !pending) st256(a.st.last_rpm, i, rpm[0], rpm[1], rpm[2], rpm[3]);
+        if (a.st.last_rpm) st256(a.st.last_rpm, i, rpm[0], rpm[1], rpm[2], rpm[3]);
         if (pid_act) store_pid(a.st.pid, N, i, pst);
         if (dslot == 0 && want_epilogue) {
             if (pending) {

@@ -95,10 +95,18 @@ class BaseRLAviary(BaseAviary):
         actions, but the drone state stays in registers and the action history in shared memory between ticks.
 
         Vector API only.  `actions`: float32 CUDA tensor [T, E, D, A], or None for uniform[-1, 1) actions generated on the
-        device from (`seed`, tick, drone) -- the synthetic random-action workload.  Autoreset must be "same_step" or
-        disabled.  Returns a dict of CUDA tensors in rollout-buffer layout:
+        device from (`seed`, tick, drone) -- the synthetic random-action workload.  Every autoreset mode of the env is
+        honoured.  Returns a dict of CUDA tensors in rollout-buffer layout:
         obs [T, E, D, obs_dim] (observation AFTER each tick), actions [T, E, D, A], rewards / terminated / truncated [T, E].
         `out` may pass a previous result dict to reuse its buffers.
+
+        With autoreset="next_step" (gymnasium >= 1.0, CleanRL-style loops) an aviary that finishes at tick k is reset by tick
+        k+1, which ignores its action: obs[k+1] is the reset observation, rewards[k+1] = 0, terminated / truncated[k+1] = False.
+        The result then also holds `autoreset` [T, E] bool, the ticks that only reset an aviary (a learner masks these
+        transitions out): autoreset[0] is the env's pending reset from before the call, autoreset[k] = terminated[k-1] |
+        truncated[k-1] after it.  obs[k] is then the terminal observation, so no final_obs is needed, and with a critic the
+        time-out bootstrap value V(obs[k]) is values[k+1] where autoreset[k+1]; for the last tick it is the next rollout's
+        values[0].
 
         `final_obs=True` (same-step autoreset only) adds `final_obs` [T, E, D, obs_dim]: the terminal observation of every
         aviary that finished at tick k, bit for bit `step()`'s `info["final_obs"]`; `final_values=True` (with a policy that has
@@ -117,8 +125,6 @@ class BaseRLAviary(BaseAviary):
         reason."""
         if not self.VECTORIZED:
             raise ValueError("rollout() needs the vector API (num_envs=...)")
-        if self._flags & N.FLAG_AUTORESET_NEXT_STEP:
-            raise ValueError("rollout() supports autoreset='same_step' or disabled")
         if self._dw_fz is not None:
             raise ValueError("rollout() needs drones_per_env <= 128")
         if (final_obs or final_values) and not (self._flags & N.FLAG_AUTORESET_SAME_STEP):
@@ -160,6 +166,9 @@ class BaseRLAviary(BaseAviary):
             out["final_obs"] = torch.empty((T, E, D, od), dtype=torch.float32, device=dev)
         if final_values and "final_values" not in out:
             out["final_values"] = torch.empty((T, E), dtype=torch.float32, device=dev)
+        next_step = bool(self._flags & N.FLAG_AUTORESET_NEXT_STEP)
+        if next_step and "autoreset" not in out:
+            out["autoreset"] = torch.empty((T, E), dtype=torch.bool, device=dev)
         tmax = self._lib.qs_rollout_max_ticks(self._act_type(), self._B, D)
         if tmax <= 0:
             if self._B == 0:
@@ -170,6 +179,8 @@ class BaseRLAviary(BaseAviary):
         n = self._N
         with self._on_device():
             stream = self._stream()
+            if next_step:
+                out["autoreset"][0].copy_(self._pending)             # the latch the first tick starts from (kernel-owned state)
             k0 = 0
             while k0 < T:
                 tt = min(tmax, T - k0)
@@ -190,11 +201,12 @@ class BaseRLAviary(BaseAviary):
                     io.policy = C.addressof(qp)
                     io.actions, io.actions_out = None, out["actions"][k0].data_ptr()
                 rc = self._lib.qs_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), self._act_type(), self._task(),
-                                          E, D, self.PYB_STEPS_PER_CTRL, self._effects,
-                                          self._flags & ~N.FLAG_AUTORESET_NEXT_STEP, stream)
+                                          E, D, self.PYB_STEPS_PER_CTRL, self._effects, self._flags, stream)
                 N.check(rc, "qs_rollout")
                 self._cur = 1 - cur
                 k0 += tt
+            if next_step:
+                torch.logical_or(out["terminated"][:-1], out["truncated"][:-1], out=out["autoreset"][1:])
         self._rollout_tick = int(getattr(self, "_rollout_tick", 0)) + T
         # keep the per-step outputs of the env consistent with the last tick
         self._reward.copy_(out["rewards"][-1]); self._terminated.copy_(out["terminated"][-1]); self._truncated.copy_(out["truncated"][-1])

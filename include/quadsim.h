@@ -238,9 +238,15 @@ typedef struct QsPolicy {
 } QsPolicy;
 
 /* Multi-tick rollout: T control ticks in ONE launch (SURVEY.md 8f rank 1; the caller is SB3's collect_rollouts,
- * examples/learn.py:93).  Exactly T calls of qs_step with SAME_STEP (or no) autoreset, but the drone state stays in
- * registers and the action history in shared memory between ticks: per tick only the action is read and the observation
- * row, reward and flags are written.
+ * examples/learn.py:93).  Exactly T calls of qs_step with the same flags -- SAME_STEP, NEXT_STEP or no autoreset -- but the
+ * drone state stays in registers and the action history in shared memory between ticks: per tick only the action is read and
+ * the observation row, reward and flags are written.
+ * NEXT_STEP autoreset: an aviary whose QsState.pending_reset latch is set at the start of a tick is only reset by it, as by
+ * qs_step: its action is ignored (no decode, no controller, no physics; actions_out and, with a policy, logprob / values are
+ * still written), its observation is the reset pose with the action history unshifted (zeroed with CLEARS_HISTORY), reward 0,
+ * terminated / truncated 0.  The latch is carried from tick to tick (a tick's done sets it for the next) and stored at the end,
+ * so it crosses launches and mixes with qs_step.  obs[k] of an aviary that finished at k is its terminal observation, and the
+ * policy's values[k+1] the critic on it.
  * Terminal observations (SAME_STEP autoreset): at tick k the kernel writes final_obs[k][i] for every drone i of an aviary that
  * finished at k, bit for bit the row qs_step writes to QsStepIO.final_obs, and with a policy critic final_values[k][e] = the
  * critic on that aviary's terminal rows (the value SB3 bootstraps a truncated episode with).  Entries of the aviaries that did
@@ -266,7 +272,7 @@ typedef struct QsRolloutIO {
                                    samples.  Every action type; effects none, GND, DRAG, DW or all three (GND|DRAG, GND|DW and
                                    DRAG|DW return QS_ERR_UNSUPPORTED); drones_per_env <= 64; hidden 64. */
     float* final_obs;           /* out [T][N][12+B*A] terminal observations (see above); nullable.  Needs QS_FLAG_AUTORESET_SAME_STEP
-                                   (QS_ERR_UNSUPPORTED otherwise) */
+                                   (QS_ERR_UNSUPPORTED otherwise; under NEXT_STEP obs[k] already is the terminal observation) */
     float* final_values;        /* out [T][E] critic on the terminal observations; nullable.  Needs SAME_STEP autoreset
                                    (QS_ERR_UNSUPPORTED) and a policy with a critic (QS_ERR_NULL) */
 } QsRolloutIO;
@@ -342,8 +348,10 @@ int qs_step_call(const QsStepCall* c, void* stream);
 int qs_step_host(const QsParams* p, const QsState* st, const QsStepIO* io, const QsHostIO* h, int act_type, int task,
                  int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 
-/* T fused control ticks (see QsRolloutIO).  RL action types, KIN observations, drones_per_env <= 128, autoreset SAME_STEP or
- * none (flags as qs_step; the terminal observations go to QsRolloutIO.final_obs, their critic values to final_values).
+/* T fused control ticks (see QsRolloutIO).  RL action types, KIN observations, drones_per_env <= 128, autoreset SAME_STEP,
+ * NEXT_STEP or none (flags as qs_step: both modes together return QS_ERR_ENUM, NEXT_STEP needs QsState.pending_reset
+ * (QS_ERR_NULL) and the init tables; under SAME_STEP the terminal observations go to QsRolloutIO.final_obs, their critic values
+ * to final_values).
  * qs_rollout_max_ticks gives the largest T for an observation width. */
 int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int act_type, int task,
                int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
