@@ -12,7 +12,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))    # override: A/B builds in tools/
 _CSRC = os.path.join(_HERE, "csrc")
-SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "formation.cu")]
+SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_ctrl.cu",
+                                             "formation.cu")]
 HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
@@ -31,6 +32,7 @@ FLAG_AUTORESET_SAME_STEP, FLAG_AUTORESET_NEXT_STEP, FLAG_RPY_F32 = 1, 2, 4
 FLAG_AUTORESET_CLEARS_PID, FLAG_AUTORESET_CLEARS_HISTORY = 8, 16
 FLAG_OBS_STATE20 = 32
 FLAG_SKIP_EPILOGUE, FLAG_RPM_FROM_LAST, FLAG_ACTION_F64 = 0x100, 0x200, 0x400
+CTRL_RAW, CTRL_VEL, CTRL_TRACK = 0, 1, 2          # qs_ctrl_rollout modes
 ABI_VERSION = 4
 PHYS_WIDTH = 16          # float64 columns of one QsState.phys row
 
@@ -104,6 +106,15 @@ class QsLogRing(C.Structure):
     _fields_ = [("ring", C.c_void_p), ("head", C.c_void_p), ("capacity", C.c_int), ("first_drone", C.c_int), ("n_drones", C.c_int), ("kin_rows", C.c_int)]
 
 
+class QsCtrlRolloutIO(C.Structure):
+    _fields_ = [("T", C.c_int), ("log_targets", C.c_int), ("actions", C.c_void_p),
+                ("ctrl_params", C.c_void_p), ("pid_state", C.c_void_p), ("control_timestep", C.c_double),
+                ("waypoints", C.c_void_p), ("W", C.c_int), ("M", C.c_int), ("start", C.c_void_p), ("offset", C.c_void_p),
+                ("target_rpy", C.c_void_p), ("target_vel", C.c_void_p), ("target_rpy_rates", C.c_void_p),
+                ("obs", C.c_void_p), ("rpm", C.c_void_p), ("pos_e", C.c_void_p), ("yaw_e", C.c_void_p), ("obs_last", C.c_void_p),
+                ("log", C.c_void_p), ("log_controls", C.c_void_p)]
+
+
 class QsStepCall(C.Structure):
     _fields_ = [("p", C.c_void_p), ("st", C.c_void_p), ("io", C.c_void_p),
                 ("act_type", C.c_int), ("task", C.c_int), ("n_envs", C.c_int), ("drones_per_env", C.c_int), ("substeps", C.c_int),
@@ -112,7 +123,8 @@ class QsStepCall(C.Structure):
 
 EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_state", "qs_sizeof_step_io",
            "qs_sizeof_rollout_io", "qs_sizeof_host_io", "qs_step", "qs_step_call", "qs_step_host", "qs_rollout", "qs_rollout_max_ticks", "qs_dyn_substeps", "qs_dyn_substeps_pub", "qs_pid_control",
-           "qs_downwash", "qs_downwash_boxed", "qs_dw_gathered_floats", "qs_dw_boxes", "qs_downwash_rows", "qs_dw_publish", "qs_enable_peer_access", "qs_ipc_export", "qs_ipc_import", "qs_adjacency", "qs_reset", "qs_reset_heads", "qs_host_is_pinned", "qs_log_append", "qs_sizeof_log_ring", "qs_wait_flags", "qs_pid_control_state"]
+           "qs_downwash", "qs_downwash_boxed", "qs_dw_gathered_floats", "qs_dw_boxes", "qs_downwash_rows", "qs_dw_publish", "qs_enable_peer_access", "qs_ipc_export", "qs_ipc_import", "qs_adjacency", "qs_reset", "qs_reset_heads", "qs_host_is_pinned", "qs_log_append", "qs_sizeof_log_ring", "qs_wait_flags", "qs_pid_control_state",
+           "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io"]
 MAX_PEERS = 16
 
 
@@ -182,6 +194,10 @@ def lib():
                              C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
     L.qs_rollout_max_ticks.restype = C.c_int
     L.qs_rollout_max_ticks.argtypes = [C.c_int, C.c_int, C.c_int]
+    L.qs_ctrl_rollout.restype = C.c_int
+    L.qs_ctrl_rollout.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.c_int, C.c_int, C.c_int,
+                                  C.c_int, C.c_uint, C.c_uint, C.c_void_p]
+    L.qs_sizeof_ctrl_rollout_io.restype = C.c_int
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -234,8 +250,9 @@ def lib():
     if (L.qs_sizeof_params(), L.qs_sizeof_state(), L.qs_sizeof_step_io(), L.qs_sizeof_rollout_io()) != \
             (C.sizeof(QsParams), C.sizeof(QsState), C.sizeof(QsStepIO), C.sizeof(QsRolloutIO)):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror: rebuild")
-    if L.qs_sizeof_log_ring() != C.sizeof(QsLogRing) or L.qs_sizeof_host_io() != C.sizeof(QsHostIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io): rebuild")
+    if L.qs_sizeof_log_ring() != C.sizeof(QsLogRing) or L.qs_sizeof_host_io() != C.sizeof(QsHostIO) or \
+            L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io): rebuild")
     _lib = L
     return L
 

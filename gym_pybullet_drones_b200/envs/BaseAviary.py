@@ -626,6 +626,124 @@ class BaseAviary(Env):
             self._log_append()
         return self._obs_buf[self._cur]
 
+    def _ctrl_rollout(self, mode, actions=None, controller=None, num_steps=None, waypoints=None, start=None, offset=None,
+                      target_rpy=None, target_vel=None, target_rpy_rates=None, control_timestep=None, record=True, errors=False,
+                      out=None, log_targets=False):
+        """rollout() of the state-vector envs (CtrlAviary, VelocityAviary): one qs_ctrl_rollout launch of T ticks in `mode`
+        (N.CTRL_RAW / CTRL_VEL / CTRL_TRACK); see CtrlAviary.rollout."""
+        if not self.VECTORIZED:
+            raise ValueError("rollout() needs the vector API (num_envs=...)")
+        if self._py_hooks:
+            raise ValueError("rollout() evaluates the built-in hooks inside the kernel: not available when a subclass overrides them")
+        if self._EXTERNAL_DOWNWASH:
+            raise ValueError("rollout() is not available with external downwash (formations)")
+        E, D, n, dev = self._E, self._D, self._N, self.device
+        io = N.QsCtrlRolloutIO()
+        flags = self._flags & N.FLAG_RPY_F32
+        keep = []                                            # device inputs that must live until the launch is enqueued
+
+        def rows3(x, name):
+            if x is None:
+                return None
+            t = x if isinstance(x, torch.Tensor) else torch.as_tensor(np.asarray(x, dtype=np.float64))
+            t = t.to(device=dev, dtype=torch.float64)
+            if t.numel() == 3:
+                t = t.reshape(1, 3).expand(n, 3)
+            elif t.numel() != n * 3:
+                raise ValueError("%s must be [3], [%d, %d, 3] or [%d, 3]" % (name, E, D, n))
+            t = t.reshape(n, 3).contiguous()
+            keep.append(t)
+            return t.data_ptr()
+        if mode == N.CTRL_TRACK:
+            if actions is not None:
+                raise ValueError("pass either actions or a controller")
+            if controller is None:
+                raise ValueError("rollout() needs actions [T, E, D, 4] or a controller")
+            if getattr(controller, "num_drones", None) != n or not hasattr(controller, "_state"):
+                raise ValueError("the controller must be a DSLPIDControl for the env's %d drones (num_drones=%d)" % (n, n))
+            if torch.device(controller.device) != dev:
+                raise ValueError("the controller's state is on %s, the env's on %s" % (controller.device, dev))
+            if waypoints is None:
+                raise ValueError("a controller rollout needs waypoints [W, 3] or [W, E, D, 3]")
+            wp = waypoints if isinstance(waypoints, torch.Tensor) else torch.as_tensor(np.asarray(waypoints, dtype=np.float64))
+            wp = wp.to(device=dev, dtype=torch.float64).contiguous()
+            if wp.dim() == 2 and wp.shape[1] == 3:
+                W, M = wp.shape[0], 1
+            elif wp.dim() >= 3 and wp.shape[-1] == 3 and wp[0].numel() == n * 3:
+                W, M = wp.shape[0], n
+            else:
+                raise ValueError("waypoints must be [W, 3] (one path for every drone) or [W, %d, %d, 3] (one per drone)" % (E, D))
+            if W == 0:
+                raise ValueError("waypoints must hold at least one row")
+            T = W if num_steps is None else int(num_steps)
+            if start is None:
+                st0 = torch.zeros((n,), dtype=torch.int32, device=dev)
+            else:
+                st0 = start if isinstance(start, torch.Tensor) else torch.as_tensor(np.asarray(start))
+                st0 = st0.to(device=dev, dtype=torch.int32)
+                st0 = (st0.reshape(1).expand(n) if st0.numel() == 1 else st0.reshape(n)).contiguous()
+            keep += [wp, st0]
+            io.ctrl_params = C.addressof(controller._P)
+            io.pid_state = controller._state.data_ptr()
+            io.control_timestep = float(self.CTRL_TIMESTEP if control_timestep is None else control_timestep)
+            io.waypoints, io.W, io.M, io.start = wp.data_ptr(), W, M, st0.data_ptr()
+            io.offset = rows3(offset, "offset")
+            io.target_rpy, io.target_vel = rows3(target_rpy, "target_rpy"), rows3(target_vel, "target_vel")
+            io.target_rpy_rates = rows3(target_rpy_rates, "target_rpy_rates")
+            io.log_targets = 1 if log_targets else 0
+        else:
+            if controller is not None:
+                raise ValueError("pass either actions or a controller" if actions is not None else "%s.rollout() takes no controller" % type(self).__name__)
+            if actions is None:
+                raise ValueError("rollout() needs actions [T, %d, %d, 4]" % (E, D))
+            if errors:
+                raise ValueError("errors=True (pos_e / yaw_e) needs a controller rollout")
+            a = actions if isinstance(actions, torch.Tensor) else torch.as_tensor(np.asarray(actions))
+            f64 = mode == N.CTRL_RAW and a.dtype == torch.float64
+            a = a.to(device=dev, dtype=torch.float64 if f64 else torch.float32).contiguous()
+            if a.numel() == 0 or a.numel() % (n * 4) or a.shape[-1] != 4:
+                raise ValueError("actions must be [T, %d, %d, 4]" % (E, D))
+            if a.data_ptr() % 32:
+                a = a.clone()
+            keep.append(a)
+            T = a.numel() // (n * 4)
+            io.actions = a.data_ptr()
+            if f64:
+                flags |= N.FLAG_ACTION_F64
+        if T <= 0:
+            raise ValueError("num_steps must be > 0")
+        shapes = dict(obs=((T, E, D, 20), torch.float32), rpm=((T, E, D, 4), torch.float64))
+        if errors:
+            shapes.update(pos_e=((T, E, D, 3), torch.float32), yaw_e=((T, E, D), torch.float32))
+        if not record:
+            del shapes["obs"]
+        res = {}
+        for k, (shp, dt) in shapes.items():
+            b = out.get(k) if out is not None else None
+            if b is None:
+                b = torch.empty(shp, dtype=dt, device=dev)
+            elif tuple(b.shape) != shp or b.dtype != dt or b.device != dev or not b.is_contiguous():
+                raise ValueError("out[%r] must be a contiguous %s tensor of shape %s on %s" % (k, dt, shp, dev))
+            res[k] = b
+        ptr = lambda k: res[k].data_ptr() if k in res else None      # noqa: E731
+        io.T = T
+        io.obs, io.rpm, io.pos_e, io.yaw_e = ptr("obs"), ptr("rpm"), ptr("pos_e"), ptr("yaw_e")
+        tgt = self._cur ^ (T & 1)                          # the buffer T step() calls would leave current
+        io.obs_last = self._obs_ptr[tgt]
+        if self._log is not None:
+            ring, controls = self._log
+            io.log = C.addressof(ring)
+            io.log_controls = controls.data_ptr() if controls is not None else None
+        with self._on_device():
+            self._reward.fill_(-1.0)                       # dummy task (CtrlAviary.py:144-185)
+            rc = self._lib.qs_ctrl_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), mode, E, D, self.PYB_STEPS_PER_CTRL,
+                                           self._effects, flags, self._stream())
+        N.check(rc, "qs_ctrl_rollout")
+        self._cur = tgt
+        if controller is not None:
+            controller.control_counter += T
+        return res
+
     def _dyn_substep(self, rpm_ptr, state20_ptr, flags, stream):
         """One DYN substep with the downwash force of `_downwash_stage` (raw-RPM envs, split loop); FormationShard fuses its
         position exchange into this launch."""

@@ -53,6 +53,14 @@ class VelocityAviary(BaseAviary):
         hi = np.array([[np.inf, np.inf, np.inf, 1., 1., 1., 1., np.pi, np.pi, np.pi, np.inf, np.inf, np.inf, np.inf, np.inf, np.inf, m, m, m, m] for i in range(self.NUM_DRONES)])
         return spaces.Box(low=lo, high=hi, dtype=np.float32)
 
+    def rollout(self, actions, record=True, out=None):
+        """T control ticks in ONE kernel launch (qs_ctrl_rollout): exactly T calls of `step(actions[k])`, bit for bit, with the
+        drone and embedded-controller state in registers between ticks.  Vector API only; `actions` [T, E, D, 4] float32.
+        Returns a dict of CUDA tensors: `obs` [T, E, D, 20] (absent with `record=False`) and `rpm` [T, E, D, 4] float64 (the RPMs
+        the controller produced); `out` reuses the buffers of a previous result.  The env ends where T step() calls leave it
+        (state, controller state, step counters, current observation, an attached Logger).  See CtrlAviary.rollout."""
+        return self._ctrl_rollout(N.CTRL_VEL, actions=actions, record=record, out=out)
+
     def _computeObs(self):
         obs = self._obs_buf[self._cur]
         return self._shape_obs(obs) if self.VECTORIZED else self._obs_to_host_single(obs)

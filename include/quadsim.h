@@ -19,6 +19,7 @@
  *   qs_adjacency     <- BaseAviary._getAdjacencyMatrix (envs/BaseAviary.py:658-675)
  *   qs_reset         <- BaseAviary.reset/_housekeeping (envs/BaseAviary.py:220-255,451-505)
  *   qs_log_append    <- Logger.log (utils/Logger.py:83-119): one entry per logged drone and tick, kept on the device
+ *   qs_ctrl_rollout  <- T ticks of the CtrlAviary / VelocityAviary loops (examples/pid.py:131-150, pid_velocity.py, downwash.py)
  *
  * Conventions
  *   - plain C, no CUDA/torch types: device buffers are raw pointers owned by the caller; the
@@ -458,6 +459,49 @@ typedef struct QsLogRing {
 int qs_sizeof_log_ring(void);
 int qs_log_append(const QsParams* p, const QsState* st, const float* obs, int obs_dim, const float* controls,
                   const QsLogRing* ring, int n_envs, int drones_per_env, void* stream);
+
+/* Control-env rollout: T control ticks of CtrlAviary / VelocityAviary in ONE launch, the drone state, the controller state and
+ * the previous RPMs in registers between ticks.  Modes:
+ *   QS_CTRL_RAW    CtrlAviary with given RPMs: T x qs_dyn_substeps (float32 actions, or float64 with QS_FLAG_ACTION_F64)
+ *   QS_CTRL_VEL    VelocityAviary: T x qs_step(QS_ACT_VEL, QS_FLAG_OBS_STATE20), the embedded controller on QsState.pid
+ *   QS_CTRL_TRACK  CtrlAviary driven by a DSLPIDControl (examples/pid.py:131-150): per tick qs_pid_control_state with the
+ *                  controller's own QsParams on its [9][N] state and the tick's targets (RPMs clipped to the controller's max_rpm),
+ *                  then qs_dyn_substeps(QS_FLAG_ACTION_F64) on those RPMs.  Target position of drone i at tick k of the launch:
+ *                      waypoints[(start[i] + k) mod W][M == 1 ? 0 : i] + offset[i]      (mod as Python's %, never negative)
+ *                  one shared path with per-drone phases (pid.py), per-drone paths (M = N), a full schedule (W = T, M = N).
+ * Each tick gives the bits of the per-tick calls it replaces.  DYN+ effects: none, GND, DRAG, DW (in-CTA, drones_per_env <= 128)
+ * or all three; flags: QS_FLAG_RPY_F32, QS_FLAG_ACTION_F64 (RAW).  The per-tick outputs are nullable: without obs only obs_last
+ * (the env's observation buffer) receives the last tick's rows. */
+enum { QS_CTRL_RAW = 0, QS_CTRL_VEL = 1, QS_CTRL_TRACK = 2 };
+typedef struct QsCtrlRolloutIO {
+    int T;                          /* ticks in this launch */
+    int log_targets;                /* TRACK with a log ring: 1 = log the tick's targets as the 12 controls (target_pos, target_rpy,
+                                       target_vel, target_rpy_rates, as float32: pid.py's layout); 0 = log_controls */
+    const void* actions;            /* RAW / VEL: [T][N][4] float32 (16-byte aligned), RAW with QS_FLAG_ACTION_F64: float64 (32-byte aligned) */
+    /* TRACK: the controller */
+    const QsParams* ctrl_params;    /* HOST pointer: the controller's QsParams (pid_* gains and model constants, max_rpm) */
+    double* pid_state;              /* [9][N] the controller's state (read at the start, stored at the end) */
+    double control_timestep;        /* the controller's dt (CTRL_TIMESTEP) */
+    const double* waypoints;        /* [W][M][3] */
+    int W, M;                       /* W > 0; M = 1 or N */
+    const int* start;               /* [N] */
+    const double* offset;           /* [N][3], nullable = zeros */
+    const double* target_rpy;       /* [N][3] constant targets, each nullable = zeros */
+    const double* target_vel;
+    const double* target_rpy_rates;
+    /* per-tick outputs, all nullable */
+    float* obs;                     /* out [T][N][20] _getDroneStateVector rows (16-byte aligned) */
+    double* rpm;                    /* out [T][N][4] the applied (clipped) RPMs (32-byte aligned) */
+    float* pos_e;                   /* out [T][N][3] TRACK: position error, as computeControlFromEnv returns it */
+    float* yaw_e;                   /* out [T][N]    TRACK: yaw error */
+    float* obs_last;                /* out [N][20] the last tick's rows (16-byte aligned); nullable */
+    const QsLogRing* log;           /* HOST pointer, nullable: one entry per logged drone and tick, the bytes of qs_log_append after
+                                       every tick of the per-tick loop; the kernel then advances *head by T */
+    const float* log_controls;      /* [n_drones][12] controls logged without log_targets; nullable = zeros */
+} QsCtrlRolloutIO;
+int qs_sizeof_ctrl_rollout_io(void);
+int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, int mode, int n_envs, int drones_per_env,
+                    int substeps, unsigned effects, unsigned flags, void* stream);
 
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
