@@ -12,9 +12,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))    # override: A/B builds in tools/
 _CSRC = os.path.join(_HERE, "csrc")
-SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_ctrl.cu",
+SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -34,6 +34,8 @@ FLAG_OBS_STATE20 = 32
 FLAG_SKIP_EPILOGUE, FLAG_RPM_FROM_LAST, FLAG_ACTION_F64 = 0x100, 0x200, 0x400
 CTRL_RAW, CTRL_VEL, CTRL_TRACK = 0, 1, 2          # qs_ctrl_rollout modes
 ABI_VERSION = 4
+MLP_TANH, MLP_RELU = 0, 1                         # QsMlpPolicy.activation
+MLP_MAX_HIDDEN, MLP_MAX_WIDTH = 4, 256
 PHYS_WIDTH = 16          # float64 columns of one QsState.phys row
 
 _d = C.c_double
@@ -91,6 +93,16 @@ class QsPolicy(C.Structure):
                                           "noise", "logprob", "values")] + [("in_dim", C.c_int), ("out_dim", C.c_int), ("nt3", C.c_int), ("pad_", C.c_int)]
 
 
+class QsMlpNet(C.Structure):
+    _fields_ = [("w", C.c_void_p * (MLP_MAX_HIDDEN + 1)), ("b", C.c_void_p * (MLP_MAX_HIDDEN + 1)), ("depth", C.c_int),
+                ("width", C.c_int * MLP_MAX_HIDDEN), ("out_tiles", C.c_int)]
+
+
+class QsMlpPolicy(C.Structure):
+    _fields_ = [("actor", QsMlpNet), ("critic", QsMlpNet), ("activation", C.c_int), ("in_dim", C.c_int), ("out_dim", C.c_int),
+                ("pad_", C.c_int), ("log_std", C.c_void_p), ("noise", C.c_void_p), ("logprob", C.c_void_p), ("values", C.c_void_p)]
+
+
 class QsDwPublish(C.Structure):
     _fields_ = [("gathered", C.POINTER(C.c_void_p)), ("flags", C.POINTER(C.c_void_p)), ("counter", C.c_void_p),
                 ("n_total", C.c_int), ("world", C.c_int), ("rank", C.c_int), ("offset", C.c_int), ("seq", C.c_uint), ("pad_", C.c_int)]
@@ -124,7 +136,7 @@ class QsStepCall(C.Structure):
 EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_state", "qs_sizeof_step_io",
            "qs_sizeof_rollout_io", "qs_sizeof_host_io", "qs_step", "qs_step_call", "qs_step_host", "qs_rollout", "qs_rollout_max_ticks", "qs_dyn_substeps", "qs_dyn_substeps_pub", "qs_pid_control",
            "qs_downwash", "qs_downwash_boxed", "qs_dw_gathered_floats", "qs_dw_boxes", "qs_downwash_rows", "qs_dw_publish", "qs_enable_peer_access", "qs_ipc_export", "qs_ipc_import", "qs_adjacency", "qs_reset", "qs_reset_heads", "qs_host_is_pinned", "qs_log_append", "qs_sizeof_log_ring", "qs_wait_flags", "qs_pid_control_state",
-           "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io"]
+           "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io", "qs_rollout_mlp", "qs_rollout_mlp_max_ticks", "qs_sizeof_mlp_policy"]
 MAX_PEERS = 16
 
 
@@ -194,6 +206,12 @@ def lib():
                              C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
     L.qs_rollout_max_ticks.restype = C.c_int
     L.qs_rollout_max_ticks.argtypes = [C.c_int, C.c_int, C.c_int]
+    L.qs_rollout_mlp.restype = C.c_int
+    L.qs_rollout_mlp.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsRolloutIO), C.POINTER(QsMlpPolicy), C.c_int, C.c_int,
+                                 C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
+    L.qs_rollout_mlp_max_ticks.restype = C.c_int
+    L.qs_rollout_mlp_max_ticks.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+    L.qs_sizeof_mlp_policy.restype = C.c_int
     L.qs_ctrl_rollout.restype = C.c_int
     L.qs_ctrl_rollout.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -251,8 +269,9 @@ def lib():
             (C.sizeof(QsParams), C.sizeof(QsState), C.sizeof(QsStepIO), C.sizeof(QsRolloutIO)):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror: rebuild")
     if L.qs_sizeof_log_ring() != C.sizeof(QsLogRing) or L.qs_sizeof_host_io() != C.sizeof(QsHostIO) or \
-            L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io): rebuild")
+            L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy): "
+                          "rebuild")
     _lib = L
     return L
 

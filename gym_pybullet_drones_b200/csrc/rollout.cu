@@ -17,6 +17,23 @@ int qs_rollout_max_ticks(int act_type, int act_buffer_size, int drones_per_env) 
 
 int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int act_type, int task,
                int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
+    RolloutArgs a;
+    bool pid_act = false;
+    if (int rc = prepare_rollout(p, st, io, act_type, task, n_envs, drones_per_env, substeps, effects, flags,
+                                 io && io->policy && io->policy->vw1, a, pid_act))
+        return rc;
+    if (flags & QS_FLAG_AUTORESET_NEXT_STEP) return launch_rollout_next(a, io, pid_act, stream);
+    if (io->final_obs || io->final_values)
+        return a.st.phys ? launch_rollout<true, kRolloutFin>(a, io, pid_act, stream) : launch_rollout<false, kRolloutFin>(a, io, pid_act, stream);
+    return a.st.phys ? launch_rollout<true, kRolloutNone>(a, io, pid_act, stream) : launch_rollout<false, kRolloutNone>(a, io, pid_act, stream);
+}
+
+}  // extern "C"
+
+namespace qsi {
+
+int prepare_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int act_type, int task, int n_envs, int drones_per_env,
+                    int substeps, unsigned effects, unsigned flags, bool has_critic, RolloutArgs& a, bool& pid_act) {
     if (!p || !io) return fail(QS_ERR_NULL, "qs_rollout: NULL params/io");
     const bool next_step = flags & QS_FLAG_AUTORESET_NEXT_STEP;
     if (int rc = check_state(st, (flags & (QS_FLAG_AUTORESET_SAME_STEP | QS_FLAG_AUTORESET_NEXT_STEP)) ? 1 : 0)) return rc;
@@ -33,16 +50,15 @@ int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int 
     if (!io->obs_init || !io->obs || !io->reward || !io->terminated || !io->truncated) return fail(QS_ERR_NULL, "qs_rollout: NULL buffer");
     if ((io->final_obs || io->final_values) && !(flags & QS_FLAG_AUTORESET_SAME_STEP))
         return fail(QS_ERR_UNSUPPORTED, "qs_rollout: final_obs / final_values need QS_FLAG_AUTORESET_SAME_STEP");
-    if (io->final_values && !(io->policy && io->policy->vw1)) return fail(QS_ERR_NULL, "qs_rollout: final_values requested without a policy critic");
+    if (io->final_values && !has_critic) return fail(QS_ERR_NULL, "qs_rollout: final_values requested without a policy critic");
     if (io->act_buffer_size <= 0) return fail(QS_ERR_SIZE, "qs_rollout: act_buffer_size must be > 0");
     if (io->T > qs_rollout_max_ticks(act_type, io->act_buffer_size, drones_per_env)) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: T exceeds qs_rollout_max_ticks (split the rollout)");
     if (task == QS_TASK_HOVER && (!st->target_pos || !aligned32(st->target_pos))) return fail(QS_ERR_NULL, "qs_rollout: target_pos NULL/misaligned");
-    const bool pid_act = act_type == QS_ACT_PID || act_type == QS_ACT_VEL || act_type == QS_ACT_ONE_D_PID;
+    pid_act = act_type == QS_ACT_PID || act_type == QS_ACT_VEL || act_type == QS_ACT_ONE_D_PID;
     if (pid_act && !st->pid) return fail(QS_ERR_NULL, "qs_rollout: PID action type needs QsState.pid");
     if ((effects & QS_EFFECT_DRAG) && !st->last_rpm) return fail(QS_ERR_NULL, "qs_rollout: DRAG needs QsState.last_rpm");
     if (A == 4 && ((io->actions && !aligned16(io->actions)) || (io->actions_out && !aligned16(io->actions_out)) || !aligned16(io->obs) || (io->obs_last && !aligned16(io->obs_last))))
         return fail(QS_ERR_ALIGN, "qs_rollout: [N][4]-wide buffers must be 16-byte aligned");
-    RolloutArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.st = *st; a.io = *io;
     a.act_type = act_type; a.task = task; a.n_envs = n_envs; a.D = drones_per_env; a.substeps = substeps;
@@ -56,10 +72,16 @@ int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int 
         const bool aligned = aligned16(io->obs_init) && (span % 16 == 0) && ((row_bytes * ((size_t)a.N % a.tpb)) % 16 == 0);
         a.stage_mode = (aligned && A == 4) ? 1 : 2;
     }
-    if (next_step) return launch_rollout_next(a, io, pid_act, stream);
-    if (io->final_obs || io->final_values)
-        return a.st.phys ? launch_rollout<true, kRolloutFin>(a, io, pid_act, stream) : launch_rollout<false, kRolloutFin>(a, io, pid_act, stream);
-    return a.st.phys ? launch_rollout<true, kRolloutNone>(a, io, pid_act, stream) : launch_rollout<false, kRolloutNone>(a, io, pid_act, stream);
+    return 0;
 }
 
-}  // extern "C"
+int check_policy_config(const RolloutArgs& a, const QsRolloutIO* io) {
+    const unsigned eff = a.effects & 7u;
+    if (eff != 0 && eff != QS_EFFECT_GND && eff != QS_EFFECT_DRAG && eff != QS_EFFECT_DW && eff != 7u)
+        return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports no DYN+ effect, GND, DRAG, DW or all three; not GND|DRAG, GND|DW or DRAG|DW");
+    if (a.cap > 64) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports drones_per_env <= 64");
+    if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: pass either actions or a policy");
+    return 0;
+}
+
+}  // namespace qsi

@@ -121,8 +121,9 @@ class BaseRLAviary(BaseAviary):
         stores), the env applied them clipped to [-1, 1].  Every action type (RPM, ONE_D_RPM, and PID, VEL, ONE_D_PID through the
         embedded DSLPID controller), every `Physics` mode (DYN and the ground effect, drag and downwash variants) and a per-aviary
         `set_physical_params` table are supported; the physics is bit for bit that of `rollout(actions)` fed the clipped actions.
-        Up to 64 drones per aviary and 32 action outputs (D * A) per aviary; what the kernel refuses raises ValueError with the
-        reason."""
+        Up to 64 drones per aviary and 32 action outputs (D * A) per aviary, and any SB3 net_arch of 1 to 4 hidden layers of up
+        to 256 units per network, Tanh or ReLU, with separate actor and critic shapes (`MlpPolicy`; larger networks run as
+        `forward_torch` + `step()` per tick); what the kernel refuses raises ValueError with the reason."""
         if not self.VECTORIZED:
             raise ValueError("rollout() needs the vector API (num_envs=...)")
         if self._dw_fz is not None:
@@ -169,7 +170,9 @@ class BaseRLAviary(BaseAviary):
         next_step = bool(self._flags & N.FLAG_AUTORESET_NEXT_STEP)
         if next_step and "autoreset" not in out:
             out["autoreset"] = torch.empty((T, E), dtype=torch.bool, device=dev)
-        tmax = self._lib.qs_rollout_max_ticks(self._act_type(), self._B, D)
+        general = policy is not None and not policy.classic       # any other net_arch than [64, 64] Tanh: qs_rollout_mlp
+        tmax = self._lib.qs_rollout_mlp_max_ticks(self._act_type(), self._B, D, policy.max_width) if general else \
+            self._lib.qs_rollout_max_ticks(self._act_type(), self._B, D)
         if tmax <= 0:
             if self._B == 0:
                 raise ValueError("rollout() needs an action buffer: ctrl_freq=%d gives ACTION_BUFFER_SIZE = 0" % self.CTRL_FREQ)
@@ -196,13 +199,19 @@ class BaseRLAviary(BaseAviary):
                 io.final_values = out["final_values"][k0].data_ptr() if final_values else None
                 io.tick0, io.T = int(getattr(self, "_rollout_tick", 0)) + k0, tt
                 if policy is not None:
-                    qp = policy.c_struct(None if noise is None else noise.view(T, -1)[k0], out["log_probs"][k0],
-                                         out["values"][k0] if policy.critic is not None else None)
-                    io.policy = C.addressof(qp)
+                    pargs = (None if noise is None else noise.view(T, -1)[k0], out["log_probs"][k0],
+                             out["values"][k0] if policy.critic is not None else None)
+                    qp = policy.mlp_struct(*pargs) if general else policy.c_struct(*pargs)
+                    io.policy = None if general else C.addressof(qp)
                     io.actions, io.actions_out = None, out["actions"][k0].data_ptr()
-                rc = self._lib.qs_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), self._act_type(), self._task(),
-                                          E, D, self.PYB_STEPS_PER_CTRL, self._effects, self._flags, stream)
-                N.check(rc, "qs_rollout")
+                if general:
+                    rc = self._lib.qs_rollout_mlp(C.byref(self._P), C.byref(self._st), C.byref(io), C.byref(qp), self._act_type(), self._task(),
+                                                  E, D, self.PYB_STEPS_PER_CTRL, self._effects, self._flags, stream)
+                    N.check(rc, "qs_rollout_mlp")
+                else:
+                    rc = self._lib.qs_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), self._act_type(), self._task(),
+                                              E, D, self.PYB_STEPS_PER_CTRL, self._effects, self._flags, stream)
+                    N.check(rc, "qs_rollout")
                 self._cur = 1 - cur
                 k0 += tt
             if next_step:

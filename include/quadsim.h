@@ -222,7 +222,8 @@ int qs_wait_flags(const unsigned* flags, unsigned seq, int world, unsigned* err_
  * with (ka, kb) = (2 t, 2 t + 8) for layers 2 and 3 -- the B fragment of mma.m16n8k16 -- and (ka, kb) = (4 t, 4 t + 2) for
  * layer 1 (its A operand is read as 4 consecutive observation elements per lane; any permutation of k inside a k-step is
  * allowed as long as A and B agree).  gym_pybullet_drones_b200/policy.py prepares the arrays (16-byte aligned).
- * in_dim = drones_per_env * obs_dim and out_dim = drones_per_env * A for any action type (A = 4, 3 or 1), out_dim <= 32. */
+ * in_dim = drones_per_env * obs_dim and out_dim = drones_per_env * A for any action type (A = 4, 3 or 1), out_dim <= 32.
+ * QsPolicy is SB3's default shape only; QsMlpPolicy (qs_rollout_mlp, below) describes every other supported net_arch. */
 typedef struct QsPolicy {
     const unsigned* w1; const float* b1;      /* [ceil(in_dim / 16)][8][32][4], [64]   in_dim = D * obs_dim */
     const unsigned* w2; const float* b2;      /* [4][8][32][4], [64] */
@@ -271,7 +272,8 @@ typedef struct QsRolloutIO {
                                    stores), the env applies them clipped to [-1, 1], through the embedded DSLPID controller
                                    for PID / VEL / ONE_D_PID: the physics is bit for bit that of `actions` = the clipped
                                    samples.  Every action type; effects none, GND, DRAG, DW or all three (GND|DRAG, GND|DW and
-                                   DRAG|DW return QS_ERR_UNSUPPORTED); drones_per_env <= 64; hidden 64. */
+                                   DRAG|DW return QS_ERR_UNSUPPORTED); drones_per_env <= 64; QsPolicy is the 64 tanh -> 64 tanh
+                                   network only: other shapes go through qs_rollout_mlp (QsMlpPolicy) with policy = NULL here. */
     float* final_obs;           /* out [T][N][12+B*A] terminal observations (see above); nullable.  Needs QS_FLAG_AUTORESET_SAME_STEP
                                    (QS_ERR_UNSUPPORTED otherwise; under NEXT_STEP obs[k] already is the terminal observation) */
     float* final_values;        /* out [T][E] critic on the terminal observations; nullable.  Needs SAME_STEP autoreset
@@ -357,6 +359,46 @@ int qs_step_host(const QsParams* p, const QsState* st, const QsStepIO* io, const
 int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int act_type, int task,
                int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 int qs_rollout_max_ticks(int act_type, int act_buffer_size, int drones_per_env);
+
+/* On-device policy of any SB3 MlpPolicy net_arch in scope, for qs_rollout_mlp: per network 1 to QS_MLP_MAX_HIDDEN hidden layers
+ * of 1 to QS_MLP_MAX_WIDTH units, one activation for the whole policy after every hidden layer, linear output layers, and
+ * independent actor and critic shapes (SB3's net_arch = dict(pi = [...], vf = [...])).  The arithmetic is QsPolicy's (two-term
+ * fp16 split of both operands, fp32 accumulation, the same saturation of the observation); a [64, 64] tanh network gives the
+ * bits of qs_rollout with the QsPolicy of the same weights.
+ * Layer l = 0 .. depth maps K_l inputs to N_l outputs: K_0 = in_dim padded to a multiple of 16, K_l = N_(l-1); the hidden
+ * widths N_0 .. N_(depth-1) are padded with zero columns (and zero biases) to a multiple of 64, the output layer to
+ * N_depth = 8 out_tiles.  w[l] is W_l[K_l][N_l] in QsPolicy's FRAGMENT ORDER, [K_l / 16][N_l / 8][32][4] words, with the
+ * (4 t, 4 t + 2) permutation of k for layer 0 and the mma B fragment's (2 t, 2 t + 8) for the others; b[l] is [N_l]. */
+#define QS_MLP_MAX_HIDDEN 4
+#define QS_MLP_MAX_WIDTH 256
+enum { QS_MLP_TANH = 0, QS_MLP_RELU = 1 };
+typedef struct QsMlpNet {
+    const unsigned* w[QS_MLP_MAX_HIDDEN + 1];   /* device, 16-byte aligned */
+    const float* b[QS_MLP_MAX_HIDDEN + 1];
+    int depth;                                  /* hidden layers, 1 .. QS_MLP_MAX_HIDDEN; 0 = no network (critic only) */
+    int width[QS_MLP_MAX_HIDDEN];               /* padded hidden widths N_0 .. N_(depth-1): multiples of 64, <= QS_MLP_MAX_WIDTH */
+    int out_tiles;                              /* N_depth / 8: 1, 2 or 4 for the actor (out_dim real columns), 1 for the critic */
+} QsMlpNet;
+typedef struct QsMlpPolicy {
+    QsMlpNet actor;
+    QsMlpNet critic;           /* depth 0 = no critic */
+    int activation;            /* QS_MLP_TANH or QS_MLP_RELU */
+    int in_dim, out_dim;       /* as QsPolicy: D * obs_dim and D * A (<= 32) */
+    int pad_;
+    const float* log_std;      /* [out_dim] */
+    const float* noise;        /* as QsPolicy */
+    float* logprob;
+    float* values;             /* nullable; requires a critic */
+} QsMlpPolicy;
+int qs_sizeof_mlp_policy(void);
+
+/* qs_rollout with the actions of a QsMlpPolicy (io->policy must be NULL, io->actions too): the same outputs, autoreset modes,
+ * action types, effects and per-aviary table as qs_rollout with a QsPolicy.  Every warp stages the split activations of the
+ * hidden layers in shared memory, 2 x 16 rows x max width x 4 bytes, which the per-launch tick limit accounts for:
+ * qs_rollout_mlp_max_ticks(act_type, act_buffer_size, drones_per_env, max padded hidden width of the two networks). */
+int qs_rollout_mlp(const QsParams* p, const QsState* st, const QsRolloutIO* io, const QsMlpPolicy* policy, int act_type, int task,
+                   int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
+int qs_rollout_mlp_max_ticks(int act_type, int act_buffer_size, int drones_per_env, int max_width);
 
 /* CtrlAviary semantics: rpm[N][4] (float32) clipped to [0, MAX_RPM], `substeps` x DYN, optional [N][20] state vectors.
  * With QS_FLAG_RPM_FROM_LAST `rpm` is ignored and the rpm of the previous call is re-read from QsState.last_rpm. */
