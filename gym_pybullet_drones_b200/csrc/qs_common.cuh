@@ -50,8 +50,9 @@ struct StepArgs {
     int early_store;     // experiments (QS_EARLY_STORE): 1 = history written back as soon as it has landed (A = 4)
     int dbg_slot;        // QS_TIMELINE builds: which timeline buffer this launch stamps
     int row_loads;       // experiments (QS_ROW_LOADS): 1 = A = 4 fetches only the 16(B-1) history bytes of every row (one bulk copy per lane)
-    int first_warp, n_warps;   // fast kernels: launch over warps [first_warp, first_warp + n_warps) of the batch only (n_warps = 0: all);
-                         // qs_step_host pipelines chunks of the batch against their host copies
+    int first_warp, n_warps;   // fast kernels: launch over 32-drone tiles [first_warp, first_warp + n_warps) of the batch only (n_warps = 0:
+                         // all); qs_step_host pipelines chunks of the batch against their host copies
+    int pipe_tiles;      // fast kernels, A = 4: tiles per warp of step_pipe_kernel (2 or 4; QS_FAST_PIPE), 0 = the classic kernel
     // formation exchange fused into the dynamics kernel (qs_dyn_substeps_pub; general kernel only): pub_world > 0 = on
     float* pub_dst[QS_MAX_PEERS];
     unsigned* pub_flags[QS_MAX_PEERS];
@@ -308,6 +309,7 @@ inline int block_size_for(int D, int cap = kMaxTPB) { return D <= cap ? D * (cap
 // pdl_ok = false: an ordinary stream-ordered launch (not a programmatic dependent of the previous kernel)
 cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s);      // step_general.cu
 bool step_fast_eligible(const StepArgs& a);                                                       // step_fast.cu
+constexpr int kPipeTilesDefault = 4;      // tiles per warp of the pipelined fast kernel unless QS_FAST_PIPE says otherwise (DESIGN.md 6)
 cudaError_t launch_step_fast(const StepArgs& a, cudaStream_t s);                                  // step_fast.cu
 
 // What the last library launch on a stream that lets its successor start early (griddepcontrol.launch_dependents) was:

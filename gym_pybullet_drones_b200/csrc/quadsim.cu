@@ -436,6 +436,10 @@ static int prepare_step(const QsParams* p, const QsState* st, const QsStepIO* io
         if (io->obs && io->act_buffer_size > 0 && !state20 && span <= kStageLimit) a.stage_rows = (aligned && A == 4) ? 1 : 2;
     }
     const bool fast_off = getenv("QS_FAST") && atoi(getenv("QS_FAST")) == 0;      // A/B and bit-identity tests: force the general kernel
+    {   // A/B and bit-identity tests: QS_FAST_PIPE=0 forces the classic fast kernel, 2 or 4 the tiles per warp of the pipelined one
+        const int v = getenv("QS_FAST_PIPE") ? atoi(getenv("QS_FAST_PIPE")) : kPipeTilesDefault;
+        a.pipe_tiles = v <= 1 ? 0 : (v < 4 ? 2 : 4);
+    }
     if (io->obs_gather) {
         if (fast_off || !step_fast_eligible(a)) return fail(QS_ERR_UNSUPPORTED, "qs_step: obs_gather needs a configuration of step_fast.cu (RPM / ONE_D_RPM, no effects, D | 32)");
         if (!aligned16(io->obs_gather)) return fail(QS_ERR_ALIGN, "qs_step: obs_gather must be 16-byte aligned");

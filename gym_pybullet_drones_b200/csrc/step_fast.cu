@@ -21,8 +21,10 @@
 __device__ unsigned long long g_timeline[4][8192 * 16];
 static int g_dbg_slot = 0;
 #define QS_STAMP(k) do { if (lane == 0 && wg < 8192) g_timeline[a.dbg_slot & 3][wg * 16 + (k)] = globaltimer_ns(); } while (0)
+#define QS_TSTAMP(t, k) do { if (lane == 0 && (t) < 8192) g_timeline[a.dbg_slot & 3][(t) * 16 + (k)] = globaltimer_ns(); } while (0)
 #else
 #define QS_STAMP(k) do { } while (0)
+#define QS_TSTAMP(t, k) do { } while (0)
 #endif
 
 namespace qsi {
@@ -358,6 +360,281 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
     QS_STAMP(9);
 }
 
+// ---- the pipelined kernel (A = 4): K consecutive 32-drone tiles per warp, two shared-memory stages ----------------------------
+// A tile is the classic kernel's warp unit (its own span of rows, ticket word and done word).  While tile k runs its physics,
+// tile k+1's state and actions are on their way into registers and its old span into the other stage, and tile k-1's bulk
+// store is still being written.  A tile is published once its bulk store has completed, which the warp checks only after it has
+// committed the next tile's store, so the completion round trip is off the critical path too.  Same arithmetic, same order:
+// the output bits are the classic kernel's.
+// The state and actions travel through registers, not shared memory: 20 KB per warp (B = 15) fit 10 warps on an SM.
+struct PipeSmem {
+    static __host__ __device__ constexpr int bar_off(int od) { return FastSmem<4>::x_floats(od) * 4; }
+    // [old span + 16-byte tail][its mbarrier], 128-byte multiple
+    static __host__ __device__ constexpr int stage_bytes(int od) { return (bar_off(od) + 8 + 127) / 128 * 128; }
+    static __host__ __device__ constexpr int total_bytes(int od, bool fin) { return 2 * stage_bytes(od) + (fin ? 32 * 12 * 4 : 0); }
+};
+
+template <bool TASK, bool RESET, bool RPYF, bool PHYS, int K>
+__global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ StepArgs a) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const QsParams& P = a.P;
+    const int lane = threadIdx.x;
+    const int od = a.obs_dim;
+    const long long N = a.N;
+    const long long tiles = (N + 31) / 32;
+    const long long t_end = a.n_warps > 0 && (long long)a.first_warp + a.n_warps < tiles ? (long long)a.first_warp + a.n_warps : tiles;
+    const long long t0 = (long long)a.first_warp + (long long)blockIdx.x * K;      // first tile of this warp
+    if (t0 >= t_end) return;
+    const int nt = (int)(t_end - t0 < K ? t_end - t0 : K);
+    const bool want_fin = RESET && a.io.final_obs != nullptr;
+    const int SB = PipeSmem::stage_bytes(od);
+    float* fin_s = reinterpret_cast<float*>(smem_raw + 2 * SB);
+    auto stage = [&](int k) { return smem_raw + (k & 1) * SB; };
+    auto bar_of = [&](int k) { return reinterpret_cast<unsigned long long*>(stage(k) + PipeSmem::bar_off(od)); };
+    const int D = a.D, dmask = D - 1;
+    QS_TSTAMP(t0, 0);
+    if (lane == 0) { mbar_init(bar_of(0), 1); mbar_init(bar_of(1), 1); }
+
+    // ---- readiness, per tile (DESIGN.md 4.1): lane j takes the ticket of tile j before the next grid may launch, then tries
+    // its tile's done word once; a tile found not ready is waited for when its turn comes
+    const bool ticketed = a.io.warp_ticket != nullptr;
+    unsigned my_ticket = 0;
+    if (ticketed && lane < nt) my_ticket = atomicAdd(a.io.warp_ticket + t0 + lane, 1u);
+    const unsigned ticket0 = __shfl_sync(0xffffffffu, my_ticket, 0);           // (every lane's atomic has returned)
+    if (a.grid_wait) asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    bool rdy = !ticketed;
+    if (ticketed && lane < nt) {
+        unsigned v;
+        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a.io.warp_done + t0 + lane) : "memory");
+        rdy = v == my_ticket;
+        if (rdy) asm volatile("fence.proxy.async.global;" ::: "memory");
+    }
+    const unsigned ready_mask = __ballot_sync(0xffffffffu, rdy);
+    auto try_turn = [&](int k) -> bool {
+        if ((ready_mask >> k) & 1u) return true;
+        const unsigned tk = __shfl_sync(0xffffffffu, my_ticket, k);
+        int ok = 0;
+        if (lane == 0) {
+            unsigned v;
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a.io.warp_done + t0 + k) : "memory");
+            ok = v == tk;
+            if (ok) asm volatile("fence.proxy.async.global;" ::: "memory");
+        }
+        return __shfl_sync(0xffffffffu, ok, 0) != 0;
+    };
+    auto wait_turn = [&](int k, unsigned tk) {          // blocking: the warp holds no finished, unpublished tile here
+        if (!((ready_mask >> k) & 1u) && lane == 0) warp_wait_turn(a.io.warp_done + t0 + k, tk, a.io.ready_err);
+    };
+    auto publish = [&](int k, bool all_done) {          // tile k's stores have completed: all_done = no later group outstanding
+        if (!ticketed) return;
+        const unsigned tk = __shfl_sync(0xffffffffu, my_ticket, k);
+        if (lane == 0) {
+            if (all_done) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+            else asm volatile("cp.async.bulk.wait_group 1;" ::: "memory");
+        }
+        warp_publish(a.io.warp_done + t0 + k, tk + 1u);
+        QS_TSTAMP(t0 + k, 7);
+    };
+    // tile k's loads, after its readiness: state and action into registers (consumed when tile k starts), the old span into
+    // stage k & 1.  Dead lanes of a ragged last tile shadow its first drone, as in the classic kernel.
+    qs::Drone dn;
+    float4 an;
+    auto issue = [&](int k) {
+        __syncwarp();
+        const long long w0 = (t0 + k) * 32;
+        const long long il = w0 + lane < N ? w0 + lane : w0;
+        load_drone(a.st.planes, N, il, dn);
+        an = ldg4(a.io.action, il);
+        if (lane == 0) {
+            const int rows = (int)(N - w0 < 32 ? N - w0 : 32);
+            asm volatile("fence.proxy.async.global;" ::: "memory");
+            tma_bulk_g2s_read_once(stage(k), a.io.obs_prev + w0 * od, (unsigned)(rows * od * 4), bar_of(k));
+        }
+        QS_TSTAMP(t0 + k, 1);
+    };
+#ifdef QS_TIMELINE
+    for (int k = 1; k < nt; ++k) QS_TSTAMP(t0 + k, 0);
+#endif
+    __syncwarp();
+    wait_turn(0, ticket0);
+    issue(0);
+
+    int pend = -1;                                      // finished tile whose publish is outstanding
+    for (int k = 0; k < nt; ++k) {
+        const long long tg = t0 + k;
+        const unsigned par = (unsigned)(k >> 1) & 1u;
+        qs::Drone d = dn;
+        const float4 av = an;
+        bool pre = false;
+        if (k + 1 < nt && try_turn(k + 1)) {
+            // stage (k + 1) & 1 held tile k-1, whose bulk store must have finished reading it
+            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+            issue(k + 1);
+            pre = true;
+        }
+        const long long w0 = tg * 32;
+        const long long i = w0 + lane;
+        const bool live = i < N;
+        const int rows = (int)((N - w0) < 32 ? (N - w0) : 32);
+        const long long il = live ? i : w0;
+        const long long e = il >> a.log2D;
+        const int dslot = (int)il & dmask;
+        const long long tbl = a.st.tables_per_env ? il : dslot;
+        unsigned long long* bar = bar_of(k);
+        float* xs = reinterpret_cast<float*>(stage(k));
+        double tpx = 0.0, tpy = 0.0, tpz = 0.0;
+        if (TASK) { const D4 tp = ld256_nc(a.st.target_pos, tbl); tpx = tp.x; tpy = tp.y; tpz = tp.z; }
+        int sc = a.st.step_counter[e];
+        qs::PhysRow ph;
+        if constexpr (PHYS) ph = load_phys(a.st.phys, e);
+
+        QS_TSTAMP(tg, 2);
+        float act[4] = {av.x, av.y, av.z, av.w};
+
+        // ---- action decode (BaseRLAviary.py:192,225) + S substeps ----------------------------------------------------------
+        double rpm[4];
+        {
+            qs::PidState none = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+            if constexpr (PHYS) qs::decode_action_k<false>(P, ph, QS_ACT_RPM, act, d, 0.0, none, rpm);
+            else qs::decode_action<false>(P, QS_ACT_RPM, act, d, 0.0, none, rpm);
+        }
+        double R_last[9];
+        if constexpr (PHYS) qs::dyn_tick_k<0>(P, ph, d, rpm, rpm, 0.0, a.substeps, R_last);
+        else qs::dyn_tick<0>(P, d, rpm, rpm, 0.0, a.substeps, R_last);
+        QS_TSTAMP(tg, 3);
+        qs::Derived o;
+        qs::derive<RPYF>(d, R_last, o);
+
+        // ---- task terms, reduced over the D drones of the aviary in index order (MultiHoverAviary.py:75-130) ------------------
+        bool env_done = false;
+        if (TASK) {
+            const qs::TaskTerms tt = qs::hover_terms(P, d, o, tpx, tpy, tpz);
+            double rew = 0.0, dist = 0.0;
+            const int base = lane & ~dmask;
+            for (int j = 0; j < D; ++j) {
+                rew += __shfl_sync(0xffffffffu, tt.reward, base + j);
+                dist += __shfl_sync(0xffffffffu, tt.dist, base + j);
+            }
+            const unsigned oobs = __ballot_sync(0xffffffffu, tt.out_of_bounds && live);
+            const unsigned gmask = (D == 32 ? 0xffffffffu : ((1u << D) - 1u)) << base;
+            const bool term = dist < P.term_dist;                                     // HoverAviary.py:91
+            const bool trunc = (oobs & gmask) != 0u || sc >= a.sc_limit;              // HoverAviary.py:113
+            env_done = term || trunc;
+            if (live && dslot == 0) {
+                a.io.reward[e] = (float)rew;
+                a.io.terminated[e] = term ? 1 : 0;
+                a.io.truncated[e] = trunc ? 1 : 0;
+                if (a.io.done) a.io.done[e] = env_done ? 1 : 0;
+            }
+        } else if (live && dslot == 0) {
+            a.io.reward[e] = -1.0f; a.io.terminated[e] = 0; a.io.truncated[e] = 0;     // CtrlAviary-style dummy task
+            if (a.io.done) a.io.done[e] = 0;
+        }
+
+        // ---- observation head, autoreset, state store ----------------------------------------------------------------------
+        float h[12];
+        h[0] = (float)d.px; h[1] = (float)d.py; h[2] = (float)d.pz;                    // BaseRLAviary.py:310-315
+        h[3] = (float)o.roll; h[4] = (float)o.pitch; h[5] = (float)o.yaw;
+        h[6] = (float)d.vx; h[7] = (float)d.vy; h[8] = (float)d.vz;
+        h[9] = (float)o.ax; h[10] = (float)o.ay; h[11] = (float)o.az;
+        const bool reset_me = RESET && env_done;
+        if (reset_me) {
+            if (want_fin) {
+                float4* f4 = reinterpret_cast<float4*>(fin_s + 12 * lane);
+                f4[0] = make_float4(h[0], h[1], h[2], h[3]); f4[1] = make_float4(h[4], h[5], h[6], h[7]); f4[2] = make_float4(h[8], h[9], h[10], h[11]);
+            }
+            init_drone(a.st, tbl, d);                                                  // BaseAviary.py:451-505
+            const float4* rh = reinterpret_cast<const float4*>(a.st.reset_head) + 3 * tbl;
+            const float4 r0 = __ldg(rh), r1 = __ldg(rh + 1), r2 = __ldg(rh + 2);
+            h[0] = r0.x; h[1] = r0.y; h[2] = r0.z; h[3] = r0.w; h[4] = r1.x; h[5] = r1.y; h[6] = r1.z; h[7] = r1.w;
+            h[8] = r2.x; h[9] = r2.y; h[10] = r2.z; h[11] = r2.w;
+            rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                                   // last_clipped_action = 0
+            sc = -a.counter_inc;
+        }
+        if (live) {
+            store_drone(a.st, N, i, d);
+            if (a.st.last_rpm) st256(a.st.last_rpm, i, rpm[0], rpm[1], rpm[2], rpm[3]);
+            if (dslot == 0) a.st.step_counter[e] = sc + a.counter_inc;                 // BaseAviary.py:382
+        }
+        QS_TSTAMP(tg, 4);
+
+        // ---- observation rows: patched in shared memory, one bulk store of the shifted span ----------------------------------
+        const unsigned fin_rows = want_fin ? __ballot_sync(0xffffffffu, reset_me && live) : 0u;
+        mbar_wait(bar, par);
+        QS_TSTAMP(tg, 5);
+        if (live) {             // new head -> slots [4, 16) of my row, new action -> the 4 slots after it (in place)
+            float* row = xs + (size_t)lane * od;
+            float4* r4 = reinterpret_cast<float4*>(row + 4);
+            r4[0] = make_float4(h[0], h[1], h[2], h[3]); r4[1] = make_float4(h[4], h[5], h[6], h[7]); r4[2] = make_float4(h[8], h[9], h[10], h[11]);
+            *reinterpret_cast<float4*>(row + od) = make_float4(act[0], act[1], act[2], act[3]);
+        }
+        __syncwarp();
+        const float4* shifted = reinterpret_cast<const float4*>(xs) + 1;
+        if (lane == 0) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                         ::"l"(a.io.obs + w0 * od), "r"(smem_u32(shifted)), "r"((unsigned)(rows * od * 4)) : "memory");
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        }
+        if (want_fin) {                                                                // terminal observations: head from fin_s, history from the span
+            const int c4n = od >> 2;
+            float4* fin = reinterpret_cast<float4*>(a.io.final_obs + w0 * od);
+            for (unsigned m = fin_rows; m; m &= m - 1) {
+                const int r = __ffs(m) - 1;
+                for (int c = lane; c < c4n; c += 32)
+                    fin[r * c4n + c] = c < 3 ? reinterpret_cast<const float4*>(fin_s + 12 * r)[c] : shifted[r * c4n + c];
+            }
+            __syncwarp();                                                              // fin_s is rewritten by the next tile
+        }
+        QS_TSTAMP(tg, 6);
+        if (pend >= 0) publish(pend, false);            // tile k-1: every group but tile k's has completed
+        pend = k;
+        if (k + 1 < nt && !pre) {
+            // tile k+1 was not ready: never spin while holding an unpublished tile
+            publish(k, true);
+            pend = -1;
+            wait_turn(k + 1, __shfl_sync(0xffffffffu, my_ticket, k + 1));
+            issue(k + 1);
+        }
+    }
+    if (ticketed) publish(pend, true);
+    else if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // shared memory must outlive the bulk store's reads
+}
+
+template <bool TASK, bool RESET, bool RPYF, bool PHYS, int K>
+cudaError_t launch_pipe(const StepArgs& a, cudaStream_t s) {
+    const long long tiles = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
+    const int blocks = (int)((tiles + K - 1) / K);
+    const size_t sm = (size_t)PipeSmem::total_bytes(a.obs_dim, RESET && a.io.final_obs != nullptr);
+    static const bool pdl = !(getenv("QS_PDL") && atoi(getenv("QS_PDL")) == 0);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = sm; cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+    if (sm > 48 * 1024)
+        cudaFuncSetAttribute(step_pipe_kernel<TASK, RESET, RPYF, PHYS, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    return cudaLaunchKernelEx(&cfg, step_pipe_kernel<TASK, RESET, RPYF, PHYS, K>, a);
+}
+
+template <int K, bool PHYS>
+cudaError_t launch_pipe_modes(const StepArgs& a, cudaStream_t s) {
+    const bool task = a.task == QS_TASK_HOVER, reset = a.flags & QS_FLAG_AUTORESET_SAME_STEP, rpyf = a.flags & QS_FLAG_RPY_F32;
+    const int key = (task ? 4 : 0) | (reset ? 2 : 0) | (rpyf ? 1 : 0);
+    switch (key) {
+        case 0: return launch_pipe<false, false, false, PHYS, K>(a, s);
+        case 1: return launch_pipe<false, false, true, PHYS, K>(a, s);
+        case 2: return launch_pipe<false, true, false, PHYS, K>(a, s);
+        case 3: return launch_pipe<false, true, true, PHYS, K>(a, s);
+        case 4: return launch_pipe<true, false, false, PHYS, K>(a, s);
+        case 5: return launch_pipe<true, false, true, PHYS, K>(a, s);
+        case 6: return launch_pipe<true, true, false, PHYS, K>(a, s);
+        default: return launch_pipe<true, true, true, PHYS, K>(a, s);
+    }
+}
+
 template <int A, bool TASK, bool RESET, bool RPYF, int WARPS, bool PHYS>
 cudaError_t launch_one(const StepArgs& a, cudaStream_t s) {
     const long long warps = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
@@ -430,6 +707,11 @@ cudaError_t launch_step_fast(const StepArgs& a_in, cudaStream_t s) {
     const StepArgs& a = a_in;
 #endif
     static const int warps = getenv("QS_FAST_WARPS") ? atoi(getenv("QS_FAST_WARPS")) : 1;      // measured default (DESIGN.md 6)
+    // the pipelined kernel takes A = 4 without the fused gather; the experiment switches keep their meaning on the classic one
+    if (a.A == 4 && a.pipe_tiles > 0 && !a.io.obs_gather && warps == 1 && a.early_store && a.flags_late_tma && !a.row_loads) {
+        if (a.pipe_tiles == 4) return a.st.phys ? launch_pipe_modes<4, true>(a, s) : launch_pipe_modes<4, false>(a, s);
+        return a.st.phys ? launch_pipe_modes<2, true>(a, s) : launch_pipe_modes<2, false>(a, s);
+    }
     if (a.st.phys) return launch_warps<true>(a, warps, s);
     return launch_warps<false>(a, warps, s);
 }

@@ -194,11 +194,11 @@ typedef struct QsStepIO {
     unsigned* gather_counter;           /* one zeroed device word owned by the caller (arrival count); required with gather_flag */
     unsigned gather_seq;
     unsigned pad_;
-    /* Per-warp readiness of the fast step kernels (DESIGN.md 4.1): device words owned by the caller, zero-initialised once, and
-     * passed with EVERY qs_step / qs_step_host call on the same state and observation buffers (or never).  With them a warp of
-     * 32 drones waits only for the warp of the previous step on these buffers that owns the same 32 drones, instead of for the
-     * whole previous kernel of the stream, so consecutive steps overlap.  All NULL = the whole-grid wait.
-     * ready_err becomes non-zero if a warp ever waited longer than ~1 s for its turn (the step then went ahead unordered). */
+    /* Per-tile readiness of the fast step kernels (DESIGN.md 4.1), one word each per tile of 32 consecutive drones: device words
+     * owned by the caller, zero-initialised once, and passed with EVERY qs_step / qs_step_host call on the same state and
+     * observation buffers (or never).  With them a tile waits only for the same tile of the previous step on these buffers,
+     * instead of for the whole previous kernel of the stream, so consecutive steps overlap.  All NULL = the whole-grid wait.
+     * ready_err becomes non-zero if a tile ever waited longer than ~1 s for its turn (the step then went ahead unordered). */
     unsigned* warp_ticket;              /* [ceil(N / 32)] */
     unsigned* warp_done;                /* [ceil(N / 32)] */
     unsigned* ready_err;                /* one word */
