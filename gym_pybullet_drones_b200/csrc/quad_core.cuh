@@ -128,6 +128,16 @@ QS_HD void quat_to_euler(double x, double y, double z, double w, double& roll, d
     }
 }
 
+// The reference's ground-effect switch (BaseAviary.py:742): |roll| < np.pi/2 and |pitch| < np.pi/2 on its float64 rpy, without
+// trig.  |pitch| < fl(pi/2) iff sarg is off the gimbal guard.  Roll = RN(atan2(ra, rb)): for rb <= 0 (and not ra = rb = 0, where
+// atan2 = 0) |roll| >= fl(pi/2).  For rb > 0, t = rb/|ra| and roll = pi/2 - t + O(t^3) near the switch, which rounds below fl(pi/2)
+// iff pi/2 - t < fl(pi/2) - 2^-53, i.e. t > (pi/2 - fl(pi/2)) + 2^-53 = 6.123233995736766e-17 + 1.1102230246251565e-16.  So a
+// drone at roll = pi/2 - 1e-16 is not upright, as in the reference.
+QS_HD bool upright(double sarg, double ra, double rb) {
+    const double T = 1.722546424198833e-16;
+    return (sarg > -0.99999) && (sarg < 0.99999) && (rb > T * fabs(ra) || (rb == 0.0 && ra == 0.0));
+}
+
 // cos(theta) and sin(theta)/|w| for theta = |w| dt/2, from n2 = |w|^2 -- both are even in theta, so for the
 // small angles of a 240 Hz substep they are 5- or 8-term series in theta^2 (truncation < 2^-53 in both ranges):
 // no sqrt, no division, no range reduction.  Large rates fall back to sqrt/sincos.
@@ -255,15 +265,14 @@ QS_HD void dyn_tick_k(const QsParams& P, const K& c, Drone& d, const double rpm[
             const double sarg = -2.0 * (x * z - w * y);
             const double ra = 2.0 * (y * z + w * x);
             const double rb = w * w - x * x - y * y + z * z;
-            // |roll| < pi/2 and |pitch| < pi/2 (:742) without trig: roll = atan2(ra, rb), pitch = asin(sarg) w/ guard
-            const bool upright = (sarg > -0.99999) && (sarg < 0.99999) && (rb > 0.0 || (rb == 0.0 && ra == 0.0));
+            const bool up = upright(sarg, ra, rb);                                  // :742
             double g[4];
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const double hz = d.pz + r20 * P.prop_xyz[i][0] + r21 * P.prop_xyz[i][1] + r22 * P.prop_xyz[i][2];
                 const double h = hz < P.gnd_eff_h_clip ? P.gnd_eff_h_clip : hz;       // :739-740
                 const double rr = P.prop_radius / (4.0 * h);
-                g[i] = upright ? rpm[i] * rpm[i] * c.kf * P.gnd_eff_coeff * (rr * rr) : 0.0;   // :741
+                g[i] = up ? rpm[i] * rpm[i] * c.kf * P.gnd_eff_coeff * (rr * rr) : 0.0;   // :741
             }
             const double f0 = f[0] + g[0], f1 = f[1] + g[1], f2 = f[2] + g[2], f3 = f[3] + g[3];
             thrust = f0 + f1 + f2 + f3;
@@ -439,6 +448,22 @@ QS_HD void decode_action(const QsParams& P, int act_type, const float a[4], cons
 // ---- task: Hover / MultiHover per-drone terms ----------------------------------------------------
 struct TaskTerms { double reward, dist; bool out_of_bounds; };
 
+// |roll| or |pitch| > tilt_bound (HoverAviary.py:110-111), decided on float64 angles as the reference decides it on its float64
+// rpy.  With RPY_F32, `o` holds atan2f/asinf of float32-rounded arguments: the rounding moves roll by at most 2^-24 rad and pitch
+// by at most 2^-24 tan|pitch|, and CUDA's atan2f/asinf add at most 3 ulp (3 * 2^-23 |a|).  At the tasks' bound of 0.4 that is
+// < 3.4 * 2^-24; the band of 2^-18 max(1, bound) is 19x wider (and at least 4x for any bound up to 1.5 rad).  Within the band the
+// angles are recomputed from the quaternion in float64 (a rare branch); outside it the float32 angle is on the float64 one's side.
+// The common case (both angles below bound - band) costs the two compares of a plain float32 decision.
+QS_HD bool tilted(const QsParams& P, const Drone& d, const Derived& o) {
+    const double band = (1.0 / 262144.0) * (P.tilt_bound > 1.0 ? P.tilt_bound : 1.0);      // 2^-18 max(1, bound)
+    const double ar = fabs(o.roll), ap = fabs(o.pitch);
+    if (!(ar > P.tilt_bound - band || ap > P.tilt_bound - band)) return false;
+    if (ar > P.tilt_bound + band || ap > P.tilt_bound + band) return true;
+    double roll, pitch, yaw;                                                   // within the band: float64 angles decide
+    quat_to_euler<false>(d.qx, d.qy, d.qz, d.qw, roll, pitch, yaw);
+    return fabs(roll) > P.tilt_bound || fabs(pitch) > P.tilt_bound;
+}
+
 QS_HD TaskTerms hover_terms(const QsParams& P, const Drone& d, const Derived& o, double tx, double ty, double tz) {
     const double ex = tx - d.px, ey = ty - d.py, ez = tz - d.pz;
     const double n = sqrt(ex * ex + ey * ey + ez * ez);                              // HoverAviary.py:77
@@ -447,8 +472,7 @@ QS_HD TaskTerms hover_terms(const QsParams& P, const Drone& d, const Derived& o,
     const double r = 2.0 - n2 * n2;
     t.reward = r > 0.0 ? r : 0.0;                                                    // max(0, 2 - |e|^4)
     t.dist = n;
-    t.out_of_bounds = fabs(d.px) > P.xy_bound || fabs(d.py) > P.xy_bound || d.pz > P.z_bound ||
-                      fabs(o.roll) > P.tilt_bound || fabs(o.pitch) > P.tilt_bound;   // HoverAviary.py:109-111
+    t.out_of_bounds = fabs(d.px) > P.xy_bound || fabs(d.py) > P.xy_bound || d.pz > P.z_bound || tilted(P, d, o);   // HoverAviary.py:109-111
     return t;
 }
 

@@ -220,14 +220,16 @@ __global__ void log_append_kernel(QsParams P, QsState st, const float* __restric
 }
 __global__ void log_advance_kernel(long long* head) { *head += 1; }      // after every CTA of the append has read it (stream order)
 
-__global__ void reset_heads_kernel(QsState st, int rows, int rpyf, float* __restrict__ out) {
+// the head of a freshly reset drone carries float64 angles whatever QS_FLAG_RPY_F32 is: the same bits as reset_kernel writes, so an
+// aviary's first observation does not depend on whether reset() or an autoreset produced it
+__global__ void reset_heads_kernel(QsState st, int rows, float* __restrict__ out) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= rows) return;
     qs::Drone d;
     init_drone(st, r, d);
     qs::Derived o;
     const double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    if (rpyf) qs::derive<true>(d, R, o); else qs::derive<false>(d, R, o);
+    qs::derive<false>(d, R, o);
     float* h = out + 12 * (long long)r;
     h[0] = (float)d.px; h[1] = (float)d.py; h[2] = (float)d.pz;
     h[3] = (float)o.roll; h[4] = (float)o.pitch; h[5] = (float)o.yaw;
@@ -734,7 +736,8 @@ int qs_reset_heads(const QsState* st, int rows, unsigned flags, float* out, void
     if (!st || !st->init_pos || !st->init_quat || !out) return fail(QS_ERR_NULL, "qs_reset_heads: NULL argument");
     if (!aligned32(st->init_pos) || !aligned32(st->init_quat) || !aligned16(out)) return fail(QS_ERR_ALIGN, "qs_reset_heads: misaligned table");
     if (rows <= 0) return fail(QS_ERR_SIZE, "qs_reset_heads: rows must be > 0");
-    reset_heads_kernel<<<(rows + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*st, rows, (flags & QS_FLAG_RPY_F32) ? 1 : 0, out);
+    (void)flags;
+    reset_heads_kernel<<<(rows + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*st, rows, out);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_reset_heads launch");
 }

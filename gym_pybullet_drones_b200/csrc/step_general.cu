@@ -221,7 +221,8 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
             if (a.flags & QS_FLAG_AUTORESET_CLEARS_PID) pst = {0, 0, 0, 0, 0, 0, 0, 0, 0};
             rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                               // last_clipped_action = 0 (BaseAviary.py:468)
         }
-        if (a.flags & QS_FLAG_RPY_F32) qs::derive<true>(d, R_last, o); else qs::derive<false>(d, R_last, o);
+        // a reset drone's head carries float64 angles in every mode (qs_reset_heads)
+        if ((a.flags & QS_FLAG_RPY_F32) && !pending) qs::derive<true>(d, R_last, o); else qs::derive<false>(d, R_last, o);
         if (pending) { o.ax = o.ay = o.az = 0.0; }
     }
     const bool want_epilogue = !(a.flags & QS_FLAG_SKIP_EPILOGUE);
@@ -281,7 +282,7 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
                 if (a.flags & QS_FLAG_AUTORESET_CLEARS_PID) pst = {0, 0, 0, 0, 0, 0, 0, 0, 0};
                 init_drone(a.st, tbl, d);                                          // BaseAviary.py:451-505
                 double Rr[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-                if (a.flags & QS_FLAG_RPY_F32) qs::derive<true>(d, Rr, o); else qs::derive<false>(d, Rr, o);
+                qs::derive<false>(d, Rr, o);                                       // float64 angles, as qs_reset_heads
                 rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                           // last_clipped_action = 0
                 sc = -a.counter_inc;                                               // -> 0 after the increment below
             }

@@ -26,7 +26,7 @@ import torch
 from .. import _native as N
 from .._compat import (AUTORESET_DISABLED, AUTORESET_NEXT_STEP, AUTORESET_SAME_STEP, Env, batch_box, spaces)
 from ..params import (PHYS_KEYS, AviaryConstants, coerce_physical_args, fill_params, nominal_properties, physical_rows,
-                      quaternion_from_euler)
+                      euler_from_quaternion, quaternion_from_euler)
 from ..utils.enums import DroneModel, Physics
 
 _PHYSICS_EFFECTS = {
@@ -100,7 +100,9 @@ class BaseAviary(Env):
             buffer (quirk kept by default); set to clear them when an env auto-resets.
         rpy_f32 : bool
             Evaluate the reported roll/pitch/yaw with float32 atan2f/asinf on float64 arguments (default; error ~2e-7 rad,
-            far inside the 1e-5 parity bound); False = float64 atan2/asin.
+            far inside the 1e-5 parity bound); False = float64 atan2/asin.  Only the reported angles change: the tilt
+            truncation is decided on float64 angles, and the observation of a freshly reset drone carries float64 angles,
+            in both modes.
         track_last_action : bool | None
             Keep `last_clipped_action` (BaseAviary.py:372, 32 bytes written per drone and tick).  None = only where the model
             needs it (drag, CtrlAviary/VelocityAviary state vectors, formations) or for the single-env API.
@@ -1016,12 +1018,7 @@ class BaseAviary(Env):
     def _getDroneStateVectors(self):
         """[E, D, 20] float64 ndarray of _getDroneStateVector (BaseAviary.py:541-561), computed from the state planes."""
         pos, quat, vel = self._plane[0, :, 0:3], self._plane[1], self._plane[2, :, 0:3]
-        x, y, z, w = quat[:, 0], quat[:, 1], quat[:, 2], quat[:, 3]
-        sarg = -2.0 * (x * z - w * y)
-        roll = torch.atan2(2.0 * (y * z + w * x), w * w - x * x - y * y + z * z)
-        pitch = torch.asin(sarg.clamp(-1, 1))
-        yaw = torch.atan2(2.0 * (x * y + w * z), w * w + x * x - y * y - z * z)
-        rpy = torch.stack([roll, pitch, yaw], dim=1)
+        rpy = euler_from_quaternion(quat)
         obs = self._obs_buf[self._cur]
         ang_v = obs[:, 13:16].double() if self._state20_obs() else obs[:, 9:12].double()      # (a KIN row can be 20 wide)
         sv = torch.cat([pos, quat, rpy, vel, ang_v, self._last_rpm], dim=1)

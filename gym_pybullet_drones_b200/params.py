@@ -234,4 +234,15 @@ def quaternion_from_euler(rpy):
     return q / np.linalg.norm(q, axis=-1, keepdims=True)
 
 
-_ = math
+def euler_from_quaternion(quat):
+    """pybullet.getEulerFromQuaternion (call site envs/BaseAviary.py:518) on a float64 tensor [..., 4] (x,y,z,w) -> [..., 3],
+    with Bullet's gimbal guard: where sarg = -2(xz - wy) reaches +-0.99999, roll = 0, pitch = +-pi/2 and yaw = 2 atan2(-+x, +-y)."""
+    import torch
+    x, y, z, w = quat.unbind(-1)
+    sarg = -2.0 * (x * z - w * y)
+    lo, hi = sarg <= -0.99999, sarg >= 0.99999
+    roll = torch.where(lo | hi, 0.0, torch.atan2(2.0 * (y * z + w * x), w * w - x * x - y * y + z * z))
+    pitch = torch.where(lo, -0.5 * math.pi, torch.where(hi, 0.5 * math.pi, torch.asin(sarg.clamp(-1, 1))))
+    yaw = torch.where(lo, 2.0 * torch.atan2(x, -y),
+                      torch.where(hi, 2.0 * torch.atan2(-x, y), torch.atan2(2.0 * (x * y + w * z), w * w + x * x - y * y - z * z)))
+    return torch.stack([roll, pitch, yaw], dim=-1)

@@ -62,7 +62,8 @@ enum { QS_FLAG_AUTORESET_SAME_STEP = 1,   /* SB3 VecEnv semantics: done envs are
                                              terminal observation goes to QsStepIO.final_obs */
        QS_FLAG_AUTORESET_NEXT_STEP = 2,   /* gymnasium>=1.0 default: a done env is reset by the NEXT step call,
                                              which ignores that env's action */
-       QS_FLAG_RPY_F32 = 4,               /* evaluate the output roll/pitch/yaw with float32 atan2/asin */
+       QS_FLAG_RPY_F32 = 4,               /* evaluate the output roll/pitch/yaw with float32 atan2/asin; decisions (tilt
+                                             truncation) and reset observations still use float64 angles */
        /* The reference's reset() clears neither the embedded PID controllers nor the action buffer
           (SURVEY.md 3.3); autoreset keeps that behaviour unless asked otherwise: */
        QS_FLAG_AUTORESET_CLEARS_PID = 8,
@@ -481,8 +482,9 @@ int qs_enable_peer_access(int peer_device);
 int qs_adjacency(const QsState* st, int n_envs, int drones_per_env, double radius, unsigned char* out, void* stream);
 
 /* Fills `out` ([rows][12] float32, 16-byte aligned; rows = D or N like the init tables) with the observation head of a freshly
- * reset drone: (float)INIT_XYZS, rpy of the initial quaternion (float32 atan2f/asinf iff flags has QS_FLAG_RPY_F32), zeros --
- * exactly what the tick writes for an aviary it resets.  Point QsState.reset_head at it afterwards. */
+ * reset drone: (float)INIT_XYZS, float32 casts of the float64 rpy of the initial quaternion, zeros -- exactly what qs_reset and
+ * the tick write for an aviary they reset, with or without QS_FLAG_RPY_F32 (`flags` is accepted and ignored).  Point
+ * QsState.reset_head at it afterwards. */
 int qs_reset_heads(const QsState* st, int rows, unsigned flags, float* out, void* stream);
 
 /* Device-side trajectory ring in the reference Logger's layout (utils/Logger.py:83-127).  One call appends ONE entry for

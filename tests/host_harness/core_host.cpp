@@ -75,6 +75,35 @@ void hh_pid(const QsParams* P, double* st, double dt, const double* pos, const d
                     tpos[0], tpos[1], tpos[2], tyaw, tvel[0], tvel[1], tvel[2], trr[0], trr[1], trr[2], rpm, pos_e, *yaw_e);
     st[0] = s.ipx; st[1] = s.ipy; st[2] = s.ipz; st[3] = s.lr; st[4] = s.lp; st[5] = s.ly; st[6] = s.irx; st[7] = s.iry; st[8] = s.irz;
 }
+// getEulerFromQuaternion of the kernels for n quaternions [n][4] (x,y,z,w) -> rpy [n][3]; f32 = the RPY_F32 variant
+void hh_quat_to_euler(const double* q, int n, int f32, double* rpy) {
+    for (int i = 0; i < n; ++i) {
+        const double* v = q + 4 * i; double* r = rpy + 3 * i;
+        if (f32) qs::quat_to_euler<true>(v[0], v[1], v[2], v[3], r[0], r[1], r[2]);
+        else qs::quat_to_euler<false>(v[0], v[1], v[2], v[3], r[0], r[1], r[2]);
+    }
+}
+// the ground-effect switch of dyn_tick_k on n quaternions -> out[n] (0/1)
+void hh_upright(const double* q, int n, unsigned char* out) {
+    for (int i = 0; i < n; ++i) {
+        const double x = q[4 * i], y = q[4 * i + 1], z = q[4 * i + 2], w = q[4 * i + 3];
+        out[i] = qs::upright(-2.0 * (x * z - w * y), 2.0 * (y * z + w * x), w * w - x * x - y * y + z * z) ? 1 : 0;
+    }
+}
+// hover_terms on n drones: pos [n][3], quat [n][4], target [n][3]; the task's angles come from derive<f32> as in the kernels.
+// out [n][5]: reward, dist, out_of_bounds, roll, pitch (the angles the kernel reports)
+void hh_hover_terms(const QsParams* P, const double* pos, const double* quat, const double* tgt, int n, int f32, double* out) {
+    const double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    for (int i = 0; i < n; ++i) {
+        qs::Drone d = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], quat[4 * i], quat[4 * i + 1], quat[4 * i + 2], quat[4 * i + 3],
+                       0, 0, 0, 0, 0, 0};
+        qs::Derived o;
+        if (f32) qs::derive<true>(d, R, o); else qs::derive<false>(d, R, o);
+        const qs::TaskTerms t = qs::hover_terms(*P, d, o, tgt[3 * i], tgt[3 * i + 1], tgt[3 * i + 2]);
+        double* r = out + 5 * i;
+        r[0] = t.reward; r[1] = t.dist; r[2] = t.out_of_bounds ? 1.0 : 0.0; r[3] = o.roll; r[4] = o.pitch;
+    }
+}
 double hh_downwash_pair(const QsParams* P, double dz, double dxy2) { return qs::downwash_pair(*P, dz, dxy2); }
 void hh_half_angle(double n2, double dt, double* c, double* s) { qs::half_angle_terms(n2, dt, *c, *s); }
 }

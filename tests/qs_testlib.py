@@ -68,6 +68,9 @@ def host_harness():
     L.hh_half_angle.argtypes = [C.c_double, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     L.hh_tick.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p]
     L.hh_pid.argtypes = [C.c_void_p] + [C.c_void_p, C.c_double] + [C.c_void_p] * 4 + [C.c_double] + [C.c_void_p] * 5
+    L.hh_quat_to_euler.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    L.hh_upright.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.hh_hover_terms.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_void_p]
     _HH = L
     return L
 

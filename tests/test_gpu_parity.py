@@ -244,14 +244,42 @@ def test_velocity_aviary_golden(golden):
 # ---------------------------------------------------------------------------------------------------------------
 # (b) seeded inputs against the float64 oracle
 # ---------------------------------------------------------------------------------------------------------------
-def _borderline(ora, eps=1e-4):
-    """[E] bool: some truncation test of the oracle state sits within eps of its threshold."""
-    m = np.minimum.reduce([np.abs(np.abs(ora.pos[..., 0]) - ora.xy_bound), np.abs(np.abs(ora.pos[..., 1]) - ora.xy_bound),
-                           np.abs(ora.pos[..., 2] - 2.0), np.abs(np.abs(ora.rpy[..., 0]) - 0.4), np.abs(np.abs(ora.rpy[..., 1]) - 0.4)])
-    return np.any(m < eps, axis=1)
+BORDERLINE = {"ticks": 0, "old": 0, "new": 0}     # aviary-ticks seen, and excluded by the former fixed 1e-4 window and by this one
+
+
+def _borderline(ora, tol):
+    """[E] bool: some truncation test of the oracle state sits so close to its threshold that the kernel's state may lie on the
+    other side.  The caller holds that state to `tol`: positions relative to max(|x|, 1) (<= 2 at the bounds), the unit quaternion
+    absolutely, so |d(roll)|, |d(pitch)| <= 6 tol / cos(pitch) (test_gpu_configs._rpy_bound).  The window is 10x those.  The
+    kernel decides on float64 angles (quad_core.cuh, qs::tilted), so nothing wider is needed; test_gpu_thresholds.py pins the
+    decisions themselves to the ulp.  Callers that assert the state only at the end of a rollout (and the observations, at
+    OBS_TOL, on the way) rely on the state error not shrinking over the rollout, which holds for these runs: the state
+    differs from the oracle's by rounding that accumulates.  Each caller starts with _reset_borderline()."""
+    cosp = np.maximum(np.abs(np.cos(ora.rpy[..., 1])), 0.02)
+    wp, wa = 10.0 * tol * 2.0, 10.0 * 6.0 * tol / cosp
+    dp = np.minimum.reduce([np.abs(np.abs(ora.pos[..., 0]) - ora.xy_bound), np.abs(np.abs(ora.pos[..., 1]) - ora.xy_bound),
+                            np.abs(ora.pos[..., 2] - 2.0)])
+    da = np.minimum(np.abs(np.abs(ora.rpy[..., 0]) - 0.4), np.abs(np.abs(ora.rpy[..., 1]) - 0.4))
+    near = np.any((dp < wp) | (da < wa), axis=1)
+    BORDERLINE["ticks"] += near.size
+    BORDERLINE["old"] += int(np.any(np.minimum(dp, da) < 1e-4, axis=1).sum())
+    BORDERLINE["new"] += int(near.sum())
+    return near
+
+
+def _reset_borderline():
+    BORDERLINE.update(ticks=0, old=0, new=0)
+
+
+def _report_borderline(name):
+    """Prints and clears the counts of _borderline since the last report."""
+    print("[borderline] %s: %d aviary-ticks, truncation unchecked on %d (fixed 1e-4 window: %d)"
+          % (name, BORDERLINE["ticks"], BORDERLINE["new"], BORDERLINE["old"]))
+    BORDERLINE.update(ticks=0, old=0, new=0)
 
 
 def _compare_with_oracle(env, ora, acts, tol, check_obs_every=5):
+    _reset_borderline()
     obs, _ = env.reset()
     o_obs = ora.reset()
     assert relerr(obs.cpu().numpy(), o_obs) < 1e-6
@@ -273,11 +301,12 @@ def _compare_with_oracle(env, ora, acts, tol, check_obs_every=5):
             assert e <= (max(tol, OBS_TOL) if f in OBS_FIELDS else tol), (f, t, e)
         assert relerr(rew.cpu().numpy(), o_rew) < max(tol, OBS_TOL)
         assert np.array_equal(term.cpu().numpy(), o_term), t
-        # a truncation bound crossed within rounding distance of the threshold may legitimately flip: skip those envs
-        clear = ~_borderline(ora)
+        # a truncation bound crossed within the state tolerance of the threshold may legitimately flip: skip those envs
+        clear = ~_borderline(ora, tol)
         assert np.array_equal(trunc.cpu().numpy()[clear], o_trunc[clear]), t
         if t % check_obs_every == 0:
             assert relerr(obs.cpu().numpy(), o_obs) < max(tol, OBS_TOL)
+    _report_borderline("compare_with_oracle tol=%g" % tol)
 
 
 @pytest.mark.parametrize("act,A", [("RPM", 4), ("ONE_D_RPM", 1)])
@@ -654,8 +683,9 @@ def test_config3_full_size_65536_drones_125_ticks_vs_oracle():
             assert relerr(st["vel"], ora.vel) < TIGHT and relerr(st["rpy_rates"], ora.rpy_rates) < TIGHT, t
             assert relerr(obs.cpu().numpy()[..., 6:], o_obs[..., 6:]) < OBS_TOL and relerr(rew.cpu().numpy(), o_rew) < OBS_TOL, t
             assert np.array_equal(term.cpu().numpy(), o_term)
-            clear = ~_borderline(ora)
+            clear = ~_borderline(ora, TIGHT)
             assert np.array_equal(trunc.cpu().numpy()[clear], o_trunc[clear]), t
+    _report_borderline("65536 drones")
 
 
 def test_config2_pid_4096_30hz_teacher_forced_vs_oracle():
@@ -758,8 +788,9 @@ def test_rollout_vs_oracle_directly():
     for t in range(T):
         o_obs, o_rew, o_term, o_trunc = ora.step(acts[t])
         assert relerr(obs[t], o_obs) < OBS_TOL and relerr(rew[t], o_rew) < OBS_TOL, t
-        clear = ~_borderline(ora)
+        clear = ~_borderline(ora, TIGHT)       # the end state is held to TIGHT below
         assert np.array_equal(te[t], o_term) and np.array_equal(tr[t][clear], o_trunc[clear]), t
+    _report_borderline("rollout")
     st = state_of(env)
     assert relerr(st["pos"], ora.pos) < TIGHT and quat_err(st["quat"], ora.quat) < TIGHT
     assert relerr(st["vel"], ora.vel) < TIGHT and relerr(st["rpy_rates"], ora.rpy_rates) < TIGHT

@@ -201,7 +201,7 @@ def _small_policy(in_dim, out_dim, seed, scale):
 @pytest.mark.parametrize("case", ORACLE_CASES, ids=[c[0] for c in ORACLE_CASES])
 def test_policy_rollout_vs_oracle(case):
     from test_gpu_configs import _force_from_snapshot, _snapshot, _state_ratio, make_env, make_oracle
-    from test_gpu_parity import OBS_TOL, _borderline, state_of
+    from test_gpu_parity import OBS_TOL, _borderline, _report_borderline, state_of
     name, kind, D, model, pyb, ctrl, act, E, T, teacher, tol, opts = case
     kw = {"initial_xyzs": opts["xyzs"]} if "xyzs" in opts else {}
     env = make_env(kind, D, model, pyb, ctrl, act, E, physics=opts.get("physics", "DYN"), **kw)
@@ -217,7 +217,7 @@ def test_policy_rollout_vs_oracle(case):
         o_obs, o_rew, o_term, o_trunc = ora.step(out_actions[t])
         r = max(relerr(rew.cpu().numpy(), o_rew) / max(tol, OBS_TOL), relerr(obs.cpu().numpy(), o_obs) / max(tol, OBS_TOL))
         assert np.array_equal(term.cpu().numpy(), o_term), t
-        clear = ~_borderline(ora)
+        clear = ~_borderline(ora, tol)
         assert np.array_equal(trunc.cpu().numpy()[clear], o_trunc[clear]), t
         return r
 
@@ -244,6 +244,7 @@ def test_policy_rollout_vs_oracle(case):
         r = _state_ratio(state_of(env), ora, tol)
         assert r <= 1.0, (name, "final state", r)
         worst = max(worst, r)
+    _report_borderline("policy " + name)
     _report("oracle-" + name, {"state": worst})
 
 
