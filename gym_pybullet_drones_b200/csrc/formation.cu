@@ -286,89 +286,15 @@ struct AdjArgs {
 };
 
 constexpr int kAdjCols = 512, kAdjRows = 256;
-#ifndef QS_ADJ_DEFAULT
-#define QS_ADJ_DEFAULT 4
-#endif
-
-__global__ void __launch_bounds__(256) adjacency_kernel(const __grid_constant__ AdjArgs a) {
-    __shared__ float4 rows_s[kAdjRows];
-    int b = blockIdx.x;
-    const int ct = b % a.col_tiles; b /= a.col_tiles;
-    const int rt = b % a.row_tiles;
-    const int env = b / a.row_tiles;
-    const long long base = (long long)env * a.D;
-    const int c0 = ct * kAdjCols, r0 = rt * kAdjRows;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int k = threadIdx.x; k < kAdjRows; k += blockDim.x) {
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r0 + k < a.D) { const D4 p = ld256(a.planes, base + r0 + k); v = make_float4((float)p.x, (float)p.y, (float)p.z, 0.f); }
-        rows_s[k] = v;
-    }
-    const int j0 = c0 + 16 * lane;                         // my 16 columns
-    float cx[16], cy[16], cz[16];
-#pragma unroll
-    for (int q = 0; q < 16; ++q) {
-        if (j0 + q < a.D) { const D4 p = ld256(a.planes, base + j0 + q); cx[q] = (float)p.x; cy[q] = (float)p.y; cz[q] = (float)p.z; }
-        else { cx[q] = 3e30f; cy[q] = 3e30f; cz[q] = 3e30f; }
-    }
-    __syncthreads();
-    const float r2f = (float)(a.radius * a.radius);
-    float r2lo = r2f * (1.f - 2e-4f), r2hi = r2f * (1.f + 2e-4f);           // outside [lo, hi] float32 decides
-    if (a.radius < 0.0) r2lo = r2hi = -1.f;                                 // |d| < negative radius: never
-    const bool vec = (a.D % 16) == 0;
-    for (int rr = warp; rr < kAdjRows; rr += 8) {
-        const int i = r0 + rr;
-        if (i >= a.D) break;
-        const float4 me = rows_s[rr];                                       // warp-uniform (broadcast)
-        unsigned w[4] = {0u, 0u, 0u, 0u};
-        unsigned amb = 0u;                                                  // bit q: pair q is within 2e-4 of the threshold
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            const float dx = cx[q] - me.x, dy = cy[q] - me.y, dz = cz[q] - me.z;
-            const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-            const bool near = d2 < r2lo;
-            amb |= (!near && !(d2 > r2hi)) ? (1u << q) : 0u;
-            w[q >> 2] |= near ? (1u << (8 * (q & 3))) : 0u;
-        }
-        if (__any_sync(0xffffffffu, amb != 0u)) {                           // rare: the reference's float64 arithmetic decides
-            if (amb) {
-                const D4 md = ld256(a.planes, base + i);
-                for (unsigned m = amb; m; m &= m - 1) {
-                    const int q = __ffs(m) - 1;
-                    if (j0 + q >= a.D) continue;
-                    const D4 od = ld256(a.planes, base + j0 + q);          // BaseAviary.py:670
-                    const double ex = md.x - od.x, ey = md.y - od.y, ez = md.z - od.z;
-                    const bool near = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey)), __dmul_rn(ez, ez))) < a.radius;
-                    const unsigned bit = near ? (1u << (8 * (q & 3))) : 0u;
-                    if ((q >> 2) == 0) w[0] |= bit; else if ((q >> 2) == 1) w[1] |= bit; else if ((q >> 2) == 2) w[2] |= bit; else w[3] |= bit;
-                }
-            }
-        }
-        const int dj = i - j0;                                              // identity (BaseAviary.py:666)
-        if ((unsigned)dj < 16u) {
-            const unsigned bit = 1u << (8 * (dj & 3));
-            if ((dj >> 2) == 0) w[0] |= bit; else if ((dj >> 2) == 1) w[1] |= bit; else if ((dj >> 2) == 2) w[2] |= bit; else w[3] |= bit;
-        }
-        unsigned char* dst = a.out + ((size_t)(base + i)) * a.D + j0;
-        if (vec) {
-            if (j0 < a.D) *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
-        } else {
-            for (int q = 0; q < 16 && j0 + q < a.D; ++q) dst[q] = (unsigned char)((w[q >> 2] >> (8 * (q & 3))) & 0xffu);
-        }
-    }
-}
-
-
-// ---- adjacency, second version: column pairs, sign-bit decisions ------------------------------------------------------------
-// Same tiles, same decision rule, fewer instructions per pair.  A lane's 16 columns are 8 register PAIRS per
-// coordinate; one pair operation handles two columns: 3 x add2 (differences: the row is stored NEGATED and duplicated in
-// shared memory, so it arrives as paired operands by LDS.128 + LDS.64), mul2 + 2 x fma2 (squared distance),
-// add2 s = d2 - r2lo and add2 u = s - (r2hi - r2lo).  The SIGN BITS carry the decisions: sign(s) = "near",
-// ~sign(s) & sign(u) = "inside the float32 band" (accumulated over the 16 pairs with one LOP3 per pair, tested once per row);
-// the 16 result bytes are built from the sign bits by PRMT with sign replication (3 PRMT + 1 LOP3 per 4 pairs) -- no FSETP,
-// no SEL.  Rows whose band bit came up are re-evaluated exactly like in the first version (float32 band per pair, then the
+// ---- adjacency kernel: column pairs, sign-bit decisions --------------------------------------------------------------------
+// A lane's 16 columns are 8 register PAIRS per coordinate; one pair operation handles two columns: 3 x add2 (differences:
+// the row is stored NEGATED and duplicated in shared memory, so it arrives as paired operands by LDS.128 + LDS.64), mul2 +
+// 2 x fma2 (squared distance), add2 s = d2 - r2lo and add2 u = s - (r2hi - r2lo).  The SIGN BITS carry the decisions:
+// sign(s) = "near", ~sign(s) & sign(u) = "inside the float32 band" (accumulated over the 16 pairs with one LOP3 per pair,
+// tested once per row); the 16 result bytes are built from the sign bits by PRMT with sign replication (3 PRMT + 1 LOP3 per
+// 4 pairs) -- no FSETP, no SEL.  Rows whose band bit came up are re-evaluated pair by pair (float32 band per pair, then the
 // reference's float64 arithmetic on the float64 positions).  The tile's 512 column positions are converted to float32 once
-// per CTA through shared memory (the first version converted them in every warp: 48 F2F.F32.F64 per thread).
+// per CTA through shared memory.  Registers are capped for 3 CTAs per SM.
 // sm_90 has no packed float32 instructions: each pair operation is two scalar round-to-nearest operations (explicit
 // intrinsics, so the compiler cannot contract a multiply and an add into an FFMA), which gives the packed forms' bits.
 typedef unsigned long long u64;
@@ -381,8 +307,7 @@ __device__ __forceinline__ u64 mul2(u64 a, u64 b) { return pack2(__fmul_rn(lo2(a
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { return pack2(__fmaf_rn(lo2(a), lo2(b), lo2(c)), __fmaf_rn(hi2(a), hi2(b), hi2(c))); }
 __device__ __forceinline__ unsigned prmt(unsigned a, unsigned b, unsigned c) { unsigned r; asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
 
-template <bool MIX, int MINB>
-__global__ void __launch_bounds__(256, MINB) adjacency2_kernel(const __grid_constant__ AdjArgs a) {
+__global__ void __launch_bounds__(256, 3) adjacency_kernel(const __grid_constant__ AdjArgs a) {
     __shared__ __align__(16) float4 rows_a[kAdjRows];          // {-x, -x, -y, -y} of the tile's rows
     __shared__ __align__(16) float2 rows_b[kAdjRows];          // {-z, -z}
     __shared__ __align__(16) float cols_s[3][kAdjCols];        // x[], y[], z[] of the tile's columns (float32)
@@ -437,25 +362,6 @@ __global__ void __launch_bounds__(256, MINB) adjacency2_kernel(const __grid_cons
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int q = 2 * g + h;
-                if (MIX && h == 1) {
-                    // every second column pair with SCALAR instructions: the packed ones issue to the FMA-heavy pipe only (ncu:
-                    // fmaheavy 54 % busy, math-pipe throttle the top stall, fmalite idle), scalar FADD / FMUL / FFMA can take the
-                    // lite pipe -- same arithmetic, same bits
-                    unsigned cxl, cxh, cyl, cyh, czl, czh;
-                    unpack2(cx[q], cxl, cxh); unpack2(cy[q], cyl, cyh); unpack2(cz[q], czl, czh);
-                    const float nlo = -r2lo;
-#pragma unroll
-                    for (int k = 0; k < 2; ++k) {
-                        const float dx = __uint_as_float(k ? cxh : cxl) + ma.x, dy = __uint_as_float(k ? cyh : cyl) + ma.z,
-                                    dz = __uint_as_float(k ? czh : czl) + mb.x;
-                        const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-                        const float sf = d2 + nlo, uf = sf + nbw;
-                        const unsigned sb = __float_as_uint(sf), ub = __float_as_uint(uf);
-                        band |= ~sb & ub;
-                        sg[2 + k] = sb;
-                    }
-                    continue;
-                }
                 const u64 dx = add2(cx[q], mx), dy = add2(cy[q], my), dz = add2(cz[q], mz);
                 const u64 d2 = fma2(dz, dz, fma2(dy, dy, mul2(dx, dx)));
                 const u64 s = add2(d2, nlo2);                               // < 0: nearer than the lower band edge
@@ -651,16 +557,7 @@ int qs_adjacency(const QsState* st, int n_envs, int drones_per_env, double radiu
     a.col_tiles = (drones_per_env + kAdjCols - 1) / kAdjCols; a.row_tiles = (drones_per_env + kAdjRows - 1) / kAdjRows;
     const long long blocks = (long long)n_envs * a.col_tiles * a.row_tiles;
     if (blocks > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_adjacency: too many tiles");
-    // QS_ADJ_V=1: the first version (scalar float32 arithmetic, FSETP + SEL packing), kept for A/B measurements
-    // 2: all packed; 3: half packed, half scalar; 4 / 5: the same two with registers capped for 3 CTAs per SM (read per call: A/B tool)
-    const char* ve = getenv("QS_ADJ_V");
-    const int version = ve ? atoi(ve) : QS_ADJ_DEFAULT;
-    cudaStream_t cs = (cudaStream_t)stream;
-    if (version == 1) adjacency_kernel<<<(unsigned)blocks, 256, 0, cs>>>(a);
-    else if (version == 3) adjacency2_kernel<true, 2><<<(unsigned)blocks, 256, 0, cs>>>(a);
-    else if (version == 4) adjacency2_kernel<false, 3><<<(unsigned)blocks, 256, 0, cs>>>(a);
-    else if (version == 5) adjacency2_kernel<true, 3><<<(unsigned)blocks, 256, 0, cs>>>(a);
-    else adjacency2_kernel<false, 2><<<(unsigned)blocks, 256, 0, cs>>>(a);
+    adjacency_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_adjacency launch");
 }

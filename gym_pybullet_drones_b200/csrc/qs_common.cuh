@@ -45,14 +45,11 @@ struct StepArgs {
     int cap;             // CTA capacity in drones (64 or 128): sizes the shared-memory arrays
     int log2D;           // log2(D) when D is a power of two, else -1
     int sc_limit;        // smallest step counter with (double)sc / pyb_freq > episode_len_sec (HoverAviary.py:113)
-    int flags_late_tma;  // experiments (QS_LATE_TMA): 1 = issue the bulk copy only after the state loads have landed
     int grid_wait;       // fast kernels: 1 = griddepcontrol.wait for the whole previous grid (quadsim.cu launch_step_tracked, DESIGN.md 4.1)
-    int early_store;     // experiments (QS_EARLY_STORE): 1 = history written back as soon as it has landed (A = 4)
     int dbg_slot;        // QS_TIMELINE builds: which timeline buffer this launch stamps
-    int row_loads;       // experiments (QS_ROW_LOADS): 1 = A = 4 fetches only the 16(B-1) history bytes of every row (one bulk copy per lane)
+    int pipe;            // fast kernels, A = 4: 1 = step_pipe_kernel, 0 = the classic kernel (QS_FAST_PIPE=0)
     int first_warp, n_warps;   // fast kernels: launch over 32-drone tiles [first_warp, first_warp + n_warps) of the batch only (n_warps = 0:
                          // all); qs_step_host pipelines chunks of the batch against their host copies
-    int pipe_tiles;      // fast kernels, A = 4: tiles per warp of step_pipe_kernel (2 or 4; QS_FAST_PIPE), 0 = the classic kernel
     // formation exchange fused into the dynamics kernel (qs_dyn_substeps_pub; general kernel only): pub_world > 0 = on
     float* pub_dst[QS_MAX_PEERS];
     unsigned* pub_flags[QS_MAX_PEERS];
@@ -159,13 +156,6 @@ __device__ __forceinline__ void tma_bulk_g2s_read_once(void* dst_smem, const voi
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, unsigned bytes, unsigned long long* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
     unsigned ok;
@@ -309,8 +299,27 @@ inline int block_size_for(int D, int cap = kMaxTPB) { return D <= cap ? D * (cap
 // pdl_ok = false: an ordinary stream-ordered launch (not a programmatic dependent of the previous kernel)
 cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s);      // step_general.cu
 bool step_fast_eligible(const StepArgs& a);                                                       // step_fast.cu
-constexpr int kPipeTilesDefault = 4;      // tiles per warp of the pipelined fast kernel unless QS_FAST_PIPE says otherwise (DESIGN.md 6)
 cudaError_t launch_step_fast(const StepArgs& a, cudaStream_t s);                                  // step_fast.cu
+
+// QS_PDL=0 (a debugging switch for the ordering protocol): the step kernels are ordinary stream-ordered launches
+inline bool pdl_enabled() {
+    static const bool on = !(getenv("QS_PDL") && atoi(getenv("QS_PDL")) == 0);
+    return on;
+}
+// kernel<<<blocks, threads, smem, s>>>(a), a programmatic dependent of the previous kernel on s when pdl is set (the kernel's
+// griddepcontrol instructions then decide what overlaps).  Above 48 KB, the kernel's dynamic shared-memory limit is first
+// raised to smem_limit.
+inline cudaError_t launch_step_kernel(void (*kernel)(StepArgs), int blocks, int threads, size_t smem, size_t smem_limit, bool pdl,
+                                      cudaStream_t s, const StepArgs& a) {
+    if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kernel, a);
+}
 
 // What the last library launch on a stream that lets its successor start early (griddepcontrol.launch_dependents) was:
 // nothing yet, a fast step, or another kernel (general step, formation publish).  Only the library's own early-triggering

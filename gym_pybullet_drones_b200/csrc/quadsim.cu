@@ -410,13 +410,7 @@ static int prepare_step(const QsParams* p, const QsState* st, const QsStepIO* io
     a.tpb = block_size_for(drones_per_env, a.cap);
     a.counter_inc = io->tick_substeps > 0 ? io->tick_substeps : substeps;
     a.effects = effects; a.flags = flags;
-    {
-        static const int late = getenv("QS_LATE_TMA") ? atoi(getenv("QS_LATE_TMA")) : 1;
-        static const int early = getenv("QS_EARLY_STORE") ? atoi(getenv("QS_EARLY_STORE")) : 1;
-        static const int rowl = getenv("QS_ROW_LOADS") ? atoi(getenv("QS_ROW_LOADS")) : 0;
-        a.flags_late_tma = late; a.early_store = early; a.row_loads = rowl;
-        a.grid_wait = 1;
-    }
+    a.grid_wait = 1;
     if ((io->warp_ticket == nullptr) != (io->warp_done == nullptr)) return fail(QS_ERR_NULL, "qs_step: warp_ticket and warp_done go together");
     if ((reinterpret_cast<uintptr_t>(io->warp_ticket) | reinterpret_cast<uintptr_t>(io->warp_done) | reinterpret_cast<uintptr_t>(io->ready_err)) & 3u)
         return fail(QS_ERR_ALIGN, "qs_step: warp_ticket / warp_done / ready_err must be 4-byte aligned");
@@ -438,10 +432,7 @@ static int prepare_step(const QsParams* p, const QsState* st, const QsStepIO* io
         if (io->obs && io->act_buffer_size > 0 && !state20 && span <= kStageLimit) a.stage_rows = (aligned && A == 4) ? 1 : 2;
     }
     const bool fast_off = getenv("QS_FAST") && atoi(getenv("QS_FAST")) == 0;      // A/B and bit-identity tests: force the general kernel
-    {   // A/B and bit-identity tests: QS_FAST_PIPE=0 forces the classic fast kernel, 2 or 4 the tiles per warp of the pipelined one
-        const int v = getenv("QS_FAST_PIPE") ? atoi(getenv("QS_FAST_PIPE")) : kPipeTilesDefault;
-        a.pipe_tiles = v <= 1 ? 0 : (v < 4 ? 2 : 4);
-    }
+    a.pipe = !(getenv("QS_FAST_PIPE") && atoi(getenv("QS_FAST_PIPE")) == 0);      // bit-identity tests: 0 forces the classic fast kernel
     if (io->obs_gather) {
         if (fast_off || !step_fast_eligible(a)) return fail(QS_ERR_UNSUPPORTED, "qs_step: obs_gather needs a configuration of step_fast.cu (RPM / ONE_D_RPM, no effects, D | 32)");
         if (!aligned16(io->obs_gather)) return fail(QS_ERR_ALIGN, "qs_step: obs_gather must be 16-byte aligned");
@@ -578,8 +569,7 @@ int qs_step_host(const QsParams* p, const QsState* st, const QsStepIO* io, const
             }
             // the per-aviary outputs travel by kernel stores into the (mapped) host arrays on the side stream as well
             float* rew_h = nullptr; unsigned char *te_h = nullptr, *tr_h = nullptr, *dn_h = nullptr;
-            static const bool small_kernel = !(getenv("QS_SMALL_OUT") && atoi(getenv("QS_SMALL_OUT")) == 0);
-            if (small_kernel && cudaHostGetDevicePointer(reinterpret_cast<void**>(&rew_h), h->reward_host, 0) == cudaSuccess &&
+            if (cudaHostGetDevicePointer(reinterpret_cast<void**>(&rew_h), h->reward_host, 0) == cudaSuccess &&
                 cudaHostGetDevicePointer(reinterpret_cast<void**>(&te_h), h->terminated_host, 0) == cudaSuccess &&
                 cudaHostGetDevicePointer(reinterpret_cast<void**>(&tr_h), h->truncated_host, 0) == cudaSuccess &&
                 cudaHostGetDevicePointer(reinterpret_cast<void**>(&dn_h), h->done_host, 0) == cudaSuccess) {

@@ -3,15 +3,18 @@
 // embedded PID, aviaries of 1, 2, 4, ... 32 drones, autoreset SAME_STEP or none.  Everything else takes step_general.cu.
 //
 // Same arithmetic as the general kernel (the per-drone functions of quad_core.cuh), different skeleton:
-//   * a WARP is the unit of work: 32 consecutive drones = one contiguous span of observation rows with its own mbarrier
-//     and shared-memory window; no __syncthreads anywhere, the aviary reduction is a warp shuffle (aviaries never straddle
-//     warps), so warps of a CTA run completely out of phase
+//   * a TILE of 32 consecutive drones = one contiguous span of observation rows with its own mbarrier and shared-memory
+//     window is the unit of work, run by one warp; each CTA is one warp, no __syncthreads anywhere, the aviary reduction is
+//     a warp shuffle (aviaries never straddle tiles)
+//   * two kernels run one tile's work (tile_step): step_fast_kernel, one tile per warp, and step_pipe_kernel (A = 4 without
+//     the fused gather), four tiles per warp with the next tile's loads issued under the current tile's physics
 //   * A, the task, the autoreset mode and the rpy precision are template parameters: the instruction stream of an
 //     instantiation contains no mode switches (round 1's kernel: 268 IMAD, 101 BRA per warp)
 //   * state in/out as 3 x 32 bytes (two 16-byte vector accesses each) + 1 x 8 bytes per thread (float64 planes, no conversions)
-//   * A = 4: the old span is TMA-loaded, patched in place (head -> slots [A, A+12), new action -> the A slots after the
-//     row) and TMA-stored shifted by one action (16 bytes); A = 1: the span is TMA-loaded, funnel-shifted by one float with
-//     128-bit shared-memory accesses into a second 16-byte-aligned window, patched there and TMA-stored
+//   * A = 4: the old span is TMA-loaded and TMA-stored shifted by one action (16 bytes); the new heads and actions go into the
+//     span in shared memory first (pipelined kernel) or over the stored rows afterwards (classic kernel, whose store starts
+//     as soon as the span has landed); A = 1: the span is TMA-loaded, funnel-shifted by one float with 128-bit shared-memory
+//     accesses into a second 16-byte-aligned window, patched there and TMA-stored
 //   * the observation of a freshly reset drone (SAME_STEP autoreset) comes from a precomputed table (qs_reset_heads),
 //     not from two atan2f and an asinf in the epilogue
 #include "qs_common.cuh"
@@ -43,35 +46,159 @@ struct FastSmem {
     }
 };
 
-// A: action width (4 = RPM, 1 = ONE_D_RPM).  TASK: Hover/MultiHover reward + flags (else the CtrlAviary-style dummy task).
-// RESET: SAME_STEP autoreset.  RPYF: float32 atan2f/asinf for the reported rpy.  WARPS: warps per CTA (independent).
-// PHYS: the drone's physical constants come from its aviary's row of QsState.phys (else from QsParams).
-template <int A, bool TASK, bool RESET, bool RPYF, int WARPS, bool PHYS>
-__global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_constant__ StepArgs a) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
+// Dead lanes of a ragged last tile shadow the tile's first drone (il) for their loads and store nothing.
+struct TileLane { long long i, il, e, tbl; int dslot; bool live; };
+__device__ __forceinline__ TileLane tile_lane(const StepArgs& a, long long N, int D, long long w0, int lane) {
+    TileLane t;
+    t.i = w0 + lane;
+    t.live = t.i < N;
+    t.il = t.live ? t.i : w0;
+    t.e = t.il >> a.log2D;
+    t.dslot = (int)t.il & (D - 1);                                          // D is a power of two <= 32
+    t.tbl = a.st.tables_per_env ? t.il : t.dslot;
+    return t;
+}
+
+// What the kernels still need after tile_step: whether the drone was reset (its terminal head is then in fin_s), and for the
+// fused gather its aviary's reward and flags.
+struct TileEnd { bool reset_me; float rew; bool term, trunc; };
+
+// One 32-drone tile's work, from the action decode to the state stores: S substeps, the task terms reduced over the aviary, the
+// per-aviary outputs, the observation head h (the reset table's head for a drone reset in this step) and the state, last_rpm and
+// step-counter stores.  Both fast kernels run it, so they give the same bits.  substep(s) runs between substeps (the classic
+// kernel's early store); stamp(p) marks point p of the tile for the timeline build: 0 physics done, 1 derived, 2 task terms
+// stored, 3 state stored.
+template <int A, bool TASK, bool RESET, bool RPYF, bool PHYS, class Substep, class Stamp>
+__device__ __forceinline__ TileEnd tile_step(const StepArgs& a, long long N, int D, const TileLane& t, int lane, qs::Drone& d, const float act[4], int sc,
+                                             const qs::PhysRow& ph, const D4& tp, bool want_fin, float* fin_s, float h[12],
+                                             Substep substep, Stamp stamp) {
     const QsParams& P = a.P;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int dmask = D - 1;
+
+    // ---- action decode (BaseRLAviary.py:192,225) + S substeps ---------------------------------------------------------------
+    double rpm[4];
+    {
+        qs::PidState none = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        if constexpr (PHYS) qs::decode_action_k<false>(P, ph, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
+        else qs::decode_action<false>(P, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
+    }
+    double R_last[9];
+    if constexpr (PHYS) qs::dyn_tick_k<0>(P, ph, d, rpm, rpm, 0.0, a.substeps, R_last, substep);
+    else qs::dyn_tick<0>(P, d, rpm, rpm, 0.0, a.substeps, R_last, substep);
+    stamp(0);
+    qs::Derived o;
+    qs::derive<RPYF>(d, R_last, o);
+    stamp(1);
+
+    // ---- task terms, reduced over the D drones of the aviary in index order (MultiHoverAviary.py:75-130) ----------------------
+    TileEnd r = {false, -1.0f, false, false};
+    bool env_done = false;
+    if (TASK) {
+        const qs::TaskTerms tt = qs::hover_terms(P, d, o, tp.x, tp.y, tp.z);
+        double rew = 0.0, dist = 0.0;
+        const int base = lane & ~dmask;
+        for (int k = 0; k < D; ++k) {
+            rew += __shfl_sync(0xffffffffu, tt.reward, base + k);
+            dist += __shfl_sync(0xffffffffu, tt.dist, base + k);
+        }
+        const unsigned oobs = __ballot_sync(0xffffffffu, tt.out_of_bounds && t.live);
+        const unsigned gmask = (D == 32 ? 0xffffffffu : ((1u << D) - 1u)) << base;
+        const bool term = dist < P.term_dist;                                     // HoverAviary.py:91
+        const bool trunc = (oobs & gmask) != 0u || sc >= a.sc_limit;              // HoverAviary.py:113 (sc/PYB_FREQ > EPISODE_LEN_SEC)
+        env_done = term || trunc;
+        r.rew = (float)rew; r.term = term; r.trunc = trunc;
+        if (t.live && t.dslot == 0) {
+            a.io.reward[t.e] = (float)rew;
+            a.io.terminated[t.e] = term ? 1 : 0;
+            a.io.truncated[t.e] = trunc ? 1 : 0;
+            if (a.io.done) a.io.done[t.e] = env_done ? 1 : 0;
+        }
+    } else if (t.live && t.dslot == 0) {
+        a.io.reward[t.e] = -1.0f; a.io.terminated[t.e] = 0; a.io.truncated[t.e] = 0;     // CtrlAviary-style dummy task
+        if (a.io.done) a.io.done[t.e] = 0;
+    }
+    stamp(2);
+
+    // ---- observation head, autoreset, state store ----------------------------------------------------------------------------
+    h[0] = (float)d.px; h[1] = (float)d.py; h[2] = (float)d.pz;                    // BaseRLAviary.py:310-315
+    h[3] = (float)o.roll; h[4] = (float)o.pitch; h[5] = (float)o.yaw;
+    h[6] = (float)d.vx; h[7] = (float)d.vy; h[8] = (float)d.vz;
+    h[9] = (float)o.ax; h[10] = (float)o.ay; h[11] = (float)o.az;
+    r.reset_me = RESET && env_done;
+    if (r.reset_me) {
+        if (want_fin) {                                                            // terminal head, for final_obs
+            float4* f4 = reinterpret_cast<float4*>(fin_s + 12 * lane);
+            f4[0] = make_float4(h[0], h[1], h[2], h[3]); f4[1] = make_float4(h[4], h[5], h[6], h[7]); f4[2] = make_float4(h[8], h[9], h[10], h[11]);
+        }
+        init_drone(a.st, t.tbl, d);                                                // BaseAviary.py:451-505
+        const float4* rh = reinterpret_cast<const float4*>(a.st.reset_head) + 3 * t.tbl;
+        const float4 r0 = __ldg(rh), r1 = __ldg(rh + 1), r2 = __ldg(rh + 2);
+        h[0] = r0.x; h[1] = r0.y; h[2] = r0.z; h[3] = r0.w; h[4] = r1.x; h[5] = r1.y; h[6] = r1.z; h[7] = r1.w;
+        h[8] = r2.x; h[9] = r2.y; h[10] = r2.z; h[11] = r2.w;
+        rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                                   // last_clipped_action = 0
+        sc = -a.counter_inc;
+    }
+    if (t.live) {
+        store_drone(a.st, N, t.i, d);
+        if (a.st.last_rpm) st256(a.st.last_rpm, t.i, rpm[0], rpm[1], rpm[2], rpm[3]);
+        if (t.dslot == 0) a.st.step_counter[t.e] = sc + a.counter_inc;             // BaseAviary.py:382
+    }
+    stamp(3);
+    return r;
+}
+
+// A = 4: the drone's new head -> slots [4, 16) of its row of the old span in shared memory, its new action -> the 4 slots after
+// the row.  The span read 16 bytes further on (shifted) is then the tile's new span.
+__device__ __forceinline__ void patch_row_a4(float* xs, int od, int lane, bool live, const float h[12], const float act[4]) {
+    if (live) {
+        float* row = xs + (size_t)lane * od;
+        float4* r4 = reinterpret_cast<float4*>(row + 4);
+        r4[0] = make_float4(h[0], h[1], h[2], h[3]); r4[1] = make_float4(h[4], h[5], h[6], h[7]); r4[2] = make_float4(h[8], h[9], h[10], h[11]);
+        *reinterpret_cast<float4*>(row + od) = make_float4(act[0], act[1], act[2], act[3]);
+    }
+    __syncwarp();
+}
+
+// A = 4: the terminal observations (final_obs rows of the tile) of the rows in m: the head from fin_s, the history from the
+// shifted span.  The newest action comes from the span when patch_row_a4 has run (PATCHED), else from lane r's act.
+template <bool PATCHED>
+__device__ __forceinline__ void store_final_rows(float* final_obs, const float* fin_s, const float4* shifted, int od, unsigned m, int lane,
+                                                 const float act[4]) {
+    const int c4n = od >> 2;
+    float4* fin = reinterpret_cast<float4*>(final_obs);
+    for (; m; m &= m - 1) {
+        const int r = __ffs(m) - 1;
+        float4 ar = make_float4(0.f, 0.f, 0.f, 0.f);
+        if constexpr (!PATCHED)
+            ar = make_float4(__shfl_sync(0xffffffffu, act[0], r), __shfl_sync(0xffffffffu, act[1], r),
+                             __shfl_sync(0xffffffffu, act[2], r), __shfl_sync(0xffffffffu, act[3], r));
+        for (int c = lane; c < c4n; c += 32)
+            fin[r * c4n + c] = c < 3 ? reinterpret_cast<const float4*>(fin_s + 12 * r)[c] : (PATCHED || c < c4n - 1 ? shifted[r * c4n + c] : ar);
+    }
+}
+
+// ---- the classic kernel: one 32-drone tile per warp, one warp per CTA ------------------------------------------------------------
+// A: action width (4 = RPM, 1 = ONE_D_RPM).  TASK: Hover/MultiHover reward + flags (else the CtrlAviary-style dummy task).
+// RESET: SAME_STEP autoreset.  RPYF: float32 atan2f/asinf for the reported rpy.
+// PHYS: the drone's physical constants come from its aviary's row of QsState.phys (else from QsParams).
+template <int A, bool TASK, bool RESET, bool RPYF, bool PHYS>
+__global__ void __launch_bounds__(32) step_fast_kernel(const __grid_constant__ StepArgs a) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const int lane = threadIdx.x;
     const int od = a.obs_dim;
     const long long N = a.N;
-    const long long wg = (long long)a.first_warp + (long long)blockIdx.x * WARPS + warp;      // global warp index (a launch may cover a chunk)
+    const long long wg = (long long)a.first_warp + (long long)blockIdx.x;  // global warp index (a launch may cover a chunk)
     const long long w0 = wg * 32;                                           // first drone of this warp
-    if (w0 >= N) return;                                                    // (whole warp: no barrier is shared between warps)
-    if (WARPS > 1 && a.n_warps > 0 && wg >= (long long)a.first_warp + a.n_warps) return;     // past the chunk (a later launch owns these drones)
-    const long long i = w0 + lane;
-    const bool live = i < N;
+    if (w0 >= N) return;
+    const int D = a.D;
+    const TileLane t = tile_lane(a, N, D, w0, lane);
     const int rows = (int)((N - w0) < 32 ? (N - w0) : 32);
     const bool want_fin = RESET && a.io.final_obs != nullptr;
 
-    float* xs = reinterpret_cast<float*>(smem_raw + (size_t)warp * FastSmem<A>::total_bytes(od, want_fin));
+    float* xs = reinterpret_cast<float*>(smem_raw);
     float* ys = xs + FastSmem<A>::x_floats(od);
     float* fin_s = ys + FastSmem<A>::y_floats(od);
     unsigned long long* bar = reinterpret_cast<unsigned long long*>(fin_s + FastSmem<A>::fin_floats(want_fin));
-
-    const int D = a.D, dmask = D - 1;                                       // D is a power of two <= 32
-    const long long il = live ? i : w0;                                     // dead lanes of a ragged last warp shadow the first drone
-    const long long e = il >> a.log2D;
-    const int dslot = (int)il & dmask;
-    const long long tbl = a.st.tables_per_env ? il : dslot;
 
     const float* span_src = a.io.obs_prev + w0 * od;
     float* span_dst = a.io.obs + w0 * od;
@@ -79,8 +206,8 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
     QS_STAMP(0);
     if (lane == 0) mbar_init(bar, 1);
     // read-only tables (never written by a kernel): safe ahead of the dependency wait
-    double tpx = 0.0, tpy = 0.0, tpz = 0.0;
-    if (TASK) { const D4 tp = ld256_nc(a.st.target_pos, tbl); tpx = tp.x; tpy = tp.y; tpz = tp.z; }
+    D4 tp = {0.0, 0.0, 0.0, 0.0};
+    if (TASK) tp = ld256_nc(a.st.target_pos, t.tbl);
 
     // ---- readiness (DESIGN.md 4.1) ----------------------------------------------------------------------------------------
     // This warp's ticket among the steps on these buffers: taken (the atomic has returned, hence the shuffle) BEFORE the CTA lets
@@ -109,51 +236,32 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
     qs::Drone d;
     float act[4] = {0.f, 0.f, 0.f, 0.f};
     int sc = 0;
-    load_drone(a.st.planes, N, il, d);
+    load_drone(a.st.planes, N, t.il, d);
     if (A == 4) {
-        const float4 v = ldg4(a.io.action, il);
+        const float4 v = ldg4(a.io.action, t.il);
         act[0] = v.x; act[1] = v.y; act[2] = v.z; act[3] = v.w;
     } else {
-        act[0] = __ldg(a.io.action + il);
+        act[0] = __ldg(a.io.action + t.il);
     }
-    sc = a.st.step_counter[e];
+    sc = a.st.step_counter[t.e];
     qs::PhysRow ph;
-    if constexpr (PHYS) ph = load_phys(a.st.phys, e);                      // one row per aviary: aviaries never straddle warps
+    if constexpr (PHYS) ph = load_phys(a.st.phys, t.e);                    // one row per aviary: aviaries never straddle warps
     // The bulk copy of the old span (9 KB per warp) is issued only once the step counter -- and with it the batch of small
     // state loads issued just before it -- has ARRIVED: warps issue in order, so the comparison below stalls until then, and
     // the memory system serves every warp's 120 bytes of state ahead of the 19 MB of history the physics does not need yet.
     // (The comparison is always true for a valid counter; the compiler cannot know.)
-    // Experiment (QS_ROW_LOADS=1, off): every lane fetches only the history of its own row, leaving the 48-byte head and the
-    // dropped oldest action (64 of 288 bytes per row) in HBM.  32 small bulk copies per warp measured SLOWER than one copy of
-    // the whole span (13.2 vs 12.3 us per step): the default moves the span.
-    const bool by_rows = A == 4 && a.row_loads;
     auto load_span = [&]() {
-        if (by_rows) {
-            const unsigned hb = (unsigned)(od - 16) * 4u;
-            if (lane == 0) mbar_expect_tx(bar, hb * (unsigned)rows);
-            if (ticketed) asm volatile("fence.proxy.async.global;" ::: "memory");     // every lane issues an async-proxy read
-            __syncwarp();
-            if (live) bulk_g2s(xs + (size_t)lane * od + 16, span_src + (size_t)lane * od + 16, hb, bar);
-        } else if (lane == 0) {
-            // the old span is dead once copied (the next launch on these buffers overwrites it): evict-first in L2, so its 19 MB
-            // make room for this launch's stores and the next launch's state instead of pushing them out (+3 % per step, DESIGN.md 6)
-            tma_bulk_g2s_read_once(xs, span_src, span_bytes, bar);
-        }
+        // the old span is dead once copied (the next launch on these buffers overwrites it): evict-first in L2, so its 19 MB
+        // make room for this launch's stores and the next launch's state instead of pushing them out (+3 % per step, DESIGN.md 6)
+        if (lane == 0) tma_bulk_g2s_read_once(xs, span_src, span_bytes, bar);
     };
     bool issued = false;
-    if (a.flags_late_tma == 0 || __shfl_sync(0xffffffffu, sc, 0) != (int)0x80000000) {
+    if (__shfl_sync(0xffffffffu, sc, 0) != (int)0x80000000) {
         load_span();
         issued = true;
     }
     QS_STAMP(2);
 
-    // ---- action decode (BaseRLAviary.py:192,225) + S substeps ---------------------------------------------------------------
-    double rpm[4];
-    {
-        qs::PidState none = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-        if constexpr (PHYS) qs::decode_action_k<false>(P, ph, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
-        else qs::decode_action<false>(P, A == 4 ? QS_ACT_RPM : QS_ACT_ONE_D_RPM, act, d, 0.0, none, rpm);
-    }
     // A = 4: the history part of the new rows does not depend on the physics: as soon as the old span has landed (polled between
     // substeps) the copy engine writes it back shifted by one action; the heads and the new actions follow at the end as
     // ordinary stores.  So the 19 MB of history stores overlap the FP64 loop instead of following it.
@@ -167,80 +275,19 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
         stored = true;
     };
     auto poll = [&](int s) {
-        if (A == 4 && a.early_store && issued && !stored && (s & 1)) {
+        if (A == 4 && issued && !stored && (s & 1)) {
             int ok = 0;
             if (lane == 0) ok = mbar_test(bar, 0) ? 1 : 0;
             if (__shfl_sync(0xffffffffu, ok, 0)) store_span();
         }
     };
-    double R_last[9];
-    if constexpr (PHYS) qs::dyn_tick_k<0>(P, ph, d, rpm, rpm, 0.0, a.substeps, R_last, poll);
-    else qs::dyn_tick<0>(P, d, rpm, rpm, 0.0, a.substeps, R_last, poll);
-    QS_STAMP(3);
-    qs::Derived o;
-    qs::derive<RPYF>(d, R_last, o);
-    QS_STAMP(4);
-
-    // ---- task terms, reduced over the D drones of the aviary in index order (MultiHoverAviary.py:75-130) ----------------------
-    bool env_done = false;
-    float g_rew = -1.0f;
-    bool g_term = false, g_trunc = false;
-    if (TASK) {
-        const qs::TaskTerms tt = qs::hover_terms(P, d, o, tpx, tpy, tpz);
-        double rew = 0.0, dist = 0.0;
-        const int base = lane & ~dmask;
-        for (int k = 0; k < D; ++k) {
-            rew += __shfl_sync(0xffffffffu, tt.reward, base + k);
-            dist += __shfl_sync(0xffffffffu, tt.dist, base + k);
-        }
-        const unsigned oobs = __ballot_sync(0xffffffffu, tt.out_of_bounds && live);
-        const unsigned gmask = (D == 32 ? 0xffffffffu : ((1u << D) - 1u)) << base;
-        const bool term = dist < P.term_dist;                                     // HoverAviary.py:91
-        const bool trunc = (oobs & gmask) != 0u || sc >= a.sc_limit;              // HoverAviary.py:113 (sc/PYB_FREQ > EPISODE_LEN_SEC)
-        env_done = term || trunc;
-        g_rew = (float)rew; g_term = term; g_trunc = trunc;
-        if (live && dslot == 0) {
-            a.io.reward[e] = (float)rew;
-            a.io.terminated[e] = term ? 1 : 0;
-            a.io.truncated[e] = trunc ? 1 : 0;
-            if (a.io.done) a.io.done[e] = env_done ? 1 : 0;
-        }
-    } else if (live && dslot == 0) {
-        a.io.reward[e] = -1.0f; a.io.terminated[e] = 0; a.io.truncated[e] = 0;     // CtrlAviary-style dummy task
-        if (a.io.done) a.io.done[e] = 0;
-    }
-    QS_STAMP(5);
-
-    // ---- observation head, autoreset, state store ----------------------------------------------------------------------------
     float h[12];
-    h[0] = (float)d.px; h[1] = (float)d.py; h[2] = (float)d.pz;                    // BaseRLAviary.py:310-315
-    h[3] = (float)o.roll; h[4] = (float)o.pitch; h[5] = (float)o.yaw;
-    h[6] = (float)d.vx; h[7] = (float)d.vy; h[8] = (float)d.vz;
-    h[9] = (float)o.ax; h[10] = (float)o.ay; h[11] = (float)o.az;
-    const bool reset_me = RESET && env_done;
-    if (reset_me) {
-        if (want_fin) {                                                            // terminal head, for final_obs
-            float4* f4 = reinterpret_cast<float4*>(fin_s + 12 * lane);
-            f4[0] = make_float4(h[0], h[1], h[2], h[3]); f4[1] = make_float4(h[4], h[5], h[6], h[7]); f4[2] = make_float4(h[8], h[9], h[10], h[11]);
-        }
-        init_drone(a.st, tbl, d);                                                  // BaseAviary.py:451-505
-        const float4* rh = reinterpret_cast<const float4*>(a.st.reset_head) + 3 * tbl;
-        const float4 r0 = __ldg(rh), r1 = __ldg(rh + 1), r2 = __ldg(rh + 2);
-        h[0] = r0.x; h[1] = r0.y; h[2] = r0.z; h[3] = r0.w; h[4] = r1.x; h[5] = r1.y; h[6] = r1.z; h[7] = r1.w;
-        h[8] = r2.x; h[9] = r2.y; h[10] = r2.z; h[11] = r2.w;
-        rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                                   // last_clipped_action = 0
-        sc = -a.counter_inc;
-    }
-    if (live) {
-        store_drone(a.st, N, i, d);
-        if (a.st.last_rpm) st256(a.st.last_rpm, i, rpm[0], rpm[1], rpm[2], rpm[3]);
-        if (dslot == 0) a.st.step_counter[e] = sc + a.counter_inc;                 // BaseAviary.py:382
-    }
-    QS_STAMP(6);
+    const TileEnd te = tile_step<A, TASK, RESET, RPYF, PHYS>(a, N, D, t, lane, d, act, sc, ph, tp, want_fin, fin_s, h, poll,
+                                                             [&](int p) { QS_STAMP(3 + p); });
 
     // ---- observation rows --------------------------------------------------------------------------------------------------------
     if (!issued) load_span();
-    const unsigned fin_rows = want_fin ? __ballot_sync(0xffffffffu, reset_me && live) : 0u;
+    const unsigned fin_rows = want_fin ? __ballot_sync(0xffffffffu, te.reset_me && t.live) : 0u;
     // Fused observation gather: the finished rows go a second time, straight from shared memory, to the learner's tensor
     // (peer memory over NVLink), the per-aviary outputs with them; the last warp of the grid raises the learner's flag.
     auto gather = [&](const void* rows_smem) {
@@ -250,10 +297,10 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
                          ::"l"(a.io.obs_gather + w0 * od), "r"(smem_u32(rows_smem)), "r"(span_bytes) : "memory");
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
-        if (live && dslot == 0) {
-            if (a.io.reward_gather) a.io.reward_gather[e] = g_rew;
-            if (a.io.terminated_gather) a.io.terminated_gather[e] = g_term ? 1 : 0;
-            if (a.io.truncated_gather) a.io.truncated_gather[e] = g_trunc ? 1 : 0;
+        if (t.live && t.dslot == 0) {
+            if (a.io.reward_gather) a.io.reward_gather[t.e] = te.rew;
+            if (a.io.terminated_gather) a.io.terminated_gather[t.e] = te.term ? 1 : 0;
+            if (a.io.truncated_gather) a.io.truncated_gather[t.e] = te.trunc ? 1 : 0;
         }
         if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // rows written (not only read) before the flag
         __syncwarp();
@@ -269,104 +316,74 @@ __global__ void __launch_bounds__(32 * WARPS) step_fast_kernel(const __grid_cons
             }
         }
     };
-    auto patch_rows_a4 = [&]() {            // new head -> slots [A, A+12) of my row, new action -> the A slots after it (in place)
-        if (live) {
-            float* row = xs + (size_t)lane * od;
-            float4* r4 = reinterpret_cast<float4*>(row + 4);
-            r4[0] = make_float4(h[0], h[1], h[2], h[3]); r4[1] = make_float4(h[4], h[5], h[6], h[7]); r4[2] = make_float4(h[8], h[9], h[10], h[11]);
-            *reinterpret_cast<float4*>(row + od) = make_float4(act[0], act[1], act[2], act[3]);
-        }
-        __syncwarp();
-    };
-    if (A == 4 && a.early_store) {
+    if (A == 4) {
         if (!stored) { mbar_wait(bar, 0); store_span(); }
-        if (want_fin) {                                                            // terminal observations: head from fin_s, history from the span
+        if (want_fin) {
             __syncwarp();
-            const int c4n = od >> 2;
-            float4* fin = reinterpret_cast<float4*>(a.io.final_obs + w0 * od);
-            for (unsigned m = fin_rows; m; m &= m - 1) {
-                const int r = __ffs(m) - 1;
-                const float4 ar = make_float4(__shfl_sync(0xffffffffu, act[0], r), __shfl_sync(0xffffffffu, act[1], r),
-                                              __shfl_sync(0xffffffffu, act[2], r), __shfl_sync(0xffffffffu, act[3], r));
-                for (int c = lane; c < c4n; c += 32)
-                    fin[r * c4n + c] = c < 3 ? reinterpret_cast<const float4*>(fin_s + 12 * r)[c] : (c < c4n - 1 ? shifted[r * c4n + c] : ar);
-            }
+            store_final_rows<false>(a.io.final_obs + w0 * od, fin_s, shifted, od, fin_rows, lane, act);
         }
         QS_STAMP(7);
         // the bulk store wrote stale values into the head and newest-action slots of every row: wait until it has completed,
         // then overwrite them (same addresses: the generic stores must be ordered after the asynchronous ones)
         if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
         __syncwarp();
-        if (live) {
-            float4* row = reinterpret_cast<float4*>(a.io.obs + i * od);
+        if (t.live) {
+            float4* row = reinterpret_cast<float4*>(a.io.obs + t.i * od);
             row[0] = make_float4(h[0], h[1], h[2], h[3]); row[1] = make_float4(h[4], h[5], h[6], h[7]); row[2] = make_float4(h[8], h[9], h[10], h[11]);
             row[(od >> 2) - 1] = make_float4(act[0], act[1], act[2], act[3]);
         }
         QS_STAMP(8);
-        if (a.io.obs_gather) { patch_rows_a4(); gather(shifted); }      // (the early bulk store has completed: shared memory is free)
+        if (a.io.obs_gather) { patch_row_a4(xs, od, lane, t.live, h, act); gather(shifted); }      // (the bulk store has completed: shared memory is free)
         publish();
         return;
     }
+    // A = 1: funnel shift by one float, ys[j] = xs[j + 1], four floats per thread and iteration (LDS.128 + one shuffle + STS.128)
     mbar_wait(bar, 0);
     QS_STAMP(7);
-    if (A == 4) {
-        patch_rows_a4();
-        if (lane == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        store_span();
-        if (want_fin) {                                                            // terminal observations: head from fin_s, history from the span
-            const int c4n = od >> 2;
-            float4* fin = reinterpret_cast<float4*>(a.io.final_obs + w0 * od);
-            for (unsigned m = fin_rows; m; m &= m - 1) {
-                const int r = __ffs(m) - 1;
-                for (int c = lane; c < c4n; c += 32)
-                    fin[r * c4n + c] = c < 3 ? reinterpret_cast<const float4*>(fin_s + 12 * r)[c] : shifted[r * c4n + c];
-            }
-        }
-    } else {
-        // funnel shift by one float: ys[j] = xs[j + 1], four floats per thread and iteration (LDS.128 + one shuffle + STS.128)
-        const int n4 = (rows * od + 3) >> 2;
-        for (int j = lane; j < ((n4 + 31) & ~31); j += 32) {
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (j <= n4) v = reinterpret_cast<const float4*>(xs)[j];              // j == n4: the float past the span (padding)
-            float nx = __shfl_down_sync(0xffffffffu, v.x, 1);
-            if (lane == 31 && j + 1 <= n4) nx = xs[4 * (j + 1)];
-            if (j < n4) reinterpret_cast<float4*>(ys)[j] = make_float4(v.y, v.z, v.w, nx);
-        }
-        __syncwarp();
-        if (live) {
-            float* row = ys + (size_t)lane * od;                                  // od = 12 + B: odd word stride for B = 15, conflict-free
+    const int n4 = (rows * od + 3) >> 2;
+    for (int j = lane; j < ((n4 + 31) & ~31); j += 32) {
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (j <= n4) v = reinterpret_cast<const float4*>(xs)[j];              // j == n4: the float past the span (padding)
+        float nx = __shfl_down_sync(0xffffffffu, v.x, 1);
+        if (lane == 31 && j + 1 <= n4) nx = xs[4 * (j + 1)];
+        if (j < n4) reinterpret_cast<float4*>(ys)[j] = make_float4(v.y, v.z, v.w, nx);
+    }
+    __syncwarp();
+    if (t.live) {
+        float* row = ys + (size_t)lane * od;                                  // od = 12 + B: odd word stride for B = 15, conflict-free
 #pragma unroll
-            for (int k = 0; k < 12; ++k) row[k] = h[k];
-            row[od - 1] = act[0];
-        }
-        __syncwarp();
-        if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(span_dst), "r"(smem_u32(ys)), "r"(span_bytes) : "memory");
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        if (want_fin) {
-            float* fin = a.io.final_obs + w0 * od;
-            for (unsigned m = fin_rows; m; m &= m - 1) {
-                const int r = __ffs(m) - 1;
-                for (int c = lane; c < od; c += 32) fin[r * od + c] = c < 12 ? fin_s[12 * r + c] : ys[r * od + c];
-            }
+        for (int k = 0; k < 12; ++k) row[k] = h[k];
+        row[od - 1] = act[0];
+    }
+    __syncwarp();
+    if (lane == 0) {
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(span_dst), "r"(smem_u32(ys)), "r"(span_bytes) : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+    if (want_fin) {
+        float* fin = a.io.final_obs + w0 * od;
+        for (unsigned m = fin_rows; m; m &= m - 1) {
+            const int r = __ffs(m) - 1;
+            for (int c = lane; c < od; c += 32) fin[r * od + c] = c < 12 ? fin_s[12 * r + c] : ys[r * od + c];
         }
     }
     QS_STAMP(8);
-    if (a.io.obs_gather) { gather(A == 4 ? (const void*)shifted : (const void*)ys); publish(); return; }
+    if (a.io.obs_gather) { gather(ys); publish(); return; }
     if (ticketed) publish();
     else if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // shared memory must outlive the bulk store's reads
     QS_STAMP(9);
 }
 
-// ---- the pipelined kernel (A = 4): K consecutive 32-drone tiles per warp, two shared-memory stages ----------------------------
+// ---- the pipelined kernel (A = 4): kPipeTiles consecutive 32-drone tiles per warp, two shared-memory stages -------------------
 // A tile is the classic kernel's warp unit (its own span of rows, ticket word and done word).  While tile k runs its physics,
 // tile k+1's state and actions are on their way into registers and its old span into the other stage, and tile k-1's bulk
 // store is still being written.  A tile is published once its bulk store has completed, which the warp checks only after it has
-// committed the next tile's store, so the completion round trip is off the critical path too.  Same arithmetic, same order:
-// the output bits are the classic kernel's.
+// committed the next tile's store, so the completion round trip is off the critical path too.  Same tile_step as the classic
+// kernel: the output bits are the classic kernel's.
 // The state and actions travel through registers, not shared memory: 20 KB per warp (B = 15) fit 10 warps on an SM.
+// Four tiles per warp measured faster than two on the bench, at 262 144 and at 1 M drones (DESIGN.md 6).
+constexpr int kPipeTiles = 4;
 struct PipeSmem {
     static __host__ __device__ constexpr int bar_off(int od) { return FastSmem<4>::x_floats(od) * 4; }
     // [old span + 16-byte tail][its mbarrier], 128-byte multiple
@@ -374,10 +391,10 @@ struct PipeSmem {
     static __host__ __device__ constexpr int total_bytes(int od, bool fin) { return 2 * stage_bytes(od) + (fin ? 32 * 12 * 4 : 0); }
 };
 
-template <bool TASK, bool RESET, bool RPYF, bool PHYS, int K>
+template <bool TASK, bool RESET, bool RPYF, bool PHYS>
 __global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ StepArgs a) {
+    constexpr int K = kPipeTiles;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    const QsParams& P = a.P;
     const int lane = threadIdx.x;
     const int od = a.obs_dim;
     const long long N = a.N;
@@ -391,7 +408,7 @@ __global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ S
     float* fin_s = reinterpret_cast<float*>(smem_raw + 2 * SB);
     auto stage = [&](int k) { return smem_raw + (k & 1) * SB; };
     auto bar_of = [&](int k) { return reinterpret_cast<unsigned long long*>(stage(k) + PipeSmem::bar_off(od)); };
-    const int D = a.D, dmask = D - 1;
+    const int D = a.D;
     QS_TSTAMP(t0, 0);
     if (lane == 0) { mbar_init(bar_of(0), 1); mbar_init(bar_of(1), 1); }
 
@@ -474,102 +491,27 @@ __global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ S
             pre = true;
         }
         const long long w0 = tg * 32;
-        const long long i = w0 + lane;
-        const bool live = i < N;
+        const TileLane t = tile_lane(a, N, D, w0, lane);
         const int rows = (int)((N - w0) < 32 ? (N - w0) : 32);
-        const long long il = live ? i : w0;
-        const long long e = il >> a.log2D;
-        const int dslot = (int)il & dmask;
-        const long long tbl = a.st.tables_per_env ? il : dslot;
         unsigned long long* bar = bar_of(k);
         float* xs = reinterpret_cast<float*>(stage(k));
-        double tpx = 0.0, tpy = 0.0, tpz = 0.0;
-        if (TASK) { const D4 tp = ld256_nc(a.st.target_pos, tbl); tpx = tp.x; tpy = tp.y; tpz = tp.z; }
-        int sc = a.st.step_counter[e];
+        D4 tp = {0.0, 0.0, 0.0, 0.0};
+        if (TASK) tp = ld256_nc(a.st.target_pos, t.tbl);
+        const int sc = a.st.step_counter[t.e];
         qs::PhysRow ph;
-        if constexpr (PHYS) ph = load_phys(a.st.phys, e);
+        if constexpr (PHYS) ph = load_phys(a.st.phys, t.e);
 
         QS_TSTAMP(tg, 2);
-        float act[4] = {av.x, av.y, av.z, av.w};
-
-        // ---- action decode (BaseRLAviary.py:192,225) + S substeps ----------------------------------------------------------
-        double rpm[4];
-        {
-            qs::PidState none = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-            if constexpr (PHYS) qs::decode_action_k<false>(P, ph, QS_ACT_RPM, act, d, 0.0, none, rpm);
-            else qs::decode_action<false>(P, QS_ACT_RPM, act, d, 0.0, none, rpm);
-        }
-        double R_last[9];
-        if constexpr (PHYS) qs::dyn_tick_k<0>(P, ph, d, rpm, rpm, 0.0, a.substeps, R_last);
-        else qs::dyn_tick<0>(P, d, rpm, rpm, 0.0, a.substeps, R_last);
-        QS_TSTAMP(tg, 3);
-        qs::Derived o;
-        qs::derive<RPYF>(d, R_last, o);
-
-        // ---- task terms, reduced over the D drones of the aviary in index order (MultiHoverAviary.py:75-130) ------------------
-        bool env_done = false;
-        if (TASK) {
-            const qs::TaskTerms tt = qs::hover_terms(P, d, o, tpx, tpy, tpz);
-            double rew = 0.0, dist = 0.0;
-            const int base = lane & ~dmask;
-            for (int j = 0; j < D; ++j) {
-                rew += __shfl_sync(0xffffffffu, tt.reward, base + j);
-                dist += __shfl_sync(0xffffffffu, tt.dist, base + j);
-            }
-            const unsigned oobs = __ballot_sync(0xffffffffu, tt.out_of_bounds && live);
-            const unsigned gmask = (D == 32 ? 0xffffffffu : ((1u << D) - 1u)) << base;
-            const bool term = dist < P.term_dist;                                     // HoverAviary.py:91
-            const bool trunc = (oobs & gmask) != 0u || sc >= a.sc_limit;              // HoverAviary.py:113
-            env_done = term || trunc;
-            if (live && dslot == 0) {
-                a.io.reward[e] = (float)rew;
-                a.io.terminated[e] = term ? 1 : 0;
-                a.io.truncated[e] = trunc ? 1 : 0;
-                if (a.io.done) a.io.done[e] = env_done ? 1 : 0;
-            }
-        } else if (live && dslot == 0) {
-            a.io.reward[e] = -1.0f; a.io.terminated[e] = 0; a.io.truncated[e] = 0;     // CtrlAviary-style dummy task
-            if (a.io.done) a.io.done[e] = 0;
-        }
-
-        // ---- observation head, autoreset, state store ----------------------------------------------------------------------
+        const float act[4] = {av.x, av.y, av.z, av.w};
         float h[12];
-        h[0] = (float)d.px; h[1] = (float)d.py; h[2] = (float)d.pz;                    // BaseRLAviary.py:310-315
-        h[3] = (float)o.roll; h[4] = (float)o.pitch; h[5] = (float)o.yaw;
-        h[6] = (float)d.vx; h[7] = (float)d.vy; h[8] = (float)d.vz;
-        h[9] = (float)o.ax; h[10] = (float)o.ay; h[11] = (float)o.az;
-        const bool reset_me = RESET && env_done;
-        if (reset_me) {
-            if (want_fin) {
-                float4* f4 = reinterpret_cast<float4*>(fin_s + 12 * lane);
-                f4[0] = make_float4(h[0], h[1], h[2], h[3]); f4[1] = make_float4(h[4], h[5], h[6], h[7]); f4[2] = make_float4(h[8], h[9], h[10], h[11]);
-            }
-            init_drone(a.st, tbl, d);                                                  // BaseAviary.py:451-505
-            const float4* rh = reinterpret_cast<const float4*>(a.st.reset_head) + 3 * tbl;
-            const float4 r0 = __ldg(rh), r1 = __ldg(rh + 1), r2 = __ldg(rh + 2);
-            h[0] = r0.x; h[1] = r0.y; h[2] = r0.z; h[3] = r0.w; h[4] = r1.x; h[5] = r1.y; h[6] = r1.z; h[7] = r1.w;
-            h[8] = r2.x; h[9] = r2.y; h[10] = r2.z; h[11] = r2.w;
-            rpm[0] = rpm[1] = rpm[2] = rpm[3] = 0.0;                                   // last_clipped_action = 0
-            sc = -a.counter_inc;
-        }
-        if (live) {
-            store_drone(a.st, N, i, d);
-            if (a.st.last_rpm) st256(a.st.last_rpm, i, rpm[0], rpm[1], rpm[2], rpm[3]);
-            if (dslot == 0) a.st.step_counter[e] = sc + a.counter_inc;                 // BaseAviary.py:382
-        }
-        QS_TSTAMP(tg, 4);
+        const TileEnd te = tile_step<4, TASK, RESET, RPYF, PHYS>(a, N, D, t, lane, d, act, sc, ph, tp, want_fin, fin_s, h, qs::NoHook(),
+                                                                 [&](int p) { if (p == 0) QS_TSTAMP(tg, 3); else if (p == 3) QS_TSTAMP(tg, 4); });
 
         // ---- observation rows: patched in shared memory, one bulk store of the shifted span ----------------------------------
-        const unsigned fin_rows = want_fin ? __ballot_sync(0xffffffffu, reset_me && live) : 0u;
+        const unsigned fin_rows = want_fin ? __ballot_sync(0xffffffffu, te.reset_me && t.live) : 0u;
         mbar_wait(bar, par);
         QS_TSTAMP(tg, 5);
-        if (live) {             // new head -> slots [4, 16) of my row, new action -> the 4 slots after it (in place)
-            float* row = xs + (size_t)lane * od;
-            float4* r4 = reinterpret_cast<float4*>(row + 4);
-            r4[0] = make_float4(h[0], h[1], h[2], h[3]); r4[1] = make_float4(h[4], h[5], h[6], h[7]); r4[2] = make_float4(h[8], h[9], h[10], h[11]);
-            *reinterpret_cast<float4*>(row + od) = make_float4(act[0], act[1], act[2], act[3]);
-        }
-        __syncwarp();
+        patch_row_a4(xs, od, lane, t.live, h, act);
         const float4* shifted = reinterpret_cast<const float4*>(xs) + 1;
         if (lane == 0) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -577,14 +519,8 @@ __global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ S
                          ::"l"(a.io.obs + w0 * od), "r"(smem_u32(shifted)), "r"((unsigned)(rows * od * 4)) : "memory");
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
-        if (want_fin) {                                                                // terminal observations: head from fin_s, history from the span
-            const int c4n = od >> 2;
-            float4* fin = reinterpret_cast<float4*>(a.io.final_obs + w0 * od);
-            for (unsigned m = fin_rows; m; m &= m - 1) {
-                const int r = __ffs(m) - 1;
-                for (int c = lane; c < c4n; c += 32)
-                    fin[r * c4n + c] = c < 3 ? reinterpret_cast<const float4*>(fin_s + 12 * r)[c] : shifted[r * c4n + c];
-            }
+        if (want_fin) {
+            store_final_rows<true>(a.io.final_obs + w0 * od, fin_s, shifted, od, fin_rows, lane, act);
             __syncwarp();                                                              // fin_s is rewritten by the next tile
         }
         QS_TSTAMP(tg, 6);
@@ -602,83 +538,42 @@ __global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ S
     else if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // shared memory must outlive the bulk store's reads
 }
 
-template <bool TASK, bool RESET, bool RPYF, bool PHYS, int K>
-cudaError_t launch_pipe(const StepArgs& a, cudaStream_t s) {
-    const long long tiles = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
-    const int blocks = (int)((tiles + K - 1) / K);
-    const size_t sm = (size_t)PipeSmem::total_bytes(a.obs_dim, RESET && a.io.final_obs != nullptr);
-    static const bool pdl = !(getenv("QS_PDL") && atoi(getenv("QS_PDL")) == 0);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = sm; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    if (sm > 48 * 1024)
-        cudaFuncSetAttribute(step_pipe_kernel<TASK, RESET, RPYF, PHYS, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    return cudaLaunchKernelEx(&cfg, step_pipe_kernel<TASK, RESET, RPYF, PHYS, K>, a);
-}
-
-template <int K, bool PHYS>
-cudaError_t launch_pipe_modes(const StepArgs& a, cudaStream_t s) {
-    const bool task = a.task == QS_TASK_HOVER, reset = a.flags & QS_FLAG_AUTORESET_SAME_STEP, rpyf = a.flags & QS_FLAG_RPY_F32;
-    const int key = (task ? 4 : 0) | (reset ? 2 : 0) | (rpyf ? 1 : 0);
-    switch (key) {
-        case 0: return launch_pipe<false, false, false, PHYS, K>(a, s);
-        case 1: return launch_pipe<false, false, true, PHYS, K>(a, s);
-        case 2: return launch_pipe<false, true, false, PHYS, K>(a, s);
-        case 3: return launch_pipe<false, true, true, PHYS, K>(a, s);
-        case 4: return launch_pipe<true, false, false, PHYS, K>(a, s);
-        case 5: return launch_pipe<true, false, true, PHYS, K>(a, s);
-        case 6: return launch_pipe<true, true, false, PHYS, K>(a, s);
-        default: return launch_pipe<true, true, true, PHYS, K>(a, s);
+// ---- launch ------------------------------------------------------------------------------------------------------------------
+template <int A, bool PHYS>
+struct LaunchClassic {
+    template <bool TASK, bool RESET, bool RPYF>
+    static cudaError_t run(const StepArgs& a, cudaStream_t s) {
+        const long long warps = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
+        const size_t sm = (size_t)FastSmem<A>::total_bytes(a.obs_dim, RESET && a.io.final_obs != nullptr);
+        return launch_step_kernel(step_fast_kernel<A, TASK, RESET, RPYF, PHYS>, (int)warps, 32, sm, sm, pdl_enabled(), s, a);
     }
-}
-
-template <int A, bool TASK, bool RESET, bool RPYF, int WARPS, bool PHYS>
-cudaError_t launch_one(const StepArgs& a, cudaStream_t s) {
-    const long long warps = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
-    const int blocks = (int)((warps + WARPS - 1) / WARPS);
-    const bool fin = RESET && a.io.final_obs != nullptr;
-    const size_t sm = (size_t)WARPS * FastSmem<A>::total_bytes(a.obs_dim, fin);
-    static const bool pdl = !(getenv("QS_PDL") && atoi(getenv("QS_PDL")) == 0);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(32 * WARPS); cfg.dynamicSmemBytes = sm; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    if (sm > 48 * 1024)
-        cudaFuncSetAttribute(step_fast_kernel<A, TASK, RESET, RPYF, WARPS, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    return cudaLaunchKernelEx(&cfg, step_fast_kernel<A, TASK, RESET, RPYF, WARPS, PHYS>, a);
-}
-
-template <int A, int WARPS, bool PHYS>
-cudaError_t launch_modes(const StepArgs& a, cudaStream_t s) {
-    const bool task = a.task == QS_TASK_HOVER, reset = a.flags & QS_FLAG_AUTORESET_SAME_STEP, rpyf = a.flags & QS_FLAG_RPY_F32;
-    const int key = (task ? 4 : 0) | (reset ? 2 : 0) | (rpyf ? 1 : 0);
-    switch (key) {
-        case 0: return launch_one<A, false, false, false, WARPS, PHYS>(a, s);
-        case 1: return launch_one<A, false, false, true, WARPS, PHYS>(a, s);
-        case 2: return launch_one<A, false, true, false, WARPS, PHYS>(a, s);
-        case 3: return launch_one<A, false, true, true, WARPS, PHYS>(a, s);
-        case 4: return launch_one<A, true, false, false, WARPS, PHYS>(a, s);
-        case 5: return launch_one<A, true, false, true, WARPS, PHYS>(a, s);
-        case 6: return launch_one<A, true, true, false, WARPS, PHYS>(a, s);
-        default: return launch_one<A, true, true, true, WARPS, PHYS>(a, s);
-    }
-}
+};
 
 template <bool PHYS>
-cudaError_t launch_warps(const StepArgs& a, int warps, cudaStream_t s) {
-    if (a.A == 4) {
-        if (warps == 4) return launch_modes<4, 4, PHYS>(a, s);
-        if (warps == 2) return launch_modes<4, 2, PHYS>(a, s);
-        return launch_modes<4, 1, PHYS>(a, s);
+struct LaunchPipe {
+    template <bool TASK, bool RESET, bool RPYF>
+    static cudaError_t run(const StepArgs& a, cudaStream_t s) {
+        const long long tiles = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
+        const size_t sm = (size_t)PipeSmem::total_bytes(a.obs_dim, RESET && a.io.final_obs != nullptr);
+        return launch_step_kernel(step_pipe_kernel<TASK, RESET, RPYF, PHYS>, (int)((tiles + kPipeTiles - 1) / kPipeTiles), 32, sm, sm,
+                                  pdl_enabled(), s, a);
     }
-    if (warps == 4) return launch_modes<1, 4, PHYS>(a, s);
-    if (warps == 2) return launch_modes<1, 2, PHYS>(a, s);
-    return launch_modes<1, 1, PHYS>(a, s);
+};
+
+// L::run<TASK, RESET, RPYF> for the step's task, autoreset mode and rpy precision
+template <class L>
+cudaError_t launch_modes(const StepArgs& a, cudaStream_t s) {
+    const bool task = a.task == QS_TASK_HOVER, reset = a.flags & QS_FLAG_AUTORESET_SAME_STEP, rpyf = a.flags & QS_FLAG_RPY_F32;
+    switch ((task ? 4 : 0) | (reset ? 2 : 0) | (rpyf ? 1 : 0)) {
+        case 0: return L::template run<false, false, false>(a, s);
+        case 1: return L::template run<false, false, true>(a, s);
+        case 2: return L::template run<false, true, false>(a, s);
+        case 3: return L::template run<false, true, true>(a, s);
+        case 4: return L::template run<true, false, false>(a, s);
+        case 5: return L::template run<true, false, true>(a, s);
+        case 6: return L::template run<true, true, false>(a, s);
+        default: return L::template run<true, true, true>(a, s);
+    }
 }
 
 }  // namespace
@@ -706,14 +601,10 @@ cudaError_t launch_step_fast(const StepArgs& a_in, cudaStream_t s) {
 #else
     const StepArgs& a = a_in;
 #endif
-    static const int warps = getenv("QS_FAST_WARPS") ? atoi(getenv("QS_FAST_WARPS")) : 1;      // measured default (DESIGN.md 6)
-    // the pipelined kernel takes A = 4 without the fused gather; the experiment switches keep their meaning on the classic one
-    if (a.A == 4 && a.pipe_tiles > 0 && !a.io.obs_gather && warps == 1 && a.early_store && a.flags_late_tma && !a.row_loads) {
-        if (a.pipe_tiles == 4) return a.st.phys ? launch_pipe_modes<4, true>(a, s) : launch_pipe_modes<4, false>(a, s);
-        return a.st.phys ? launch_pipe_modes<2, true>(a, s) : launch_pipe_modes<2, false>(a, s);
-    }
-    if (a.st.phys) return launch_warps<true>(a, warps, s);
-    return launch_warps<false>(a, warps, s);
+    // the pipelined kernel takes A = 4 without the fused gather
+    if (a.A == 4 && a.pipe && !a.io.obs_gather) return a.st.phys ? launch_modes<LaunchPipe<true>>(a, s) : launch_modes<LaunchPipe<false>>(a, s);
+    if (a.A == 4) return a.st.phys ? launch_modes<LaunchClassic<4, true>>(a, s) : launch_modes<LaunchClassic<4, false>>(a, s);
+    return a.st.phys ? launch_modes<LaunchClassic<1, true>>(a, s) : launch_modes<LaunchClassic<1, false>>(a, s);
 }
 
 }  // namespace qsi

@@ -427,20 +427,10 @@ cudaError_t launch_step(const StepArgs& a, bool pdl_ok, cudaStream_t s) {
     const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
     const int threads = ((a.tpb + 31) / 32) * 32;
     const size_t sm = step_smem_bytes(a);
-    static const bool pdl = !(getenv("QS_PDL") && atoi(getenv("QS_PDL")) == 0);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = sm; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = (pdl && pdl_ok) ? 1 : 0;
-#define QS_CASE(E)                                                                                               \
-    case E: {                                                                                                    \
-        if (sm > 48 * 1024)      /* per device and cheap: no process-wide "already set" flag */                 \
-            cudaFuncSetAttribute(step_kernel<E, RAW, PIDACT, PHYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                 (int)(kStepSmemFixed + kStageLimit + 32));                                      \
-        return cudaLaunchKernelEx(&cfg, step_kernel<E, RAW, PIDACT, PHYS>, a);                                   \
-    }
+    const bool pdl = pdl_enabled() && pdl_ok;
+    // the shared-memory limit is the largest step_smem_bytes, the same for every launch of a kernel
+#define QS_CASE(E)                                                                                                     \
+    case E: return launch_step_kernel(step_kernel<E, RAW, PIDACT, PHYS>, blocks, threads, sm, kStepSmemFixed + kStageLimit + 32, pdl, s, a);
     switch (a.effects & 7u) {
         QS_CASE(0) QS_CASE(1) QS_CASE(2) QS_CASE(3) QS_CASE(4) QS_CASE(5) QS_CASE(6) QS_CASE(7)
     }

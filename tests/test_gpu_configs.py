@@ -568,9 +568,8 @@ def test_negative_control_episode_length_moves_the_time_out():
 # 3. launch variants of the environment knobs (read once per process: one subprocess per setting)
 # ---------------------------------------------------------------------------------------------------------------
 VARIANT_ROWS = ["1", "5", "7", "9"]
-VARIANTS = [{}, {"QS_FAST_WARPS": "2"}, {"QS_FAST_WARPS": "4"}, {"QS_EARLY_STORE": "0"}, {"QS_LATE_TMA": "0"}, {"QS_ROW_LOADS": "1"},
-            {"QS_PDL": "0"}, {"QS_CTA_CAP": "64", "QS_FAST": "0"}, {"QS_CTA_CAP": "128", "QS_FAST": "0"}]
-_KNOBS = ("QS_FAST", "QS_FAST_WARPS", "QS_EARLY_STORE", "QS_LATE_TMA", "QS_ROW_LOADS", "QS_PDL", "QS_CTA_CAP", "QS_HOST_CHUNKS")
+VARIANTS = [{}, {"QS_FAST_PIPE": "0"}, {"QS_PDL": "0"}, {"QS_CTA_CAP": "64", "QS_FAST": "0"}, {"QS_CTA_CAP": "128", "QS_FAST": "0"}]
+_KNOBS = ("QS_FAST", "QS_FAST_PIPE", "QS_PDL", "QS_CTA_CAP", "QS_HOST_CHUNKS")
 
 
 def play_variant_sequence(path):

@@ -56,13 +56,8 @@ def _fz(N, env, cull=True, boxed=False):
     return fz.cpu().numpy()
 
 
-ADJ_VERSIONS = [1, 2, 3, 4, 5]      # kernel versions of qs_adjacency (QS_ADJ_V, read per call): all must give the reference's bits
-
-
-@pytest.mark.parametrize("version", ADJ_VERSIONS)
-def test_adjacency_golden(golden, version, monkeypatch):
+def test_adjacency_golden(golden):
     """BaseAviary._getAdjacencyMatrix of the unmodified reference on three random swarms: bit-exact."""
-    monkeypatch.setenv("QS_ADJ_V", str(version))
     N, CtrlAviary, _, _, Physics, _ = _imports()
     g = golden("adjacency")
     for k in range(3):
@@ -72,12 +67,10 @@ def test_adjacency_golden(golden, version, monkeypatch):
         assert adj.dtype == np.float64 and np.array_equal(adj, g["case%d_adjacency" % k])
 
 
-@pytest.mark.parametrize("version", ADJ_VERSIONS)
 @pytest.mark.parametrize("E,D,radius", [(3, 1000, 0.7), (1, 4096, 1.1), (5, 37, np.inf), (2, 512, 0.0), (2, 48, -1.0)])
-def test_adjacency_vs_oracle(E, D, radius, version, monkeypatch):
+def test_adjacency_vs_oracle(E, D, radius):
     """Vector query [E, D, D] against the NumPy restatement: ragged D (scalar stores), D % 16 == 0 (16-byte stores),
     several column tiles, radius 0 and negative (identity) and inf (all ones)."""
-    monkeypatch.setenv("QS_ADJ_V", str(version))
     N, CtrlAviary, _, _, Physics, O = _imports()
     rng = np.random.default_rng(3)
     pos = rng.uniform(-2, 2, (E, D, 3)).astype(np.float32).astype(np.float64)
@@ -89,14 +82,12 @@ def test_adjacency_vs_oracle(E, D, radius, version, monkeypatch):
     assert np.array_equal(adj, adj.transpose(0, 2, 1))
 
 
-@pytest.mark.parametrize("version", ADJ_VERSIONS)
 @pytest.mark.parametrize("D", [864, 1000])
-def test_adjacency_pairs_on_the_threshold(D, version, monkeypatch):
+def test_adjacency_pairs_on_the_threshold(D):
     """A lattice with 0.25 m pitch and radius 1.0: thousands of pairs sit EXACTLY on the threshold (4 steps along an axis,
     3-4-5 triangles ... -- the reference's `<` says no) and, after perturbing random coordinates by 1e-9 ... 1e-6, within a
     few float32 ulps of it on either side.  The float32 fast decision must hand every such pair to the float64 arithmetic of
-    the reference (the band logic of both kernel versions): bit-exact against the float64 restatement."""
-    monkeypatch.setenv("QS_ADJ_V", str(version))
+    the reference (the kernel's band logic): bit-exact against the float64 restatement."""
     N, CtrlAviary, _, _, Physics, O = _imports()
     k = np.arange(D)
     pos = np.stack([0.25 * (k % 12), 0.25 * ((k // 12) % 12), 0.25 * (k // 144)], axis=1).astype(np.float64)

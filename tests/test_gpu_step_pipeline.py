@@ -1,4 +1,4 @@
-"""The pipelined fast step kernel (step_pipe_kernel, DESIGN.md 4.1): K consecutive 32-drone tiles per warp, two shared-memory
+"""The pipelined fast step kernel (step_pipe_kernel, DESIGN.md 4.1): 4 consecutive 32-drone tiles per warp, two shared-memory
 stages, per-tile readiness.  Every test runs the same sequence with the default kernel, with the classic one-tile-per-warp
 kernel (QS_FAST_PIPE=0) and with the general kernel (QS_FAST=0), and compares the bits of everything a step writes; the
 readiness words agree and the readiness error word stays zero."""
@@ -70,14 +70,11 @@ def _outputs(env, final_obs=True):
     return {k: v.clone() for k, v in out.items()}
 
 
-def _run_modes(make_envs, body, modes=("pipe", "classic", "general"), pipe_tiles=None):
+def _run_modes(make_envs, body, modes=("pipe", "classic", "general")):
     """body(envs) once per kernel; returns {mode: envs}."""
     res = {}
     for m in modes:
-        values = dict(MODES[m])
-        if m == "pipe" and pipe_tiles is not None:
-            values["QS_FAST_PIPE"] = pipe_tiles
-        with _env_vars(values):
+        with _env_vars(MODES[m]):
             envs = make_envs()
             body(envs)
             torch.cuda.synchronize()
@@ -118,12 +115,14 @@ def test_bench_pattern_eight_envs_rotating():
     assert int(torch.stack(dones).sum()) > 0                       # same-step resets happened
 
 
-# 35 tiles per env (a ragged last tile, a tile count no K divides), every aviary size, every tile count
-@pytest.mark.parametrize("pipe_tiles", ["2", "4"])
-@pytest.mark.parametrize("D,E", [(1, 1100), (2, 550), (4, 275), (32, 35)])
-def test_ragged_batches_every_aviary_size(D, E, pipe_tiles):
+# 33, 34 or 35 tiles per env, so the last warp holds 1, 2 or 3 of its 4 tiles; a ragged last tile of 12 drones for D < 32;
+# every aviary size
+@pytest.mark.parametrize("tiles", [33, 34, 35])
+@pytest.mark.parametrize("D", [1, 2, 4, 32])
+def test_ragged_batches_every_aviary_size(D, tiles):
+    E = tiles if D == 32 else (32 * (tiles - 1) + 12) // D
     dones = []
-    res = _run_modes(lambda: [_make(E, D), _make(E, D)], _stepper(48, 200 + D, dones), pipe_tiles=pipe_tiles)
+    res = _run_modes(lambda: [_make(E, D), _make(E, D)], _stepper(48, 200 + D, dones))
     _assert_same(res)
     assert int(torch.stack(dones).sum()) > 0
 

@@ -25,7 +25,7 @@ import threshold_sweeps as S
 pytestmark = pytest.mark.gpu
 
 BAND_ULPS = 16
-MODES = {"pipe4": {"QS_FAST_PIPE": "4"}, "pipe2": {"QS_FAST_PIPE": "2"}, "classic": {"QS_FAST_PIPE": "0"}, "general": {"QS_FAST": "0"}}
+MODES = {"pipe": {}, "classic": {"QS_FAST_PIPE": "0"}, "general": {"QS_FAST": "0"}}
 
 
 @contextlib.contextmanager
@@ -158,7 +158,7 @@ def test_s1_per_aviary_constants_row():
     counts = {}
     E = 3040
     pos, q = _tilt_state("hover", E)
-    for mode in ("pipe4", "general"):
+    for mode in ("pipe", "general"):
         with _env_vars(MODES[mode]):
             env = _make("hover", E)
             m = torch.full((E,), 0.027, dtype=torch.float64, device="cuda")
@@ -232,7 +232,7 @@ def test_s3_termination(kind, D):
     ks = np.arange(-64, 65)
     E = ks.size
     counts = {}
-    for mode in ("pipe4", "classic", "general"):
+    for mode in ("pipe", "classic", "general"):
         with _env_vars(MODES[mode]):
             env = _make(kind, E, D=D)
             tgt = env._target[:, 0:3].cpu().numpy()          # [D, 3]
@@ -310,7 +310,7 @@ def test_s7_reset_observation_every_path(rpy_f32):
     heads["reset"] = obs.cpu().numpy().reshape(E, -1)[:, 0:12]
     init_q = env._init_quat.cpu().numpy().reshape(-1, 4)[:, 0:4]
     ref = np.float32(S.euler(init_q))
-    for mode in ("pipe4", "classic", "general"):
+    for mode in ("pipe", "classic", "general"):
         with _env_vars(MODES[mode]):
             env = _make("hover", E, rpy_f32=rpy_f32, autoreset="same_step", initial_rpys=rpys)
             _place(env, far, env._init_quat.cpu().numpy()[:, 0:4])

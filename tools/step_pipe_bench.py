@@ -3,8 +3,7 @@
 Prints the card (name, power limit, max SM clock), then the copy ceiling: a device-to-device copy with the step kernel's
 read/write volume per launch of 65 536 drones (~27 MB read + ~26 MB written), rotated over buffers much larger than the 50 MB
 L2 and timed with CUDA events.  Then it alternates the kernel variants (QS_FAST_PIPE=0: the classic one-tile-per-warp kernel,
-2 and 4: tiles per warp of the pipelined kernel), each in a fresh process because the library reads the knob once, and
-times, in µs per launch:
+4: the pipelined kernel, four tiles per warp), each in a fresh process, and times, in µs per launch:
   bench      the bench.py workload: 32 768 MultiHoverAviary x 2 drones, RPM, 8 batches rotating on one stream
   n262144    262 144 drones, 2 batches alternating
   n1048576   1 048 576 drones, 2 batches alternating
@@ -12,7 +11,7 @@ times, in µs per launch:
   two_streams  even / odd batches on two streams
 Each variant's bytes actually moved per launch over its time are printed against the ceiling.
 
-    python tools/step_pipe_bench.py [--variants 0,2,4] [--runs 3] [--lib A=path ...]
+    python tools/step_pipe_bench.py [--variants 0,4] [--runs 3] [--lib A=path ...]
 """
 import argparse
 import json
@@ -143,7 +142,7 @@ def worker(steps):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--variants", default="0,2,4", help="QS_FAST_PIPE values, alternated")
+    ap.add_argument("--variants", default="0,4", help="QS_FAST_PIPE values, alternated")
     ap.add_argument("--lib", action="append", default=[], help="NAME=path: an extra variant running another libquadsim.so")
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--steps", type=int, default=2000)

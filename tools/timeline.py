@@ -1,8 +1,8 @@
 """Per-warp phase timeline of the fast step kernel (tools, not product): builds a -DQS_TIMELINE copy of the library
 (build/libquadsim_timeline.so, %globaltimer stamps by lane 0 of every warp), runs the bench workload and prints where a
-warp's time goes.  Stamps: 0 start, 1 after the readiness wait (per-warp ticket, and griddepcontrol.wait when kept), 2 loads issued / bulk copy issued (= state arrived with
-QS_LATE_TMA=1), 3 physics done, 4 state stored, 5 old span arrived, 6 bulk store + terminal rows issued, 7 exit.
-The pipelined kernel (A = 4, QS_FAST_PIPE != 0) stamps per 32-drone tile: 0 its warp started, 1 its loads issued (after its
+warp's time goes.  Stamps: 0 start, 1 after the readiness wait (per-warp ticket, and griddepcontrol.wait when kept), 2 loads issued / bulk copy issued (once the state loads
+have arrived), 3 physics done, 4 state stored, 5 old span arrived, 6 bulk store + terminal rows issued, 7 exit.
+The pipelined kernel (A = 4 unless QS_FAST_PIPE=0) stamps per 32-drone tile: 0 its warp started, 1 its loads issued (after its
 readiness), 2 tile started (its state and actions in registers), 3 physics done, 4 state stored, 5 old span arrived, 6 bulk store + terminal rows issued, 7 published.
 
     python tools/timeline.py --build          # here (nvcc)
@@ -92,7 +92,7 @@ def main():
     t0 = t[:, 0].min()
     rel = (t - t0) / 1e3            # us since the first warp started
     all_names = ["start", "after_pdl_wait", "state_arrived", "physics_done", "derived", "task_done", "state_stored", "span_stored/arrived", "rows_done", "exit"]
-    if a.act == "RPM" and os.environ.get("QS_FAST_PIPE", "2") != "0":     # step_pipe_kernel: one row per 32-drone tile
+    if a.act == "RPM" and os.environ.get("QS_FAST_PIPE") != "0":     # step_pipe_kernel: one row per 32-drone tile
         all_names = ["warp_start", "loads_issued", "tile_start", "physics_done", "state_stored", "span_arrived", "span_store_issued", "published"]
     names = [all_names[k] if k < len(all_names) else "s%d" % k for k in used]
     out = {"act": a.act, "n": n, "isolated": a.isolated, "env": {k: v for k, v in os.environ.items() if k.startswith("QS_") and k != "QS_LIBQUADSIM"}, "warps": nw, "phases_us": {}}
