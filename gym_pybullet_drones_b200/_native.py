@@ -13,8 +13,8 @@ _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))    # override: A/B builds in tools/
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
-                                             "formation.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
+                                             "formation.cu", "mrac.cu")]
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -33,6 +33,8 @@ FLAG_AUTORESET_CLEARS_PID, FLAG_AUTORESET_CLEARS_HISTORY = 8, 16
 FLAG_OBS_STATE20 = 32
 FLAG_SKIP_EPILOGUE, FLAG_RPM_FROM_LAST, FLAG_ACTION_F64 = 0x100, 0x200, 0x400
 CTRL_RAW, CTRL_VEL, CTRL_TRACK = 0, 1, 2          # qs_ctrl_rollout modes
+CTRL_MRAC = 3                                     # qs_ctrl_rollout_mrac
+MRAC_STATE = 76                                   # doubles of one MRAC's adaptive state (Kx 48, Kr 16, Xm 12)
 ABI_VERSION = 4
 MLP_TANH, MLP_RELU = 0, 1                         # QsMlpPolicy.activation
 MLP_MAX_HIDDEN, MLP_MAX_WIDTH = 4, 256
@@ -127,6 +129,16 @@ class QsCtrlRolloutIO(C.Structure):
                 ("log", C.c_void_p), ("log_controls", C.c_void_p)]
 
 
+class QsMracParams(C.Structure):
+    _fields_ = [("Am", (_d * 12) * 12), ("bm", _d * 4), ("PBm", (_d * 4) * 12), ("Kr_ref", (_d * 12) * 4),
+                ("gamma_x", _d), ("gamma_r", _d), ("mixer", (_d * 3) * 4),
+                ("kf", _d), ("pwm2rpm_scale", _d), ("pwm2rpm_const", _d), ("min_pwm", _d), ("max_pwm", _d), ("max_rpm", _d)]
+
+
+class QsMracRolloutIO(C.Structure):
+    _fields_ = [("params", C.c_void_p), ("state", C.c_void_p), ("init", C.c_int), ("pad_", C.c_int), ("rpy_e", C.c_void_p)]
+
+
 class QsStepCall(C.Structure):
     _fields_ = [("p", C.c_void_p), ("st", C.c_void_p), ("io", C.c_void_p),
                 ("act_type", C.c_int), ("task", C.c_int), ("n_envs", C.c_int), ("drones_per_env", C.c_int), ("substeps", C.c_int),
@@ -136,7 +148,8 @@ class QsStepCall(C.Structure):
 EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_state", "qs_sizeof_step_io",
            "qs_sizeof_rollout_io", "qs_sizeof_host_io", "qs_step", "qs_step_call", "qs_step_host", "qs_rollout", "qs_rollout_max_ticks", "qs_dyn_substeps", "qs_dyn_substeps_pub", "qs_pid_control",
            "qs_downwash", "qs_downwash_boxed", "qs_dw_gathered_floats", "qs_dw_boxes", "qs_downwash_rows", "qs_dw_publish", "qs_enable_peer_access", "qs_ipc_export", "qs_ipc_import", "qs_adjacency", "qs_reset", "qs_reset_heads", "qs_host_is_pinned", "qs_log_append", "qs_sizeof_log_ring", "qs_wait_flags", "qs_pid_control_state",
-           "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io", "qs_rollout_mlp", "qs_rollout_mlp_max_ticks", "qs_sizeof_mlp_policy"]
+           "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io", "qs_rollout_mlp", "qs_rollout_mlp_max_ticks", "qs_sizeof_mlp_policy",
+           "qs_mrac_control", "qs_mrac_control_state", "qs_ctrl_rollout_mrac", "qs_sizeof_mrac_params", "qs_sizeof_mrac_rollout_io"]
 MAX_PEERS = 16
 
 
@@ -216,6 +229,17 @@ def lib():
     L.qs_ctrl_rollout.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_uint, C.c_uint, C.c_void_p]
     L.qs_sizeof_ctrl_rollout_io.restype = C.c_int
+    L.qs_ctrl_rollout_mrac.restype = C.c_int
+    L.qs_ctrl_rollout_mrac.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.POINTER(QsMracRolloutIO),
+                                       C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
+    L.qs_mrac_control.restype = C.c_int
+    L.qs_mrac_control.argtypes = [C.POINTER(QsMracParams), C.c_void_p, C.c_int, C.c_double] + [C.c_void_p] * 8 + \
+        [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.qs_mrac_control_state.restype = C.c_int
+    L.qs_mrac_control_state.argtypes = [C.POINTER(QsMracParams), C.c_void_p, C.c_int, C.c_double, C.POINTER(QsState), C.c_int] + \
+        [C.c_void_p] * 8
+    L.qs_sizeof_mrac_params.restype = C.c_int
+    L.qs_sizeof_mrac_rollout_io.restype = C.c_int
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -269,8 +293,9 @@ def lib():
             (C.sizeof(QsParams), C.sizeof(QsState), C.sizeof(QsStepIO), C.sizeof(QsRolloutIO)):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror: rebuild")
     if L.qs_sizeof_log_ring() != C.sizeof(QsLogRing) or L.qs_sizeof_host_io() != C.sizeof(QsHostIO) or \
-            L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy): "
+            L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy) or \
+            L.qs_sizeof_mrac_params() != C.sizeof(QsMracParams) or L.qs_sizeof_mrac_rollout_io() != C.sizeof(QsMracRolloutIO):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac): "
                           "rebuild")
     _lib = L
     return L

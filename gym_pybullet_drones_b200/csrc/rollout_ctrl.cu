@@ -4,6 +4,7 @@
 // is no action history: the state vector rows are written from registers through a small shared-memory stage, so this is a
 // translation unit of its own and leaves every rollout_kernel entry as it was.
 #include "qs_common.cuh"
+#include "mrac_core.cuh"
 
 namespace qsi {
 namespace {
@@ -21,6 +22,20 @@ struct CtrlRolloutArgs {
     unsigned flags;
     int has_log;
 };
+
+// QS_CTRL_MRAC: the controller's constants and state travel with the launch; the other modes keep CtrlRolloutArgs
+struct CtrlMracArgs : CtrlRolloutArgs {
+    QsMracParams M;
+    QsMracRolloutIO mio;
+};
+template <int MODE> struct CtrlArgsOf { using type = CtrlRolloutArgs; };
+template <> struct CtrlArgsOf<QS_CTRL_MRAC> { using type = CtrlMracArgs; };
+
+// MRAC: threads per CTA (each keeps its controller's 76 doubles in shared memory, [76][tpb]: 86 KB per CTA with the row stage)
+// and CTAs per SM.  64-thread CTAs (43 KB, up to 5 per SM) ran as fast within the spread on the H100 (DESIGN.md 4.1e).
+constexpr int kMracTPB = 128;
+constexpr int kMracMinBlocks = 2;
+constexpr size_t mrac_smem(int tpb) { return (size_t)tpb * QS_MRAC_STATE * 8; }
 
 // the state stored back at the end of the rollout: the quaternion is already renormalised (round_to_planes after every tick), so
 // it is stored as it is -- store_drone would renormalise a second time and could move the last bit
@@ -57,8 +72,12 @@ __device__ __forceinline__ void const_target(const double* p, long long i, doubl
 // in the same order, so the rollout gives their bits.
 // 128 registers (4 CTAs of 128 threads per SM): the entries with the controller in the loop spill some of their state at that
 // size, but on the H100 the occupancy pays more than the registers (168 or 255 registers were slower, DESIGN.md 4.1e).
+// QS_CTRL_MRAC: the same loop with mrac_control in place of pid_control; the adaptive state (76 doubles per drone) cannot share the
+// register file with the drone, so it lives in dynamic shared memory as [76][tpb] (consecutive threads, consecutive words), loaded
+// once at the start and stored once at the end.
 template <int EFF, int MODE, bool PHYS>
-__global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_constant__ CtrlRolloutArgs a) {
+__global__ void __launch_bounds__(kCtrlTPB, MODE == QS_CTRL_MRAC ? kMracMinBlocks : 4)
+ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const QsParams& P = a.P;
     const QsCtrlRolloutIO& io = a.io;
@@ -70,6 +89,7 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
     const int rows = (int)((N - c0) < tpb ? (N - c0) : tpb);
     float* row_s = reinterpret_cast<float*>(smem_raw);                               // [tpb][20] state vector rows
     double* pos_s = reinterpret_cast<double*>(row_s + (size_t)tpb * 20);              // [tpb][3] in-CTA downwash
+    double* ms = pos_s + ((EFF & QS_EFFECT_DW) ? (size_t)tpb * 3 : 0);                  // MRAC: [76][tpb] controller state
     const long long e = live ? i / D : 0;
     const int le = t / D;
 
@@ -83,6 +103,9 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
         if ((EFF & QS_EFFECT_DRAG) && a.st.last_rpm) load_rpm(a.st.last_rpm, i, rpm_prev);
         if (MODE == QS_CTRL_VEL) load_pid(a.st.pid, N, i, pst);
         if (MODE == QS_CTRL_TRACK) load_pid(io.pid_state, N, i, pst);
+        if constexpr (MODE == QS_CTRL_MRAC) {
+            for (int q = 0; q < QS_MRAC_STATE; ++q) ms[(size_t)q * tpb + t] = a.mio.state[q * N + i];
+        }
         sc = a.st.step_counter[e];
         if (a.has_log && i >= a.rg.first_drone && i < (long long)a.rg.first_drone + a.rg.n_drones) {
             lj = i - a.rg.first_drone;
@@ -96,6 +119,7 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
         double R_last[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
         qs::PhysRow ph;
         double pe[3] = {0, 0, 0}, ye = 0.0;
+        double re[3] = {0, 0, 0};                                // MRAC: rpy_e
         if (live) {
             if constexpr (MODE == QS_CTRL_RAW) {
                 const double mr = PHYS ? load_phys_rpm(a.st.phys, e).max_rpm : P.max_rpm;
@@ -115,7 +139,7 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
                 qs::quat_to_euler<false>(d.qx, d.qy, d.qz, d.qw, r_, p_, cur_yaw);
                 if constexpr (PHYS) qs::decode_action_k<true>(P, load_phys_rpm(a.st.phys, e), QS_ACT_VEL, act, d, cur_yaw, pst, rpm);
                 else qs::decode_action<true>(P, QS_ACT_VEL, act, d, cur_yaw, pst, rpm);
-            } else {
+            } else if constexpr (MODE == QS_CTRL_TRACK) {
                 // computeControlFromEnv (pid_state_kernel): the controller's constants, its max_rpm clip, then the env's clip
                 double tx, ty, tz, rx, ry, rz, vx, vy, vz, wx, wy, wz;
                 track_target(io, N, i, k, tx, ty, tz);
@@ -127,6 +151,22 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
                 const double mr = PHYS ? load_phys_rpm(a.st.phys, e).max_rpm : P.max_rpm;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) rpm[j] = qs::clampd(qs::clampd(rpm[j], 0.0, a.CP.max_rpm), 0.0, mr);
+            } else {
+                // MRAC.computeControlFromEnv (mrac_kernel on the planes): the tick's targets, ang_v rebuilt from the state, the
+                // controller's max_rpm clip, then the env's
+                double r[12];
+                track_target(io, N, i, k, r[0], r[1], r[2]);
+                const_target(io.target_rpy, i, r[3], r[4], r[5]);
+                const_target(io.target_vel, i, r[6], r[7], r[8]);
+                const_target(io.target_rpy_rates, i, r[9], r[10], r[11]);
+                const double pos[3] = {d.px, d.py, d.pz}, quat[4] = {d.qx, d.qy, d.qz, d.qw}, vel[3] = {d.vx, d.vy, d.vz};
+                double av[3];
+                qs::mrac_ang_v(d, av);
+                const qs::MracState S = {ms + t, tpb};
+                qs::mrac_control(a.M, S, k == 0 && a.mio.init != 0, io.control_timestep, pos, quat, vel, av, r, rpm, pe, re);
+                const double mr = PHYS ? load_phys_rpm(a.st.phys, e).max_rpm : P.max_rpm;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) rpm[j] = qs::clampd(qs::clampd(rpm[j], 0.0, a.M.max_rpm), 0.0, mr);
             }
             if constexpr (PHYS && !(EFF & QS_EFFECT_DW)) ph = load_phys(a.st.phys, e);       // after the controller
         }
@@ -173,6 +213,10 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
                 if (io.pos_e) { float* pp = io.pos_e + 3 * ki; pp[0] = (float)pe[0]; pp[1] = (float)pe[1]; pp[2] = (float)pe[2]; }
                 if (io.yaw_e) io.yaw_e[ki] = (float)ye;
             }
+            if constexpr (MODE == QS_CTRL_MRAC) {
+                if (io.pos_e) { float* pp = io.pos_e + 3 * ki; pp[0] = (float)pe[0]; pp[1] = (float)pe[1]; pp[2] = (float)pe[2]; }
+                if (a.mio.rpy_e) { float* pp = a.mio.rpy_e + 3 * ki; pp[0] = (float)re[0]; pp[1] = (float)re[1]; pp[2] = (float)re[2]; }
+            }
             // _getDroneStateVector (BaseAviary.py:541-561), the row of qs_dyn_substeps: quaternion normalised, ang_v of the last substep
             float h[20];
             h[0] = (float)d.px; h[1] = (float)d.py; h[2] = (float)d.pz;
@@ -197,7 +241,7 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
                 ow[9] = h[13]; ow[10] = h[14]; ow[11] = h[15];
                 const bool lr = a.st.last_rpm != nullptr;
                 ow[12] = lr ? rpm[0] : 0.0; ow[13] = lr ? rpm[1] : 0.0; ow[14] = lr ? rpm[2] : 0.0; ow[15] = lr ? rpm[3] : 0.0;
-                if (MODE == QS_CTRL_TRACK && io.log_targets) {
+                if ((MODE == QS_CTRL_TRACK || MODE == QS_CTRL_MRAC) && io.log_targets) {
                     // pid.py's controls: the tick's targets (target_pos, target_rpy, target_vel, target_rpy_rates), as float32
                     double c[12];
                     track_target(io, N, i, k, c[0], c[1], c[2]);
@@ -232,6 +276,9 @@ __global__ void __launch_bounds__(kCtrlTPB, 4) ctrl_rollout_kernel(const __grid_
         if (a.st.last_rpm) st256(a.st.last_rpm, i, rpm[0], rpm[1], rpm[2], rpm[3]);
         if (MODE == QS_CTRL_VEL) store_pid(a.st.pid, N, i, pst);
         if (MODE == QS_CTRL_TRACK) store_pid(io.pid_state, N, i, pst);
+        if constexpr (MODE == QS_CTRL_MRAC) {
+            for (int q = 0; q < QS_MRAC_STATE; ++q) a.mio.state[q * N + i] = ms[(size_t)q * tpb + t];
+        }
         if (i - e * D == 0) a.st.step_counter[e] = sc;
     }
 }
@@ -242,7 +289,13 @@ template <int EFF, bool PHYS>
 void launch_eff(const CtrlRolloutArgs& a, int mode, int blocks, int threads, size_t sm, cudaStream_t s) {
     if (mode == QS_CTRL_RAW) ctrl_rollout_kernel<EFF, QS_CTRL_RAW, PHYS><<<blocks, threads, sm, s>>>(a);
     else if (mode == QS_CTRL_VEL) ctrl_rollout_kernel<EFF, QS_CTRL_VEL, PHYS><<<blocks, threads, sm, s>>>(a);
-    else ctrl_rollout_kernel<EFF, QS_CTRL_TRACK, PHYS><<<blocks, threads, sm, s>>>(a);
+    else if (mode == QS_CTRL_TRACK) ctrl_rollout_kernel<EFF, QS_CTRL_TRACK, PHYS><<<blocks, threads, sm, s>>>(a);
+    else {
+        // more than the default 48 KB of dynamic shared memory; the launch reports a failure of the attribute call
+        void (*k)(CtrlMracArgs) = ctrl_rollout_kernel<EFF, QS_CTRL_MRAC, PHYS>;
+        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm) == cudaSuccess)
+            k<<<blocks, threads, sm, s>>>(static_cast<const CtrlMracArgs&>(a));
+    }
 }
 
 template <bool PHYS>
@@ -265,13 +318,18 @@ extern "C" {
 
 int qs_sizeof_ctrl_rollout_io(void) { return (int)sizeof(QsCtrlRolloutIO); }
 
-int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, int mode, int n_envs, int drones_per_env,
-                    int substeps, unsigned effects, unsigned flags, void* stream) {
+}  // extern "C"
+
+namespace {
+// qs_ctrl_rollout (mio == NULL) and qs_ctrl_rollout_mrac (mode QS_CTRL_MRAC, mio != NULL)
+int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int mode, int n_envs,
+                 int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
     if (!p || !io) return fail(QS_ERR_NULL, "qs_ctrl_rollout: NULL params/io");
     if (int rc = check_state(st, 0)) return rc;
     if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: n_envs, drones_per_env, substeps and T must be > 0");
     if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: n_envs * drones_per_env exceeds 2^31-1");
-    if (mode != QS_CTRL_RAW && mode != QS_CTRL_VEL && mode != QS_CTRL_TRACK) return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad mode (QS_CTRL_RAW, QS_CTRL_VEL or QS_CTRL_TRACK)");
+    if (mio ? mode != QS_CTRL_MRAC : (mode != QS_CTRL_RAW && mode != QS_CTRL_VEL && mode != QS_CTRL_TRACK))
+        return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad mode (QS_CTRL_RAW, QS_CTRL_VEL or QS_CTRL_TRACK; QS_CTRL_MRAC is qs_ctrl_rollout_mrac)");
     if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad effects");
     const unsigned eff = effects & 7u;
     if (eff != 0 && eff != QS_EFFECT_GND && eff != QS_EFFECT_DRAG && eff != QS_EFFECT_DW && eff != 7u)
@@ -283,9 +341,14 @@ int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO*
     const bool f64 = flags & QS_FLAG_ACTION_F64;
     if (f64 && mode != QS_CTRL_RAW) return fail(QS_ERR_UNSUPPORTED, "qs_ctrl_rollout: QS_FLAG_ACTION_F64 is for QS_CTRL_RAW actions");
     if ((eff & QS_EFFECT_DRAG) && !st->last_rpm) return fail(QS_ERR_NULL, "qs_ctrl_rollout: DRAG needs QsState.last_rpm");
-    if (mode == QS_CTRL_TRACK) {
-        if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_ctrl_rollout: QS_CTRL_TRACK takes a controller, not actions");
-        if (!io->ctrl_params || !io->pid_state) return fail(QS_ERR_NULL, "qs_ctrl_rollout: QS_CTRL_TRACK needs a controller (ctrl_params, pid_state)");
+    if (mode == QS_CTRL_TRACK || mode == QS_CTRL_MRAC) {
+        if (io->actions)
+            return fail(QS_ERR_UNSUPPORTED, mode == QS_CTRL_TRACK ? "qs_ctrl_rollout: QS_CTRL_TRACK takes a controller, not actions"
+                                                                  : "qs_ctrl_rollout_mrac: takes a controller, not actions");
+        if (mode == QS_CTRL_TRACK && (!io->ctrl_params || !io->pid_state))
+            return fail(QS_ERR_NULL, "qs_ctrl_rollout: QS_CTRL_TRACK needs a controller (ctrl_params, pid_state)");
+        if (mode == QS_CTRL_MRAC && (!mio->params || !mio->state))
+            return fail(QS_ERR_NULL, "qs_ctrl_rollout_mrac: needs a controller (params, state)");
         if (!io->waypoints || !io->start) return fail(QS_ERR_NULL, "qs_ctrl_rollout: QS_CTRL_TRACK needs waypoints and start");
         if (io->W <= 0) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: W (waypoint rows) must be > 0");
         if (io->M != 1 && (long long)io->M != (long long)n_envs * drones_per_env) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: M (waypoint columns) must be 1 or N");
@@ -299,16 +362,20 @@ int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO*
     if (io->rpm && !aligned32(io->rpm)) return fail(QS_ERR_ALIGN, "qs_ctrl_rollout: rpm must be 32-byte aligned");
     if ((io->obs && !aligned16(io->obs)) || (io->obs_last && !aligned16(io->obs_last)))
         return fail(QS_ERR_ALIGN, "qs_ctrl_rollout: obs / obs_last must be 16-byte aligned");
-    CtrlRolloutArgs a;
-    memset(&a, 0, sizeof(a));
+    CtrlRolloutArgs a0;
+    memset(&a0, 0, sizeof(a0));
     if (io->log) {
         const QsLogRing& r = *io->log;
         if (!r.ring || !r.head) return fail(QS_ERR_NULL, "qs_ctrl_rollout: NULL log ring");
         if (r.capacity <= 0 || r.n_drones <= 0 || r.first_drone < 0 || (long long)r.first_drone + r.n_drones > (long long)n_envs * drones_per_env)
             return fail(QS_ERR_SIZE, "qs_ctrl_rollout: bad log ring geometry");
-        a.rg = r;
-        a.has_log = 1;
+        a0.rg = r;
+        a0.has_log = 1;
     }
+    CtrlMracArgs ma;                         // MRAC: the derived arguments, of which `a` is the base
+    CtrlRolloutArgs& a = mio ? static_cast<CtrlRolloutArgs&>(ma) : a0;
+    memset(&ma, 0, sizeof(ma));
+    if (mio) { a = a0; ma.M = *mio->params; ma.mio = *mio; }
     a.P = *p;
     if (mode == QS_CTRL_TRACK) a.CP = *io->ctrl_params;
     a.st = *st; a.io = *io;
@@ -317,9 +384,12 @@ int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO*
     // in-CTA downwash: whole aviaries per CTA; otherwise any 128 consecutive drones (one-warp CTAs for downwash, as the step kernels
     // use up to 32 drones per aviary, measured slower on the H100: DESIGN.md 4.1e)
     a.tpb = (eff & QS_EFFECT_DW) ? block_size_for(drones_per_env, kCtrlTPB) : kCtrlTPB;
+    if (mode == QS_CTRL_MRAC)                 // whole aviaries per CTA still, for downwash aviaries larger than kMracTPB too
+        a.tpb = (eff & QS_EFFECT_DW) ? block_size_for(drones_per_env, drones_per_env > kMracTPB ? kCtrlTPB : kMracTPB) : kMracTPB;
     const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
     const int threads = ((a.tpb + 31) / 32) * 32;
-    const size_t sm = (size_t)a.tpb * 20 * 4 + ((eff & QS_EFFECT_DW) ? (size_t)a.tpb * 3 * 8 : 0);
+    size_t sm = (size_t)a.tpb * 20 * 4 + ((eff & QS_EFFECT_DW) ? (size_t)a.tpb * 3 * 8 : 0);
+    if (mode == QS_CTRL_MRAC) sm += mrac_smem(a.tpb);
     cudaStream_t s = (cudaStream_t)stream;
     if (st->phys) launch_ctrl<true>(a, mode, eff, blocks, threads, sm, s);
     else launch_ctrl<false>(a, mode, eff, blocks, threads, sm, s);
@@ -329,6 +399,22 @@ int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO*
         e = cudaGetLastError();
     }
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_ctrl_rollout launch");
+}
+}  // namespace
+
+extern "C" {
+
+int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, int mode, int n_envs, int drones_per_env,
+                    int substeps, unsigned effects, unsigned flags, void* stream) {
+    return ctrl_rollout(p, st, io, nullptr, mode, n_envs, drones_per_env, substeps, effects, flags, stream);
+}
+
+int qs_sizeof_mrac_rollout_io(void) { return (int)sizeof(QsMracRolloutIO); }
+
+int qs_ctrl_rollout_mrac(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int n_envs,
+                         int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
+    if (!mio) return fail(QS_ERR_NULL, "qs_ctrl_rollout_mrac: NULL mio");
+    return ctrl_rollout(p, st, io, mio, QS_CTRL_MRAC, n_envs, drones_per_env, substeps, effects, flags, stream);
 }
 
 }  // extern "C"

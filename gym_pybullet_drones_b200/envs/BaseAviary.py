@@ -632,7 +632,7 @@ class BaseAviary(Env):
                       target_rpy=None, target_vel=None, target_rpy_rates=None, control_timestep=None, record=True, errors=False,
                       out=None, log_targets=False):
         """rollout() of the state-vector envs (CtrlAviary, VelocityAviary): one qs_ctrl_rollout launch of T ticks in `mode`
-        (N.CTRL_RAW / CTRL_VEL / CTRL_TRACK); see CtrlAviary.rollout."""
+        (N.CTRL_RAW / CTRL_VEL / CTRL_TRACK), or of qs_ctrl_rollout_mrac (N.CTRL_MRAC); see CtrlAviary.rollout."""
         if not self.VECTORIZED:
             raise ValueError("rollout() needs the vector API (num_envs=...)")
         if self._py_hooks:
@@ -656,13 +656,14 @@ class BaseAviary(Env):
             t = t.reshape(n, 3).contiguous()
             keep.append(t)
             return t.data_ptr()
-        if mode == N.CTRL_TRACK:
+        mio = None
+        if mode in (N.CTRL_TRACK, N.CTRL_MRAC):
             if actions is not None:
                 raise ValueError("pass either actions or a controller")
             if controller is None:
                 raise ValueError("rollout() needs actions [T, E, D, 4] or a controller")
             if getattr(controller, "num_drones", None) != n or not hasattr(controller, "_state"):
-                raise ValueError("the controller must be a DSLPIDControl for the env's %d drones (num_drones=%d)" % (n, n))
+                raise ValueError("the controller must be a DSLPIDControl or an MRAC for the env's %d drones (num_drones=%d)" % (n, n))
             if torch.device(controller.device) != dev:
                 raise ValueError("the controller's state is on %s, the env's on %s" % (controller.device, dev))
             if waypoints is None:
@@ -685,8 +686,13 @@ class BaseAviary(Env):
                 st0 = st0.to(device=dev, dtype=torch.int32)
                 st0 = (st0.reshape(1).expand(n) if st0.numel() == 1 else st0.reshape(n)).contiguous()
             keep += [wp, st0]
-            io.ctrl_params = C.addressof(controller._P)
-            io.pid_state = controller._state.data_ptr()
+            if mode == N.CTRL_TRACK:
+                io.ctrl_params = C.addressof(controller._P)
+                io.pid_state = controller._state.data_ptr()
+            else:
+                mio = N.QsMracRolloutIO()
+                mio.params, mio.state = C.addressof(controller._P), controller._state.data_ptr()
+                mio.init = 1 if controller.control_counter == 0 else 0          # MRAC.py:123-124, at tick 0
             io.control_timestep = float(self.CTRL_TIMESTEP if control_timestep is None else control_timestep)
             io.waypoints, io.W, io.M, io.start = wp.data_ptr(), W, M, st0.data_ptr()
             io.offset = rows3(offset, "offset")
@@ -716,7 +722,11 @@ class BaseAviary(Env):
             raise ValueError("num_steps must be > 0")
         shapes = dict(obs=((T, E, D, 20), torch.float32), rpm=((T, E, D, 4), torch.float64))
         if errors:
-            shapes.update(pos_e=((T, E, D, 3), torch.float32), yaw_e=((T, E, D), torch.float32))
+            shapes.update(pos_e=((T, E, D, 3), torch.float32))
+            if mode == N.CTRL_MRAC:
+                shapes.update(rpy_e=((T, E, D, 3), torch.float32))
+            else:
+                shapes.update(yaw_e=((T, E, D), torch.float32))
         if not record:
             del shapes["obs"]
         res = {}
@@ -730,6 +740,8 @@ class BaseAviary(Env):
         ptr = lambda k: res[k].data_ptr() if k in res else None      # noqa: E731
         io.T = T
         io.obs, io.rpm, io.pos_e, io.yaw_e = ptr("obs"), ptr("rpm"), ptr("pos_e"), ptr("yaw_e")
+        if mio is not None:
+            mio.rpy_e = ptr("rpy_e")
         tgt = self._cur ^ (T & 1)                          # the buffer T step() calls would leave current
         io.obs_last = self._obs_ptr[tgt]
         if self._log is not None:
@@ -738,9 +750,13 @@ class BaseAviary(Env):
             io.log_controls = controls.data_ptr() if controls is not None else None
         with self._on_device():
             self._reward.fill_(-1.0)                       # dummy task (CtrlAviary.py:144-185)
-            rc = self._lib.qs_ctrl_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), mode, E, D, self.PYB_STEPS_PER_CTRL,
-                                           self._effects, flags, self._stream())
-        N.check(rc, "qs_ctrl_rollout")
+            if mio is not None:
+                rc = self._lib.qs_ctrl_rollout_mrac(C.byref(self._P), C.byref(self._st), C.byref(io), C.byref(mio), E, D,
+                                                    self.PYB_STEPS_PER_CTRL, self._effects, flags, self._stream())
+            else:
+                rc = self._lib.qs_ctrl_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), mode, E, D, self.PYB_STEPS_PER_CTRL,
+                                               self._effects, flags, self._stream())
+        N.check(rc, "qs_ctrl_rollout" if mio is None else "qs_ctrl_rollout_mrac")
         self._cur = tgt
         if controller is not None:
             controller.control_counter += T

@@ -71,10 +71,17 @@ class CtrlAviary(BaseAviary):
         Afterwards the env is exactly where T step() calls leave it: state, last_clipped_action, step counters, current
         observation, reward -1 and an attached Logger (one entry per tick; `log_targets=True` logs the tick's targets as the
         controls, pid.py's layout, instead of the Logger's current controls).
+        * `controller`: an `MRAC(num_drones=E*D)` on the env's device, with the same schedule arguments: tick k runs
+          `rpm = controller.computeControlFromEnv(env, target_pos, ...)` and `step(rpm)`, bit for bit; tick 0 initialises the
+          reference model Xm when `controller.control_counter` is 0.  With `errors=True` the result holds `pos_e` and `rpy_e`
+          [T, E, D, 3] (float32) instead of `yaw_e`.
+
         What the kernel refuses (downwash with more than 128 drones per aviary, a controller of the wrong size or device, both
-        actions and a controller, the single-env API) raises ValueError."""
+        actions and a controller, the single-env API, external downwash) raises ValueError."""
         if controller is not None or actions is None:
-            return self._ctrl_rollout(N.CTRL_TRACK, actions=actions, controller=controller, num_steps=num_steps, waypoints=waypoints,
+            from ..control.MRAC import MRAC
+            mode = N.CTRL_MRAC if isinstance(controller, MRAC) else N.CTRL_TRACK
+            return self._ctrl_rollout(mode, actions=actions, controller=controller, num_steps=num_steps, waypoints=waypoints,
                                       start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
                                       target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, record=record,
                                       errors=errors, out=out, log_targets=log_targets)

@@ -547,6 +547,64 @@ int qs_sizeof_ctrl_rollout_io(void);
 int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, int mode, int n_envs, int drones_per_env,
                     int substeps, unsigned effects, unsigned flags, void* stream);
 
+/* MRAC (control/MRAC.py): the model reference adaptive controller, float64, one controller per drone.
+ * QsMracParams holds the per-model constants the gains were synthesised into (MRAC._compute_K with psi = 0, on the host):
+ * Am = A - B K, the diagonal of the nonzero block Bm[8:12][0:4], P Bm with P = solve_lyapunov(Am^T, -600 I), Kr_ref_gain =
+ * pinv(B) Am, the adaptation rates Gamma_x = gamma_x I and Gamma_r = gamma_r I, the mixer and the PWM constants.
+ * The adaptive state of N controllers is double[QS_MRAC_STATE][N]: rows 0-47 Kx[12][4] (row-major), 48-63 Kr[4][4], 64-75 Xm[12].
+ * `init` != 0 is the reference's control_counter == 0: the call first sets Xm to the current state X.
+ * One call per drone (MRAC.computeControl, MRAC.py:109-155):
+ *   rpy = getEulerFromQuaternion(q); w_b = R_XYZ(rpy)^T cur_ang_vel (scipy's intrinsic 'XYZ' on Bullet's rpy, as the reference);
+ *   X = [pos, rpy, vel, w_b]; rt = -Kr_ref_gain [tpos, trpy, tvel, trates]; u = Kx^T X + Kr^T rt; e = X - Xm;
+ *   Kx += dt (-gamma_x X e^T P Bm); Kr += dt (-gamma_r rt e^T P Bm); thrust = max(0, u0); tau = clip(u1..3, +-3200);
+ *   rpm = 0.2685 clip((sqrt(thrust / 4 KF) - 4070.3) / 0.2685 + MIX tau, 20000, 65535) + 4070.3; pos_e = tpos - pos;
+ *   rpy_e = trpy - rpy; Xm += dt (Am Xm + Bm rt). */
+#define QS_MRAC_STATE 76
+typedef struct QsMracParams {
+    double Am[12][12];
+    double bm[4];                   /* Bm[8 + j][j]; every other entry of Bm is 0 */
+    double PBm[12][4];              /* P Bm */
+    double Kr_ref[4][12];           /* Kr_ref_gain */
+    double gamma_x, gamma_r;
+    double mixer[4][3];
+    double kf, pwm2rpm_scale, pwm2rpm_const, min_pwm, max_pwm;
+    double max_rpm;                 /* qs_mrac_control_state and the rollout clip the RPMs to [0, max_rpm] (CtrlAviary.py:140) */
+} QsMracParams;
+int qs_sizeof_mrac_params(void);
+
+/* MRAC.computeControl for n drones: cur_pos / cur_vel / cur_ang_vel / target_* are float64 [n][3], cur_quat float64 [n][4]
+ * (target_rpy / target_vel / target_rpy_rates nullable = zeros).  rpm_out: float64 [n][4], the reference's unclipped RPMs;
+ * pos_e_out / rpy_e_out: float32 [n][3], nullable. */
+int qs_mrac_control(const QsMracParams* p, double* mrac_state, int init, double control_timestep,
+                    const double* cur_pos, const double* cur_quat, const double* cur_vel, const double* cur_ang_vel,
+                    const double* target_pos, const double* target_rpy, const double* target_vel, const double* target_rpy_rates,
+                    int n, double* rpm_out, float* pos_e_out, float* rpy_e_out, void* stream);
+
+/* The same controller for the n drones of a simulator state, as qs_pid_control_state: pos / quat / vel / rates from the float64
+ * planes, cur_ang_vel = getMatrixFromQuaternion(q) w (the state vector's ang_v, BaseAviary.py:873, rebuilt in float64: the
+ * quaternion increment is body-frame, so R_old w = R_new w), RPMs clipped to [0, max_rpm] into rpm_out (float64 [n][4], 32-byte
+ * aligned), e.g. the env's float64 command buffer. */
+int qs_mrac_control_state(const QsMracParams* p, double* mrac_state, int init, double control_timestep, const QsState* st, int n,
+                          const double* target_pos, const double* target_rpy, const double* target_vel, const double* target_rpy_rates,
+                          double* rpm_out, float* pos_e_out, float* rpy_e_out, void* stream);
+
+/* qs_ctrl_rollout with an MRAC in the loop (mode QS_CTRL_MRAC): per tick qs_mrac_control_state on the tick's targets (the TRACK
+ * schedule of QsCtrlRolloutIO: waypoints, start, offset, target_rpy, target_vel, target_rpy_rates, control_timestep), then
+ * qs_dyn_substeps(QS_FLAG_ACTION_F64) on those RPMs; tick 0 initialises Xm iff mio->init.  QsCtrlRolloutIO.ctrl_params,
+ * pid_state and yaw_e are not used; its obs, rpm, pos_e, obs_last and log outputs are written as for QS_CTRL_TRACK.
+ * Each thread keeps its controller's 76 doubles in shared memory for the whole launch. */
+enum { QS_CTRL_MRAC = 3 };
+typedef struct QsMracRolloutIO {
+    const QsMracParams* params;     /* HOST pointer */
+    double* state;                  /* [QS_MRAC_STATE][N] (read at the start, stored at the end) */
+    int init;                       /* 1: tick 0 sets Xm = X (the controller's control_counter is 0) */
+    int pad_;
+    float* rpy_e;                   /* out [T][N][3], nullable */
+} QsMracRolloutIO;
+int qs_sizeof_mrac_rollout_io(void);
+int qs_ctrl_rollout_mrac(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int n_envs,
+                         int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
