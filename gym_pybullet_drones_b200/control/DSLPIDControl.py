@@ -88,26 +88,38 @@ class DSLPIDControl(BaseControl):
         """computeControl for every drone of `env` (num_drones == env's drone count), reading pos / quat / vel from the env's
         float64 state on the device (qs_pid_control_state) and returning float64 RPMs [n, 4] in the env's float64
         command buffer: `env.step(rpm)` with that tensor applies them without a copy or a float32 rounding
-        -- the pid.py loop (examples/pid.py:131-150) in float64 end to end.  Targets: [n, 3] arrays / tensors (float64)."""
+        -- the pid.py loop (examples/pid.py:131-150) in float64 end to end.  Targets: [n, 3] arrays / tensors (float64).
+        Targets, RPMs and the controller state are indexed by drone id, also after `env.reorder_by_morton()`."""
         n = env._N
         if n != self.num_drones:
             raise ValueError("controller for %d drones used with an env of %d" % (self.num_drones, n))
         self.control_counter += 1
         dev = self.device
+        order = env._order                       # reorder_by_morton(): the kernel pairs env storage slot i with row / column i
 
         def t64(x):
             if x is None:
                 return None
             t = x if isinstance(x, torch.Tensor) else torch.as_tensor(np.asarray(x, dtype=np.float64))
-            return t.to(device=dev, dtype=torch.float64).reshape(n, 3).contiguous()
+            t = t.to(device=dev, dtype=torch.float64).reshape(n, 3)
+            return t.contiguous() if order is None else t[order]
         tp, tr, tv, trr = t64(target_pos), t64(target_rpy), t64(target_vel), t64(target_rpy_rates)
         ptr = lambda t: None if t is None else t.data_ptr()      # noqa: E731
         dt = float(env.CTRL_TIMESTEP if control_timestep is None else control_timestep)
         with torch.cuda.device(dev):
-            rc = self._lib.qs_pid_control_state(C.byref(self._P), self._state.data_ptr(), dt, C.byref(env._st), n,
-                                                ptr(tp), ptr(tr), ptr(tv), ptr(trr), env._rpm_cmd.data_ptr(),
-                                                self._pos_e.data_ptr(), self._yaw_e.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        N.check(rc, "qs_pid_control_state")
+            if order is None:
+                state, rpm, pos_e, yaw_e = self._state, env._rpm_cmd, self._pos_e, self._yaw_e
+            else:                                # run in storage order, then scatter back to drone ids
+                state, rpm = self._state[:, order], torch.empty_like(env._rpm_cmd)
+                pos_e, yaw_e = torch.empty_like(self._pos_e), torch.empty_like(self._yaw_e)
+            rc = self._lib.qs_pid_control_state(C.byref(self._P), state.data_ptr(), dt, C.byref(env._st), n,
+                                                ptr(tp), ptr(tr), ptr(tv), ptr(trr), rpm.data_ptr(),
+                                                pos_e.data_ptr(), yaw_e.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+            N.check(rc, "qs_pid_control_state")
+            if order is not None:
+                self._state[:, order] = state
+                env._rpm_cmd[order] = rpm
+                self._pos_e[order], self._yaw_e[order] = pos_e, yaw_e
         return env._rpm_cmd.view(env._E, env._D, 4) if env.VECTORIZED else env._rpm_cmd
 
     def computeControl(self, control_timestep, cur_pos, cur_quat, cur_vel, cur_ang_vel, target_pos,

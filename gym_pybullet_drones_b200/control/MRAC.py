@@ -124,7 +124,8 @@ class MRAC(BaseControl):
         """computeControl for every drone of `env` (num_drones == env's drone count), reading pos / quat / vel / ang_v from the env's
         float64 state on the device (qs_mrac_control_state) and returning float64 RPMs [n, 4] in the env's float64 command buffer:
         `env.step(rpm)` with that tensor applies them without a copy -- the mrac.py loop in float64 end to end.  Targets: [n, 3]
-        arrays / tensors (float64).  The position and rpy errors of the call are in `last_pos_e` / `last_rpy_e`."""
+        arrays / tensors (float64).  The position and rpy errors of the call are in `last_pos_e` / `last_rpy_e`.  Targets, RPMs,
+        errors and the adaptive state are indexed by drone id, also after `env.reorder_by_morton()`."""
         n = env._N
         if n != self.num_drones:
             raise ValueError("controller for %d drones used with an env of %d" % (self.num_drones, n))
@@ -132,15 +133,27 @@ class MRAC(BaseControl):
             raise ValueError("computeControlFromEnv needs an env with raw RPM actions (CtrlAviary)")
         if torch.device(env.device) != self.device:
             raise ValueError("the controller's state is on %s, the env's on %s" % (self.device, env.device))
+        order = env._order                       # reorder_by_morton(): the kernel pairs env storage slot i with row / column i
         tp, tr, tv, trr = (self._dev(x, 3) for x in (target_pos, target_rpy, target_vel, target_rpy_rates))
+        if order is not None:
+            tp, tr, tv, trr = (None if t is None else t[order] for t in (tp, tr, tv, trr))
         ptr = lambda t: None if t is None else t.data_ptr()      # noqa: E731
         dt = float(env.CTRL_TIMESTEP if control_timestep is None else control_timestep)
         init = self._init_flag()
         with torch.cuda.device(self.device):
-            rc = self._lib.qs_mrac_control_state(C.byref(self._P), self._state.data_ptr(), init, dt, C.byref(env._st), n,
-                                                 ptr(tp), ptr(tr), ptr(tv), ptr(trr), env._rpm_cmd.data_ptr(),
-                                                 self._pos_e.data_ptr(), self._rpy_e.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
-        N.check(rc, "qs_mrac_control_state")
+            if order is None:
+                state, rpm, pos_e, rpy_e = self._state, env._rpm_cmd, self._pos_e, self._rpy_e
+            else:                                # run in storage order, then scatter back to drone ids
+                state, rpm = self._state[:, order], torch.empty_like(env._rpm_cmd)
+                pos_e, rpy_e = torch.empty_like(self._pos_e), torch.empty_like(self._rpy_e)
+            rc = self._lib.qs_mrac_control_state(C.byref(self._P), state.data_ptr(), init, dt, C.byref(env._st), n,
+                                                 ptr(tp), ptr(tr), ptr(tv), ptr(trr), rpm.data_ptr(),
+                                                 pos_e.data_ptr(), rpy_e.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+            N.check(rc, "qs_mrac_control_state")
+            if order is not None:
+                self._state[:, order] = state
+                env._rpm_cmd[order] = rpm
+                self._pos_e[order], self._rpy_e[order] = pos_e, rpy_e
         return env._rpm_cmd.view(env._E, env._D, 4) if env.VECTORIZED else env._rpm_cmd
 
     @property

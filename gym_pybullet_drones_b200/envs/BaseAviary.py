@@ -406,23 +406,32 @@ class BaseAviary(Env):
         return self._h_action_view
 
     ################################################################################
-    # state views (float32 CUDA tensors; names follow BaseAviary.py:470-476)
+    # state views (float64 CUDA tensors; names follow BaseAviary.py:470-476).  Vector API: views of the state planes, except
+    # after reorder_by_morton(), where they are copies gathered into drone-id order.
+
+    def _by_id(self, t):
+        """Per-drone rows [N, ...] of the storage order in drone-id order: `t` itself unless reorder_by_morton() has permuted
+        the storage (then a gathered copy)."""
+        return t if self._inv is None else t[self._inv]
 
     @property
     def pos(self):
-        return self._plane[0, :, 0:3].view(self._E, self._D, 3) if self.VECTORIZED else self._host(self._plane[0, :, 0:3])
+        p = self._by_id(self._plane[0, :, 0:3])
+        return p.view(self._E, self._D, 3) if self.VECTORIZED else self._host(p)
 
     @property
     def quat(self):
-        return self._plane[1].view(self._E, self._D, 4) if self.VECTORIZED else self._host(self._plane[1])
+        q = self._by_id(self._plane[1])
+        return q.view(self._E, self._D, 4) if self.VECTORIZED else self._host(q)
 
     @property
     def vel(self):
-        return self._plane[2, :, 0:3].view(self._E, self._D, 3) if self.VECTORIZED else self._host(self._plane[2, :, 0:3])
+        v = self._by_id(self._plane[2, :, 0:3])
+        return v.view(self._E, self._D, 3) if self.VECTORIZED else self._host(v)
 
     @property
     def rpy_rates(self):
-        w = torch.stack([self._plane[0, :, 3], self._plane[2, :, 3], self._wz], dim=1)
+        w = self._by_id(torch.stack([self._plane[0, :, 3], self._plane[2, :, 3], self._wz], dim=1))
         return w.view(self._E, self._D, 3) if self.VECTORIZED else w.cpu().numpy()
 
     @property
@@ -433,7 +442,8 @@ class BaseAviary(Env):
     def last_clipped_action(self):
         if not self._track_last_action:
             raise AttributeError("last_clipped_action is not tracked by this env (pass track_last_action=True)")
-        return self._last_rpm.view(self._E, self._D, 4) if self.VECTORIZED else self._host(self._last_rpm)
+        r = self._by_id(self._last_rpm)
+        return r.view(self._E, self._D, 4) if self.VECTORIZED else self._host(r)
 
     @staticmethod
     def _host(t):
@@ -441,15 +451,20 @@ class BaseAviary(Env):
 
     @property
     def pid_state(self):
-        """[9, E*D] float64 CUDA tensor of the embedded controllers (integral_pos_e, last_rpy, integral_rpy_e) or None."""
-        return self._pid
+        """[9, E*D] float64 CUDA tensor of the embedded controllers (integral_pos_e, last_rpy, integral_rpy_e) or None.  The
+        controllers' own state, columns in drone-id order; after reorder_by_morton() a gathered copy."""
+        if self._pid is None or self._inv is None:
+            return self._pid
+        return self._pid[:, self._inv]
 
     def set_state(self, pos=None, quat=None, vel=None, rpy_rates=None, step_counter=None):
-        """Overwrites (parts of) the kinematic state; arrays are [E,D,k] / [D,k] (stored as float64)."""
+        """Overwrites (parts of) the kinematic state; arrays are [E,D,k] / [D,k] in drone-id order (stored as float64)."""
         def dev(a, k):
             if isinstance(a, torch.Tensor):
-                return a.to(device=self.device, dtype=torch.float64).reshape(self._N, k)
-            return torch.as_tensor(np.asarray(a, dtype=np.float64).reshape(self._N, k), device=self.device)
+                t = a.to(device=self.device, dtype=torch.float64).reshape(self._N, k)
+            else:
+                t = torch.as_tensor(np.asarray(a, dtype=np.float64).reshape(self._N, k), device=self.device)
+            return t if self._order is None else t[self._order]          # storage slot i holds drone _order[i]
         if pos is not None:
             self._plane[0, :, 0:3] = dev(pos, 3)
             if self._pos_f32 is not None:
@@ -794,13 +809,24 @@ class BaseAviary(Env):
         """Re-bins a large formation on the device (SURVEY.md 8f rank 3; BaseAviary.py:785-811): the downwash kernels skip
         32-drone chunks whose bounding boxes cannot interact, which only pays while consecutive indices are neighbours in
         space.  This sorts the STORAGE order of the drones along a Z-order curve of their current xy positions (keys, sort and
-        the permutation of every per-drone buffer run on the GPU); actions and observations keep the caller's drone ids
-        (`step` gathers / scatters through the permutation).  Call it every K ticks for formations that mix.
-        One aviary per env (num_envs == 1), unsharded."""
+        the permutation of every per-drone buffer run on the GPU).  Call it every K ticks for formations that mix.
+        One aviary per env (num_envs == 1), unsharded.
+
+        Everything a caller passes or receives keeps the caller's drone ids: the actions and float64 RPMs of `step` (NumPy or
+        torch, vector or single-env API), its observations and `info["final_obs"]`, `reset`, `set_state`, the state views
+        (`pos`, `quat`, `vel`, `rpy_rates`, `last_clipped_action`, `pid_state`: copies gathered into drone-id order rather
+        than views once the env is reordered), `_getDroneStateVectors` / `_getDroneStateVector` / `render`, `adjacency` /
+        `_getAdjacencyMatrix`, and the targets, controller state and RPMs of `DSLPIDControl` / `MRAC.computeControlFromEnv`.
+        The device-side Logger ring records storage slots, so a Logger cannot be attached to a reordered env and a reorder
+        is refused while one is attached (ValueError); `Logger.detach()` first.  Returns the permutation (storage slot i
+        holds drone `order[i]`)."""
         if self._E != 1 or self._dw_fz is None:
             raise ValueError("reorder_by_morton() is for one large aviary with external downwash (num_drones > 128, num_envs == 1)")
         if getattr(self, "shard", None) is not None and self.shard.world > 1:
             raise ValueError("reorder_by_morton() does not move drones between GPUs")
+        if self._log is not None:
+            raise ValueError("reorder_by_morton() with a Logger attached: the device ring records storage slots, which the "
+                             "reorder would mix between two entries; detach() the Logger first")
         n = self._N
         with self._on_device():
             xy = self._plane[0, :, 0:2]
@@ -817,7 +843,8 @@ class BaseAviary(Env):
             perm = torch.argsort(spread(q[:, 0]) | (spread(q[:, 1]) << 1), stable=True)      # new slot i <- old slot perm[i]
             self._plane.copy_(self._plane[:, perm].clone())
             self._wz.copy_(self._wz[perm].clone())
-            for t in (self._last_rpm, self._pos_f32, self._obs_buf[0], self._obs_buf[1], self._dw_fz, self._rpm_cmd):
+            # (_rpm_cmd and _action_dev are not permuted: they hold the caller's commands in drone-id order)
+            for t in (self._last_rpm, self._pos_f32, self._obs_buf[0], self._obs_buf[1], self._dw_fz):
                 if t is not None:
                     t.copy_(t[perm].clone())
             if self._pid is not None:
@@ -888,7 +915,7 @@ class BaseAviary(Env):
                     return self._single_result(obs)
                 info = {}
                 if self._final_obs is not None:
-                    info = {"final_obs": self._final_obs.view(self._E, self._D, self._obs_dim), "_final_obs": self._done}
+                    info = {"final_obs": self._by_id(self._final_obs).view(self._E, self._D, self._obs_dim), "_final_obs": self._done}
                 return self._shape_obs(obs), self._reward, self._terminated, self._truncated, info
             #### NumPy path: pinned H2D of the action, D2H of the results, all inside this call ####
             if self._rpm_cmd is not None and isinstance(action, np.ndarray) and action.dtype == np.float64:
@@ -910,7 +937,7 @@ class BaseAviary(Env):
             k = self._hcur
             self._hcur = 1 - k
             h_obs, h_rew, h_te, h_tr = self._h_obs[k], self._h_reward[k], self._h_term[k], self._h_trunc[k]
-            h_obs.copy_(obs, non_blocking=True)
+            h_obs.copy_(self._by_id(obs), non_blocking=True)
             h_rew.copy_(self._reward, non_blocking=True)
             h_te.copy_(self._terminated, non_blocking=True)
             h_tr.copy_(self._truncated, non_blocking=True)
@@ -1037,7 +1064,7 @@ class BaseAviary(Env):
         rpy = euler_from_quaternion(quat)
         obs = self._obs_buf[self._cur]
         ang_v = obs[:, 13:16].double() if self._state20_obs() else obs[:, 9:12].double()      # (a KIN row can be 20 wide)
-        sv = torch.cat([pos, quat, rpy, vel, ang_v, self._last_rpm], dim=1)
+        sv = self._by_id(torch.cat([pos, quat, rpy, vel, ang_v, self._last_rpm], dim=1))
         return sv.view(self._E, self._D, 20).cpu().numpy()
 
     def _getDroneStateVector(self, nth_drone):
@@ -1045,12 +1072,14 @@ class BaseAviary(Env):
 
     def adjacency(self, out=None):
         """Neighbourhood query for every aviary: uint8 tensor [E, D, D], 1 where i == j or the drones are closer
-        than NEIGHBOURHOOD_RADIUS (BaseAviary._getAdjacencyMatrix, BaseAviary.py:658-675)."""
+        than NEIGHBOURHOOD_RADIUS (BaseAviary._getAdjacencyMatrix, BaseAviary.py:658-675).  Rows and columns are drone ids."""
         if out is None:
             out = torch.empty((self._E, self._D, self._D), dtype=torch.uint8, device=self.device)
         with self._on_device():
             N.check(self._lib.qs_adjacency(C.byref(self._st), self._E, self._D, float(self.NEIGHBOURHOOD_RADIUS),
                                            out.data_ptr(), self._stream()), "qs_adjacency")
+            if self._inv is not None:                      # the kernel indexes storage slots (E == 1 after reorder_by_morton)
+                out[0] = out[0][self._inv][:, self._inv]
         return out
 
     def _getAdjacencyMatrix(self):

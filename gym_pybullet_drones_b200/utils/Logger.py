@@ -65,12 +65,17 @@ class Logger(object):
     # ---- device-side ring (SURVEY.md 8f rank 4) --------------------------------------------------------------------------
     def attach(self, env, aviary: int = 0, capacity: int = None):
         """Starts logging every control tick of `env`'s aviary `aviary` (its NUM_DRONES drones) on the device.
-        `capacity` = ticks the ring holds between two flush() calls (default: duration_sec * logging_freq_hz, else 4096)."""
+        `capacity` = ticks the ring holds between two flush() calls (default: duration_sec * logging_freq_hz, else 4096).
+        The ring records the env's storage slots, so an env whose storage `reorder_by_morton()` has permuted is refused
+        (ValueError), and so is a reorder while a Logger is attached; log such a formation with `log_all` and its observations."""
         import ctypes as C
         import torch
         from .. import _native as N
         if env.NUM_DRONES != self.NUM_DRONES:
             raise ValueError("Logger(num_drones=%d) attached to an env with %d drones per aviary" % (self.NUM_DRONES, env.NUM_DRONES))
+        if getattr(env, "_order", None) is not None:
+            raise ValueError("Logger.attach() on an env reordered by reorder_by_morton(): the device ring records storage slots, "
+                             "not drone ids; log its observations with log_all() instead")
         if not 0 <= aviary < env.num_envs:
             raise ValueError("aviary index out of range")
         cap = int(capacity or (self.timestamps.shape[1] if self.PREALLOCATED_ARRAYS else 4096))
