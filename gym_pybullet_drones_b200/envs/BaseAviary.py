@@ -553,6 +553,28 @@ class BaseAviary(Env):
             return {k: torch.full((self._E,), nom[k], dtype=torch.float64, device=self.device) for k in PHYS_KEYS}
         return {k: self._phys_props[:, j].clone() for j, k in enumerate(PHYS_KEYS)}
 
+    def differentiable_rollout(self, rpm, *, state=None, last_rpm=None, phys=None):
+        """T control ticks of raw RPMs as a differentiable function (torch.autograd), without changing the env.
+
+        rpm: [T, E, D, 4] float64 CUDA tensor; tick k applies clip(rpm[k], 0, MAX_RPM) for PYB_STEPS_PER_CTRL substeps, exactly
+        as CtrlAviary.step(rpm[k]) does with float64 RPMs.  state: optional dict pos / quat / vel / rpy_rates of [E, D, k] float64
+        tensors (default: a detached copy of the env's state).  last_rpm: [E, D, 4], the previous tick's clipped RPMs that drag
+        reads in the first substep (default: last_clipped_action, or zeros when the env does not track it).  phys: optional dict
+        of some PHYS_KEYS -> [E] float64 tensors (the rest from physical_params()).  Any of these may require grad.  Returns
+        {pos, quat, vel, rpy_rates} as [T, E, D, k] float64 tensors, entry k the state after tick k; indices are drone ids,
+        also after reorder_by_morton().  The state, counters, observation buffers, Logger ring and constants table stay as
+        they were.
+
+        The forward is the kernels' function bit for bit.  The backward (one adjoint kernel, DESIGN.md 4.5) differentiates:
+        _integrateQ's exponential map everywhere, also where the forward keeps the quaternion (np.isclose(|w|, 0)); the
+        quaternion renormalisation on tick entry (the gradient w.r.t. state["quat"] has no radial part); the RPM clip as
+        torch.clamp (the gradient passes for 0 <= rpm <= MAX_RPM and goes to MAX_RPM above); the ground-effect height clip with
+        the forward's predicate; the upright switch as a constant.  Drag's first substep reads the previous tick's RPMs, so
+        their gradient flows to rpm[k-1], or to last_rpm for k = 0.  Physics.DYN, PYB, PYB_GND and PYB_DRAG; downwash, inputs
+        that are not float64 CUDA tensors of the right shape on the env's device, and double backward raise ValueError."""
+        from ..diff import differentiable_rollout
+        return differentiable_rollout(self, rpm, state=state, last_rpm=last_rpm, phys=phys)
+
     ################################################################################
 
     def _stream(self):

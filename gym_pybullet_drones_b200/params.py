@@ -123,7 +123,11 @@ def _sqrt(t):
     # correctly rounded like np.sqrt: CUDA's float64 sqrt is; torch's vectorised CPU sqrt is not (1 ulp apart now and then)
     if t.device.type == "cpu":
         import torch
-        return torch.from_numpy(np.sqrt(t.numpy()))
+        r = torch.from_numpy(np.sqrt(t.detach().numpy()))
+        if t.requires_grad:                  # np.sqrt's value with sqrt's derivative (s - s.detach() is exactly 0)
+            s = t.sqrt()
+            r = r + (s - s.detach())
+        return r
     return t.sqrt()
 
 

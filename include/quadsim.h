@@ -605,6 +605,37 @@ int qs_sizeof_mrac_rollout_io(void);
 int qs_ctrl_rollout_mrac(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int n_envs,
                          int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 
+/* Differentiable raw-RPM trajectories (DESIGN.md 4.5): T control ticks of Physics.DYN (+ GND and/or DRAG, no downwash) from a
+ * given state, and the reverse-mode product (VJP) of that trajectory with cotangents of its T states.  The env is not touched:
+ * every input and output is a caller-owned float64 device array.  A "state" is 13 N doubles in QsState.planes' layout
+ * ([pos|w.x] [quat] [vel|w.y] as [N][4] each, then w.z [N]).  Tick k applies clip(rpm[k], 0, MAX_RPM) for `substeps` substeps,
+ * exactly as qs_dyn_substeps(QS_FLAG_ACTION_F64) does, and drag's first substep reads the previous tick's clipped RPMs (last_rpm
+ * for tick 0).  The VJP differentiates the exponential map of _integrateQ everywhere (also where |w| <= 1e-8, where the forward
+ * keeps the quaternion) and the quaternion renormalisation on tick entry; the RPM clip passes the gradient for
+ * 0 <= rpm <= MAX_RPM and gives it to MAX_RPM above; the ground-effect height clip and the upright switch are differentiated
+ * with the forward's predicates.  One thread per drone; deterministic. */
+typedef struct QsDynTrajIO {
+    int T;                          /* ticks, > 0 */
+    int pad_;
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* rpm;              /* [T][N][4] RPM commands (clipped in the kernel) */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows; nullable = the constants of QsParams */
+    double* states;                 /* qs_dyn_traj out: [T][13 N], entry k = the state after tick k */
+    /* qs_dyn_traj_vjp: `states` is read (the forward's output), and */
+    const double* g_states;         /* [T][13 N] cotangents of the states */
+    double* g_rpm;                  /* out [T][N][4] */
+    double* g_state0;               /* out [13 N] */
+    double* g_last_rpm;             /* out [N][4], nullable */
+    double* g_phys;                 /* out [N][16]: PER DRONE (sum the drones of an aviary for its row); nullable */
+    double* scratch;                /* [substeps][13][N] workspace (the substep states of one tick) */
+} QsDynTrajIO;
+int qs_sizeof_dyn_traj_io(void);
+/* effects: 0, QS_EFFECT_GND, QS_EFFECT_DRAG or both (QS_EFFECT_DW: QS_ERR_UNSUPPORTED) */
+int qs_dyn_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects, void* stream);
+int qs_dyn_traj_vjp(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                    void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
