@@ -26,10 +26,12 @@ def unpack_states(planes, n):
 class DynTrajectory(torch.autograd.Function):
     """states [T, 13 N] = the T ticks of qs_dyn_traj from planes0 [13 N] with rpm [T, N, 4], last_rpm [N, 4] and the per-aviary
     rows [E, 16]; backward = qs_dyn_traj_vjp, its per-drone row gradients summed over each aviary's drones (torch, deterministic).
-    `cfg` = (QsParams, E, D, substeps, effects).  Double backward raises ValueError."""
+    `cfg` = (QsParams, E, D, substeps, effects).  The inputs may have any strides (the kernels read dense buffers: they get
+    contiguous copies).  Double backward raises ValueError."""
 
     @staticmethod
     def forward(ctx, rpm, planes0, last_rpm, rows, cfg):
+        rpm, planes0, last_rpm, rows = (x.contiguous() for x in (rpm, planes0, last_rpm, rows))
         P, E, D, S, eff = cfg
         T, n = rpm.shape[0], E * D
         states = torch.empty((T, 13 * n), dtype=torch.float64, device=rpm.device)

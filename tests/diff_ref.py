@@ -32,7 +32,7 @@ def half_angle(n2, dt, exact_branch=False):
     """cos(theta) and sin(theta)/|w| for theta = |w| dt / 2, from n2 = |w|^2.  exact_branch=True: the reference's
     np.isclose(|w|, 0) identity (c = 1, s = 0 where |w| <= 1e-8), whose derivative is zero there -- a negative control only."""
     h = 0.5 * dt
-    t = n2 * (h * h)
+    t = n2 * h * h                                   # half_angle_terms' order: both take the same side of t = 1/4
     small = t < 0.25
     ts = torch.where(small, t, torch.zeros_like(t))
     c_ser = torch.zeros_like(t)
@@ -55,8 +55,9 @@ def upright(sarg, ra, rb):
     return (sarg > -0.99999) & (sarg < 0.99999) & ((rb > _UPRIGHT_T * ra.abs()) | ((rb == 0) & (ra == 0)))
 
 
-def substep(K, rows, x, u, ds, effects, exact_branch=False):
-    """One _dynamics substep (BaseAviary.py:815-877) from x [B, 13] with clipped rpm u [B, 4] and drag sum ds [B]."""
+def substep(K, rows, x, u, ds, effects, exact_branch=False, gnd_clip_le=False):
+    """One _dynamics substep (BaseAviary.py:815-877) from x [B, 13] with clipped rpm u [B, 4] and drag sum ds [B].
+    gnd_clip_le=True: the height clip as `hz <= clip`, which clips at equality -- a negative control only."""
     dt = K["dt"]
     p, q, v, w = x[:, 0:3], x[:, 3:7], x[:, 7:10], x[:, 10:13]
     X, Y, Z, W = q.unbind(1)
@@ -69,7 +70,7 @@ def substep(K, rows, x, u, ds, effects, exact_branch=False):
         up = upright(-2.0 * (X * Z - W * Y), 2.0 * (Y * Z + W * X), W * W - X * X - Y * Y + Z * Z).detach()
         Pp = K["props"]
         hz = p[:, 2:3] + r20[:, None] * Pp[:, 0] + r21[:, None] * Pp[:, 1] + r22[:, None] * Pp[:, 2]
-        h = torch.where(hz < K["h_clip"], torch.full_like(hz, K["h_clip"]), hz)
+        h = torch.where(hz <= K["h_clip"] if gnd_clip_le else hz < K["h_clip"], torch.full_like(hz, K["h_clip"]), hz)
         rr = K["prop_radius"] / (4 * h)
         g = u * u * kf[:, None] * K["gnd_coeff"] * (rr * rr)
         f = f + torch.where(up[:, None], g, torch.zeros_like(g))
@@ -91,16 +92,21 @@ def substep(K, rows, x, u, ds, effects, exact_branch=False):
     return torch.cat([pn, qn, vn, wn], dim=1)
 
 
-def tick(K, rows, x, rpm, up, S, effects, renormalise=True, exact_branch=False):
-    """One control tick: clip(rpm, 0, MAX_RPM) for S substeps from x [B, 13]; up = the previous tick's clipped rpm (drag)."""
-    u = torch.clamp(rpm, min=torch.zeros_like(rpm), max=rows[:, 13:14].expand_as(rpm))
+def tick(K, rows, x, rpm, up, S, effects, renormalise=True, strict_clamp=False, **sub):
+    """One control tick: clip(rpm, 0, MAX_RPM) for S substeps from x [B, 13]; up = the previous tick's clipped rpm (drag).
+    strict_clamp=True: a clip whose gradient reaches rpm only strictly below MAX_RPM (at equality it goes to MAX_RPM) -- a
+    negative control only.  `sub`: substep's exact_branch and gnd_clip_le."""
+    mx = rows[:, 13:14].expand_as(rpm)
+    u = torch.clamp(rpm, min=torch.zeros_like(rpm), max=mx)
+    if strict_clamp:
+        u = torch.where(rpm < mx, u, mx)
     if renormalise:
         q = x[:, 3:7]
         x = torch.cat([x[:, 0:3], q / torch.sqrt((q * q).sum(1, keepdim=True)), x[:, 7:13]], dim=1)
     k = 2 * math.pi
     ds_prev, ds_cur = (k * up / 60).sum(1), (k * u / 60).sum(1)
     for s in range(S):
-        x = substep(K, rows, x, u, ds_prev if s == 0 else ds_cur, effects, exact_branch)
+        x = substep(K, rows, x, u, ds_prev if s == 0 else ds_cur, effects, **sub)
     return x, u
 
 
