@@ -44,12 +44,6 @@ __device__ __forceinline__ void clip_rpm(const double raw[4], double max_rpm, do
     for (int j = 0; j < 4; ++j) u[j] = qs::clampd(raw[j], 0.0, max_rpm);            // CtrlAviary.py:140
 }
 
-// what store_drone + load_drone do to the state between two ticks
-__device__ __forceinline__ void round_quat(qs::Drone& d) {
-    const double inv = rsqrt(qs::quat_norm2(d.qx, d.qy, d.qz, d.qw));
-    d.qx = __dmul_rn(d.qx, inv); d.qy = __dmul_rn(d.qy, inv); d.qz = __dmul_rn(d.qz, inv); d.qw = __dmul_rn(d.qw, inv);
-}
-
 template <int EFF>
 __global__ void __launch_bounds__(kTrajTPB) dyn_traj_kernel(const __grid_constant__ TrajArgs a) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -66,7 +60,7 @@ __global__ void __launch_bounds__(kTrajTPB) dyn_traj_kernel(const __grid_constan
         clip_rpm(raw, c.max_rpm, u);
         double R_last[9];
         qs::dyn_tick_k<EFF>(a.P, c, d, u, up, 0.0, a.substeps, R_last);
-        round_quat(d);
+        round_to_planes(d);
         st_state(io.states + (long long)k * 13 * N, N, i, d);
 #pragma unroll
         for (int j = 0; j < 4; ++j) up[j] = u[j];
@@ -162,18 +156,11 @@ int launch_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones
     a.D = drones_per_env; a.substeps = substeps;
     const unsigned blocks = (unsigned)((a.N + kTrajTPB - 1) / kTrajTPB);
     cudaStream_t s = (cudaStream_t)stream;
-    switch (effects) {
-        case 0: if (VJP) dyn_traj_vjp_kernel<0><<<blocks, kTrajTPB, 0, s>>>(a); else dyn_traj_kernel<0><<<blocks, kTrajTPB, 0, s>>>(a); break;
-        case QS_EFFECT_GND:
-            if (VJP) dyn_traj_vjp_kernel<QS_EFFECT_GND><<<blocks, kTrajTPB, 0, s>>>(a); else dyn_traj_kernel<QS_EFFECT_GND><<<blocks, kTrajTPB, 0, s>>>(a);
-            break;
-        case QS_EFFECT_DRAG:
-            if (VJP) dyn_traj_vjp_kernel<QS_EFFECT_DRAG><<<blocks, kTrajTPB, 0, s>>>(a); else dyn_traj_kernel<QS_EFFECT_DRAG><<<blocks, kTrajTPB, 0, s>>>(a);
-            break;
-        default:
-            if (VJP) dyn_traj_vjp_kernel<3><<<blocks, kTrajTPB, 0, s>>>(a); else dyn_traj_kernel<3><<<blocks, kTrajTPB, 0, s>>>(a);
-            break;
-    }
+    // the checks above leave TrajEffects only (no bit above 7, no DW)
+    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
+        auto* k = VJP ? dyn_traj_vjp_kernel<decltype(EFF)::value> : dyn_traj_kernel<decltype(EFF)::value>;
+        k<<<blocks, kTrajTPB, 0, s>>>(a);
+    });
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_fail(e, what);
 }

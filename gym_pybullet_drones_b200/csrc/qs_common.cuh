@@ -1,5 +1,6 @@
 // qs_common.cuh -- shared by the translation units of libquadsim.so: error convention, argument structs, the state
-// load/store helpers (float64 planes, 32-byte accesses), TMA bulk-copy / mbarrier wrappers, launch geometry.
+// load/store helpers (float64 planes, 32-byte accesses), TMA bulk-copy / mbarrier wrappers, launch geometry, the dispatch from
+// run-time options to kernel instantiations.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,6 +8,7 @@
 #include <string.h>
 #include <stdlib.h>
 #include <time.h>
+#include <type_traits>
 
 #include "quad_core.cuh"
 
@@ -236,6 +238,13 @@ __device__ __forceinline__ void store_drone(const QsState& st, long long N, long
     if (st.pos_f32) st4(st.pos_f32, i, make_float4((float)d.px, (float)d.py, (float)d.pz, 0.f));
 }
 
+// what store_drone + load_drone do to the state between two ticks of a multi-tick kernel: the quaternion is renormalised, nothing
+// is rounded (the planes are float64), so T fused ticks equal T single-tick calls bit for bit
+__device__ __forceinline__ void round_to_planes(qs::Drone& d) {
+    const double inv = rsqrt(qs::quat_norm2(d.qx, d.qy, d.qz, d.qw));
+    d.qx = __dmul_rn(d.qx, inv); d.qy = __dmul_rn(d.qy, inv); d.qz = __dmul_rn(d.qz, inv); d.qw = __dmul_rn(d.qw, inv);
+}
+
 __device__ __forceinline__ void init_drone(const QsState& st, long long tbl, qs::Drone& d) {
     const D4 ip = ld256_nc(st.init_pos, tbl), iq = ld256_nc(st.init_quat, tbl);
     d.px = ip.x; d.py = ip.y; d.pz = ip.z;
@@ -290,6 +299,24 @@ inline int act_width(int act_type) {
         default: return -1;
     }
 }
+
+// ---- from run-time options to a kernel instantiation (host code).  Every launcher picks its template arguments through these
+// two: the generic lambda f receives the value as a type and names the kernel once.
+template <int... Vs> struct IntList {};
+// f(std::integral_constant<int, V>{}) for the V of the list that equals v; false, and no call, when none does
+template <int... Vs, class F>
+bool with_int(IntList<Vs...>, int v, F&& f) {
+    return ((v == Vs && (f(std::integral_constant<int, Vs>{}), true)) || ...);
+}
+// f(std::true_type{}) or f(std::false_type{}); returns what f returns
+template <class F>
+auto with_bool(bool b, F&& f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
+
+// the DYN+ effect sets that have kernels, written here only
+using AllEffects = IntList<0, 1, 2, 3, 4, 5, 6, 7>;                                                  // general step, action rollout
+using PolicyEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_DW, 7>;                    // policy and control rollouts
+using TrajEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_GND | QS_EFFECT_DRAG>;       // differentiable trajectories
+inline bool policy_effects_supported(unsigned eff) { return with_int(PolicyEffects{}, (int)eff, [](auto) {}); }
 
 int check_state(const QsState* st, int need_tables);                      // quadsim.cu
 int cta_capacity(long long N, int D, bool rollout = false);               // quadsim.cu

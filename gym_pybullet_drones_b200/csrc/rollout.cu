@@ -23,9 +23,12 @@ int qs_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io, int 
                                  io && io->policy && io->policy->vw1, a, pid_act))
         return rc;
     if (flags & QS_FLAG_AUTORESET_NEXT_STEP) return launch_rollout_next(a, io, pid_act, stream);
-    if (io->final_obs || io->final_values)
-        return a.st.phys ? launch_rollout<true, kRolloutFin>(a, io, pid_act, stream) : launch_rollout<false, kRolloutFin>(a, io, pid_act, stream);
-    return a.st.phys ? launch_rollout<true, kRolloutNone>(a, io, pid_act, stream) : launch_rollout<false, kRolloutNone>(a, io, pid_act, stream);
+    const bool fin = io->final_obs || io->final_values;
+    return with_bool(a.st.phys != nullptr, [&](auto PHYS) {
+        return with_bool(fin, [&](auto FIN) {
+            return launch_rollout<decltype(PHYS)::value, decltype(FIN)::value ? kRolloutFin : kRolloutNone>(a, io, pid_act, stream);
+        });
+    });
 }
 
 }  // extern "C"
@@ -76,11 +79,24 @@ int prepare_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io,
 }
 
 int check_policy_config(const RolloutArgs& a, const QsRolloutIO* io) {
-    const unsigned eff = a.effects & 7u;
-    if (eff != 0 && eff != QS_EFFECT_GND && eff != QS_EFFECT_DRAG && eff != QS_EFFECT_DW && eff != 7u)
+    if (!policy_effects_supported(a.effects & 7u))
         return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports no DYN+ effect, GND, DRAG, DW or all three; not GND|DRAG, GND|DW or DRAG|DW");
     if (a.cap > 64) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: the on-device policy supports drones_per_env <= 64");
     if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: pass either actions or a policy");
+    return 0;
+}
+
+int check_classic_policy(const RolloutArgs& a, const QsRolloutIO* io) {
+    const QsPolicy& q = *io->policy;
+    if (int rc = check_policy_config(a, io)) return rc;
+    if (!q.w1 || !q.b1 || !q.w2 || !q.b2 || !q.w3 || !q.b3 || !q.log_std) return fail(QS_ERR_NULL, "qs_rollout: policy weights are NULL");
+    if (q.nt3 != 1 && q.nt3 != 2 && q.nt3 != 4) return fail(QS_ERR_SIZE, "qs_rollout: policy nt3 (padded output tiles of 8) must be 1, 2 or 4");
+    if (q.out_dim > 8 * q.nt3) return fail(QS_ERR_SIZE, "qs_rollout: policy out_dim exceeds the padded output width");
+    if (q.in_dim != a.D * a.obs_dim || q.out_dim != a.D * a.A) return fail(QS_ERR_SIZE, "qs_rollout: policy in_dim/out_dim must be D*obs_dim / D*A");
+    if (q.vw1 && (!q.vb1 || !q.vw2 || !q.vb2 || !q.vw3 || !q.vb3)) return fail(QS_ERR_NULL, "qs_rollout: incomplete critic");
+    if (q.values && !q.vw1) return fail(QS_ERR_NULL, "qs_rollout: values requested without a critic");
+    if (!aligned16(q.w1) || !aligned16(q.w2) || !aligned16(q.w3) || (q.vw1 && (!aligned16(q.vw1) || !aligned16(q.vw2) || !aligned16(q.vw3))))
+        return fail(QS_ERR_ALIGN, "qs_rollout: policy weight arrays must be 16-byte aligned");
     return 0;
 }
 

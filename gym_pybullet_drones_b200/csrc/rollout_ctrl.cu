@@ -47,12 +47,6 @@ __device__ __forceinline__ void store_drone_rounded(const QsState& st, long long
     if (st.pos_f32) st4(st.pos_f32, i, make_float4((float)d.px, (float)d.py, (float)d.pz, 0.f));
 }
 
-// what store_drone + load_drone do to the state between two ticks (the rollout kernel's helper): the quaternion is renormalised
-__device__ __forceinline__ void round_to_planes(qs::Drone& d) {
-    const double inv = rsqrt(qs::quat_norm2(d.qx, d.qy, d.qz, d.qw));
-    d.qx = __dmul_rn(d.qx, inv); d.qy = __dmul_rn(d.qy, inv); d.qz = __dmul_rn(d.qz, inv); d.qw = __dmul_rn(d.qw, inv);
-}
-
 // TRACK targets of drone i at tick k (include/quadsim.h, QsCtrlRolloutIO): the waypoint row (start[i] + k) mod W, column 0 (M = 1)
 // or i (M = N), plus offset[i]
 __device__ __forceinline__ void track_target(const QsCtrlRolloutIO& io, long long N, long long i, int k, double& tx, double& ty, double& tz) {
@@ -285,30 +279,6 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
 
 __global__ void ctrl_log_advance_kernel(long long* head, int T) { *head += T; }      // after every CTA has read it (stream order)
 
-template <int EFF, bool PHYS>
-void launch_eff(const CtrlRolloutArgs& a, int mode, int blocks, int threads, size_t sm, cudaStream_t s) {
-    if (mode == QS_CTRL_RAW) ctrl_rollout_kernel<EFF, QS_CTRL_RAW, PHYS><<<blocks, threads, sm, s>>>(a);
-    else if (mode == QS_CTRL_VEL) ctrl_rollout_kernel<EFF, QS_CTRL_VEL, PHYS><<<blocks, threads, sm, s>>>(a);
-    else if (mode == QS_CTRL_TRACK) ctrl_rollout_kernel<EFF, QS_CTRL_TRACK, PHYS><<<blocks, threads, sm, s>>>(a);
-    else {
-        // more than the default 48 KB of dynamic shared memory; the launch reports a failure of the attribute call
-        void (*k)(CtrlMracArgs) = ctrl_rollout_kernel<EFF, QS_CTRL_MRAC, PHYS>;
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm) == cudaSuccess)
-            k<<<blocks, threads, sm, s>>>(static_cast<const CtrlMracArgs&>(a));
-    }
-}
-
-template <bool PHYS>
-void launch_ctrl(const CtrlRolloutArgs& a, int mode, unsigned eff, int blocks, int threads, size_t sm, cudaStream_t s) {
-    switch (eff) {
-        case 0: launch_eff<0, PHYS>(a, mode, blocks, threads, sm, s); break;
-        case QS_EFFECT_GND: launch_eff<QS_EFFECT_GND, PHYS>(a, mode, blocks, threads, sm, s); break;
-        case QS_EFFECT_DRAG: launch_eff<QS_EFFECT_DRAG, PHYS>(a, mode, blocks, threads, sm, s); break;
-        case QS_EFFECT_DW: launch_eff<QS_EFFECT_DW, PHYS>(a, mode, blocks, threads, sm, s); break;
-        default: launch_eff<7, PHYS>(a, mode, blocks, threads, sm, s); break;
-    }
-}
-
 }  // namespace
 }  // namespace qsi
 
@@ -332,7 +302,7 @@ int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io
         return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad mode (QS_CTRL_RAW, QS_CTRL_VEL or QS_CTRL_TRACK; QS_CTRL_MRAC is qs_ctrl_rollout_mrac)");
     if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad effects");
     const unsigned eff = effects & 7u;
-    if (eff != 0 && eff != QS_EFFECT_GND && eff != QS_EFFECT_DRAG && eff != QS_EFFECT_DW && eff != 7u)
+    if (!policy_effects_supported(eff))
         return fail(QS_ERR_UNSUPPORTED, "qs_ctrl_rollout: supports no DYN+ effect, GND, DRAG, DW or all three; not GND|DRAG, GND|DW or DRAG|DW");
     if ((eff & QS_EFFECT_DW) && drones_per_env > kCtrlTPB)
         return fail(QS_ERR_UNSUPPORTED, "qs_ctrl_rollout: downwash needs drones_per_env <= 128 (larger aviaries take the per-tick qs_downwash + qs_dyn_substeps path)");
@@ -391,8 +361,18 @@ int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io
     size_t sm = (size_t)a.tpb * 20 * 4 + ((eff & QS_EFFECT_DW) ? (size_t)a.tpb * 3 * 8 : 0);
     if (mode == QS_CTRL_MRAC) sm += mrac_smem(a.tpb);
     cudaStream_t s = (cudaStream_t)stream;
-    if (st->phys) launch_ctrl<true>(a, mode, eff, blocks, threads, sm, s);
-    else launch_ctrl<false>(a, mode, eff, blocks, threads, sm, s);
+    // eff is one of PolicyEffects and mode one of the four (both checked above)
+    with_int(PolicyEffects{}, (int)eff, [&](auto EFF) {
+        with_int(IntList<QS_CTRL_RAW, QS_CTRL_VEL, QS_CTRL_TRACK, QS_CTRL_MRAC>{}, mode, [&](auto MODE) {
+            with_bool(st->phys != nullptr, [&](auto PHYS) {
+                using Args = typename CtrlArgsOf<decltype(MODE)::value>::type;
+                void (*k)(Args) = ctrl_rollout_kernel<decltype(EFF)::value, decltype(MODE)::value, decltype(PHYS)::value>;
+                // MRAC takes more than the default 48 KB of dynamic shared memory; the launch reports a failure of the attribute call
+                if (decltype(MODE)::value != QS_CTRL_MRAC || cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm) == cudaSuccess)
+                    k<<<blocks, threads, sm, s>>>(static_cast<const Args&>(a));
+            });
+        });
+    });
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess && a.has_log) {
         ctrl_log_advance_kernel<<<1, 1, 0, s>>>(a.rg.head, io->T);

@@ -3,7 +3,6 @@
 #pragma once
 #include "qs_common.cuh"
 #include <cuda_fp16.h>
-#include <type_traits>
 
 namespace qsi {
 
@@ -41,6 +40,8 @@ int prepare_rollout(const QsParams* p, const QsState* st, const QsRolloutIO* io,
                     int substeps, unsigned effects, unsigned flags, bool has_critic, RolloutArgs& a, bool& pid_act);
 // the checks every on-device policy shares: effect set, drones per aviary, no caller actions
 int check_policy_config(const RolloutArgs& a, const QsRolloutIO* io);
+// check_policy_config, then the checks of the classic network io->policy (rollout.cu)
+int check_classic_policy(const RolloutArgs& a, const QsRolloutIO* io);
 
 namespace {
 
@@ -419,13 +420,6 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
 }
 __device__ __forceinline__ float u32_to_pm1(unsigned u) { return (float)(u >> 8) * (1.0f / 8388608.0f) - 1.0f; }   // [-1, 1)
 
-// what store_drone + load_drone do to the state between two ticks: the quaternion is renormalised, nothing is rounded
-// (the planes are float64), so T fused ticks equal T calls of qs_step bit for bit
-__device__ __forceinline__ void round_to_planes(qs::Drone& d) {
-    const double inv = rsqrt(qs::quat_norm2(d.qx, d.qy, d.qz, d.qw));
-    d.qx = __dmul_rn(d.qx, inv); d.qy = __dmul_rn(d.qy, inv); d.qz = __dmul_rn(d.qz, inv); d.qw = __dmul_rn(d.qw, inv);
-}
-
 // Fixed part of a POLICY CTA's dynamic shared memory: red_s [64][2] doubles, oob [64], done [64], and with in-CTA downwash the
 // positions pos_s [64][3] doubles; the mbarrier sits in the last 16 bytes.  1280 bytes without downwash, 2816 with it.
 __host__ __device__ constexpr size_t policy_smem_fixed(int eff) {
@@ -436,6 +430,20 @@ constexpr size_t kPolicyPosOffset = 64 * 2 * 8 + 64 + 64;       // pos_s of the 
 // 128 registers; the in-CTA downwash substep loop (positions of the aviary's drones, barriers, all three effects) spills the drone
 // state at 128, so those variants get 6 CTAs and 168 registers (DESIGN.md 4.1b)
 __host__ __device__ constexpr int policy_ctas(int eff) { return (eff & QS_EFFECT_DW) ? 6 : 7; }
+// the rest of a policy CTA's dynamic shared memory (the general network adds its staging): window, means, values, log-prob terms
+inline size_t policy_smem_var(int tpb, int obs_dim, int T, int A, int D, int out_tiles) {
+    const int n_av_max = 64 / D;
+    return (size_t)tpb * obs_dim * 4 + (size_t)(T + 1) * A * 4 + 32 + (size_t)(n_av_max * 8 * out_tiles + n_av_max * 8 + 64) * 4 + 16;
+}
+constexpr size_t kPolicySmemLimit = 200 * 1024;      // what a policy CTA may use
+// shared-memory carve-out of a policy kernel: just enough for `ctas` resident CTAs of `sm` bytes, so that the weights find the
+// rest of the 256 KB as L1
+template <class K>
+void set_policy_carveout(K* kernel, int ctas, size_t sm) {
+    const size_t need = (size_t)ctas * (sm + 1024);
+    const int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
+    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
+}
 
 // PHYS: the physical constants come from the aviary's row of QsState.phys, re-read (L1) every tick rather than held in 28
 // registers for the whole rollout -- the POLICY variants have none to spare (128 registers, 7 CTAs per SM, DESIGN.md 4.1b).
@@ -460,65 +468,41 @@ __global__ void __launch_bounds__(64, policy_ctas(EFF)) rollout_mlp_kernel(const
 // one policy variant: `sm_var` = its dynamic shared memory without the fixed part
 template <int EFF, bool PIDACT, bool PHYS, int MODE>
 void launch_policy(const RolloutArgs& a, size_t sm_var, int blocks, cudaStream_t s) {
+    auto* k = rollout_kernel<EFF, PIDACT, true, PHYS, MODE>;
     const size_t sm = policy_smem_fixed(EFF) + sm_var;
-    if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    {   // shared-memory carve-out: just enough for the resident CTAs, so that the weights find the rest of the 256 KB as L1
-        const size_t need = (size_t)policy_ctas(EFF) * (sm + 1024);
-        int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
-        cudaFuncSetAttribute(rollout_kernel<EFF, PIDACT, true, PHYS, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
-    }
-    rollout_kernel<EFF, PIDACT, true, PHYS, MODE><<<blocks, 64, sm, s>>>(a);       // two warps: 64 drones, 32 hidden units each in the MLP
+    if (sm > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    set_policy_carveout(k, policy_ctas(EFF), sm);
+    k<<<blocks, 64, sm, s>>>(a);       // two warps: 64 drones, 32 hidden units each in the MLP
 }
 
 // validates the policy (if any) and launches the rollout kernel family of `a` (PHYS: with the per-aviary table; MODE: see
 // rollout_kernel)
 template <bool PHYS, int MODE>
 int launch_rollout(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* stream) {
-    const int drones_per_env = a.D, A = a.A;
-    const unsigned effects = a.effects;
     const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
-    int threads = ((a.tpb + 31) / 32) * 32;
-    size_t sm = smem_fixed(a.cap) + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32;
+    const int eff = (int)(a.effects & 7u);
     cudaStream_t s = (cudaStream_t)stream;
     if (io->policy) {
-        const QsPolicy& q = *io->policy;
-        const unsigned eff = effects & 7u;
-        if (int rc = check_policy_config(a, io)) return rc;
-        if (!q.w1 || !q.b1 || !q.w2 || !q.b2 || !q.w3 || !q.b3 || !q.log_std) return fail(QS_ERR_NULL, "qs_rollout: policy weights are NULL");
-        if (q.nt3 != 1 && q.nt3 != 2 && q.nt3 != 4) return fail(QS_ERR_SIZE, "qs_rollout: policy nt3 (padded output tiles of 8) must be 1, 2 or 4");
-        if (q.out_dim > 8 * q.nt3) return fail(QS_ERR_SIZE, "qs_rollout: policy out_dim exceeds the padded output width");
-        if (q.in_dim != drones_per_env * a.obs_dim || q.out_dim != drones_per_env * A) return fail(QS_ERR_SIZE, "qs_rollout: policy in_dim/out_dim must be D*obs_dim / D*A");
-        if (q.vw1 && (!q.vb1 || !q.vw2 || !q.vb2 || !q.vw3 || !q.vb3)) return fail(QS_ERR_NULL, "qs_rollout: incomplete critic");
-        if (q.values && !q.vw1) return fail(QS_ERR_NULL, "qs_rollout: values requested without a critic");
-        if (!aligned16(q.w1) || !aligned16(q.w2) || !aligned16(q.w3) || (q.vw1 && (!aligned16(q.vw1) || !aligned16(q.vw2) || !aligned16(q.vw3))))
-            return fail(QS_ERR_ALIGN, "qs_rollout: policy weight arrays must be 16-byte aligned");
-        a.pol = q;
-        const int n_av_max = 64 / drones_per_env;
-        const size_t sm_var = (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * A * 4 + 32
-                            + (size_t)(n_av_max * 8 * q.nt3 + n_av_max * 8 + 64) * 4 + 16;      // window, means, values, log-prob terms
-        if (policy_smem_fixed(eff) + sm_var > 200 * 1024) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
-#define QS_PCASE(E)                                                                                                   \
-    case E:                                                                                                           \
-        if (pid_act) launch_policy<E, true, PHYS, MODE>(a, sm_var, blocks, s);                                              \
-        else launch_policy<E, false, PHYS, MODE>(a, sm_var, blocks, s);                                                     \
-        break;
-        switch (eff) { QS_PCASE(0) QS_PCASE(QS_EFFECT_GND) QS_PCASE(QS_EFFECT_DRAG) QS_PCASE(QS_EFFECT_DW) QS_PCASE(7) }
-#undef QS_PCASE
+        if (int rc = check_classic_policy(a, io)) return rc;
+        a.pol = *io->policy;
+        const size_t sm_var = policy_smem_var(a.tpb, a.obs_dim, io->T, a.A, a.D, a.pol.nt3);
+        if (policy_smem_fixed(eff) + sm_var > kPolicySmemLimit) return fail(QS_ERR_UNSUPPORTED, "qs_rollout: policy + window exceed shared memory");
+        // check_policy_config has rejected every effect set outside PolicyEffects
+        with_int(PolicyEffects{}, eff, [&](auto EFF) {
+            with_bool(pid_act, [&](auto PIDACT) { launch_policy<decltype(EFF)::value, decltype(PIDACT)::value, PHYS, MODE>(a, sm_var, blocks, s); });
+        });
         const cudaError_t e = cudaGetLastError();
         return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout (policy) launch");
     }
-#define QS_RCASE(E)                                                                                                   \
-    case E: {                                                                                                         \
-        if (pid_act) {                                                                                                \
-            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, true, false, PHYS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
-            rollout_kernel<E, true, false, PHYS, MODE><<<blocks, threads, sm, s>>>(a);                                            \
-        } else {                                                                                                      \
-            if (sm > 48 * 1024) cudaFuncSetAttribute(rollout_kernel<E, false, false, PHYS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32)); \
-            rollout_kernel<E, false, false, PHYS, MODE><<<blocks, threads, sm, s>>>(a);                                           \
-        }                                                                                                             \
-    } break;
-    switch (effects & 7u) { QS_RCASE(0) QS_RCASE(1) QS_RCASE(2) QS_RCASE(3) QS_RCASE(4) QS_RCASE(5) QS_RCASE(6) QS_RCASE(7) }
-#undef QS_RCASE
+    const int threads = ((a.tpb + 31) / 32) * 32;
+    const size_t sm = smem_fixed(a.cap) + (size_t)a.tpb * a.obs_dim * 4 + (size_t)(io->T + 1) * a.A * 4 + 32;
+    with_int(AllEffects{}, eff, [&](auto EFF) {
+        with_bool(pid_act, [&](auto PIDACT) {
+            auto* k = rollout_kernel<decltype(EFF)::value, decltype(PIDACT)::value, false, PHYS, MODE>;
+            if (sm > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kStepSmemFixed + kStageLimit + 32));
+            k<<<blocks, threads, sm, s>>>(a);
+        });
+    });
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout launch");
 }

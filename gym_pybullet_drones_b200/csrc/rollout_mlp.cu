@@ -6,14 +6,8 @@ using namespace qsi;
 
 namespace {
 
-// shared memory of a policy CTA besides the fixed part and the staging: window, means, values, log-prob terms (launch_rollout)
-size_t mlp_smem_var(int tpb, int obs_dim, int T, int A, int D, int out_tiles) {
-    const int n_av_max = 64 / D;
-    return (size_t)tpb * obs_dim * 4 + (size_t)(T + 1) * A * 4 + 32 + (size_t)(n_av_max * 8 * out_tiles + n_av_max * 8 + 64) * 4 + 16;
-}
 // the two staging buffers of both warps: 2 warps x 2 buffers x (max width / 16) k-steps x 1 KB
 size_t mlp_stage_bytes(int max_width) { return (size_t)2 * 2 * (max_width / 16) * 1024; }
-constexpr size_t kPolicySmemLimit = 200 * 1024;      // what launch_rollout allows a policy CTA
 
 int net_max_width(const QsMlpNet& n) {
     int w = 0;
@@ -52,29 +46,12 @@ void launch_mlp(const MlpRolloutArgs& a, int blocks, cudaStream_t s) {
     auto* k = rollout_mlp_kernel<EFF, PIDACT, PHYS, MODE>;
     const size_t sm = (size_t)a.stage_off + mlp_stage_bytes(a.stage_ks * 16);
     if (sm > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    {   // carve-out: the resident CTAs (as many as the staging leaves room for, at most the register limit), the rest is L1
-        int ctas = (int)((228 * 1024) / (sm + 1024));
-        if (ctas > policy_ctas(EFF)) ctas = policy_ctas(EFF);
-        if (ctas < 1) ctas = 1;
-        const size_t need = (size_t)ctas * (sm + 1024);
-        int pct = (int)((need * 100 + 228 * 1024 - 1) / (228 * 1024));
-        cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
-    }
+    // carve-out: the resident CTAs (as many as the staging leaves room for, at most the register limit), the rest is L1
+    int ctas = (int)((228 * 1024) / (sm + 1024));
+    if (ctas > policy_ctas(EFF)) ctas = policy_ctas(EFF);
+    if (ctas < 1) ctas = 1;
+    set_policy_carveout(k, ctas, sm);
     k<<<blocks, 64, sm, s>>>(a);
-}
-
-template <bool PHYS, int MODE>
-int launch_mlp_family(const MlpRolloutArgs& a, bool pid_act, cudaStream_t s) {
-    const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
-#define QS_MCASE(E)                                                                                                   \
-    case E:                                                                                                           \
-        if (pid_act) launch_mlp<E, true, PHYS, MODE>(a, blocks, s);                                                  \
-        else launch_mlp<E, false, PHYS, MODE>(a, blocks, s);                                                         \
-        break;
-    switch (a.effects & 7u) { QS_MCASE(0) QS_MCASE(QS_EFFECT_GND) QS_MCASE(QS_EFFECT_DRAG) QS_MCASE(QS_EFFECT_DW) QS_MCASE(7) }
-#undef QS_MCASE
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout_mlp launch");
 }
 
 }  // namespace
@@ -90,7 +67,7 @@ int qs_rollout_mlp_max_ticks(int act_type, int act_buffer_size, int drones_per_e
     const int wpad = (max_width + 63) / 64 * 64;
     // the window grows by A floats per tick; everything else is fixed: downwash's fixed part (the larger), the staging, the
     // scratch with the widest action outputs
-    const size_t fixed = policy_smem_fixed(QS_EFFECT_DW) + mlp_stage_bytes(wpad) + 15 + mlp_smem_var(block_size_for(D, 64), 12 + act_buffer_size * A, 0, A, D, 4);
+    const size_t fixed = policy_smem_fixed(QS_EFFECT_DW) + mlp_stage_bytes(wpad) + 15 + policy_smem_var(block_size_for(D, 64), 12 + act_buffer_size * A, 0, A, D, 4);
     if (fixed + (size_t)A * 4 > kPolicySmemLimit) return 0;
     const int t_smem = (int)((kPolicySmemLimit - fixed) / ((size_t)A * 4));
     return t_smem < tmax ? t_smem : tmax;
@@ -122,14 +99,24 @@ int qs_rollout_mlp(const QsParams* p, const QsState* st, const QsRolloutIO* io, 
     a.pol.log_std = q.log_std; a.pol.noise = q.noise; a.pol.logprob = q.logprob; a.pol.values = q.values;
     a.pol.in_dim = q.in_dim; a.pol.out_dim = q.out_dim; a.pol.nt3 = q.actor.out_tiles;
     a.pol.vw1 = q.critic.depth ? q.critic.w[0] : nullptr;
-    const size_t sm_var = mlp_smem_var(a.tpb, a.obs_dim, io->T, a.A, drones_per_env, q.actor.out_tiles);
+    const size_t sm_var = policy_smem_var(a.tpb, a.obs_dim, io->T, a.A, drones_per_env, q.actor.out_tiles);
     a.stage_off = (int)((policy_smem_fixed(a.effects & 7u) + sm_var + 15) / 16 * 16);
     a.stage_ks = wmax / 16;
     cudaStream_t s = (cudaStream_t)stream;
     const int mode = (flags & QS_FLAG_AUTORESET_NEXT_STEP) ? kRolloutNext : (io->final_obs || io->final_values) ? kRolloutFin : kRolloutNone;
-    if (mode == kRolloutNext) return a.st.phys ? launch_mlp_family<true, kRolloutNext>(a, pid_act, s) : launch_mlp_family<false, kRolloutNext>(a, pid_act, s);
-    if (mode == kRolloutFin) return a.st.phys ? launch_mlp_family<true, kRolloutFin>(a, pid_act, s) : launch_mlp_family<false, kRolloutFin>(a, pid_act, s);
-    return a.st.phys ? launch_mlp_family<true, kRolloutNone>(a, pid_act, s) : launch_mlp_family<false, kRolloutNone>(a, pid_act, s);
+    const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
+    // check_policy_config has rejected every effect set outside PolicyEffects
+    with_int(PolicyEffects{}, (int)(a.effects & 7u), [&](auto EFF) {
+        with_bool(pid_act, [&](auto PIDACT) {
+            with_bool(a.st.phys != nullptr, [&](auto PHYS) {
+                with_int(IntList<kRolloutNone, kRolloutFin, kRolloutNext>{}, mode, [&](auto MODE) {
+                    launch_mlp<decltype(EFF)::value, decltype(PIDACT)::value, decltype(PHYS)::value, decltype(MODE)::value>(a, blocks, s);
+                });
+            });
+        });
+    });
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout_mlp launch");
 }
 
 }  // extern "C"

@@ -5,7 +5,7 @@
 namespace qsi {
 
 int launch_rollout_next(RolloutArgs& a, const QsRolloutIO* io, bool pid_act, void* stream) {
-    return a.st.phys ? launch_rollout<true, kRolloutNext>(a, io, pid_act, stream) : launch_rollout<false, kRolloutNext>(a, io, pid_act, stream);
+    return with_bool(a.st.phys != nullptr, [&](auto PHYS) { return launch_rollout<decltype(PHYS)::value, kRolloutNext>(a, io, pid_act, stream); });
 }
 
 }  // namespace qsi

@@ -538,44 +538,6 @@ __global__ void __launch_bounds__(32) step_pipe_kernel(const __grid_constant__ S
     else if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // shared memory must outlive the bulk store's reads
 }
 
-// ---- launch ------------------------------------------------------------------------------------------------------------------
-template <int A, bool PHYS>
-struct LaunchClassic {
-    template <bool TASK, bool RESET, bool RPYF>
-    static cudaError_t run(const StepArgs& a, cudaStream_t s) {
-        const long long warps = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
-        const size_t sm = (size_t)FastSmem<A>::total_bytes(a.obs_dim, RESET && a.io.final_obs != nullptr);
-        return launch_step_kernel(step_fast_kernel<A, TASK, RESET, RPYF, PHYS>, (int)warps, 32, sm, sm, pdl_enabled(), s, a);
-    }
-};
-
-template <bool PHYS>
-struct LaunchPipe {
-    template <bool TASK, bool RESET, bool RPYF>
-    static cudaError_t run(const StepArgs& a, cudaStream_t s) {
-        const long long tiles = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
-        const size_t sm = (size_t)PipeSmem::total_bytes(a.obs_dim, RESET && a.io.final_obs != nullptr);
-        return launch_step_kernel(step_pipe_kernel<TASK, RESET, RPYF, PHYS>, (int)((tiles + kPipeTiles - 1) / kPipeTiles), 32, sm, sm,
-                                  pdl_enabled(), s, a);
-    }
-};
-
-// L::run<TASK, RESET, RPYF> for the step's task, autoreset mode and rpy precision
-template <class L>
-cudaError_t launch_modes(const StepArgs& a, cudaStream_t s) {
-    const bool task = a.task == QS_TASK_HOVER, reset = a.flags & QS_FLAG_AUTORESET_SAME_STEP, rpyf = a.flags & QS_FLAG_RPY_F32;
-    switch ((task ? 4 : 0) | (reset ? 2 : 0) | (rpyf ? 1 : 0)) {
-        case 0: return L::template run<false, false, false>(a, s);
-        case 1: return L::template run<false, false, true>(a, s);
-        case 2: return L::template run<false, true, false>(a, s);
-        case 3: return L::template run<false, true, true>(a, s);
-        case 4: return L::template run<true, false, false>(a, s);
-        case 5: return L::template run<true, false, true>(a, s);
-        case 6: return L::template run<true, true, false>(a, s);
-        default: return L::template run<true, true, true>(a, s);
-    }
-}
-
 }  // namespace
 
 // The fast kernels cover: RL observations with an action buffer, act RPM / ONE_D_RPM, no DYN+ effects, D in {1,2,4,...,32},
@@ -601,10 +563,24 @@ cudaError_t launch_step_fast(const StepArgs& a_in, cudaStream_t s) {
 #else
     const StepArgs& a = a_in;
 #endif
-    // the pipelined kernel takes A = 4 without the fused gather
-    if (a.A == 4 && a.pipe && !a.io.obs_gather) return a.st.phys ? launch_modes<LaunchPipe<true>>(a, s) : launch_modes<LaunchPipe<false>>(a, s);
-    if (a.A == 4) return a.st.phys ? launch_modes<LaunchClassic<4, true>>(a, s) : launch_modes<LaunchClassic<4, false>>(a, s);
-    return a.st.phys ? launch_modes<LaunchClassic<1, true>>(a, s) : launch_modes<LaunchClassic<1, false>>(a, s);
+    const bool fin = (a.flags & QS_FLAG_AUTORESET_SAME_STEP) && a.io.final_obs != nullptr;
+    const long long tiles = a.n_warps > 0 ? a.n_warps : (a.N + 31) / 32;
+    return with_bool(a.task == QS_TASK_HOVER, [&](auto TASK) {
+        return with_bool((a.flags & QS_FLAG_AUTORESET_SAME_STEP) != 0, [&](auto RESET) {
+            return with_bool((a.flags & QS_FLAG_RPY_F32) != 0, [&](auto RPYF) {
+                return with_bool(a.st.phys != nullptr, [&](auto PHYS) {
+                    constexpr bool T = decltype(TASK)::value, R = decltype(RESET)::value, F = decltype(RPYF)::value, P = decltype(PHYS)::value;
+                    if (a.A == 4 && a.pipe && !a.io.obs_gather) {      // the pipelined kernel takes A = 4 without the fused gather
+                        const size_t sm = (size_t)PipeSmem::total_bytes(a.obs_dim, fin);
+                        return launch_step_kernel(step_pipe_kernel<T, R, F, P>, (int)((tiles + kPipeTiles - 1) / kPipeTiles), 32, sm, sm, pdl_enabled(), s, a);
+                    }
+                    const size_t sm = (size_t)(a.A == 4 ? FastSmem<4>::total_bytes(a.obs_dim, fin) : FastSmem<1>::total_bytes(a.obs_dim, fin));
+                    return launch_step_kernel(a.A == 4 ? step_fast_kernel<4, T, R, F, P> : step_fast_kernel<1, T, R, F, P>, (int)tiles, 32, sm, sm,
+                                              pdl_enabled(), s, a);
+                });
+            });
+        });
+    });
 }
 
 }  // namespace qsi

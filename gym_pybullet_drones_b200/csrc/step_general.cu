@@ -422,32 +422,26 @@ size_t step_smem_bytes(const StepArgs& a) {
     return smem_fixed(a.cap) + (a.stage_rows ? (size_t)a.tpb * a.obs_dim * 4 + 32 : 0);
 }
 
-template <bool RAW, bool PIDACT, bool PHYS>
-cudaError_t launch_step(const StepArgs& a, bool pdl_ok, cudaStream_t s) {
+}  // namespace
+
+cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s) {
     const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
     const int threads = ((a.tpb + 31) / 32) * 32;
     const size_t sm = step_smem_bytes(a);
     const bool pdl = pdl_enabled() && pdl_ok;
-    // the shared-memory limit is the largest step_smem_bytes, the same for every launch of a kernel
-#define QS_CASE(E)                                                                                                     \
-    case E: return launch_step_kernel(step_kernel<E, RAW, PIDACT, PHYS>, blocks, threads, sm, kStepSmemFixed + kStageLimit + 32, pdl, s, a);
-    switch (a.effects & 7u) {
-        QS_CASE(0) QS_CASE(1) QS_CASE(2) QS_CASE(3) QS_CASE(4) QS_CASE(5) QS_CASE(6) QS_CASE(7)
-    }
-#undef QS_CASE
-    return cudaGetLastError();
-}
-
-template <bool PHYS>
-cudaError_t launch_families(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s) {
-    if (raw) return pid_act ? launch_step<true, true, PHYS>(a, pdl_ok, s) : launch_step<true, false, PHYS>(a, pdl_ok, s);
-    return pid_act ? launch_step<false, true, PHYS>(a, pdl_ok, s) : launch_step<false, false, PHYS>(a, pdl_ok, s);
-}
-
-}  // namespace
-
-cudaError_t launch_step_general(const StepArgs& a, bool raw, bool pid_act, bool pdl_ok, cudaStream_t s) {
-    return a.st.phys ? launch_families<true>(a, raw, pid_act, pdl_ok, s) : launch_families<false>(a, raw, pid_act, pdl_ok, s);
+    cudaError_t err = cudaSuccess;
+    with_int(AllEffects{}, (int)(a.effects & 7u), [&](auto EFF) {
+        err = with_bool(raw, [&](auto RAW) {
+            return with_bool(pid_act, [&](auto PIDACT) {
+                return with_bool(a.st.phys != nullptr, [&](auto PHYS) {
+                    // the shared-memory limit is the largest step_smem_bytes, the same for every launch of a kernel
+                    return launch_step_kernel(step_kernel<decltype(EFF)::value, decltype(RAW)::value, decltype(PIDACT)::value, decltype(PHYS)::value>,
+                                              blocks, threads, sm, kStepSmemFixed + kStageLimit + 32, pdl, s, a);
+                });
+            });
+        });
+    });
+    return err;
 }
 
 }  // namespace qsi
