@@ -1,0 +1,225 @@
+// dyn_ctrl_traj.cu -- qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp: differentiable closed-loop trajectories of a DSLPIDControl around
+// Physics.DYN (include/quadsim.h, DESIGN.md 4.5).  One thread per drone for all T ticks.  The forward is the QS_CTRL_TRACK tick of
+// ctrl_rollout_kernel (pid_control, the controller's max_rpm clip, the env's clip, dyn_tick_k, round_to_planes) in the same order;
+// the backward walks the ticks in reverse, reloading each tick's start state and controller state from the forward's outputs and
+// running dyn_adjoint.cuh's tick adjoint, the two clip adjoints and pid_adjoint.cuh's controller adjoint.
+#include "qs_common.cuh"
+#include "pid_adjoint.cuh"
+#include "traj_io.cuh"
+
+namespace qsi {
+namespace {
+
+constexpr int kCtrlTrajTPB = 128;
+
+struct CtrlTrajArgs {
+    QsParams P;          // the env: physics, MAX_RPM clip
+    QsParams CP;         // the DSLPIDControl's own constants (gains unless io.gains, model, g, max_rpm)
+    QsDynCtrlTrajIO io;
+    long long N;
+    int D, substeps;
+};
+
+__device__ __forceinline__ qs::PhysRow ctrl_row_of(const CtrlTrajArgs& a, long long i) {
+    return a.io.phys ? load_phys(a.io.phys, i / a.D) : qs::phys_row_of(a.P);
+}
+__device__ __forceinline__ qs::PidGains gains_of(const CtrlTrajArgs& a, long long i) {
+    if (!a.io.gains) return qs::pid_gains_of(a.CP);
+    const double* g = a.io.gains + 18 * (i / a.D);
+    qs::PidGains k;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        k.pid_p_for[c] = g[c]; k.pid_i_for[c] = g[3 + c]; k.pid_d_for[c] = g[6 + c];
+        k.pid_p_tor[c] = g[9 + c]; k.pid_i_tor[c] = g[12 + c]; k.pid_d_tor[c] = g[15 + c];
+    }
+    return k;
+}
+__device__ __forceinline__ void ld3(const double* p, long long i, double v[3]) {
+    if (p) { v[0] = p[3 * i]; v[1] = p[3 * i + 1]; v[2] = p[3 * i + 2]; } else { v[0] = v[1] = v[2] = 0.0; }
+}
+// the tick's targets of drone i: target_pos of tick k, the constant target_vel, target yaw and target_rpy_rates
+__device__ __forceinline__ qs::PidTargets targets_of(const QsDynCtrlTrajIO& io, long long N, long long i, int k) {
+    qs::PidTargets t;
+    ld3(io.target_pos, (long long)k * N + i, t.tp);
+    ld3(io.target_vel, i, t.tv);
+    double r[3];
+    ld3(io.target_rpy, i, r);
+    t.tyaw = r[2];
+    ld3(io.target_rpy_rates, i, t.trr);
+    return t;
+}
+
+// computeControlFromEnv + the two clips of the TRACK tick: the raw controller RPMs, the controller's clip u1, the applied u
+__device__ __forceinline__ void control(const CtrlTrajArgs& a, const qs::PidGains& K, qs::PidState& st, const qs::Drone& d,
+                                        const qs::PidTargets& t, double mr, double raw[4], double u1[4], double u[4]) {
+    double pe[3], ye;
+    qs::pid_control_k(a.CP, K, st, a.io.control_timestep, d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz,
+                      t.tp[0], t.tp[1], t.tp[2], t.tyaw, t.tv[0], t.tv[1], t.tv[2], t.trr[0], t.trr[1], t.trr[2], raw, pe, ye);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        u1[j] = qs::clampd(raw[j], 0.0, a.CP.max_rpm);
+        u[j] = qs::clampd(u1[j], 0.0, mr);
+    }
+}
+
+template <int EFF>
+__global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_kernel(const __grid_constant__ CtrlTrajArgs a) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long N = a.N;
+    if (i >= N) return;
+    const QsDynCtrlTrajIO& io = a.io;
+    const qs::PhysRow c = ctrl_row_of(a, i);
+    const qs::PidGains K = gains_of(a, i);
+    qs::Drone d;
+    ld_state(io.state0, N, i, d);
+    qs::PidState st;
+    load_pid(io.pid0, N, i, st);
+    double up[4] = {0, 0, 0, 0}, raw[4], u1[4], u[4];
+    if ((EFF & QS_EFFECT_DRAG) && io.last_rpm) ld4(io.last_rpm, i, up);
+    for (int k = 0; k < io.T; ++k) {
+        store_pid(io.pid_states + (long long)k * 9 * N, N, i, st);
+        control(a, K, st, d, targets_of(io, N, i, k), c.max_rpm, raw, u1, u);
+        double R_last[9];
+        qs::dyn_tick_k<EFF>(a.P, c, d, u, up, 0.0, a.substeps, R_last);
+        round_to_planes(d);
+        st_state(io.states + (long long)k * 13 * N, N, i, d);
+        double* o = io.rpm + 4 * ((long long)k * N + i);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { o[j] = u[j]; up[j] = u[j]; }
+    }
+}
+
+template <int EFF>
+__global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_vjp_kernel(const __grid_constant__ CtrlTrajArgs a) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long N = a.N;
+    if (i >= N) return;
+    const QsDynCtrlTrajIO& io = a.io;
+    const qs::PhysRow c = ctrl_row_of(a, i);
+    const qs::PidGains K = gains_of(a, i);
+    ScratchRec rec = {io.scratch, N, i};
+    qs::PhysGrad G;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) G.g[j] = 0.0;
+    double Lg[18];
+#pragma unroll
+    for (int j = 0; j < 18; ++j) Lg[j] = 0.0;
+    qs::PidTargets Lt = {{0, 0, 0}, 0, {0, 0, 0}, {0, 0, 0}};
+    qs::Drone L = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    qs::PidState Ls = {0, 0, 0, 0, 0, 0, 0, 0, 0};      // the cotangent of the controller state after tick k
+    double Lup_next[4] = {0, 0, 0, 0};                 // drag: the cotangent of this tick's applied RPMs from tick k + 1
+    for (int k = io.T - 1; k >= 0; --k) {
+        qs::Drone g;
+        ld_state(io.g_states + (long long)k * 13 * N, N, i, g);
+        L.px += g.px; L.py += g.py; L.pz += g.pz; L.qx += g.qx; L.qy += g.qy; L.qz += g.qz; L.qw += g.qw;
+        L.vx += g.vx; L.vy += g.vy; L.vz += g.vz; L.wx += g.wx; L.wy += g.wy; L.wz += g.wz;
+        qs::Drone d0;
+        ld_state(k == 0 ? io.state0 : io.states + (long long)(k - 1) * 13 * N, N, i, d0);
+        qs::PidState st0;
+        load_pid(io.pid_states + (long long)k * 9 * N, N, i, st0);
+        const qs::PidTargets t = targets_of(io, N, i, k);
+        double raw[4], u1[4], u[4], up[4] = {0, 0, 0, 0};
+        {
+            qs::PidState st = st0;
+            control(a, K, st, d0, t, c.max_rpm, raw, u1, u);
+        }
+        if (EFF & QS_EFFECT_DRAG) {
+            if (k > 0) ld4(io.rpm, (long long)(k - 1) * N + i, up);
+            else if (io.last_rpm) ld4(io.last_rpm, i, up);
+        }
+        double Lu[4] = {Lup_next[0], Lup_next[1], Lup_next[2], Lup_next[3]}, Lup[4] = {0, 0, 0, 0};
+        if (io.g_rpm_out) {
+            double gr[4];
+            ld4(io.g_rpm_out, (long long)k * N + i, gr);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) Lu[j] += gr[j];
+        }
+        qs::dyn_tick_vjp<EFF>(a.P, c, d0, u, up, a.substeps, rec, L, Lu, Lup, G);
+        // the env's clip (gradient to the row's MAX_RPM), then the controller's (its max_rpm is a constant of the controller)
+        double Lu1[4], Lraw[4], g_cmax = 0.0;
+        qs::rpm_clip_vjp(u1, c.max_rpm, Lu, Lu1, G.g[13]);
+        qs::rpm_clip_vjp(raw, a.CP.max_rpm, Lu1, Lraw, g_cmax);
+        Lt.tp[0] = Lt.tp[1] = Lt.tp[2] = 0.0;             // target_pos is per tick: its cotangent is written, not carried
+        qs::pid_control_vjp(a.CP, K, st0, io.control_timestep, d0, t, Lraw, Ls, L, Lt, Lg);
+        if (io.g_target_pos) {
+            double* o = io.g_target_pos + 3 * ((long long)k * N + i);
+            o[0] = Lt.tp[0]; o[1] = Lt.tp[1]; o[2] = Lt.tp[2];
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) Lup_next[j] = Lup[j];
+    }
+    st_state(io.g_state0, N, i, L);
+    if (io.g_pid0) store_pid(io.g_pid0, N, i, Ls);
+    auto st3 = [&](double* p, const double v[3]) { if (p) { p[3 * i] = v[0]; p[3 * i + 1] = v[1]; p[3 * i + 2] = v[2]; } };
+    st3(io.g_target_vel, Lt.tv);
+    st3(io.g_target_rpy_rates, Lt.trr);
+    const double ly[3] = {0.0, 0.0, Lt.tyaw};
+    st3(io.g_target_rpy, ly);
+    if (io.g_last_rpm) {
+        double* o = io.g_last_rpm + 4 * i;
+        o[0] = Lup_next[0]; o[1] = Lup_next[1]; o[2] = Lup_next[2]; o[3] = Lup_next[3];
+    }
+    if (io.g_phys) {
+        double* o = io.g_phys + 16 * i;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) o[j] = G.g[j];
+    }
+    if (io.g_gains) {
+        double* o = io.g_gains + 18 * i;
+#pragma unroll
+        for (int j = 0; j < 18; ++j) o[j] = Lg[j];
+    }
+}
+
+template <bool VJP>
+int launch_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
+                     int substeps, unsigned effects, void* stream, const char* what) {
+    if (!p || !cp || !io)
+        return fail(QS_ERR_NULL, VJP ? "qs_dyn_ctrl_traj_vjp: NULL params / controller params / io" : "qs_dyn_ctrl_traj: NULL params / controller params / io");
+    if (!io->state0 || !io->pid0 || !io->target_pos || !io->states || !io->rpm || !io->pid_states)
+        return fail(QS_ERR_NULL, "qs_dyn_ctrl_traj: NULL state0 / pid0 / target_pos / states / rpm / pid_states");
+    if (VJP && (!io->g_states || !io->g_state0 || !io->scratch))
+        return fail(QS_ERR_NULL, "qs_dyn_ctrl_traj_vjp: NULL g_states / g_state0 / scratch");
+    if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0)
+        return fail(QS_ERR_SIZE, "qs_dyn_ctrl_traj: n_envs, drones_per_env, substeps and T must be > 0");
+    if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_dyn_ctrl_traj: n_envs * drones_per_env exceeds 2^31-1");
+    if (!(io->control_timestep > 0.0)) return fail(QS_ERR_SIZE, "qs_dyn_ctrl_traj: control_timestep must be > 0");
+    if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_dyn_ctrl_traj: bad effects");
+    if (effects & QS_EFFECT_DW) return fail(QS_ERR_UNSUPPORTED, "qs_dyn_ctrl_traj: downwash couples the drones pairwise and has no adjoint here");
+    if (io->phys && !aligned16(io->phys)) return fail(QS_ERR_ALIGN, "qs_dyn_ctrl_traj: phys rows must be 16-byte aligned");
+    CtrlTrajArgs a;
+    memset(&a, 0, sizeof(a));
+    a.P = *p; a.CP = *cp; a.io = *io;
+    a.N = (long long)n_envs * drones_per_env;
+    a.D = drones_per_env; a.substeps = substeps;
+    const unsigned blocks = (unsigned)((a.N + kCtrlTrajTPB - 1) / kCtrlTrajTPB);
+    cudaStream_t s = (cudaStream_t)stream;
+    // the checks above leave TrajEffects only (no bit above 7, no DW)
+    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
+        auto* k = VJP ? dyn_ctrl_traj_vjp_kernel<decltype(EFF)::value> : dyn_ctrl_traj_kernel<decltype(EFF)::value>;
+        k<<<blocks, kCtrlTrajTPB, 0, s>>>(a);
+    });
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_fail(e, what);
+}
+
+}  // namespace
+}  // namespace qsi
+
+using namespace qsi;
+
+extern "C" {
+
+int qs_sizeof_dyn_ctrl_traj_io(void) { return (int)sizeof(QsDynCtrlTrajIO); }
+
+int qs_dyn_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env, int substeps,
+                     unsigned effects, void* stream) {
+    return launch_ctrl_traj<false>(p, cp, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_ctrl_traj launch");
+}
+
+int qs_dyn_ctrl_traj_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
+                         int substeps, unsigned effects, void* stream) {
+    return launch_ctrl_traj<true>(p, cp, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_ctrl_traj_vjp launch");
+}
+
+}  // extern "C"

@@ -334,13 +334,15 @@ QS_HD void derive(const Drone& d, const double R_last[9], Derived& o) {
 // ---- DSLPIDControl -----------------------------------------------------------------------------
 struct PidState { double ipx, ipy, ipz, lr, lp, ly, irx, iry, irz; };   // integral_pos_e, last_rpy, integral_rpy_e
 
-// computeControl (control/DSLPIDControl.py:82-145).  Returns rpm[4], pos_e[3], yaw_e; updates st.
-QS_HD void pid_control(const QsParams& P, PidState& st, double dt,
-                       double px, double py, double pz, double qx, double qy, double qz, double qw,
-                       double vx, double vy, double vz,
-                       double tpx, double tpy, double tpz, double tyaw,
-                       double tvx, double tvy, double tvz, double trr0, double trr1, double trr2,
-                       double rpm[4], double pos_e[3], double& yaw_e) {
+// computeControl (control/DSLPIDControl.py:82-145).  Returns rpm[4], pos_e[3], yaw_e; updates st.  The 18 gains (pid_p_for ..
+// pid_d_tor) come from `K`: P itself (pid_control), or one aviary's gain set of a differentiable rollout (pid_adjoint.cuh).
+template <class K>
+QS_HD void pid_control_k(const QsParams& P, const K& G, PidState& st, double dt,
+                         double px, double py, double pz, double qx, double qy, double qz, double qw,
+                         double vx, double vy, double vz,
+                         double tpx, double tpy, double tpz, double tyaw,
+                         double tvx, double tvy, double tvz, double trr0, double trr1, double trr2,
+                         double rpm[4], double pos_e[3], double& yaw_e) {
     double R[9];
     quat_to_matrix(qx, qy, qz, qw, R);                                               // :187
     const double ex = tpx - px, ey = tpy - py, ez = tpz - pz;                        // :188
@@ -348,9 +350,9 @@ QS_HD void pid_control(const QsParams& P, PidState& st, double dt,
     st.ipx = clampd(st.ipx + ex * dt, -2.0, 2.0);                                    // :190-191
     st.ipy = clampd(st.ipy + ey * dt, -2.0, 2.0);
     st.ipz = clampd(clampd(st.ipz + ez * dt, -2.0, 2.0), -0.15, 0.15);               // :192
-    double ttx = P.pid_p_for[0] * ex + P.pid_i_for[0] * st.ipx + P.pid_d_for[0] * evx;          // :194-196
-    double tty = P.pid_p_for[1] * ey + P.pid_i_for[1] * st.ipy + P.pid_d_for[1] * evy;
-    double ttz = P.pid_p_for[2] * ez + P.pid_i_for[2] * st.ipz + P.pid_d_for[2] * evz + P.pid_gravity;
+    double ttx = G.pid_p_for[0] * ex + G.pid_i_for[0] * st.ipx + G.pid_d_for[0] * evx;          // :194-196
+    double tty = G.pid_p_for[1] * ey + G.pid_i_for[1] * st.ipy + G.pid_d_for[1] * evy;
+    double ttz = G.pid_p_for[2] * ez + G.pid_i_for[2] * st.ipz + G.pid_d_for[2] * evz + P.pid_gravity;
     double scalar = ttx * R[2] + tty * R[5] + ttz * R[8];                            // :197
     if (scalar < 0.0) scalar = 0.0;
     const double thrust = (sqrt(scalar / (4.0 * P.pid_kf)) - P.pid_pwm2rpm_const) / P.pid_pwm2rpm_scale;   // :198
@@ -387,9 +389,9 @@ QS_HD void pid_control(const QsParams& P, PidState& st, double dt,
     st.irx = clampd(clampd(st.irx - rex * dt, -1500.0, 1500.0), -1.0, 1.0);          // :249-251
     st.iry = clampd(clampd(st.iry - rey * dt, -1500.0, 1500.0), -1.0, 1.0);
     st.irz = clampd(st.irz - rez * dt, -1500.0, 1500.0);
-    double q0 = -P.pid_p_tor[0] * rex + P.pid_d_tor[0] * rrx + P.pid_i_tor[0] * st.irx;      // :253-255
-    double q1 = -P.pid_p_tor[1] * rey + P.pid_d_tor[1] * rry + P.pid_i_tor[1] * st.iry;
-    double q2 = -P.pid_p_tor[2] * rez + P.pid_d_tor[2] * rrz + P.pid_i_tor[2] * st.irz;
+    double q0 = -G.pid_p_tor[0] * rex + G.pid_d_tor[0] * rrx + G.pid_i_tor[0] * st.irx;      // :253-255
+    double q1 = -G.pid_p_tor[1] * rey + G.pid_d_tor[1] * rry + G.pid_i_tor[1] * st.iry;
+    double q2 = -G.pid_p_tor[2] * rez + G.pid_d_tor[2] * rrz + G.pid_i_tor[2] * st.irz;
     q0 = clampd(q0, -3200.0, 3200.0); q1 = clampd(q1, -3200.0, 3200.0); q2 = clampd(q2, -3200.0, 3200.0);   // :256
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -398,6 +400,16 @@ QS_HD void pid_control(const QsParams& P, PidState& st, double dt,
         rpm[i] = P.pid_pwm2rpm_scale * pwm + P.pid_pwm2rpm_const;                    // :259
     }
     yaw_e = ec - yaw;                                                                // :145
+}
+
+QS_HD void pid_control(const QsParams& P, PidState& st, double dt,
+                       double px, double py, double pz, double qx, double qy, double qz, double qw,
+                       double vx, double vy, double vz,
+                       double tpx, double tpy, double tpz, double tyaw,
+                       double tvx, double tvy, double tvz, double trr0, double trr1, double trr2,
+                       double rpm[4], double pos_e[3], double& yaw_e) {
+    pid_control_k(P, P, st, dt, px, py, pz, qx, qy, qz, qw, vx, vy, vz, tpx, tpy, tpz, tyaw, tvx, tvy, tvz, trr0, trr1, trr2,
+                  rpm, pos_e, yaw_e);
 }
 
 // ---- action decoding (BaseRLAviary._preprocessAction, envs/BaseRLAviary.py:160-239) -----------------

@@ -1,6 +1,7 @@
-"""Differentiable raw-RPM trajectories of Physics.DYN: a torch.autograd.Function over qs_dyn_traj / qs_dyn_traj_vjp
-(include/quadsim.h, DESIGN.md 4.5).  BaseAviary.differentiable_rollout is the public entry point; this module packs the state
-into the kernels' planes layout, runs the forward and backward kernels and unpacks the result."""
+"""Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs) and
+qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop) (include/quadsim.h, DESIGN.md 4.5).
+BaseAviary.differentiable_rollout is the public entry point; this module packs the state into the kernels' planes layout, runs
+the forward and backward kernels and unpacks the result."""
 import ctypes as C
 
 import torch
@@ -8,6 +9,8 @@ import torch
 from . import _native as N
 
 STATE_KEYS = (("pos", 3), ("quat", 4), ("vel", 3), ("rpy_rates", 3))
+GAIN_KEYS = ("P_COEFF_FOR", "I_COEFF_FOR", "D_COEFF_FOR", "P_COEFF_TOR", "I_COEFF_TOR", "D_COEFF_TOR")    # QsDynCtrlTrajIO.gains
+PID_KEYS = ("integral_pos_e", "last_rpy", "integral_rpy_e")                                              # rows of the [9, N] state
 
 
 def pack_state(pos, quat, vel, w):
@@ -70,6 +73,63 @@ class DynTrajectory(torch.autograd.Function):
         return g_rpm, g_state0, g_last, g_phys.view(E, D, 16).sum(dim=1), None
 
 
+class DynCtrlTrajectory(torch.autograd.Function):
+    """(states [T, 13 N], rpm [T, N, 4]) = the T ticks of qs_dyn_ctrl_traj from planes0 [13 N] and the controller state pid0
+    [9, N], with target_pos [T, N, 3], target_vel / target_rpy / target_rpy_rates [N, 3], last_rpm [N, 4], the per-aviary rows
+    [E, 16] and gain sets [E, 18]; backward = qs_dyn_ctrl_traj_vjp, its per-drone row and gain gradients summed over each
+    aviary's drones (torch, deterministic).  `cfg` = (env QsParams, controller QsParams, control_timestep, E, D, substeps,
+    effects).  The inputs may have any strides (the kernels get contiguous copies).  Double backward raises ValueError."""
+
+    @staticmethod
+    def _io(T, dt, ins, outs):
+        io = N.QsDynCtrlTrajIO()
+        io.T, io.control_timestep = T, dt
+        for k, x in list(ins.items()) + list(outs.items()):
+            setattr(io, k, x.data_ptr())
+        return io
+
+    @staticmethod
+    def forward(ctx, planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains, cfg):
+        ins = dict(zip(("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains"),
+                       (x.contiguous() for x in (planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains))))
+        P, CP, dt, E, D, S, eff = cfg
+        T, n = tpos.shape[0], E * D
+        f64 = dict(dtype=torch.float64, device=tpos.device)
+        outs = dict(states=torch.empty((T, 13 * n), **f64), rpm=torch.empty((T, n, 4), **f64), pid_states=torch.empty((T, 9, n), **f64))
+        io = DynCtrlTrajectory._io(T, dt, ins, outs)
+        with torch.cuda.device(tpos.device):
+            N.check(N.lib().qs_dyn_ctrl_traj(C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
+                    "qs_dyn_ctrl_traj")
+        ctx.save_for_backward(*ins.values(), *outs.values())
+        ctx.cfg = cfg
+        return outs["states"], outs["rpm"]
+
+    @staticmethod
+    def backward(ctx, g_states, g_rpm):
+        if torch.is_grad_enabled():
+            raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
+                             "derivative of its own")
+        saved = ctx.saved_tensors
+        ins = dict(zip(("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains"), saved[:9]))
+        outs = dict(zip(("states", "rpm", "pid_states"), saved[9:]))
+        P, CP, dt, E, D, S, eff = ctx.cfg
+        T, n = ins["target_pos"].shape[0], E * D
+        f64 = dict(dtype=torch.float64, device=ins["target_pos"].device)
+        grads = dict(g_state0=torch.empty((13 * n,), **f64), g_pid0=torch.empty((9, n), **f64), g_target_pos=torch.empty((T, n, 3), **f64),
+                     g_target_vel=torch.empty((n, 3), **f64), g_target_rpy=torch.empty((n, 3), **f64),
+                     g_target_rpy_rates=torch.empty((n, 3), **f64), g_last_rpm=torch.empty((n, 4), **f64),
+                     g_phys=torch.empty((n, 16), **f64), g_gains=torch.empty((n, 18), **f64))
+        outs.update(g_states=g_states.to(torch.float64).contiguous(), g_rpm_out=g_rpm.to(torch.float64).contiguous(),
+                    scratch=torch.empty((S, 13, n), **f64))
+        io = DynCtrlTrajectory._io(T, dt, ins, dict(outs, **grads))
+        with torch.cuda.device(ins["target_pos"].device):
+            N.check(N.lib().qs_dyn_ctrl_traj_vjp(C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff,
+                                                 torch.cuda.current_stream().cuda_stream), "qs_dyn_ctrl_traj_vjp")
+        g = grads
+        return (g["g_state0"], g["g_pid0"], g["g_target_pos"], g["g_target_vel"], g["g_target_rpy"], g["g_target_rpy_rates"],
+                g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), g["g_gains"].view(E, D, 18).sum(dim=1), None)
+
+
 def _tensor(x, name, shape, device):
     if not isinstance(x, torch.Tensor):
         raise ValueError("%s must be a torch tensor, got %s" % (name, type(x).__name__))
@@ -82,19 +142,10 @@ def _tensor(x, name, shape, device):
     return x
 
 
-def differentiable_rollout(env, rpm, state=None, last_rpm=None, phys=None):
-    """BaseAviary.differentiable_rollout (see there)."""
+def _start_state(env, state, last_rpm, phys):
+    """The planes [13 N] of the initial state, last_rpm [N, 4] and the per-aviary rows [E, 16] of differentiable_rollout."""
     from .params import PHYS_KEYS, physical_rows
-    if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
-        raise ValueError("differentiable_rollout() does not support downwash: the pairwise term has no adjoint (use Physics.DYN, PYB, "
-                         "PYB_GND or PYB_DRAG)")
     E, D, n, dev = env._E, env._D, env._N, env.device
-    if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
-        raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
-    T = rpm.shape[0]
-    if T <= 0:
-        raise ValueError("rpm must hold at least one tick")
-    _tensor(rpm, "rpm", (T, E, D, 4), dev)
     # the env's state in drone-id order (every drone is independent without downwash: the kernels need no storage order)
     cur = {"pos": env._plane[0, :, 0:3], "quat": env._plane[1], "vel": env._plane[2, :, 0:3],
            "rpy_rates": torch.stack([env._plane[0, :, 3], env._plane[2, :, 3], env._wz], dim=1)}
@@ -122,6 +173,120 @@ def differentiable_rollout(env, rpm, state=None, last_rpm=None, phys=None):
         props[k] = _tensor(v, "phys[%r]" % k, (E,), dev)
     with torch.cuda.device(dev):
         rows = physical_rows(env.DRONE_MODEL, props, env.G)
+    return planes0, last_rpm, rows
+
+
+def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, **schedule):
+    """BaseAviary.differentiable_rollout (see there)."""
+    if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
+        raise ValueError("differentiable_rollout() does not support downwash: the pairwise term has no adjoint (use Physics.DYN, PYB, "
+                         "PYB_GND or PYB_DRAG)")
+    if (rpm is None) == (controller is None):
+        raise ValueError("differentiable_rollout() takes exactly one of rpm [T, E, D, 4] (open loop) or controller= (closed loop)")
+    if controller is not None:
+        return _closed_loop(env, controller, state, last_rpm, phys, **schedule)
+    given = sorted(k for k, v in schedule.items() if v is not None)
+    if given:
+        raise ValueError("%s apply to a controller rollout only" % ", ".join(given))
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
+        raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
+    T = rpm.shape[0]
+    if T <= 0:
+        raise ValueError("rpm must hold at least one tick")
+    _tensor(rpm, "rpm", (T, E, D, 4), dev)
+    planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
+    with torch.cuda.device(dev):
         cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
         states = DynTrajectory.apply(rpm.reshape(T, n, 4).contiguous(), planes0, last_rpm.contiguous(), rows.contiguous(), cfg)
     return {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+
+
+def _rows3(x, name, E, D, dev):
+    """[E, D, 3] or [3] float64 tensor -> [E * D, 3]; None -> zeros."""
+    n = E * D
+    if x is None:
+        return torch.zeros((n, 3), dtype=torch.float64, device=dev)
+    if isinstance(x, torch.Tensor) and x.dim() == 1:
+        return _tensor(x, name, (3,), dev).expand(n, 3)
+    return _tensor(x, name, (E, D, 3), dev).reshape(n, 3)
+
+
+def schedule_targets(waypoints, start, offset, T, E, D, dev):
+    """target_pos [T, E * D, 3] of CtrlAviary.rollout's schedule: waypoints[(start[i] + k) % W][i or 0] + offset[i], built from
+    gathers, expands and sums so that its backward is deterministic (every gather index is hit once per drone)."""
+    n = E * D
+    if not isinstance(waypoints, torch.Tensor):
+        raise ValueError("waypoints must be a float64 tensor [W, 3] or [W, %d, %d, 3]" % (E, D))
+    if waypoints.dim() == 2:
+        W = waypoints.shape[0]
+        wp = _tensor(waypoints, "waypoints", (W, 3), dev)[:, None, :].expand(W, n, 3)
+    else:
+        W = waypoints.shape[0] if waypoints.dim() == 4 else 0
+        wp = _tensor(waypoints, "waypoints", (W, E, D, 3), dev).reshape(W, n, 3)
+    if W == 0:
+        raise ValueError("waypoints must hold at least one row")
+    if start is None:
+        st0 = torch.zeros((n,), dtype=torch.int64, device=dev)
+    else:
+        st0 = start if isinstance(start, torch.Tensor) else torch.as_tensor(start)
+        if st0.dtype.is_floating_point or st0.dtype == torch.bool or st0.numel() not in (1, n):
+            raise ValueError("start must be an integer or integers [%d, %d]" % (E, D))
+        st0 = st0.to(device=dev, dtype=torch.int64).reshape(-1).expand(n)
+    idx = torch.remainder(st0[None, :] + torch.arange(W, device=dev)[:, None], W)           # [W, n]: row of tick k' of drone i
+    rot = torch.gather(wp, 0, idx[:, :, None].expand(W, n, 3))                               # [W, n, 3]: tick k' (k' < W)
+    tpos = rot[:T] if T <= W else rot.repeat((T + W - 1) // W, 1, 1)[:T]
+    if offset is not None:                  # no zero offset when there is none: -0.0 + 0.0 would change the sign of a zero target
+        tpos = tpos + _rows3(offset, "offset", E, D, dev)
+    return tpos
+
+
+def _closed_loop(env, controller, state, last_rpm, phys, waypoints=None, start=None, offset=None, target_rpy=None, target_vel=None,
+                 target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None, pid_state=None):
+    from .control.DSLPIDControl import DSLPIDControl
+    from .control.MRAC import MRAC
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    if isinstance(controller, MRAC):
+        raise ValueError("differentiable_rollout() has no adjoint of MRAC: pass a DSLPIDControl")
+    if not isinstance(controller, DSLPIDControl):
+        raise ValueError("controller must be a DSLPIDControl, got %s" % type(controller).__name__)
+    if controller.num_drones != n:
+        raise ValueError("the controller must be a DSLPIDControl for the env's %d drones (num_drones=%d)" % (n, controller.num_drones))
+    if torch.device(controller.device) != dev:
+        raise ValueError("the controller's state is on %s, the env's on %s" % (controller.device, dev))
+    if waypoints is None:
+        raise ValueError("a controller rollout needs waypoints [W, 3] or [W, %d, %d, 3]" % (E, D))
+    T = (waypoints.shape[0] if isinstance(waypoints, torch.Tensor) else 0) if num_steps is None else int(num_steps)
+    if T <= 0:
+        raise ValueError("num_steps must be > 0")
+    tpos = schedule_targets(waypoints, start, offset, T, E, D, dev)
+    tvel, trpy, trr = (_rows3(x, k, E, D, dev) for x, k in ((target_vel, "target_vel"), (target_rpy, "target_rpy"),
+                                                             (target_rpy_rates, "target_rpy_rates")))
+    CP = controller._P
+    gains = dict(gains or {})
+    bad = set(gains) - set(GAIN_KEYS)
+    if bad:
+        raise ValueError("unknown gains %s (expected some of %s)" % (sorted(bad), ", ".join(GAIN_KEYS)))
+    cols = []
+    for k, f in zip(GAIN_KEYS, ("pid_p_for", "pid_i_for", "pid_d_for", "pid_p_tor", "pid_i_tor", "pid_d_tor")):
+        if k not in gains:
+            cols.append(torch.tensor(list(getattr(CP, f)), dtype=torch.float64, device=dev).expand(E, 3))
+        elif isinstance(gains[k], torch.Tensor) and gains[k].dim() == 1:
+            cols.append(_tensor(gains[k], "gains[%r]" % k, (3,), dev).expand(E, 3))
+        else:
+            cols.append(_tensor(gains[k], "gains[%r]" % k, (E, 3), dev))
+    table = torch.cat(cols, dim=1)
+    pid_state = dict(pid_state or {})
+    bad = set(pid_state) - set(PID_KEYS)
+    if bad:
+        raise ValueError("unknown pid_state keys %s (expected some of %s)" % (sorted(bad), ", ".join(PID_KEYS)))
+    pid0 = torch.cat([_tensor(pid_state[k], "pid_state[%r]" % k, (E, D, 3), dev).reshape(n, 3).t() if k in pid_state
+                      else controller._state[3 * j:3 * j + 3].detach().clone() for j, k in enumerate(PID_KEYS)])
+    planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
+    dt = float(env.CTRL_TIMESTEP if control_timestep is None else control_timestep)
+    with torch.cuda.device(dev):
+        cfg = (env._P, CP, dt, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
+        states, rpm = DynCtrlTrajectory.apply(planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, table, cfg)
+    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out["rpm"] = rpm.reshape(T, E, D, 4)
+    return out

@@ -553,8 +553,11 @@ class BaseAviary(Env):
             return {k: torch.full((self._E,), nom[k], dtype=torch.float64, device=self.device) for k in PHYS_KEYS}
         return {k: self._phys_props[:, j].clone() for j, k in enumerate(PHYS_KEYS)}
 
-    def differentiable_rollout(self, rpm, *, state=None, last_rpm=None, phys=None):
-        """T control ticks of raw RPMs as a differentiable function (torch.autograd), without changing the env.
+    def differentiable_rollout(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None,
+                               target_vel=None, target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None,
+                               pid_state=None, state=None, last_rpm=None, phys=None):
+        """T control ticks of raw RPMs, or of a DSLPIDControl tracking a waypoint schedule, as a differentiable function
+        (torch.autograd), without changing the env.  Pass exactly one of `rpm` (open loop) or `controller` (closed loop).
 
         rpm: [T, E, D, 4] float64 CUDA tensor; tick k applies clip(rpm[k], 0, MAX_RPM) for PYB_STEPS_PER_CTRL substeps, exactly
         as CtrlAviary.step(rpm[k]) does with float64 RPMs.  state: optional dict pos / quat / vel / rpy_rates of [E, D, k] float64
@@ -571,9 +574,28 @@ class BaseAviary(Env):
         torch.clamp (the gradient passes for 0 <= rpm <= MAX_RPM and goes to MAX_RPM above); the ground-effect height clip with
         the forward's predicate; the upright switch as a constant.  Drag's first substep reads the previous tick's RPMs, so
         their gradient flows to rpm[k-1], or to last_rpm for k = 0.  Physics.DYN, PYB, PYB_GND and PYB_DRAG; downwash, inputs
-        that are not float64 CUDA tensors of the right shape on the env's device, and double backward raise ValueError."""
+        that are not float64 CUDA tensors of the right shape on the env's device, and double backward raise ValueError.
+
+        Closed loop: `controller` is a DSLPIDControl(num_drones=E*D) on the env's device, and the schedule arguments mean what
+        they mean in CtrlAviary.rollout: tick k runs `rpm = controller.computeControlFromEnv(env, target_pos, target_rpy,
+        target_vel, target_rpy_rates, control_timestep)` and `step(rpm)`, with target_pos(k, i) = waypoints[(start[i] + k) % W]
+        [i or 0] + offset[i] and the constant target_rpy / target_vel / target_rpy_rates ([E, D, 3] or [3]); the forward is
+        CtrlAviary.rollout(controller=...)'s bits.  waypoints: [W, 3] or [W, E, D, 3] float64 tensor; num_steps defaults to W.
+        gains: optional dict of some of P_COEFF_FOR, I_COEFF_FOR, D_COEFF_FOR, P_COEFF_TOR, I_COEFF_TOR, D_COEFF_TOR -> [3] or
+        [E, 3] float64 tensors, one gain set per aviary (the rest are the controller's current coefficients).  pid_state:
+        optional dict of some of integral_pos_e, last_rpy, integral_rpy_e -> [E, D, 3] (default: a detached copy of the
+        controller's state).  The controller keeps its own constants (mass, KF, max_rpm of its model); `phys` changes the env's
+        physics only.  Every tensor input may require grad, waypoints and offset included.  Returns the four state entries and
+        `rpm` [T, E, D, 4], the applied (clipped) RPMs.  Unlike rollout(), the controller is not touched either: its state and
+        control_counter stay as they were.  The controller's derivative (DESIGN.md 4.5): every clip as torch.clamp (integral
+        clips, torque clip, PWM clip, max_rpm clips), zero where the thrust scalar is <= 0, the forward's branch of the Euler
+        angles' gimbal guard, the rate term without angle unwrap.  An MRAC, a controller of the wrong size or device, both rpm
+        and a controller or neither, and unknown keys raise ValueError."""
         from ..diff import differentiable_rollout
-        return differentiable_rollout(self, rpm, state=state, last_rpm=last_rpm, phys=phys)
+        return differentiable_rollout(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, waypoints=waypoints,
+                                      start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
+                                      target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps,
+                                      gains=gains, pid_state=pid_state)
 
     ################################################################################
 

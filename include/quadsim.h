@@ -636,6 +636,50 @@ int qs_dyn_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones
 int qs_dyn_traj_vjp(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                     void* stream);
 
+/* Differentiable closed-loop trajectories (DESIGN.md 4.5): T control ticks of a DSLPIDControl tracking per-tick targets around
+ * Physics.DYN (+ GND and/or DRAG, no downwash), and their VJP.  Tick k is the QS_CTRL_TRACK tick of qs_ctrl_rollout, in the same
+ * order: pid_control with the controller's QsParams `cp` (its gains, or the aviary's row of `gains`; its model constants), the
+ * controller's max_rpm clip, the env's clip (row MAX_RPM), `substeps` substeps.  States as in QsDynTrajIO; a controller state is
+ * [9][N] (integral_pos_e, last_rpy, integral_rpy_e).  The VJP follows QsDynTrajIO's decisions for the physics and clips every
+ * controller clip as torch.clamp; the target yaw is target_rpy[i][2] (the only component the controller reads).  One thread per
+ * drone; deterministic (per-drone gradients of per-aviary rows, no atomics). */
+typedef struct QsDynCtrlTrajIO {
+    int T;                          /* ticks, > 0 */
+    int pad_;
+    double control_timestep;        /* the controller's dt, > 0 */
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* pid0;             /* [9][N] the controller state before tick 0 */
+    const double* target_pos;       /* [T][N][3] */
+    const double* target_vel;       /* [N][3], nullable = zeros */
+    const double* target_rpy;       /* [N][3], nullable = zeros */
+    const double* target_rpy_rates; /* [N][3], nullable = zeros */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows; nullable = the constants of the env's QsParams */
+    const double* gains;            /* [n_envs][18] P_FOR, I_FOR, D_FOR, P_TOR, I_TOR, D_TOR; nullable = cp's */
+    double* states;                 /* qs_dyn_ctrl_traj out: [T][13 N], entry k = the state after tick k */
+    double* rpm;                    /* qs_dyn_ctrl_traj out: [T][N][4] the applied (clipped) RPMs */
+    double* pid_states;             /* qs_dyn_ctrl_traj out: [T][9][N] the controller state at the start of tick k */
+    /* qs_dyn_ctrl_traj_vjp: states, rpm and pid_states are read (the forward's outputs), and */
+    const double* g_states;         /* [T][13 N] cotangents of the states */
+    const double* g_rpm_out;        /* [T][N][4] cotangents of rpm, nullable = zeros */
+    double* g_state0;               /* out [13 N] */
+    double* g_pid0;                 /* out [9][N], nullable */
+    double* g_target_pos;           /* out [T][N][3], nullable */
+    double* g_target_vel;           /* out [N][3], nullable */
+    double* g_target_rpy;           /* out [N][3] (components 0 and 1 are zero), nullable */
+    double* g_target_rpy_rates;     /* out [N][3], nullable */
+    double* g_last_rpm;             /* out [N][4], nullable */
+    double* g_phys;                 /* out [N][16]: PER DRONE (sum the drones of an aviary for its row); nullable */
+    double* g_gains;                /* out [N][18]: PER DRONE; nullable */
+    double* scratch;                /* [substeps][13][N] workspace */
+} QsDynCtrlTrajIO;
+int qs_sizeof_dyn_ctrl_traj_io(void);
+/* cp: HOST pointer to the controller's QsParams.  effects as qs_dyn_traj. */
+int qs_dyn_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env, int substeps,
+                     unsigned effects, void* stream);
+int qs_dyn_ctrl_traj_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
+                         int substeps, unsigned effects, void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
