@@ -13,8 +13,8 @@ _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))    # override: A/B builds in tools/
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
-                                             "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
+                                             "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu")]
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -151,6 +151,14 @@ class QsDynCtrlTrajIO(C.Structure):
         "g_target_rpy", "g_target_rpy_rates", "g_last_rpm", "g_phys", "g_gains", "scratch")]
 
 
+class QsDynPolicyTrajIO(C.Structure):
+    _fields_ = [("T", C.c_int), ("act_buffer_size", C.c_int), ("activation", C.c_int), ("depth", C.c_int),
+                ("width", C.c_int * MLP_MAX_HIDDEN), ("in_dim", C.c_int), ("out_dim", C.c_int),
+                ("w", C.c_void_p * (MLP_MAX_HIDDEN + 1)), ("b", C.c_void_p * (MLP_MAX_HIDDEN + 1))] + [(n, C.c_void_p) for n in (
+        "log_std", "noise", "state0", "last_rpm", "phys", "action_buffer", "states", "actions", "obs", "g_states", "g_actions",
+        "g_raw", "g_state0", "g_last_rpm", "g_phys", "g_action_buffer", "scratch")]
+
+
 class QsStepCall(C.Structure):
     _fields_ = [("p", C.c_void_p), ("st", C.c_void_p), ("io", C.c_void_p),
                 ("act_type", C.c_int), ("task", C.c_int), ("n_envs", C.c_int), ("drones_per_env", C.c_int), ("substeps", C.c_int),
@@ -163,7 +171,7 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io", "qs_rollout_mlp", "qs_rollout_mlp_max_ticks", "qs_sizeof_mlp_policy",
            "qs_mrac_control", "qs_mrac_control_state", "qs_ctrl_rollout_mrac", "qs_sizeof_mrac_params", "qs_sizeof_mrac_rollout_io",
            "qs_dyn_traj", "qs_dyn_traj_vjp", "qs_sizeof_dyn_traj_io", "qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp",
-           "qs_sizeof_dyn_ctrl_traj_io"]
+           "qs_sizeof_dyn_ctrl_traj_io", "qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp", "qs_sizeof_dyn_policy_traj_io"]
 MAX_PEERS = 16
 
 
@@ -263,6 +271,11 @@ def lib():
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajIO), C.c_int, C.c_int, C.c_int,
                                   C.c_uint, C.c_void_p]
     L.qs_sizeof_dyn_ctrl_traj_io.restype = C.c_int
+    for n in ("qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynPolicyTrajIO), C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint,
+                                  C.c_void_p]
+    L.qs_sizeof_dyn_policy_traj_io.restype = C.c_int
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -318,9 +331,10 @@ def lib():
     if L.qs_sizeof_log_ring() != C.sizeof(QsLogRing) or L.qs_sizeof_host_io() != C.sizeof(QsHostIO) or \
             L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy) or \
             L.qs_sizeof_mrac_params() != C.sizeof(QsMracParams) or L.qs_sizeof_mrac_rollout_io() != C.sizeof(QsMracRolloutIO) or \
-            L.qs_sizeof_dyn_traj_io() != C.sizeof(QsDynTrajIO) or L.qs_sizeof_dyn_ctrl_traj_io() != C.sizeof(QsDynCtrlTrajIO):
+            L.qs_sizeof_dyn_traj_io() != C.sizeof(QsDynTrajIO) or L.qs_sizeof_dyn_ctrl_traj_io() != C.sizeof(QsDynCtrlTrajIO) or \
+            L.qs_sizeof_dyn_policy_traj_io() != C.sizeof(QsDynPolicyTrajIO):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac / "
-                          "dyn traj io / dyn ctrl traj io): "
+                          "dyn traj io / dyn ctrl traj io / dyn policy traj io): "
                           "rebuild")
     _lib = L
     return L

@@ -239,4 +239,27 @@ QS_HD void dyn_tick_vjp(const QsParams& P, const PhysRow& c, const Drone& d0, co
     L.qz = (L.qz - x0.qz * dot) * inv; L.qw = (L.qw - x0.qw * dot) * inv;
 }
 
+// Lq += d rpy / d q ^T Lrpy for rpy = quat_to_euler<false>(q), on the forward's branch of the +-0.99999 gimbal guard
+// (the controller's adjoint, pid_adjoint.cuh, and the policy loop's observation head, mlp_adjoint.cuh)
+QS_HD void quat_to_euler_vjp(double qx, double qy, double qz, double qw, const double Lrpy[3], double Lq[4]) {
+    const double sarg = -2.0 * (qx * qz - qw * qy);
+    if (sarg <= -0.99999 || sarg >= 0.99999) {
+        // roll and pitch are constants; yaw = 2 atan2(x, -y) or 2 atan2(-x, y): the same derivative
+        const double r2 = qx * qx + qy * qy;
+        Lq[0] += Lrpy[2] * (-2.0 * qy / r2);
+        Lq[1] += Lrpy[2] * (2.0 * qx / r2);
+    } else {
+        const double ra = 2.0 * (qy * qz + qw * qx), rb = qw * qw - qx * qx - qy * qy + qz * qz;
+        const double ya = 2.0 * (qx * qy + qw * qz), yb = qw * qw + qx * qx - qy * qy - qz * qz;
+        const double n_r = ra * ra + rb * rb, n_y = ya * ya + yb * yb;
+        const double Lra = Lrpy[0] * rb / n_r, Lrb = -Lrpy[0] * ra / n_r;
+        const double Ls = Lrpy[1] / sqrt(1.0 - sarg * sarg);
+        const double Lya = Lrpy[2] * yb / n_y, Lyb = -Lrpy[2] * ya / n_y;
+        Lq[0] += 2.0 * (qw * Lra - qx * Lrb - qz * Ls + qy * Lya + qx * Lyb);
+        Lq[1] += 2.0 * (qz * Lra - qy * Lrb + qw * Ls + qx * Lya - qy * Lyb);
+        Lq[2] += 2.0 * (qy * Lra + qz * Lrb - qx * Ls + qw * Lya - qz * Lyb);
+        Lq[3] += 2.0 * (qx * Lra + qw * Lrb + qy * Ls + qz * Lya + qw * Lyb);
+    }
+}
+
 }  // namespace qs

@@ -182,25 +182,9 @@ QS_HD_NOINLINE void pid_control_vjp(const QsParams& P, const PidGains& K, const 
     }
     Lst.ipx = Lip_old[0]; Lst.ipy = Lip_old[1]; Lst.ipz = Lip_old[2];
     // rpy = quat_to_euler<false>(q), on the forward's branch
-    double LX = 0.0, LY = 0.0, LZ = 0.0, LW = 0.0;
-    const double sarg = -2.0 * (qx * qz - qw * qy);
-    if (sarg <= -0.99999 || sarg >= 0.99999) {
-        // roll and pitch are constants; yaw = 2 atan2(x, -y) or 2 atan2(-x, y): the same derivative
-        const double r2 = qx * qx + qy * qy;
-        LX += Lrpy[2] * (-2.0 * qy / r2);
-        LY += Lrpy[2] * (2.0 * qx / r2);
-    } else {
-        const double ra = 2.0 * (qy * qz + qw * qx), rb = qw * qw - qx * qx - qy * qy + qz * qz;
-        const double ya = 2.0 * (qx * qy + qw * qz), yb = qw * qw + qx * qx - qy * qy - qz * qz;
-        const double n_r = ra * ra + rb * rb, n_y = ya * ya + yb * yb;
-        const double Lra = Lrpy[0] * rb / n_r, Lrb = -Lrpy[0] * ra / n_r;
-        const double Ls = Lrpy[1] / sqrt(1.0 - sarg * sarg);
-        const double Lya = Lrpy[2] * yb / n_y, Lyb = -Lrpy[2] * ya / n_y;
-        LX += 2.0 * (qw * Lra - qx * Lrb - qz * Ls + qy * Lya + qx * Lyb);
-        LY += 2.0 * (qz * Lra - qy * Lrb + qw * Ls + qx * Lya - qy * Lyb);
-        LZ += 2.0 * (qy * Lra + qz * Lrb - qx * Ls + qw * Lya - qz * Lyb);
-        LW += 2.0 * (qx * Lra + qw * Lrb + qy * Ls + qz * Lya + qw * Lyb);
-    }
+    double Lqe[4] = {0.0, 0.0, 0.0, 0.0};
+    quat_to_euler_vjp(qx, qy, qz, qw, Lrpy, Lqe);
+    double LX = Lqe[0], LY = Lqe[1], LZ = Lqe[2], LW = Lqe[3];
     // R = I + s M(q), s = 2 / |q|^2 (quat_to_matrix)
     {
         const double dq = qx * qx + qy * qy + qz * qz + qw * qw;

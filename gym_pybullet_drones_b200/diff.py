@@ -1,5 +1,6 @@
-"""Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs) and
-qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop) (include/quadsim.h, DESIGN.md 4.5).
+"""Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs),
+qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop) and qs_dyn_policy_traj / qs_dyn_policy_traj_vjp (an
+MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5).
 BaseAviary.differentiable_rollout is the public entry point; this module packs the state into the kernels' planes layout, runs
 the forward and backward kernels and unpacks the result."""
 import ctypes as C
@@ -130,6 +131,102 @@ class DynCtrlTrajectory(torch.autograd.Function):
                 g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), g["g_gains"].view(E, D, 18).sum(dim=1), None)
 
 
+def actor64(params, activation, obs, noise=None):
+    """The raw action [..., out] of the MlpPolicy actor with float64 `params` = [W1, b1, ..., Wout, bout, log_std] on observation
+    rows obs [..., in]: mean + exp(log_std) * noise (noise=None: the mean)."""
+    act = torch.tanh if activation == "tanh" else torch.relu
+    h = obs
+    for k in range(0, len(params) - 3, 2):
+        h = act(h @ params[k] + params[k + 1])
+    raw = h @ params[-3] + params[-2]
+    return raw if noise is None else raw + torch.exp(params[-1]) * noise
+
+
+class PolicyTrajectory(torch.autograd.Function):
+    """(states [T, 13 N], raw actions [T, N, A], obs [T, E, in]) = the T ticks of qs_dyn_policy_traj from planes0 [13 N] and the
+    action buffer abuf [N, B, A], with last_rpm [N, 4], the per-aviary rows [E, 16], noise [T, E, out] (or None) and the actor's
+    float64 parameters `theta` ([W1, b1, ..., Wout, bout, log_std]).  backward = qs_dyn_policy_traj_vjp, which carries the
+    sequential dependency and returns g_raw, the cotangent of every raw action; the gradients of theta and noise are then one
+    batched autograd pass of the actor over the T * E saved observation rows (deterministic, any architecture).  obs is not
+    differentiable.  `cfg` = (QsParams, act_type, activation, B, E, D, A, substeps, effects, T)."""
+
+    @staticmethod
+    def _io(cfg, T, theta, ins, outs):
+        activation, B = cfg[2], cfg[3]
+        io = N.QsDynPolicyTrajIO()
+        io.T, io.act_buffer_size, io.activation = T, B, N.MLP_TANH if activation == "tanh" else N.MLP_RELU
+        io.depth = len(theta) // 2 - 1
+        for l in range(io.depth + 1):
+            io.w[l], io.b[l] = theta[2 * l].data_ptr(), theta[2 * l + 1].data_ptr()
+            if l < io.depth:
+                io.width[l] = theta[2 * l].shape[1]
+        io.in_dim, io.out_dim = theta[0].shape[0], theta[-3].shape[1]
+        io.log_std = theta[-1].data_ptr()
+        for k, x in list(ins.items()) + list(outs.items()):
+            setattr(io, k, None if x is None else x.data_ptr())
+        return io
+
+    @staticmethod
+    def forward(ctx, planes0, last_rpm, rows, abuf, noise, cfg, *theta):
+        theta = tuple(t.contiguous() for t in theta)
+        ins = dict(state0=planes0.contiguous(), last_rpm=last_rpm.contiguous(), phys=rows.contiguous(), action_buffer=abuf.contiguous(),
+                   noise=None if noise is None else noise.contiguous())
+        P, act_type, activation, B, E, D, A, S, eff, T = cfg
+        n = E * D
+        f64 = dict(dtype=torch.float64, device=planes0.device)
+        outs = dict(states=torch.empty((T, 13 * n), **f64), actions=torch.empty((T, n, A), **f64),
+                    obs=torch.empty((T, E, theta[0].shape[0]), **f64))
+        io = PolicyTrajectory._io(cfg, T, theta, ins, outs)
+        with torch.cuda.device(planes0.device):
+            N.check(N.lib().qs_dyn_policy_traj(C.byref(P), C.byref(io), act_type, E, D, S, eff, torch.cuda.current_stream().cuda_stream),
+                    "qs_dyn_policy_traj")
+        ctx.save_for_backward(*(x for x in ins.values() if x is not None), *outs.values(), *theta)
+        ctx.cfg, ctx.has_noise = cfg, noise is not None
+        ctx.mark_non_differentiable(outs["obs"])
+        return outs["states"], outs["actions"], outs["obs"]
+
+    @staticmethod
+    def backward(ctx, g_states, g_actions, _g_obs):
+        if torch.is_grad_enabled():
+            raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
+                             "derivative of its own")
+        saved = list(ctx.saved_tensors)
+        keys = ["state0", "last_rpm", "phys", "action_buffer"] + (["noise"] if ctx.has_noise else [])
+        ins = dict(zip(keys, saved[:len(keys)]))
+        ins.setdefault("noise", None)
+        outs = dict(zip(("states", "actions", "obs"), saved[len(keys):len(keys) + 3]))
+        theta = saved[len(keys) + 3:]
+        cfg = ctx.cfg
+        P, act_type, activation, B, E, D, A, S, eff, T = cfg
+        n = E * D
+        f64 = dict(dtype=torch.float64, device=outs["states"].device)
+        grads = dict(g_raw=torch.empty((T, n, A), **f64), g_state0=torch.empty((13 * n,), **f64), g_last_rpm=torch.empty((n, 4), **f64),
+                     g_phys=torch.empty((n, 16), **f64), g_action_buffer=torch.empty((n, B, A), **f64))
+        outs.update(g_states=g_states.to(torch.float64).contiguous(), g_actions=g_actions.to(torch.float64).contiguous(),
+                    scratch=torch.empty((S, 13, n), **f64))
+        io = PolicyTrajectory._io(cfg, T, theta, ins, dict(outs, **grads))
+        with torch.cuda.device(outs["states"].device):
+            N.check(N.lib().qs_dyn_policy_traj_vjp(C.byref(P), C.byref(io), act_type, E, D, S, eff,
+                                                   torch.cuda.current_stream().cuda_stream), "qs_dyn_policy_traj_vjp")
+        # the parameters' (and the noise's) gradients: raw[k, e] = actor(obs[k, e]) + exp(log_std) noise[k, e] with cotangent g_raw
+        g_raw = grads["g_raw"].view(T, E, D * A)
+        need = [j for j in range(len(theta)) if ctx.needs_input_grad[6 + j]]
+        g_theta, g_noise = [None] * len(theta), None
+        want_noise = ctx.has_noise and ctx.needs_input_grad[4]
+        if need or want_noise:
+            with torch.enable_grad():
+                leaves = [t.detach().requires_grad_(j in need) for j, t in enumerate(theta)]
+                eps = ins["noise"].detach().requires_grad_(True) if want_noise else ins["noise"]
+                raw = actor64(leaves, activation, outs["obs"], eps)
+                got = torch.autograd.grad(raw, [leaves[j] for j in need] + ([eps] if want_noise else []), g_raw, allow_unused=True)
+            for j, g in zip(need, got):
+                g_theta[j] = g
+            if want_noise:
+                g_noise = got[-1]
+        return (grads["g_state0"], grads["g_last_rpm"], grads["g_phys"].view(E, D, 16).sum(dim=1), grads["g_action_buffer"], g_noise, None,
+                *g_theta)
+
+
 def _tensor(x, name, shape, device):
     if not isinstance(x, torch.Tensor):
         raise ValueError("%s must be a torch tensor, got %s" % (name, type(x).__name__))
@@ -176,13 +273,23 @@ def _start_state(env, state, last_rpm, phys):
     return planes0, last_rpm, rows
 
 
-def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, **schedule):
+def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
+                           action_buffer=None, **schedule):
     """BaseAviary.differentiable_rollout (see there)."""
     if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
         raise ValueError("differentiable_rollout() does not support downwash: the pairwise term has no adjoint (use Physics.DYN, PYB, "
                          "PYB_GND or PYB_DRAG)")
-    if (rpm is None) == (controller is None):
-        raise ValueError("differentiable_rollout() takes exactly one of rpm [T, E, D, 4] (open loop) or controller= (closed loop)")
+    if (rpm is not None) + (controller is not None) + (policy is not None) != 1:
+        raise ValueError("differentiable_rollout() takes exactly one of rpm [T, E, D, 4] (open loop), controller= (closed loop) or "
+                         "policy= (an MlpPolicy in the loop)")
+    if policy is not None:
+        given = sorted(k for k, v in schedule.items() if v is not None and k != "num_steps")
+        if given:
+            raise ValueError("%s apply to a controller rollout only" % ", ".join(given))
+        return _policy_loop(env, policy, params, noise, action_buffer, schedule.get("num_steps"), state, last_rpm, phys)
+    given = sorted(k for k, v in (("params", params), ("noise", noise), ("action_buffer", action_buffer)) if v is not None)
+    if given:
+        raise ValueError("%s apply to a policy rollout only" % ", ".join(given))
     if controller is not None:
         return _closed_loop(env, controller, state, last_rpm, phys, **schedule)
     given = sorted(k for k, v in schedule.items() if v is not None)
@@ -289,4 +396,55 @@ def _closed_loop(env, controller, state, last_rpm, phys, waypoints=None, start=N
         states, rpm = DynCtrlTrajectory.apply(planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, table, cfg)
     out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
     out["rpm"] = rpm.reshape(T, E, D, 4)
+    return out
+
+
+def _policy_loop(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys):
+    from .policy import MlpPolicy
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    if not isinstance(policy, MlpPolicy):
+        raise ValueError("policy must be an MlpPolicy, got %s" % type(policy).__name__)
+    act_type = env._act_type()
+    if act_type not in (N.ACT_RPM, N.ACT_ONE_D_RPM):
+        raise ValueError("differentiable_rollout(policy=) supports ActionType.RPM and ONE_D_RPM: PID, VEL and ONE_D_PID run the embedded "
+                         "DSLPID controller inside the policy loop, which has no adjoint yet")
+    A, B, od = env._A, env._B, env._obs_dim
+    if B == 0:
+        raise ValueError("differentiable_rollout(policy=) needs an action buffer: ctrl_freq=%d gives ACTION_BUFFER_SIZE = 0" % env.CTRL_FREQ)
+    if policy.in_dim != D * od or policy.out_dim != D * A:
+        raise ValueError("policy must map %d inputs to %d outputs, not %d to %d" % (D * od, D * A, policy.in_dim, policy.out_dim))
+    if torch.device(policy.device) != dev:
+        raise ValueError("the policy's weights are on %s, the env's state on %s" % (policy.device, dev))
+    shapes = [tuple(t.shape) for wb in policy.actor for t in wb] + [tuple(policy.log_std.shape)]
+    if params is None:
+        theta = [t.detach().double() for wb in policy.actor for t in wb] + [policy.log_std.detach().double()]
+    else:
+        theta = list(params)
+        if len(theta) != len(shapes):
+            raise ValueError("params must be the %d tensors of policy.parameters64() (weight and bias per actor layer, then log_std), "
+                             "got %d" % (len(shapes), len(theta)))
+        for j, (t, sh) in enumerate(zip(theta, shapes)):
+            _tensor(t, "params[%d]" % j, sh, dev)
+    if noise is None:
+        if num_steps is None:
+            raise ValueError("a policy rollout needs num_steps (or noise [T, %d, %d])" % (E, D * A))
+        T = int(num_steps)
+    else:
+        T = noise.shape[0] if isinstance(noise, torch.Tensor) and noise.dim() == 3 else 0
+        if num_steps is not None and int(num_steps) != T:
+            raise ValueError("noise must be [num_steps, %d, %d]" % (E, D * A))
+        _tensor(noise, "noise", (T, E, D * A), dev)
+    if T <= 0:
+        raise ValueError("num_steps must be > 0")
+    if action_buffer is None:
+        action_buffer = env._by_id(env._obs_buf[env._cur][:, 12:]).detach().double().reshape(n, B, A)
+    else:
+        action_buffer = _tensor(action_buffer, "action_buffer", (E, D, B, A), dev).reshape(n, B, A)
+    planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
+    with torch.cuda.device(dev):
+        cfg = (env._P, act_type, policy.activation, B, E, D, A, env.PYB_STEPS_PER_CTRL, env._effects, T)
+        states, actions, obs = PolicyTrajectory.apply(planes0, last_rpm, rows, action_buffer, noise, cfg, *theta)
+    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out["actions"] = actions.reshape(T, E, D, A)
+    out["obs"] = obs.reshape(T, E, D, od)
     return out

@@ -555,9 +555,11 @@ class BaseAviary(Env):
 
     def differentiable_rollout(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None,
                                target_vel=None, target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None,
-                               pid_state=None, state=None, last_rpm=None, phys=None):
-        """T control ticks of raw RPMs, or of a DSLPIDControl tracking a waypoint schedule, as a differentiable function
-        (torch.autograd), without changing the env.  Pass exactly one of `rpm` (open loop) or `controller` (closed loop).
+                               pid_state=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
+                               action_buffer=None):
+        """T control ticks of raw RPMs, of a DSLPIDControl tracking a waypoint schedule, or of an MlpPolicy acting on the
+        aviary's observations, as a differentiable function (torch.autograd), without changing the env.  Pass exactly one of
+        `rpm` (open loop), `controller` (closed loop) or `policy` (policy loop, at the end of this text).
 
         rpm: [T, E, D, 4] float64 CUDA tensor; tick k applies clip(rpm[k], 0, MAX_RPM) for PYB_STEPS_PER_CTRL substeps, exactly
         as CtrlAviary.step(rpm[k]) does with float64 RPMs.  state: optional dict pos / quat / vel / rpy_rates of [E, D, k] float64
@@ -590,9 +592,27 @@ class BaseAviary(Env):
         control_counter stay as they were.  The controller's derivative (DESIGN.md 4.5): every clip as torch.clamp (integral
         clips, torque clip, PWM clip, max_rpm clips), zero where the thrust scalar is <= 0, the forward's branch of the Euler
         angles' gimbal guard, the rate term without angle unwrap.  An MRAC, a controller of the wrong size or device, both rpm
-        and a controller or neither, and unknown keys raise ValueError."""
+        and a controller or neither, and unknown keys raise ValueError.
+
+        Policy loop (HoverAviary / MultiHoverAviary with ActionType.RPM or ONE_D_RPM): `policy` is an MlpPolicy mapping
+        D * obs_dim inputs to D * A outputs, `params` its float64 parameters as `policy.parameters64()` lays them out ([W1, b1,
+        ..., Wout, bout, log_std]; None: detached copies of the policy's weights), `num_steps` the tick count, `noise`
+        [T, E, D * A] float64 standard-normal draws (None: the mean action), `action_buffer` [E, D, B, A] the buffered actions
+        before tick 0, oldest first (default: a detached float64 copy of the env's).  Tick k builds the aviary's observation
+        [D, 12 + B A] in float64 from the state after tick k - 1 (pos, rpy, vel, ang_v, then the B buffered actions as
+        _computeObs lays them out), evaluates raw = actor(obs) + exp(log_std) noise[k], puts a = clip(raw, -1, 1) into the
+        buffer and flies rpm = HOVER_RPM (1 + 0.05 a) (ONE_D_RPM: on all four motors) under the MAX_RPM clip.  Returns the four
+        state entries, `actions` [T, E, D, A] (the raw, unclipped actions, differentiable) and `obs` [T, E, D, obs_dim] (what the
+        policy saw; a constant for autograd).  Gradients reach every tensor of params, state, last_rpm, phys, action_buffer and
+        noise (two kernel launches and one batched actor pass per backward, DESIGN.md 4.5); the action clip is torch.clamp,
+        ReLU passes where the unit is positive.  The whole loop is float64, so it does not have the bits of rollout(policy=),
+        which evaluates the actor at float32 accuracy on the tensor cores and decodes float32 actions: the two agree to
+        float32 level over short horizons (tests/test_gpu_diff_policy.py holds the bound).  No reward, flags or autoreset.
+        PID / VEL / ONE_D_PID actions, a policy of the wrong size or device, ctrl_freq with an empty action buffer and an
+        observation too wide for a CTA's shared memory raise ValueError."""
         from ..diff import differentiable_rollout
-        return differentiable_rollout(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, waypoints=waypoints,
+        return differentiable_rollout(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, policy=policy,
+                                      params=params, noise=noise, action_buffer=action_buffer, waypoints=waypoints,
                                       start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
                                       target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps,
                                       gains=gains, pid_state=pid_state)

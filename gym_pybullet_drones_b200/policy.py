@@ -220,6 +220,34 @@ class MlpPolicy:
         c.actor, c.critic, c.log_std = f64(self.actor), f64(self.critic), self.log_std.double()
         return c
 
+    # ---- float64 parameters of the actor (differentiable_rollout(policy=)) -------------------------------------------------
+    def parameters64(self):
+        """[W1, b1, ..., Wout, bout, log_std]: float64 CUDA copies of the actor's weights ([in, out]), biases and log_std as
+        leaves that require grad: what `differentiable_rollout(policy=self, params=...)` differentiates and an optimiser
+        updates.  The critic is not part of it."""
+        out = [t.detach().double().clone().requires_grad_(True) for wb in self.actor for t in wb]
+        return out + [self.log_std.detach().double().clone().requires_grad_(True)]
+
+    def load_parameters(self, params):
+        """Writes a `parameters64()`-shaped list back into the actor (rounded to the weights' dtype) and re-packs the fp16
+        fragments `rollout(policy=self)` reads.  The critic is left alone."""
+        params = list(params)
+        if len(params) != 2 * len(self.actor) + 1:
+            raise ValueError("load_parameters takes %d tensors (weight and bias per actor layer, then log_std), got %d"
+                             % (2 * len(self.actor) + 1, len(params)))
+        new = []
+        for k, (w, b) in enumerate(self.actor):
+            nw, nb = params[2 * k], params[2 * k + 1]
+            if tuple(nw.shape) != tuple(w.shape) or tuple(nb.shape) != tuple(b.shape):
+                raise ValueError("load_parameters: layer %d must be weight %s and bias %s" % (k, tuple(w.shape), tuple(b.shape)))
+            new.append((nw.detach().to(device=w.device, dtype=w.dtype).contiguous().clone(),
+                        nb.detach().to(device=b.device, dtype=b.dtype).contiguous().clone()))
+        if tuple(params[-1].shape) != tuple(self.log_std.shape):
+            raise ValueError("load_parameters: log_std must be %s" % (tuple(self.log_std.shape),))
+        self.actor = new
+        self.log_std = params[-1].detach().to(device=self.log_std.device, dtype=self.log_std.dtype).contiguous().clone()
+        self._split = dict(self._split, actor=self._prepare(self.actor, 8 * self.nt3))
+
     # ---- C structs ------------------------------------------------------------------------------------------------------
     def c_struct(self, noise=None, logprob=None, values=None):
         """QsPolicy (qs_rollout): the [64, 64] Tanh network only."""

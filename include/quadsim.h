@@ -680,6 +680,53 @@ int qs_dyn_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajI
 int qs_dyn_ctrl_traj_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
                          int substeps, unsigned effects, void* stream);
 
+/* Differentiable policy trajectories (DESIGN.md 4.5): T control ticks of an MLP actor driving Physics.DYN (+ GND and/or DRAG, no
+ * downwash) through the RPM or ONE_D_RPM action decode, and their VJP.  Tick k: the aviary's float64 observation
+ * [D][12 + B A] (pos, rpy, vel, ang_v = R_last w, then the B buffered clipped actions, oldest first) of the state after tick
+ * k - 1 (of state0 for k = 0, with R_last = R(q0 / |q0|)); raw = actor(obs) + exp(log_std) noise[k]; a = clip(raw, -1, 1)
+ * enters the buffer; rpm = HOVER_RPM (1 + 0.05 a) (ONE_D_RPM: on all four motors), the env's MAX_RPM clip, `substeps` substeps.
+ * The actor is flatten -> `depth` hidden layers (width[l] units, `activation` after each) -> linear, weights float64 row-major
+ * [in][out].  A CTA owns whole aviaries for all T ticks.  The VJP follows QsDynTrajIO's decisions for the physics, clips the
+ * action as torch.clamp, differentiates ReLU as h > 0 and the Euler angles on the forward's branch of the gimbal guard.  It
+ * writes g_raw, the cotangent of every raw action (what the actor's weights, log_std and the noise need: one batched pass over
+ * the saved observations); the weights' gradients themselves are not formed here.  Deterministic (no atomics). */
+typedef struct QsDynPolicyTrajIO {
+    int T;                          /* ticks, > 0 */
+    int act_buffer_size;            /* B > 0 */
+    int activation;                 /* QS_MLP_TANH or QS_MLP_RELU */
+    int depth;                      /* hidden layers, 1 .. QS_MLP_MAX_HIDDEN */
+    int width[QS_MLP_MAX_HIDDEN];   /* hidden widths, 1 .. QS_MLP_MAX_WIDTH (unpadded) */
+    int in_dim, out_dim;            /* D (12 + B A) and D A <= 32 */
+    const double* w[QS_MLP_MAX_HIDDEN + 1];   /* [in][out] row-major per layer */
+    const double* b[QS_MLP_MAX_HIDDEN + 1];   /* [out] */
+    const double* log_std;          /* [out_dim] */
+    const double* noise;            /* [T][n_envs][out_dim], nullable = the mean action */
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows; nullable = the constants of QsParams */
+    const double* action_buffer;    /* [N][B][A] the buffered actions before tick 0, oldest first */
+    double* states;                 /* qs_dyn_policy_traj out: [T][13 N], entry k = the state after tick k */
+    double* actions;                /* qs_dyn_policy_traj out: [T][N][A] the raw (unclipped) actions */
+    double* obs;                    /* qs_dyn_policy_traj out: [T][n_envs][in_dim] what the actor saw at tick k */
+    /* qs_dyn_policy_traj_vjp: states, actions and obs are read (the forward's outputs), and */
+    const double* g_states;         /* [T][13 N] cotangents of the states */
+    const double* g_actions;        /* [T][N][A] cotangents of the raw actions, nullable = zeros */
+    double* g_raw;                  /* out [T][N][A]: the whole cotangent of raw action k (g_actions included) */
+    double* g_state0;               /* out [13 N] */
+    double* g_last_rpm;             /* out [N][4], nullable */
+    double* g_phys;                 /* out [N][16]: PER DRONE (sum the drones of an aviary for its row); nullable */
+    double* g_action_buffer;        /* out [N][B][A], nullable */
+    double* scratch;                /* [substeps][13][N] workspace */
+} QsDynPolicyTrajIO;
+int qs_sizeof_dyn_policy_traj_io(void);
+/* act_type: QS_ACT_RPM or QS_ACT_ONE_D_RPM (others: QS_ERR_UNSUPPORTED).  effects as qs_dyn_traj.  QS_ERR_UNSUPPORTED also for
+ * drones_per_env > 32 or D A > 32, and where the VJP's rows of 8 aviaries (per aviary in_dim + depth * max width + out_dim +
+ * 2 max(in_dim, max width) + D B A doubles) exceed the 227 KB of a CTA's shared memory: the forward refuses what its VJP would. */
+int qs_dyn_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env, int substeps,
+                       unsigned effects, void* stream);
+int qs_dyn_policy_traj_vjp(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env,
+                           int substeps, unsigned effects, void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
