@@ -13,8 +13,8 @@ _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))    # override: A/B builds in tools/
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
-                                             "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
+                                             "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu")]
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -144,6 +144,11 @@ class QsDynTrajIO(C.Structure):
         "state0", "rpm", "last_rpm", "phys", "states", "g_states", "g_rpm", "g_state0", "g_last_rpm", "g_phys", "scratch")]
 
 
+class QsDynTrajJvpIO(C.Structure):
+    _fields_ = [("T", C.c_int), ("pad_", C.c_int)] + [(n, C.c_void_p) for n in (
+        "state0", "rpm", "last_rpm", "phys", "states", "t_state0", "t_rpm", "t_last_rpm", "t_phys", "t_states", "jac")]
+
+
 class QsDynCtrlTrajIO(C.Structure):
     _fields_ = [("T", C.c_int), ("pad_", C.c_int), ("control_timestep", C.c_double)] + [(n, C.c_void_p) for n in (
         "state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains",
@@ -171,7 +176,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_ctrl_rollout", "qs_sizeof_ctrl_rollout_io", "qs_rollout_mlp", "qs_rollout_mlp_max_ticks", "qs_sizeof_mlp_policy",
            "qs_mrac_control", "qs_mrac_control_state", "qs_ctrl_rollout_mrac", "qs_sizeof_mrac_params", "qs_sizeof_mrac_rollout_io",
            "qs_dyn_traj", "qs_dyn_traj_vjp", "qs_sizeof_dyn_traj_io", "qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp",
-           "qs_sizeof_dyn_ctrl_traj_io", "qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp", "qs_sizeof_dyn_policy_traj_io"]
+           "qs_sizeof_dyn_ctrl_traj_io", "qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp", "qs_sizeof_dyn_policy_traj_io",
+           "qs_dyn_traj_jvp", "qs_dyn_tick_jac", "qs_sizeof_dyn_traj_jvp_io"]
 MAX_PEERS = 16
 
 
@@ -266,6 +272,10 @@ def lib():
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
     L.qs_sizeof_dyn_traj_io.restype = C.c_int
+    for n in ("qs_dyn_traj_jvp", "qs_dyn_tick_jac"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajJvpIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
+    L.qs_sizeof_dyn_traj_jvp_io.restype = C.c_int
     for n in ("qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajIO), C.c_int, C.c_int, C.c_int,
@@ -332,9 +342,9 @@ def lib():
             L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy) or \
             L.qs_sizeof_mrac_params() != C.sizeof(QsMracParams) or L.qs_sizeof_mrac_rollout_io() != C.sizeof(QsMracRolloutIO) or \
             L.qs_sizeof_dyn_traj_io() != C.sizeof(QsDynTrajIO) or L.qs_sizeof_dyn_ctrl_traj_io() != C.sizeof(QsDynCtrlTrajIO) or \
-            L.qs_sizeof_dyn_policy_traj_io() != C.sizeof(QsDynPolicyTrajIO):
+            L.qs_sizeof_dyn_policy_traj_io() != C.sizeof(QsDynPolicyTrajIO) or L.qs_sizeof_dyn_traj_jvp_io() != C.sizeof(QsDynTrajJvpIO):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac / "
-                          "dyn traj io / dyn ctrl traj io / dyn policy traj io): "
+                          "dyn traj io / dyn ctrl traj io / dyn policy traj io / dyn traj jvp io): "
                           "rebuild")
     _lib = L
     return L

@@ -206,6 +206,12 @@ QS_HD void entry_normalise(Drone& d, double& inv) {
     d.qx *= inv; d.qy *= inv; d.qz *= inv; d.qw *= inv;
 }
 
+// drag's sum of the rotor speeds over four clipped RPMs (rad/s), as dyn_tick_k evaluates it
+QS_HD double drag_sum(const double r[4]) {
+    const double kk = 2.0 * 3.14159265358979323846;
+    return kk * r[0] / 60.0 + kk * r[1] / 60.0 + kk * r[2] / 60.0 + kk * r[3] / 60.0;
+}
+
 // Adjoint of dyn_tick_k<EFF>(P, c, d, u, up, 0, S, .) from the tick-start state d0 (as stored: before the entry renormalisation).
 // L: in, the cotangent of the tick's end state; out, of d0.  Lu / Lup (drag's previous RPMs) / G accumulate.  `rec` holds S - 1
 // drones: rec.store(s, d) / rec.load(s, d).
@@ -221,8 +227,7 @@ QS_HD void dyn_tick_vjp(const QsParams& P, const PhysRow& c, const Drone& d0, co
     double inv;
     entry_normalise(x0, inv);
     const double kk = 2.0 * 3.14159265358979323846;
-    const double ds_prev = kk * up[0] / 60.0 + kk * up[1] / 60.0 + kk * up[2] / 60.0 + kk * up[3] / 60.0;
-    const double ds_cur = kk * u[0] / 60.0 + kk * u[1] / 60.0 + kk * u[2] / 60.0 + kk * u[3] / 60.0;
+    const double ds_prev = drag_sum(up), ds_cur = drag_sum(u);
     double Lds_prev = 0.0, Lds_cur = 0.0;
     for (int s = S - 1; s >= 0; --s) {
         Drone x;

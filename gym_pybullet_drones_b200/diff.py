@@ -1,6 +1,7 @@
 """Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs),
 qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop) and qs_dyn_policy_traj / qs_dyn_policy_traj_vjp (an
-MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5).
+MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5), and the forward mode of the raw-RPM trajectories: DynTrajectory.jvp
+(qs_dyn_traj_jvp) and the per-tick Jacobians of linearise (qs_dyn_tick_jac).
 BaseAviary.differentiable_rollout is the public entry point; this module packs the state into the kernels' planes layout, runs
 the forward and backward kernels and unpacks the result."""
 import ctypes as C
@@ -27,27 +28,67 @@ def unpack_states(planes, n):
     return {"pos": p0[..., 0:3], "quat": q, "vel": p2[..., 0:3], "rpy_rates": w}
 
 
+def _dyn_traj(cfg, rpm, planes0, last_rpm, rows):
+    """states [T, 13 N] of qs_dyn_traj from dense rpm [T, N, 4], planes0 [13 N], last_rpm [N, 4] and rows [E, 16]."""
+    P, E, D, S, eff = cfg
+    T, n = rpm.shape[0], E * D
+    states = torch.empty((T, 13 * n), dtype=torch.float64, device=rpm.device)
+    io = N.QsDynTrajIO()
+    io.T = T
+    io.state0, io.rpm, io.last_rpm, io.phys = planes0.data_ptr(), rpm.data_ptr(), last_rpm.data_ptr(), rows.data_ptr()
+    io.states = states.data_ptr()
+    with torch.cuda.device(rpm.device):
+        N.check(N.lib().qs_dyn_traj(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream), "qs_dyn_traj")
+    return states
+
+
+def _jvp_io(rpm, planes0, last_rpm, rows, states):
+    """A QsDynTrajJvpIO over the dense primal inputs and the forward's states (no tangents, no outputs yet)."""
+    io = N.QsDynTrajJvpIO()
+    io.T = rpm.shape[0]
+    io.state0, io.rpm, io.last_rpm, io.phys = planes0.data_ptr(), rpm.data_ptr(), last_rpm.data_ptr(), rows.data_ptr()
+    io.states = states.data_ptr()
+    return io
+
+
 class DynTrajectory(torch.autograd.Function):
     """states [T, 13 N] = the T ticks of qs_dyn_traj from planes0 [13 N] with rpm [T, N, 4], last_rpm [N, 4] and the per-aviary
-    rows [E, 16]; backward = qs_dyn_traj_vjp, its per-drone row gradients summed over each aviary's drones (torch, deterministic).
-    `cfg` = (QsParams, E, D, substeps, effects).  The inputs may have any strides (the kernels read dense buffers: they get
-    contiguous copies).  Double backward raises ValueError."""
+    rows [E, 16]; backward = qs_dyn_traj_vjp, its per-drone row gradients summed over each aviary's drones (torch, deterministic);
+    jvp (torch.autograd.forward_ad) = qs_dyn_traj_jvp.  `cfg` = (QsParams, E, D, substeps, effects).  The inputs may have any
+    strides (the kernels read dense buffers: they get contiguous copies).  Double backward and tangents that require grad raise
+    ValueError."""
 
     @staticmethod
     def forward(ctx, rpm, planes0, last_rpm, rows, cfg):
         rpm, planes0, last_rpm, rows = (x.contiguous() for x in (rpm, planes0, last_rpm, rows))
-        P, E, D, S, eff = cfg
-        T, n = rpm.shape[0], E * D
-        states = torch.empty((T, 13 * n), dtype=torch.float64, device=rpm.device)
-        io = N.QsDynTrajIO()
-        io.T = T
-        io.state0, io.rpm, io.last_rpm, io.phys = planes0.data_ptr(), rpm.data_ptr(), last_rpm.data_ptr(), rows.data_ptr()
-        io.states = states.data_ptr()
-        with torch.cuda.device(rpm.device):
-            N.check(N.lib().qs_dyn_traj(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream), "qs_dyn_traj")
+        states = _dyn_traj(cfg, rpm, planes0, last_rpm, rows)
         ctx.save_for_backward(rpm, planes0, last_rpm, rows, states)
+        ctx.save_for_forward(rpm, planes0, last_rpm, rows, states)
         ctx.cfg = cfg
         return states
+
+    @staticmethod
+    def jvp(ctx, t_rpm, t_planes0, t_last_rpm, t_rows, _t_cfg):
+        """Forward mode: the tangent [T, 13 N] of the states along the inputs' tangents (qs_dyn_traj_jvp, which linearises
+        each tick at the forward's stored states).  A tangent that requires grad raises ValueError."""
+        tangents = (t_rpm, t_planes0, t_last_rpm, t_rows)
+        if any(t is not None and t.requires_grad for t in tangents):
+            raise ValueError("differentiable_rollout: a tangent that requires grad (reverse mode over forward mode) is not supported: "
+                             "the JVP kernel has no derivative of its own")
+        rpm, planes0, last_rpm, rows, states = ctx.saved_tensors
+        P, E, D, S, eff = ctx.cfg
+        t_states = torch.empty_like(states)
+        io = _jvp_io(rpm, planes0, last_rpm, rows, states)
+        dense = [None if t is None else t.to(torch.float64).contiguous() for t in tangents]
+        if dense[3] is not None and dense[3].data_ptr() % 16:          # the kernel reads t_phys rows as 16-byte pairs
+            dense[3] = dense[3].clone()
+        for k, t in zip(("t_rpm", "t_state0", "t_last_rpm", "t_phys"), dense):
+            setattr(io, k, None if t is None else t.data_ptr())
+        io.t_states = t_states.data_ptr()
+        with torch.cuda.device(rpm.device):
+            N.check(N.lib().qs_dyn_traj_jvp(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
+                    "qs_dyn_traj_jvp")
+        return t_states
 
     @staticmethod
     def backward(ctx, g_states):
@@ -447,4 +488,43 @@ def _policy_loop(env, policy, params, noise, action_buffer, num_steps, state, la
     out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
     out["actions"] = actions.reshape(T, E, D, A)
     out["obs"] = obs.reshape(T, E, D, od)
+    return out
+
+
+def tick_jacobians(cfg, rpm, planes0, last_rpm, rows):
+    """(states [T, 13 N], jac [T, N, 13, C]) of qs_dyn_traj and qs_dyn_tick_jac from dense rpm [T, N, 4], planes0 [13 N],
+    last_rpm [N, 4] and rows [E, 16]; `cfg` = (QsParams, E, D, substeps, effects), C = 17 or 21 with drag (include/quadsim.h)."""
+    P, E, D, S, eff = cfg
+    states = _dyn_traj(cfg, rpm, planes0, last_rpm, rows)
+    jac = torch.empty((rpm.shape[0], E * D, 13, 21 if eff & N.EFFECT_DRAG else 17), dtype=torch.float64, device=rpm.device)
+    io = _jvp_io(rpm, planes0, last_rpm, rows, states)
+    io.jac = jac.data_ptr()
+    with torch.cuda.device(rpm.device):
+        N.check(N.lib().qs_dyn_tick_jac(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
+                "qs_dyn_tick_jac")
+    return states, jac
+
+
+def linearise(env, rpm, state=None, last_rpm=None, phys=None):
+    """BaseAviary.linearise (see there)."""
+    if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
+        raise ValueError("linearise() does not support downwash: the pairwise term has no tangent (use Physics.DYN, PYB, PYB_GND or "
+                         "PYB_DRAG)")
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
+        raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
+    T = rpm.shape[0]
+    if T <= 0:
+        raise ValueError("rpm must hold at least one tick")
+    _tensor(rpm, "rpm", (T, E, D, 4), dev)
+    with torch.no_grad():
+        planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
+        cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
+        states, jac = tick_jacobians(cfg, *(x.detach().contiguous() for x in (rpm.reshape(T, n, 4), planes0, last_rpm, rows)))
+    cols = jac.shape[-1]
+    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    jac = jac.view(T, E, D, 13, cols)
+    out["A"], out["B"] = jac[..., :13], jac[..., 13:17]
+    if cols == 21:
+        out["B_last"] = jac[..., 17:21]
     return out

@@ -577,6 +577,9 @@ class BaseAviary(Env):
         the forward's predicate; the upright switch as a constant.  Drag's first substep reads the previous tick's RPMs, so
         their gradient flows to rpm[k-1], or to last_rpm for k = 0.  Physics.DYN, PYB, PYB_GND and PYB_DRAG; downwash, inputs
         that are not float64 CUDA tensors of the right shape on the env's device, and double backward raise ValueError.
+        Forward mode: torch.autograd.forward_ad dual tensors on rpm, state, last_rpm or phys give the tangents of the four
+        outputs (one JVP kernel launch with the same derivative decisions; the primal outputs keep their bits); a tangent that
+        itself requires grad raises ValueError.  linearise() gives the per-tick Jacobians.
 
         Closed loop: `controller` is a DSLPIDControl(num_drones=E*D) on the env's device, and the schedule arguments mean what
         they mean in CtrlAviary.rollout: tick k runs `rpm = controller.computeControlFromEnv(env, target_pos, target_rpy,
@@ -616,6 +619,27 @@ class BaseAviary(Env):
                                       start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
                                       target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps,
                                       gains=gains, pid_state=pid_state)
+
+    def linearise(self, rpm, *, state=None, last_rpm=None, phys=None):
+        """The per-tick Jacobians of every drone along the raw-RPM trajectory of differentiable_rollout(rpm, state=,
+        last_rpm=, phys=), in one kernel launch after the forward (DESIGN.md 4.5): what LQR, iLQR / DDP, EKF-style estimators
+        and stability analysis linearise at.  Arguments, checks and defaults are differentiable_rollout(rpm)'s; the result is
+        not differentiable, and the env is not touched.
+
+        Returns {pos, quat, vel, rpy_rates} of the nominal trajectory ([T, E, D, k], entry k the state after tick k, the same
+        bits as differentiable_rollout) and, for tick k,
+          A      [T, E, D, 13, 13]  d x_{k+1} / d x_k,
+          B      [T, E, D, 13, 4]   d x_{k+1} / d rpm[k] (the raw command: zero through a clipped rotor),
+          B_last [T, E, D, 13, 4]   with drag only: d x_{k+1} / d (the clipped RPMs of tick k-1, last_rpm for k = 0), which drag's
+                                    first substep reads.
+        Rows and columns are in the order pos, quat (x, y, z, w), vel, rpy_rates; indices are drone ids, also after
+        reorder_by_morton().  x_k is the state as stored, with an unnormalised quaternion: the tick renormalises it on entry, so
+        the quaternion columns of A act on the stored quaternion and A[..., :, 3:7] @ q_hat = 0.  The derivative decisions are
+        differentiable_rollout's (the exponential map everywhere, the RPM clip as torch.clamp, the height clip's predicate, the
+        upright switch constant), so the Jacobians are exactly the transposes of its backward's.  A, B and B_last are views of
+        one [T, E, D, 13, 13 + 4 (+ 4)] tensor.  Downwash and bad inputs raise ValueError."""
+        from ..diff import linearise
+        return linearise(self, rpm, state=state, last_rpm=last_rpm, phys=phys)
 
     ################################################################################
 

@@ -636,6 +636,36 @@ int qs_dyn_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones
 int qs_dyn_traj_vjp(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                     void* stream);
 
+/* Forward mode of the raw-RPM trajectories of qs_dyn_traj (DESIGN.md 4.5): the tangent of the T states along given tangents of
+ * the inputs (JVP), and the dense Jacobians of every tick.  Both read the forward's `states` and restart each tick from the
+ * stored state k-1 (state0 for k = 0), so the trajectory is linearised at the forward's bits, and both take the derivative
+ * decisions of qs_dyn_traj_vjp (they are its exact transpose).  Layouts as in QsDynTrajIO.  All indices are 64-bit. */
+typedef struct QsDynTrajJvpIO {
+    int T;                          /* ticks, > 0 */
+    int pad_;
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* rpm;              /* [T][N][4] RPM commands (clipped in the kernel) */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows; nullable = the constants of QsParams */
+    const double* states;           /* [T][13 N] qs_dyn_traj's output for these inputs */
+    /* qs_dyn_traj_jvp: tangents of the inputs, each nullable = zero */
+    const double* t_state0;         /* [13 N] */
+    const double* t_rpm;            /* [T][N][4] of the raw (unclipped) commands */
+    const double* t_last_rpm;       /* [N][4] */
+    const double* t_phys;           /* [n_envs][16], 16-byte aligned */
+    double* t_states;               /* qs_dyn_traj_jvp out: [T][13 N] the tangents of the states */
+    /* qs_dyn_tick_jac out: [T][N][13][C], C = 17 (21 with QS_EFFECT_DRAG); row r = component r of the state after tick k (pos,
+     * quat x y z w, vel, rpy_rates); columns 0..12 = the stored state before tick k, 13..16 = the raw rpm[k], and with drag
+     * 17..20 = the clipped RPMs of tick k-1 (last_rpm for k = 0) */
+    double* jac;
+} QsDynTrajJvpIO;
+int qs_sizeof_dyn_traj_jvp_io(void);
+/* effects as qs_dyn_traj; QS_ERR_SIZE also when T N C / 128 exceeds 2^31-1 CTAs (qs_dyn_tick_jac) */
+int qs_dyn_traj_jvp(const QsParams* p, const QsDynTrajJvpIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                    void* stream);
+int qs_dyn_tick_jac(const QsParams* p, const QsDynTrajJvpIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                    void* stream);
+
 /* Differentiable closed-loop trajectories (DESIGN.md 4.5): T control ticks of a DSLPIDControl tracking per-tick targets around
  * Physics.DYN (+ GND and/or DRAG, no downwash), and their VJP.  Tick k is the QS_CTRL_TRACK tick of qs_ctrl_rollout, in the same
  * order: pid_control with the controller's QsParams `cp` (its gains, or the aviary's row of `gains`; its model constants), the
