@@ -20,9 +20,6 @@ struct CtrlTrajArgs {
     int D, substeps;
 };
 
-__device__ __forceinline__ qs::PhysRow ctrl_row_of(const CtrlTrajArgs& a, long long i) {
-    return a.io.phys ? load_phys(a.io.phys, i / a.D) : qs::phys_row_of(a.P);
-}
 __device__ __forceinline__ qs::PidGains gains_of(const CtrlTrajArgs& a, long long i) {
     if (!a.io.gains) return qs::pid_gains_of(a.CP);
     const double* g = a.io.gains + 18 * (i / a.D);
@@ -68,7 +65,7 @@ __global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_kernel(const __gri
     const long long N = a.N;
     if (i >= N) return;
     const QsDynCtrlTrajIO& io = a.io;
-    const qs::PhysRow c = ctrl_row_of(a, i);
+    const qs::PhysRow c = row_of(a, i);
     const qs::PidGains K = gains_of(a, i);
     qs::Drone d;
     ld_state(io.state0, N, i, d);
@@ -95,12 +92,10 @@ __global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_vjp_kernel(const _
     const long long N = a.N;
     if (i >= N) return;
     const QsDynCtrlTrajIO& io = a.io;
-    const qs::PhysRow c = ctrl_row_of(a, i);
+    const qs::PhysRow c = row_of(a, i);
     const qs::PidGains K = gains_of(a, i);
     ScratchRec rec = {io.scratch, N, i};
-    qs::PhysGrad G;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) G.g[j] = 0.0;
+    qs::PhysGrad G = zero_phys_grad();
     double Lg[18];
 #pragma unroll
     for (int j = 0; j < 18; ++j) Lg[j] = 0.0;
@@ -109,10 +104,7 @@ __global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_vjp_kernel(const _
     qs::PidState Ls = {0, 0, 0, 0, 0, 0, 0, 0, 0};      // the cotangent of the controller state after tick k
     double Lup_next[4] = {0, 0, 0, 0};                 // drag: the cotangent of this tick's applied RPMs from tick k + 1
     for (int k = io.T - 1; k >= 0; --k) {
-        qs::Drone g;
-        ld_state(io.g_states + (long long)k * 13 * N, N, i, g);
-        L.px += g.px; L.py += g.py; L.pz += g.pz; L.qx += g.qx; L.qy += g.qy; L.qz += g.qz; L.qw += g.qw;
-        L.vx += g.vx; L.vy += g.vy; L.vz += g.vz; L.wx += g.wx; L.wy += g.wy; L.wz += g.wz;
+        add_state(io.g_states + (long long)k * 13 * N, N, i, L);
         qs::Drone d0;
         ld_state(k == 0 ? io.state0 : io.states + (long long)(k - 1) * 13 * N, N, i, d0);
         qs::PidState st0;
@@ -155,15 +147,7 @@ __global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_vjp_kernel(const _
     st3(io.g_target_rpy_rates, Lt.trr);
     const double ly[3] = {0.0, 0.0, Lt.tyaw};
     st3(io.g_target_rpy, ly);
-    if (io.g_last_rpm) {
-        double* o = io.g_last_rpm + 4 * i;
-        o[0] = Lup_next[0]; o[1] = Lup_next[1]; o[2] = Lup_next[2]; o[3] = Lup_next[3];
-    }
-    if (io.g_phys) {
-        double* o = io.g_phys + 16 * i;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) o[j] = G.g[j];
-    }
+    store_start_grads(io, i, Lup_next, G);
     if (io.g_gains) {
         double* o = io.g_gains + 18 * i;
 #pragma unroll
@@ -174,33 +158,22 @@ __global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_vjp_kernel(const _
 template <bool VJP>
 int launch_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
                      int substeps, unsigned effects, void* stream, const char* what) {
-    if (!p || !cp || !io)
-        return fail(QS_ERR_NULL, VJP ? "qs_dyn_ctrl_traj_vjp: NULL params / controller params / io" : "qs_dyn_ctrl_traj: NULL params / controller params / io");
+    if (!p || !cp || !io) return fail(QS_ERR_NULL, what, "NULL params / controller params / io");
     if (!io->state0 || !io->pid0 || !io->target_pos || !io->states || !io->rpm || !io->pid_states)
-        return fail(QS_ERR_NULL, "qs_dyn_ctrl_traj: NULL state0 / pid0 / target_pos / states / rpm / pid_states");
-    if (VJP && (!io->g_states || !io->g_state0 || !io->scratch))
-        return fail(QS_ERR_NULL, "qs_dyn_ctrl_traj_vjp: NULL g_states / g_state0 / scratch");
-    if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0)
-        return fail(QS_ERR_SIZE, "qs_dyn_ctrl_traj: n_envs, drones_per_env, substeps and T must be > 0");
-    if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_dyn_ctrl_traj: n_envs * drones_per_env exceeds 2^31-1");
-    if (!(io->control_timestep > 0.0)) return fail(QS_ERR_SIZE, "qs_dyn_ctrl_traj: control_timestep must be > 0");
-    if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_dyn_ctrl_traj: bad effects");
-    if (effects & QS_EFFECT_DW) return fail(QS_ERR_UNSUPPORTED, "qs_dyn_ctrl_traj: downwash couples the drones pairwise and has no adjoint here");
-    if (io->phys && !aligned16(io->phys)) return fail(QS_ERR_ALIGN, "qs_dyn_ctrl_traj: phys rows must be 16-byte aligned");
+        return fail(QS_ERR_NULL, what, "NULL state0 / pid0 / target_pos / states / rpm / pid_states");
+    if (VJP && (!io->g_states || !io->g_state0 || !io->scratch)) return fail(QS_ERR_NULL, what, "NULL g_states / g_state0 / scratch");
+    if (int rc = traj_check_sizes(what, n_envs, drones_per_env, substeps, io->T)) return rc;
+    if (!(io->control_timestep > 0.0)) return fail(QS_ERR_SIZE, what, "control_timestep must be > 0");
+    if (int rc = traj_check_effects(what, effects, io->phys, nullptr)) return rc;
     CtrlTrajArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.CP = *cp; a.io = *io;
     a.N = (long long)n_envs * drones_per_env;
     a.D = drones_per_env; a.substeps = substeps;
     const unsigned blocks = (unsigned)((a.N + kCtrlTrajTPB - 1) / kCtrlTrajTPB);
-    cudaStream_t s = (cudaStream_t)stream;
-    // the checks above leave TrajEffects only (no bit above 7, no DW)
-    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
-        auto* k = VJP ? dyn_ctrl_traj_vjp_kernel<decltype(EFF)::value> : dyn_ctrl_traj_kernel<decltype(EFF)::value>;
-        k<<<blocks, kCtrlTrajTPB, 0, s>>>(a);
-    });
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, what);
+    return traj_launch(what, effects, [](auto EFF) {
+        return VJP ? dyn_ctrl_traj_vjp_kernel<decltype(EFF)::value> : dyn_ctrl_traj_kernel<decltype(EFF)::value>;
+    }, blocks, kCtrlTrajTPB, 0, (cudaStream_t)stream, a);
 }
 
 }  // namespace
@@ -214,12 +187,12 @@ int qs_sizeof_dyn_ctrl_traj_io(void) { return (int)sizeof(QsDynCtrlTrajIO); }
 
 int qs_dyn_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env, int substeps,
                      unsigned effects, void* stream) {
-    return launch_ctrl_traj<false>(p, cp, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_ctrl_traj launch");
+    return launch_ctrl_traj<false>(p, cp, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_ctrl_traj");
 }
 
 int qs_dyn_ctrl_traj_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
                          int substeps, unsigned effects, void* stream) {
-    return launch_ctrl_traj<true>(p, cp, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_ctrl_traj_vjp launch");
+    return launch_ctrl_traj<true>(p, cp, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_ctrl_traj_vjp");
 }
 
 }  // extern "C"

@@ -19,43 +19,14 @@ struct JvpArgs {
     int D, substeps;
 };
 
-__device__ __forceinline__ qs::PhysRow row_of(const JvpArgs& a, long long i) {
-    return a.io.phys ? load_phys(a.io.phys, i / a.D) : qs::phys_row_of(a.P);
-}
-
 // the tangent of the constants: the aviary's row of t_phys, or zero
 __device__ __forceinline__ qs::PhysRow t_row_of(const JvpArgs& a, long long i) {
-    if (a.io.t_phys) return load_phys(a.io.t_phys, i / a.D);
-    qs::PhysRow z;
-    z.inv_m = z.gravity = z.kf = z.km = z.kx = z.ky = z.hover_rpm = z.max_rpm = 0.0;
-    for (int k = 0; k < 3; ++k) z.j[k] = z.j_inv[k] = 0.0;
-    return z;
-}
-
-__device__ __forceinline__ void clip_rpm(const double raw[4], double max_rpm, double u[4]) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) u[j] = qs::clampd(raw[j], 0.0, max_rpm);            // CtrlAviary.py:140
-}
-
-// The primal inputs of tick k of drone i: the stored start state, the raw and clipped RPMs and drag's previous clipped RPMs
-template <int EFF>
-__device__ __forceinline__ void tick_inputs(const JvpArgs& a, double max_rpm, long long i, int k, qs::Drone& d, double raw[4],
-                                            double u[4], double up[4]) {
-    const QsDynTrajJvpIO& io = a.io;
-    const long long N = a.N;
-    ld_state(k == 0 ? io.state0 : io.states + (long long)(k - 1) * 13 * N, N, i, d);
-    ld4(io.rpm, (long long)k * N + i, raw);
-    clip_rpm(raw, max_rpm, u);
-    up[0] = up[1] = up[2] = up[3] = 0.0;
-    if (EFF & QS_EFFECT_DRAG) {
-        if (k > 0) {
-            double rp[4];
-            ld4(io.rpm, (long long)(k - 1) * N + i, rp);
-            clip_rpm(rp, max_rpm, up);
-        } else if (io.last_rpm) {
-            ld4(io.last_rpm, i, up);
-        }
-    }
+    return aviary_row(a, a.io.t_phys, i, [] {
+        qs::PhysRow z;
+        z.inv_m = z.gravity = z.kf = z.km = z.kx = z.ky = z.hover_rpm = z.max_rpm = 0.0;
+        for (int k = 0; k < 3; ++k) z.j[k] = z.j_inv[k] = 0.0;
+        return z;
+    });
 }
 
 template <int EFF>
@@ -115,40 +86,25 @@ __global__ void __launch_bounds__(kJvpTPB) dyn_tick_jac_kernel(const __grid_cons
 
 template <bool JAC>
 int launch_jvp(const QsParams* p, const QsDynTrajJvpIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
-               void* stream) {
-    if (!p || !io) return fail(QS_ERR_NULL, JAC ? "qs_dyn_tick_jac: NULL params / io" : "qs_dyn_traj_jvp: NULL params / io");
-    if (!io->state0 || !io->rpm || !io->states)
-        return fail(QS_ERR_NULL, JAC ? "qs_dyn_tick_jac: NULL state0 / rpm / states" : "qs_dyn_traj_jvp: NULL state0 / rpm / states");
-    if (JAC ? !io->jac : !io->t_states) return fail(QS_ERR_NULL, JAC ? "qs_dyn_tick_jac: NULL jac" : "qs_dyn_traj_jvp: NULL t_states");
-    if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0)
-        return fail(QS_ERR_SIZE, JAC ? "qs_dyn_tick_jac: n_envs, drones_per_env, substeps and T must be > 0"
-                                     : "qs_dyn_traj_jvp: n_envs, drones_per_env, substeps and T must be > 0");
+               void* stream, const char* what) {
+    if (!p || !io) return fail(QS_ERR_NULL, what, "NULL params / io");
+    if (!io->state0 || !io->rpm || !io->states) return fail(QS_ERR_NULL, what, "NULL state0 / rpm / states");
+    if (JAC ? !io->jac : !io->t_states) return fail(QS_ERR_NULL, what, JAC ? "NULL jac" : "NULL t_states");
+    if (int rc = traj_check_sizes(what, n_envs, drones_per_env, substeps, io->T)) return rc;
+    if (int rc = traj_check_effects(what, effects, io->phys, io->t_phys)) return rc;
     const long long N = (long long)n_envs * drones_per_env;
-    if (N > 0x7fffffffLL) return fail(QS_ERR_SIZE, JAC ? "qs_dyn_tick_jac: n_envs * drones_per_env exceeds 2^31-1"
-                                                       : "qs_dyn_traj_jvp: n_envs * drones_per_env exceeds 2^31-1");
-    if (effects & ~7u) return fail(QS_ERR_ENUM, JAC ? "qs_dyn_tick_jac: bad effects" : "qs_dyn_traj_jvp: bad effects");
-    if (effects & QS_EFFECT_DW)
-        return fail(QS_ERR_UNSUPPORTED, JAC ? "qs_dyn_tick_jac: downwash couples the drones pairwise and has no tangent here"
-                                            : "qs_dyn_traj_jvp: downwash couples the drones pairwise and has no tangent here");
-    if ((io->phys && !aligned16(io->phys)) || (io->t_phys && !aligned16(io->t_phys)))
-        return fail(QS_ERR_ALIGN, JAC ? "qs_dyn_tick_jac: phys rows must be 16-byte aligned" : "qs_dyn_traj_jvp: phys and t_phys rows must be 16-byte aligned");
     const long long threads = JAC ? (long long)io->T * N * jac_cols(effects) : N;
     const long long blocks = (threads + kJvpTPB - 1) / kJvpTPB;
-    if (blocks > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_dyn_tick_jac: T * N * columns exceeds 2^31-1 CTAs of 128 threads");
+    if (blocks > 0x7fffffffLL) return fail(QS_ERR_SIZE, what, "T * N * columns exceeds 2^31-1 CTAs of 128 threads");
     JvpArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.io = *io;
     if (JAC) a.io.t_phys = nullptr;                                  // the Jacobian's columns are the state and RPM inputs only
     a.N = N;
     a.D = drones_per_env; a.substeps = substeps;
-    cudaStream_t s = (cudaStream_t)stream;
-    // the checks above leave TrajEffects only (no bit above 7, no DW)
-    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
-        auto* k = JAC ? dyn_tick_jac_kernel<decltype(EFF)::value> : dyn_traj_jvp_kernel<decltype(EFF)::value>;
-        k<<<(unsigned)blocks, kJvpTPB, 0, s>>>(a);
-    });
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, JAC ? "qs_dyn_tick_jac launch" : "qs_dyn_traj_jvp launch");
+    return traj_launch(what, effects, [](auto EFF) {
+        return JAC ? dyn_tick_jac_kernel<decltype(EFF)::value> : dyn_traj_jvp_kernel<decltype(EFF)::value>;
+    }, (unsigned)blocks, kJvpTPB, 0, (cudaStream_t)stream, a);
 }
 
 }  // namespace
@@ -162,12 +118,12 @@ int qs_sizeof_dyn_traj_jvp_io(void) { return (int)sizeof(QsDynTrajJvpIO); }
 
 int qs_dyn_traj_jvp(const QsParams* p, const QsDynTrajJvpIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                     void* stream) {
-    return launch_jvp<false>(p, io, n_envs, drones_per_env, substeps, effects, stream);
+    return launch_jvp<false>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_traj_jvp");
 }
 
 int qs_dyn_tick_jac(const QsParams* p, const QsDynTrajJvpIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                     void* stream) {
-    return launch_jvp<true>(p, io, n_envs, drones_per_env, substeps, effects, stream);
+    return launch_jvp<true>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_tick_jac");
 }
 
 }  // extern "C"

@@ -29,14 +29,6 @@ struct PolArgs {
     int maxw, cw;                   // widest hidden layer; max(maxw, in_dim): the row stride of the cotangent buffers
 };
 
-__device__ __forceinline__ qs::PhysRow pol_row_of(const PolArgs& a, long long i) {
-    return a.io.phys ? load_phys(a.io.phys, i / a.D) : qs::phys_row_of(a.P);
-}
-__device__ __forceinline__ void pol_clip_rpm(const double raw[4], double max_rpm, double u[4]) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) u[j] = qs::clampd(raw[j], 0.0, max_rpm);
-}
-
 // C[r][n] = sum_k X[r][k] Bm(k, n) for the CTA's M rows (X in shared memory, row stride ldx) and n < Nn, with
 // Bm(k, n) = W[k * sk + n * sn] read from global memory: (sk, sn) = (Nout, 1) is a layer, (1, Nout) its transpose.  epi(r, n, c)
 // receives every element once.  Every thread of the CTA calls it; no barrier inside.
@@ -162,7 +154,7 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_kernel(const __grid_c
     double up[4] = {0, 0, 0, 0}, R[9];
     double* row = obs + (size_t)tid * od;                                 // aviary m's row is D drone rows: m * in + dd * od
     if (live) {
-        c = pol_row_of(a, i);
+        c = row_of(a, i);
         ld_state(io.state0, N, i, d);
         if ((EFF & QS_EFFECT_DRAG) && io.last_rpm) ld4(io.last_rpm, i, up);
         qs::Drone x0 = d;
@@ -189,7 +181,7 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_kernel(const __grid_c
             for (int j = 0; j < (B - 1) * A; ++j) row[12 + j] = row[12 + j + A];
             for (int j = 0; j < A; ++j) row[12 + (B - 1) * A + j] = aa[j];
             qs::policy_rpm(A, c, aa, raw);
-            pol_clip_rpm(raw, c.max_rpm, u);
+            clip_rpm(raw, c.max_rpm, u);
             qs::dyn_tick_k<EFF>(a.P, c, d, u, up, 0.0, a.substeps, R);
             round_to_planes(d);
             st_state(io.states + (long long)k * 13 * N, N, i, d);
@@ -208,7 +200,7 @@ __device__ __forceinline__ void applied_rpm(const PolArgs& a, const qs::PhysRow&
         aa[j] = qs::clampd(raw_a[j], -1.0, 1.0);
     }
     qs::policy_rpm(a.A, c, aa, raw);
-    pol_clip_rpm(raw, c.max_rpm, u);
+    clip_rpm(raw, c.max_rpm, u);
 }
 
 template <int EFF>
@@ -230,11 +222,9 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_vjp_kernel(const __gr
     for (int j = tid; j < M * out; j += blockDim.x) gz[j] = 0.0;
     for (int j = tid; j < M * D * B * A; j += blockDim.x) ring[j] = 0.0;
     __syncthreads();
-    const qs::PhysRow c = live ? pol_row_of(a, i) : qs::phys_row_of(a.P);
+    const qs::PhysRow c = live ? row_of(a, i) : qs::phys_row_of(a.P);
     ScratchRec rec = {io.scratch, N, i};
-    qs::PhysGrad G;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) G.g[j] = 0.0;
+    qs::PhysGrad G = zero_phys_grad();
     qs::Drone L = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     double Lup_next[4] = {0, 0, 0, 0};          // drag: the cotangent of this tick's clipped RPMs from tick k + 1's first substep
     double Lang[3] = {0, 0, 0};                 // the cotangent of ang_v in observation k + 1
@@ -246,10 +236,7 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_vjp_kernel(const __gr
         actor_forward(a, obs, act, true, nullptr);
         qs::Drone d0 = {0, 0, 0, 0, 0, 0, 1, 0, 0, 0, 0, 0, 0};
         if (live) {
-            qs::Drone g;
-            ld_state(io.g_states + (long long)k * 13 * N, N, i, g);
-            L.px += g.px; L.py += g.py; L.pz += g.pz; L.qx += g.qx; L.qy += g.qy; L.qz += g.qz; L.qw += g.qw;
-            L.vx += g.vx; L.vy += g.vy; L.vz += g.vz; L.wx += g.wx; L.wy += g.wy; L.wz += g.wz;
+            add_state(io.g_states + (long long)k * 13 * N, N, i, L);
             ld_state(k == 0 ? io.state0 : io.states + (long long)(k - 1) * 13 * N, N, i, d0);
             double ra[4], aa[4], raw[4], u[4], up[4] = {0, 0, 0, 0};
             applied_rpm(a, c, i, k, ra, aa, raw, u);
@@ -298,15 +285,7 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_vjp_kernel(const __gr
         qs::initial_ang_v_vjp(d0, Lang, L);
     }
     st_state(io.g_state0, N, i, L);
-    if (io.g_last_rpm) {
-        double* o = io.g_last_rpm + 4 * i;
-        o[0] = Lup_next[0]; o[1] = Lup_next[1]; o[2] = Lup_next[2]; o[3] = Lup_next[3];
-    }
-    if (io.g_phys) {
-        double* o = io.g_phys + 16 * i;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) o[j] = G.g[j];
-    }
+    store_start_grads(io, i, Lup_next, G);
     if (io.g_action_buffer)
         for (int j = 0; j < B * A; ++j) io.g_action_buffer[i * B * A + j] = hist[j];
 }
@@ -314,36 +293,31 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_vjp_kernel(const __gr
 template <bool VJP>
 int launch_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env, int substeps,
                        unsigned effects, void* stream, const char* what) {
-    if (!p || !io) return fail(QS_ERR_NULL, "qs_dyn_policy_traj: NULL params / io");
+    if (!p || !io) return fail(QS_ERR_NULL, what, "NULL params / io");
     if (!io->state0 || !io->action_buffer || !io->log_std || !io->states || !io->actions || !io->obs)
-        return fail(QS_ERR_NULL, "qs_dyn_policy_traj: NULL state0 / action_buffer / log_std / states / actions / obs");
+        return fail(QS_ERR_NULL, what, "NULL state0 / action_buffer / log_std / states / actions / obs");
     if (VJP && (!io->g_states || !io->g_raw || !io->g_state0 || !io->scratch))
-        return fail(QS_ERR_NULL, "qs_dyn_policy_traj_vjp: NULL g_states / g_raw / g_state0 / scratch");
-    if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0)
-        return fail(QS_ERR_SIZE, "qs_dyn_policy_traj: n_envs, drones_per_env, substeps and T must be > 0");
-    if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_dyn_policy_traj: n_envs * drones_per_env exceeds 2^31-1");
+        return fail(QS_ERR_NULL, what, "NULL g_states / g_raw / g_state0 / scratch");
+    if (int rc = traj_check_sizes(what, n_envs, drones_per_env, substeps, io->T)) return rc;
     if (act_type != QS_ACT_RPM && act_type != QS_ACT_ONE_D_RPM)
-        return fail(QS_ERR_UNSUPPORTED, "qs_dyn_policy_traj: only the RPM and ONE_D_RPM actions have an adjoint (PID, VEL and ONE_D_PID "
-                                        "run the embedded controller)");
+        return fail(QS_ERR_UNSUPPORTED, what, "only the RPM and ONE_D_RPM actions have an adjoint (PID, VEL and ONE_D_PID run the embedded "
+                                              "controller)");
     const int A = act_width(act_type), D = drones_per_env;
-    if (io->act_buffer_size <= 0) return fail(QS_ERR_SIZE, "qs_dyn_policy_traj: act_buffer_size must be > 0");
-    if (io->activation != QS_MLP_TANH && io->activation != QS_MLP_RELU) return fail(QS_ERR_ENUM, "qs_dyn_policy_traj: bad activation");
-    if (io->depth < 1 || io->depth > QS_MLP_MAX_HIDDEN) return fail(QS_ERR_SIZE, "qs_dyn_policy_traj: 1 to 4 hidden layers");
+    if (io->act_buffer_size <= 0) return fail(QS_ERR_SIZE, what, "act_buffer_size must be > 0");
+    if (io->activation != QS_MLP_TANH && io->activation != QS_MLP_RELU) return fail(QS_ERR_ENUM, what, "bad activation");
+    if (io->depth < 1 || io->depth > QS_MLP_MAX_HIDDEN) return fail(QS_ERR_SIZE, what, "1 to 4 hidden layers");
     int maxw = 0;
     for (int l = 0; l <= io->depth; ++l) {
-        if (!io->w[l] || !io->b[l]) return fail(QS_ERR_NULL, "qs_dyn_policy_traj: NULL weight / bias");
+        if (!io->w[l] || !io->b[l]) return fail(QS_ERR_NULL, what, "NULL weight / bias");
         if (l < io->depth) {
-            if (io->width[l] < 1 || io->width[l] > QS_MLP_MAX_WIDTH) return fail(QS_ERR_SIZE, "qs_dyn_policy_traj: hidden widths must be 1 .. 256");
+            if (io->width[l] < 1 || io->width[l] > QS_MLP_MAX_WIDTH) return fail(QS_ERR_SIZE, what, "hidden widths must be 1 .. 256");
             maxw = io->width[l] > maxw ? io->width[l] : maxw;
         }
     }
-    if (D * A > 32 || D > kPolTPB / kPolMG)
-        return fail(QS_ERR_UNSUPPORTED, "qs_dyn_policy_traj: up to 32 action outputs (D * A) and 32 drones per aviary");
+    if (D * A > 32 || D > kPolTPB / kPolMG) return fail(QS_ERR_UNSUPPORTED, what, "up to 32 action outputs (D * A) and 32 drones per aviary");
     if (io->in_dim != D * (12 + io->act_buffer_size * A) || io->out_dim != D * A)
-        return fail(QS_ERR_SIZE, "qs_dyn_policy_traj: in_dim must be D (12 + B A) and out_dim D A");
-    if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_dyn_policy_traj: bad effects");
-    if (effects & QS_EFFECT_DW) return fail(QS_ERR_UNSUPPORTED, "qs_dyn_policy_traj: downwash couples the drones pairwise and has no adjoint here");
-    if (io->phys && !aligned16(io->phys)) return fail(QS_ERR_ALIGN, "qs_dyn_policy_traj: phys rows must be 16-byte aligned");
+        return fail(QS_ERR_SIZE, what, "in_dim must be D (12 + B A) and out_dim D A");
+    if (int rc = traj_check_effects(what, effects, io->phys, nullptr)) return rc;
     PolArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.io = *io;
@@ -362,21 +336,15 @@ int launch_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_t
     M = M < kPolMaxM ? M : kPolMaxM;
     M -= M % kPolMG;
     if (M < kPolMG)
-        return fail(QS_ERR_UNSUPPORTED, "qs_dyn_policy_traj: the observation rows, hidden activations and cotangents of 8 aviaries exceed the 227 KB of "
-                                        "shared memory of a CTA (shorten the action buffer with a lower ctrl_freq, or use fewer drones per aviary)");
+        return fail(QS_ERR_UNSUPPORTED, what, "the observation rows, hidden activations and cotangents of 8 aviaries exceed the 227 KB of "
+                                              "shared memory of a CTA (shorten the action buffer with a lower ctrl_freq, or use fewer drones "
+                                              "per aviary)");
     a.M = M;
     const size_t smem = per * M * sizeof(double);
     const unsigned blocks = (unsigned)((n_envs + M - 1) / M);
-    cudaStream_t s = (cudaStream_t)stream;
-    cudaError_t e = cudaSuccess;
-    // the checks above leave TrajEffects only (no bit above 7, no DW)
-    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
-        auto* k = VJP ? dyn_policy_traj_vjp_kernel<decltype(EFF)::value> : dyn_policy_traj_kernel<decltype(EFF)::value>;
-        if (smem > 48 * 1024) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) k<<<blocks, kPolTPB, smem, s>>>(a);
-    });
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, what);
+    return traj_launch(what, effects, [](auto EFF) {
+        return VJP ? dyn_policy_traj_vjp_kernel<decltype(EFF)::value> : dyn_policy_traj_kernel<decltype(EFF)::value>;
+    }, blocks, kPolTPB, smem, (cudaStream_t)stream, a);
 }
 
 }  // namespace
@@ -390,12 +358,12 @@ int qs_sizeof_dyn_policy_traj_io(void) { return (int)sizeof(QsDynPolicyTrajIO); 
 
 int qs_dyn_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env, int substeps,
                        unsigned effects, void* stream) {
-    return launch_policy_traj<false>(p, io, act_type, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_policy_traj launch");
+    return launch_policy_traj<false>(p, io, act_type, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_policy_traj");
 }
 
 int qs_dyn_policy_traj_vjp(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env, int substeps,
                            unsigned effects, void* stream) {
-    return launch_policy_traj<true>(p, io, act_type, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_policy_traj_vjp launch");
+    return launch_policy_traj<true>(p, io, act_type, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_policy_traj_vjp");
 }
 
 }  // extern "C"

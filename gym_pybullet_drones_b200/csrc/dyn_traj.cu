@@ -18,15 +18,6 @@ struct TrajArgs {
     int D, substeps;
 };
 
-__device__ __forceinline__ qs::PhysRow row_of(const TrajArgs& a, long long i) {
-    return a.io.phys ? load_phys(a.io.phys, i / a.D) : qs::phys_row_of(a.P);
-}
-
-__device__ __forceinline__ void clip_rpm(const double raw[4], double max_rpm, double u[4]) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) u[j] = qs::clampd(raw[j], 0.0, max_rpm);            // CtrlAviary.py:140
-}
-
 template <int EFF>
 __global__ void __launch_bounds__(kTrajTPB) dyn_traj_kernel(const __grid_constant__ TrajArgs a) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -58,12 +49,11 @@ __global__ void __launch_bounds__(kTrajTPB) dyn_traj_vjp_kernel(const __grid_con
     const QsDynTrajIO& io = a.io;
     const qs::PhysRow c = row_of(a, i);
     ScratchRec rec = {io.scratch, N, i};
-    qs::PhysGrad G;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) G.g[j] = 0.0;
+    qs::PhysGrad G = zero_phys_grad();
     qs::Drone L = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     double Lup_next[4] = {0, 0, 0, 0};          // drag: the cotangent of this tick's clipped RPMs from tick k + 1's first substep
     for (int k = io.T - 1; k >= 0; --k) {
+        // add_state and tick_inputs written out: through the helpers ptxas allocates this kernel's registers differently
         qs::Drone g;
         ld_state(io.g_states + (long long)k * 13 * N, N, i, g);
         L.px += g.px; L.py += g.py; L.pz += g.pz; L.qx += g.qx; L.qy += g.qy; L.qz += g.qz; L.qw += g.qw;
@@ -92,44 +82,27 @@ __global__ void __launch_bounds__(kTrajTPB) dyn_traj_vjp_kernel(const __grid_con
         for (int j = 0; j < 4; ++j) Lup_next[j] = Lup[j];
     }
     st_state(io.g_state0, N, i, L);
-    if (io.g_last_rpm) {
-        double* o = io.g_last_rpm + 4 * i;
-        o[0] = Lup_next[0]; o[1] = Lup_next[1]; o[2] = Lup_next[2]; o[3] = Lup_next[3];
-    }
-    if (io.g_phys) {
-        double* o = io.g_phys + 16 * i;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) o[j] = G.g[j];
-    }
+    store_start_grads(io, i, Lup_next, G);
 }
 
 template <bool VJP>
 int launch_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                 void* stream, const char* what) {
-    if (!p || !io) return fail(QS_ERR_NULL, VJP ? "qs_dyn_traj_vjp: NULL params / io" : "qs_dyn_traj: NULL params / io");
-    if (!io->state0 || !io->rpm || !io->states) return fail(QS_ERR_NULL, "qs_dyn_traj: NULL state0 / rpm / states");
+    if (!p || !io) return fail(QS_ERR_NULL, what, "NULL params / io");
+    if (!io->state0 || !io->rpm || !io->states) return fail(QS_ERR_NULL, what, "NULL state0 / rpm / states");
     if (VJP && (!io->g_states || !io->g_rpm || !io->g_state0 || !io->scratch))
-        return fail(QS_ERR_NULL, "qs_dyn_traj_vjp: NULL g_states / g_rpm / g_state0 / scratch");
-    if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0)
-        return fail(QS_ERR_SIZE, "qs_dyn_traj: n_envs, drones_per_env, substeps and T must be > 0");
-    if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_dyn_traj: n_envs * drones_per_env exceeds 2^31-1");
-    if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_dyn_traj: bad effects");
-    if (effects & QS_EFFECT_DW) return fail(QS_ERR_UNSUPPORTED, "qs_dyn_traj: downwash couples the drones pairwise and has no adjoint here");
-    if (io->phys && !aligned16(io->phys)) return fail(QS_ERR_ALIGN, "qs_dyn_traj: phys rows must be 16-byte aligned");
+        return fail(QS_ERR_NULL, what, "NULL g_states / g_rpm / g_state0 / scratch");
+    if (int rc = traj_check_sizes(what, n_envs, drones_per_env, substeps, io->T)) return rc;
+    if (int rc = traj_check_effects(what, effects, io->phys, nullptr)) return rc;
     TrajArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.io = *io;
     a.N = (long long)n_envs * drones_per_env;
     a.D = drones_per_env; a.substeps = substeps;
     const unsigned blocks = (unsigned)((a.N + kTrajTPB - 1) / kTrajTPB);
-    cudaStream_t s = (cudaStream_t)stream;
-    // the checks above leave TrajEffects only (no bit above 7, no DW)
-    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
-        auto* k = VJP ? dyn_traj_vjp_kernel<decltype(EFF)::value> : dyn_traj_kernel<decltype(EFF)::value>;
-        k<<<blocks, kTrajTPB, 0, s>>>(a);
-    });
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, what);
+    return traj_launch(what, effects, [](auto EFF) {
+        return VJP ? dyn_traj_vjp_kernel<decltype(EFF)::value> : dyn_traj_kernel<decltype(EFF)::value>;
+    }, blocks, kTrajTPB, 0, (cudaStream_t)stream, a);
 }
 
 }  // namespace
@@ -142,12 +115,12 @@ extern "C" {
 int qs_sizeof_dyn_traj_io(void) { return (int)sizeof(QsDynTrajIO); }
 
 int qs_dyn_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects, void* stream) {
-    return launch_traj<false>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_traj launch");
+    return launch_traj<false>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_traj");
 }
 
 int qs_dyn_traj_vjp(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                     void* stream) {
-    return launch_traj<true>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_traj_vjp launch");
+    return launch_traj<true>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_dyn_traj_vjp");
 }
 
 }  // extern "C"

@@ -20,6 +20,10 @@ inline int fail(int code, const char* msg) {
     snprintf(g_err, sizeof(g_err), "%s", msg);
     return code;
 }
+inline int fail(int code, const char* what, const char* msg) {
+    snprintf(g_err, sizeof(g_err), "%s: %s", what, msg);
+    return code;
+}
 
 inline int cuda_fail(cudaError_t e, const char* where) {
     snprintf(g_err, sizeof(g_err), "%s: %s", where, cudaGetErrorString(e));

@@ -28,27 +28,43 @@ def unpack_states(planes, n):
     return {"pos": p0[..., 0:3], "quat": q, "vel": p2[..., 0:3], "rpy_rates": w}
 
 
+def _call(name, *args, device):
+    """N.lib().<name>(*args, stream) on `device` and its current stream; a refusal or launch error raises (N.check)."""
+    with torch.cuda.device(device):
+        N.check(getattr(N.lib(), name)(*args, torch.cuda.current_stream().cuda_stream), name)
+
+
+def _io(cls, T, ptrs, **scalars):
+    """A `cls` IO struct with T, the given scalar fields and a pointer field per entry of `ptrs` (a tensor, or None: NULL)."""
+    io = cls()
+    io.T = T
+    for k, v in scalars.items():
+        setattr(io, k, v)
+    for k, x in ptrs.items():
+        setattr(io, k, None if x is None else x.data_ptr())
+    return io
+
+
+def _no_double_backward():
+    if torch.is_grad_enabled():
+        raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
+                         "derivative of its own")
+
+
+def _traj_ptrs(rpm, planes0, last_rpm, rows, states):
+    """The primal pointers of QsDynTrajIO and QsDynTrajJvpIO: dense rpm [T, N, 4], planes0 [13 N], last_rpm [N, 4], rows [E, 16]
+    and the forward's states [T, 13 N]."""
+    return dict(rpm=rpm, state0=planes0, last_rpm=last_rpm, phys=rows, states=states)
+
+
 def _dyn_traj(cfg, rpm, planes0, last_rpm, rows):
     """states [T, 13 N] of qs_dyn_traj from dense rpm [T, N, 4], planes0 [13 N], last_rpm [N, 4] and rows [E, 16]."""
     P, E, D, S, eff = cfg
     T, n = rpm.shape[0], E * D
     states = torch.empty((T, 13 * n), dtype=torch.float64, device=rpm.device)
-    io = N.QsDynTrajIO()
-    io.T = T
-    io.state0, io.rpm, io.last_rpm, io.phys = planes0.data_ptr(), rpm.data_ptr(), last_rpm.data_ptr(), rows.data_ptr()
-    io.states = states.data_ptr()
-    with torch.cuda.device(rpm.device):
-        N.check(N.lib().qs_dyn_traj(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream), "qs_dyn_traj")
+    io = _io(N.QsDynTrajIO, T, _traj_ptrs(rpm, planes0, last_rpm, rows, states))
+    _call("qs_dyn_traj", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
     return states
-
-
-def _jvp_io(rpm, planes0, last_rpm, rows, states):
-    """A QsDynTrajJvpIO over the dense primal inputs and the forward's states (no tangents, no outputs yet)."""
-    io = N.QsDynTrajJvpIO()
-    io.T = rpm.shape[0]
-    io.state0, io.rpm, io.last_rpm, io.phys = planes0.data_ptr(), rpm.data_ptr(), last_rpm.data_ptr(), rows.data_ptr()
-    io.states = states.data_ptr()
-    return io
 
 
 class DynTrajectory(torch.autograd.Function):
@@ -75,44 +91,31 @@ class DynTrajectory(torch.autograd.Function):
         if any(t is not None and t.requires_grad for t in tangents):
             raise ValueError("differentiable_rollout: a tangent that requires grad (reverse mode over forward mode) is not supported: "
                              "the JVP kernel has no derivative of its own")
-        rpm, planes0, last_rpm, rows, states = ctx.saved_tensors
         P, E, D, S, eff = ctx.cfg
+        states = ctx.saved_tensors[4]
         t_states = torch.empty_like(states)
-        io = _jvp_io(rpm, planes0, last_rpm, rows, states)
         dense = [None if t is None else t.to(torch.float64).contiguous() for t in tangents]
         if dense[3] is not None and dense[3].data_ptr() % 16:          # the kernel reads t_phys rows as 16-byte pairs
             dense[3] = dense[3].clone()
-        for k, t in zip(("t_rpm", "t_state0", "t_last_rpm", "t_phys"), dense):
-            setattr(io, k, None if t is None else t.data_ptr())
-        io.t_states = t_states.data_ptr()
-        with torch.cuda.device(rpm.device):
-            N.check(N.lib().qs_dyn_traj_jvp(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
-                    "qs_dyn_traj_jvp")
+        ptrs = dict(_traj_ptrs(*ctx.saved_tensors), t_states=t_states, **dict(zip(("t_rpm", "t_state0", "t_last_rpm", "t_phys"), dense)))
+        io = _io(N.QsDynTrajJvpIO, states.shape[0], ptrs)
+        _call("qs_dyn_traj_jvp", C.byref(P), C.byref(io), E, D, S, eff, device=states.device)
         return t_states
 
     @staticmethod
     def backward(ctx, g_states):
-        if torch.is_grad_enabled():
-            raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
-                             "derivative of its own")
-        rpm, planes0, last_rpm, rows, states = ctx.saved_tensors
+        _no_double_backward()
+        rpm = ctx.saved_tensors[0]
         P, E, D, S, eff = ctx.cfg
         T, n = rpm.shape[0], E * D
         f64 = dict(dtype=torch.float64, device=rpm.device)
-        g_states = g_states.to(torch.float64).contiguous()
-        g_rpm, g_state0 = torch.empty((T, n, 4), **f64), torch.empty((13 * n,), **f64)
-        g_last, g_phys = torch.empty((n, 4), **f64), torch.empty((n, 16), **f64)
-        scratch = torch.empty((S, 13, n), **f64)
-        io = N.QsDynTrajIO()
-        io.T = T
-        io.state0, io.rpm, io.last_rpm, io.phys = planes0.data_ptr(), rpm.data_ptr(), last_rpm.data_ptr(), rows.data_ptr()
-        io.states, io.g_states = states.data_ptr(), g_states.data_ptr()
-        io.g_rpm, io.g_state0, io.g_last_rpm, io.g_phys = g_rpm.data_ptr(), g_state0.data_ptr(), g_last.data_ptr(), g_phys.data_ptr()
-        io.scratch = scratch.data_ptr()
-        with torch.cuda.device(rpm.device):
-            N.check(N.lib().qs_dyn_traj_vjp(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
-                    "qs_dyn_traj_vjp")
-        return g_rpm, g_state0, g_last, g_phys.view(E, D, 16).sum(dim=1), None
+        g = dict(g_rpm=torch.empty((T, n, 4), **f64), g_state0=torch.empty((13 * n,), **f64), g_last_rpm=torch.empty((n, 4), **f64),
+                 g_phys=torch.empty((n, 16), **f64))
+        ptrs = dict(_traj_ptrs(*ctx.saved_tensors), g_states=g_states.to(torch.float64).contiguous(), scratch=torch.empty((S, 13, n), **f64),
+                    **g)
+        io = _io(N.QsDynTrajIO, T, ptrs)
+        _call("qs_dyn_traj_vjp", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
+        return g["g_rpm"], g["g_state0"], g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), None
 
 
 class DynCtrlTrajectory(torch.autograd.Function):
@@ -123,14 +126,6 @@ class DynCtrlTrajectory(torch.autograd.Function):
     effects).  The inputs may have any strides (the kernels get contiguous copies).  Double backward raises ValueError."""
 
     @staticmethod
-    def _io(T, dt, ins, outs):
-        io = N.QsDynCtrlTrajIO()
-        io.T, io.control_timestep = T, dt
-        for k, x in list(ins.items()) + list(outs.items()):
-            setattr(io, k, x.data_ptr())
-        return io
-
-    @staticmethod
     def forward(ctx, planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains, cfg):
         ins = dict(zip(("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains"),
                        (x.contiguous() for x in (planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains))))
@@ -138,19 +133,15 @@ class DynCtrlTrajectory(torch.autograd.Function):
         T, n = tpos.shape[0], E * D
         f64 = dict(dtype=torch.float64, device=tpos.device)
         outs = dict(states=torch.empty((T, 13 * n), **f64), rpm=torch.empty((T, n, 4), **f64), pid_states=torch.empty((T, 9, n), **f64))
-        io = DynCtrlTrajectory._io(T, dt, ins, outs)
-        with torch.cuda.device(tpos.device):
-            N.check(N.lib().qs_dyn_ctrl_traj(C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
-                    "qs_dyn_ctrl_traj")
+        io = _io(N.QsDynCtrlTrajIO, T, dict(ins, **outs), control_timestep=dt)
+        _call("qs_dyn_ctrl_traj", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=tpos.device)
         ctx.save_for_backward(*ins.values(), *outs.values())
         ctx.cfg = cfg
         return outs["states"], outs["rpm"]
 
     @staticmethod
     def backward(ctx, g_states, g_rpm):
-        if torch.is_grad_enabled():
-            raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
-                             "derivative of its own")
+        _no_double_backward()
         saved = ctx.saved_tensors
         ins = dict(zip(("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains"), saved[:9]))
         outs = dict(zip(("states", "rpm", "pid_states"), saved[9:]))
@@ -163,10 +154,8 @@ class DynCtrlTrajectory(torch.autograd.Function):
                      g_phys=torch.empty((n, 16), **f64), g_gains=torch.empty((n, 18), **f64))
         outs.update(g_states=g_states.to(torch.float64).contiguous(), g_rpm_out=g_rpm.to(torch.float64).contiguous(),
                     scratch=torch.empty((S, 13, n), **f64))
-        io = DynCtrlTrajectory._io(T, dt, ins, dict(outs, **grads))
-        with torch.cuda.device(ins["target_pos"].device):
-            N.check(N.lib().qs_dyn_ctrl_traj_vjp(C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff,
-                                                 torch.cuda.current_stream().cuda_stream), "qs_dyn_ctrl_traj_vjp")
+        io = _io(N.QsDynCtrlTrajIO, T, dict(ins, **outs, **grads), control_timestep=dt)
+        _call("qs_dyn_ctrl_traj_vjp", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=ins["target_pos"].device)
         g = grads
         return (g["g_state0"], g["g_pid0"], g["g_target_pos"], g["g_target_vel"], g["g_target_rpy"], g["g_target_rpy_rates"],
                 g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), g["g_gains"].view(E, D, 18).sum(dim=1), None)
@@ -183,6 +172,18 @@ def actor64(params, activation, obs, noise=None):
     return raw if noise is None else raw + torch.exp(params[-1]) * noise
 
 
+def _policy_io(cfg, T, theta, ptrs):
+    """The QsDynPolicyTrajIO of PolicyTrajectory: the actor's layers from the float64 parameters theta, the tensors of `ptrs`."""
+    activation, B = cfg[2], cfg[3]
+    io = _io(N.QsDynPolicyTrajIO, T, dict(ptrs, log_std=theta[-1]), act_buffer_size=B, depth=len(theta) // 2 - 1,
+             activation=N.MLP_TANH if activation == "tanh" else N.MLP_RELU, in_dim=theta[0].shape[0], out_dim=theta[-3].shape[1])
+    for l in range(io.depth + 1):
+        io.w[l], io.b[l] = theta[2 * l].data_ptr(), theta[2 * l + 1].data_ptr()
+        if l < io.depth:
+            io.width[l] = theta[2 * l].shape[1]
+    return io
+
+
 class PolicyTrajectory(torch.autograd.Function):
     """(states [T, 13 N], raw actions [T, N, A], obs [T, E, in]) = the T ticks of qs_dyn_policy_traj from planes0 [13 N] and the
     action buffer abuf [N, B, A], with last_rpm [N, 4], the per-aviary rows [E, 16], noise [T, E, out] (or None) and the actor's
@@ -190,22 +191,6 @@ class PolicyTrajectory(torch.autograd.Function):
     sequential dependency and returns g_raw, the cotangent of every raw action; the gradients of theta and noise are then one
     batched autograd pass of the actor over the T * E saved observation rows (deterministic, any architecture).  obs is not
     differentiable.  `cfg` = (QsParams, act_type, activation, B, E, D, A, substeps, effects, T)."""
-
-    @staticmethod
-    def _io(cfg, T, theta, ins, outs):
-        activation, B = cfg[2], cfg[3]
-        io = N.QsDynPolicyTrajIO()
-        io.T, io.act_buffer_size, io.activation = T, B, N.MLP_TANH if activation == "tanh" else N.MLP_RELU
-        io.depth = len(theta) // 2 - 1
-        for l in range(io.depth + 1):
-            io.w[l], io.b[l] = theta[2 * l].data_ptr(), theta[2 * l + 1].data_ptr()
-            if l < io.depth:
-                io.width[l] = theta[2 * l].shape[1]
-        io.in_dim, io.out_dim = theta[0].shape[0], theta[-3].shape[1]
-        io.log_std = theta[-1].data_ptr()
-        for k, x in list(ins.items()) + list(outs.items()):
-            setattr(io, k, None if x is None else x.data_ptr())
-        return io
 
     @staticmethod
     def forward(ctx, planes0, last_rpm, rows, abuf, noise, cfg, *theta):
@@ -217,10 +202,8 @@ class PolicyTrajectory(torch.autograd.Function):
         f64 = dict(dtype=torch.float64, device=planes0.device)
         outs = dict(states=torch.empty((T, 13 * n), **f64), actions=torch.empty((T, n, A), **f64),
                     obs=torch.empty((T, E, theta[0].shape[0]), **f64))
-        io = PolicyTrajectory._io(cfg, T, theta, ins, outs)
-        with torch.cuda.device(planes0.device):
-            N.check(N.lib().qs_dyn_policy_traj(C.byref(P), C.byref(io), act_type, E, D, S, eff, torch.cuda.current_stream().cuda_stream),
-                    "qs_dyn_policy_traj")
+        io = _policy_io(cfg, T, theta, dict(ins, **outs))
+        _call("qs_dyn_policy_traj", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=planes0.device)
         ctx.save_for_backward(*(x for x in ins.values() if x is not None), *outs.values(), *theta)
         ctx.cfg, ctx.has_noise = cfg, noise is not None
         ctx.mark_non_differentiable(outs["obs"])
@@ -228,9 +211,7 @@ class PolicyTrajectory(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_states, g_actions, _g_obs):
-        if torch.is_grad_enabled():
-            raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
-                             "derivative of its own")
+        _no_double_backward()
         saved = list(ctx.saved_tensors)
         keys = ["state0", "last_rpm", "phys", "action_buffer"] + (["noise"] if ctx.has_noise else [])
         ins = dict(zip(keys, saved[:len(keys)]))
@@ -245,10 +226,8 @@ class PolicyTrajectory(torch.autograd.Function):
                      g_phys=torch.empty((n, 16), **f64), g_action_buffer=torch.empty((n, B, A), **f64))
         outs.update(g_states=g_states.to(torch.float64).contiguous(), g_actions=g_actions.to(torch.float64).contiguous(),
                     scratch=torch.empty((S, 13, n), **f64))
-        io = PolicyTrajectory._io(cfg, T, theta, ins, dict(outs, **grads))
-        with torch.cuda.device(outs["states"].device):
-            N.check(N.lib().qs_dyn_policy_traj_vjp(C.byref(P), C.byref(io), act_type, E, D, S, eff,
-                                                   torch.cuda.current_stream().cuda_stream), "qs_dyn_policy_traj_vjp")
+        io = _policy_io(cfg, T, theta, dict(ins, **outs, **grads))
+        _call("qs_dyn_policy_traj_vjp", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=outs["states"].device)
         # the parameters' (and the noise's) gradients: raw[k, e] = actor(obs[k, e]) + exp(log_std) noise[k, e] with cotangent g_raw
         g_raw = grads["g_raw"].view(T, E, D * A)
         need = [j for j in range(len(theta)) if ctx.needs_input_grad[6 + j]]
@@ -314,12 +293,27 @@ def _start_state(env, state, last_rpm, phys):
     return planes0, last_rpm, rows
 
 
+def _refuse_downwash(env, caller, derivative):
+    if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
+        raise ValueError("%s does not support downwash: the pairwise term has no %s (use Physics.DYN, PYB, PYB_GND or PYB_DRAG)"
+                         % (caller, derivative))
+
+
+def _rpm_ticks(env, rpm):
+    """T of an rpm [T, E, D, 4] float64 tensor on the env's device; anything else raises ValueError."""
+    if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
+        raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (env._E, env._D))
+    T = rpm.shape[0]
+    if T <= 0:
+        raise ValueError("rpm must hold at least one tick")
+    _tensor(rpm, "rpm", (T, env._E, env._D, 4), env.device)
+    return T
+
+
 def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
                            action_buffer=None, **schedule):
     """BaseAviary.differentiable_rollout (see there)."""
-    if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
-        raise ValueError("differentiable_rollout() does not support downwash: the pairwise term has no adjoint (use Physics.DYN, PYB, "
-                         "PYB_GND or PYB_DRAG)")
+    _refuse_downwash(env, "differentiable_rollout()", "adjoint")
     if (rpm is not None) + (controller is not None) + (policy is not None) != 1:
         raise ValueError("differentiable_rollout() takes exactly one of rpm [T, E, D, 4] (open loop), controller= (closed loop) or "
                          "policy= (an MlpPolicy in the loop)")
@@ -337,12 +331,7 @@ def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=
     if given:
         raise ValueError("%s apply to a controller rollout only" % ", ".join(given))
     E, D, n, dev = env._E, env._D, env._N, env.device
-    if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
-        raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
-    T = rpm.shape[0]
-    if T <= 0:
-        raise ValueError("rpm must hold at least one tick")
-    _tensor(rpm, "rpm", (T, E, D, 4), dev)
+    T = _rpm_ticks(env, rpm)
     planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
     with torch.cuda.device(dev):
         cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
@@ -497,26 +486,16 @@ def tick_jacobians(cfg, rpm, planes0, last_rpm, rows):
     P, E, D, S, eff = cfg
     states = _dyn_traj(cfg, rpm, planes0, last_rpm, rows)
     jac = torch.empty((rpm.shape[0], E * D, 13, 21 if eff & N.EFFECT_DRAG else 17), dtype=torch.float64, device=rpm.device)
-    io = _jvp_io(rpm, planes0, last_rpm, rows, states)
-    io.jac = jac.data_ptr()
-    with torch.cuda.device(rpm.device):
-        N.check(N.lib().qs_dyn_tick_jac(C.byref(P), C.byref(io), E, D, S, eff, torch.cuda.current_stream().cuda_stream),
-                "qs_dyn_tick_jac")
+    io = _io(N.QsDynTrajJvpIO, rpm.shape[0], dict(_traj_ptrs(rpm, planes0, last_rpm, rows, states), jac=jac))
+    _call("qs_dyn_tick_jac", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
     return states, jac
 
 
 def linearise(env, rpm, state=None, last_rpm=None, phys=None):
     """BaseAviary.linearise (see there)."""
-    if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
-        raise ValueError("linearise() does not support downwash: the pairwise term has no tangent (use Physics.DYN, PYB, PYB_GND or "
-                         "PYB_DRAG)")
-    E, D, n, dev = env._E, env._D, env._N, env.device
-    if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
-        raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
-    T = rpm.shape[0]
-    if T <= 0:
-        raise ValueError("rpm must hold at least one tick")
-    _tensor(rpm, "rpm", (T, E, D, 4), dev)
+    _refuse_downwash(env, "linearise()", "tangent")
+    E, D, n = env._E, env._D, env._N
+    T = _rpm_ticks(env, rpm)
     with torch.no_grad():
         planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
         cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)

@@ -1,34 +1,22 @@
 """Shared helpers of the closed-loop differentiable-trajectory tests (test infrastructure): the g++ build of pid_adjoint.cuh with
 the closed-loop tick of dyn_ctrl_traj.cu, its torch counterpart, and the drone / controller batches the tests differentiate at."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import torch
 
 import diff_pid_ref as PR
 import diff_ref as R
-from diff_testlib import ROOT, quat_from_rpy
+from diff_testlib import quat_from_rpy
+from qs_testlib import harness
 
-_HH = None
 BLOCKS = ("state", "pid", "targets", "last_rpm", "phys", "gains")
 
 
 def ctrl_harness():
-    """Builds (g++) and loads tests/host_harness/diff_ctrl_host.cpp: the kernels' closed-loop tick adjoint compiled for the host."""
-    global _HH
-    if _HH is not None:
-        return _HH
-    src = os.path.join(ROOT, "tests", "host_harness", "diff_ctrl_host.cpp")
-    out = os.path.join(ROOT, "tests", "host_harness", "libdiff_ctrl_host.so")
-    csrc = os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc")
-    deps = [src, os.path.join(ROOT, "include", "quadsim.h")] + [os.path.join(csrc, f) for f in ("pid_adjoint.cuh", "dyn_adjoint.cuh", "quad_core.cuh")]
-    if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
-    L = C.CDLL(out)
+    """tests/host_harness/diff_ctrl_host.cpp: the kernels' closed-loop tick adjoint compiled for the host."""
+    L = harness("diff_ctrl_host")
     L.dh_ctrl_tick_vjp.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.c_int, C.c_double, C.c_int] + [C.c_void_p] * 18
-    _HH = L
     return L
 
 

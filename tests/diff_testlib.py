@@ -2,38 +2,20 @@
 of the dyn_traj kernels) and the drone batches the tests differentiate at."""
 import ctypes as C
 import functools
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-MODELS = ("cf2x", "cf2p", "race")
+from qs_testlib import drone_model, harness
 
-_HH = None
+MODELS = ("cf2x", "cf2p", "race")
 
 
 def diff_harness():
-    """Builds (g++) and loads tests/host_harness/diff_host.cpp: the kernels' tick adjoint compiled for the host."""
-    global _HH
-    if _HH is not None:
-        return _HH
-    src = os.path.join(ROOT, "tests", "host_harness", "diff_host.cpp")
-    out = os.path.join(ROOT, "tests", "host_harness", "libdiff_host.so")
-    csrc = os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc")
-    deps = [src, os.path.join(csrc, "dyn_adjoint.cuh"), os.path.join(csrc, "quad_core.cuh"), os.path.join(ROOT, "include", "quadsim.h")]
-    if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
-    L = C.CDLL(out)
+    """tests/host_harness/diff_host.cpp: the kernels' tick adjoint compiled for the host."""
+    L = harness("diff_host")
     L.dh_tick_vjp.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.c_int, C.c_int] + [C.c_void_p] * 9
     L.dh_half_angle_grad.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_void_p]
-    _HH = L
     return L
-
-
-def drone_model(name):
-    from gym_pybullet_drones_b200.utils.enums import DroneModel
-    return {"cf2x": DroneModel.CF2X, "cf2p": DroneModel.CF2P, "race": DroneModel.RACE}[name]
 
 
 def params_of(model, pyb_freq=240, ctrl_freq=240):

@@ -4,23 +4,10 @@
 // kernel's: pid_control_k, the controller's max_rpm clip, the env's clip, dyn_tick_k; its VJP is the kernel's backward step.
 // Never linked into or imported by the product package.
 #include <cmath>
-#include <vector>
 #include "../../gym_pybullet_drones_b200/csrc/pid_adjoint.cuh"
+#include "harness.h"
 
 namespace {
-struct HostRec {
-    std::vector<qs::Drone> v;
-    void store(int s, const qs::Drone& d) { v[s] = d; }
-    void load(int s, qs::Drone& d) const { d = v[s]; }
-};
-
-qs::PhysRow row_from(const double* r) {
-    qs::PhysRow c;
-    c.inv_m = r[0]; c.gravity = r[1]; c.kf = r[2]; c.km = r[3]; c.kx = r[4]; c.ky = r[5];
-    for (int k = 0; k < 3; ++k) { c.j[k] = r[6 + k]; c.j_inv[k] = r[9 + k]; }
-    c.hover_rpm = r[12]; c.max_rpm = r[13];
-    return c;
-}
 qs::PidGains gains_from(const double* g) {
     qs::PidGains k;
     for (int a = 0; a < 3; ++a) {
@@ -28,13 +15,6 @@ qs::PidGains gains_from(const double* g) {
         k.pid_p_tor[a] = g[9 + a]; k.pid_i_tor[a] = g[12 + a]; k.pid_d_tor[a] = g[15 + a];
     }
     return k;
-}
-qs::Drone drone_from(const double* s) {
-    return qs::Drone{s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8], s[9], s[10], s[11], s[12]};
-}
-void drone_to(const qs::Drone& d, double* s) {
-    const double v[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
-    for (int k = 0; k < 13; ++k) s[k] = v[k];
 }
 qs::PidState pid_from(const double* s) { return qs::PidState{s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8]}; }
 void pid_to(const qs::PidState& p, double* s) {
@@ -47,7 +27,7 @@ void ctrl_tick_vjp(const QsParams& P, const QsParams& CP, const double* row, con
                    const double* state, const double* pid, const double* tg, const double* up, const double* g_out,
                    const double* g_rpm, const double* g_pid, double* out, double* u_out, double* pid_out, double* g_state,
                    double* g_pid0, double* g_tg, double* g_up, double* g_row, double* g_gains) {
-    const qs::PhysRow c = row_from(row);
+    const qs::PhysRow c = row_from(P, row);
     const qs::PidGains K = gains_from(gains);
     const qs::Drone d0 = drone_from(state);
     const qs::PidState st0 = pid_from(pid);
@@ -97,11 +77,12 @@ void dh_ctrl_tick_vjp(const QsParams* P, const QsParams* CP, unsigned effects, i
                       const double* gains, const double* state, const double* pid, const double* tg, const double* up,
                       const double* g_out, const double* g_rpm, const double* g_pid, double* out, double* u_out, double* pid_out,
                       double* g_state, double* g_pid0, double* g_tg, double* g_up, double* g_row, double* g_gains) {
-    auto f = effects == 0 ? ctrl_tick_vjp<0> : effects == QS_EFFECT_GND ? ctrl_tick_vjp<QS_EFFECT_GND>
-           : effects == QS_EFFECT_DRAG ? ctrl_tick_vjp<QS_EFFECT_DRAG> : ctrl_tick_vjp<3>;
-    for (int i = 0; i < n; ++i)
-        f(*P, *CP, rows + 16 * i, gains + 18 * i, S, dt, state + 13 * i, pid + 9 * i, tg + 10 * i, up + 4 * i, g_out + 13 * i,
-          g_rpm + 4 * i, g_pid + 9 * i, out + 13 * i, u_out + 4 * i, pid_out + 9 * i, g_state + 13 * i, g_pid0 + 9 * i,
-          g_tg + 10 * i, g_up + 4 * i, g_row + 16 * i, g_gains + 18 * i);
+    with_effects(effects, [&](auto EFF) {
+        for (int i = 0; i < n; ++i)
+            ctrl_tick_vjp<decltype(EFF)::value>(*P, *CP, rows + 16 * i, gains + 18 * i, S, dt, state + 13 * i, pid + 9 * i, tg + 10 * i,
+                                                up + 4 * i, g_out + 13 * i, g_rpm + 4 * i, g_pid + 9 * i, out + 13 * i, u_out + 4 * i,
+                                                pid_out + 9 * i, g_state + 13 * i, g_pid0 + 9 * i, g_tg + 10 * i, g_up + 4 * i,
+                                                g_row + 16 * i, g_gains + 18 * i);
+    });
 }
 }

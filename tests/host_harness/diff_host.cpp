@@ -3,33 +3,10 @@
 // torch reference (tests/diff_ref.py).  A drone is 13 doubles: pos, quat (x, y, z, w), vel, rpy_rates.  Never linked into or
 // imported by the product package.
 #include <cmath>
-#include <vector>
 #include "../../gym_pybullet_drones_b200/csrc/dyn_adjoint.cuh"
+#include "harness.h"
 
 namespace {
-struct HostRec {
-    std::vector<qs::Drone> v;
-    void store(int s, const qs::Drone& d) { v[s] = d; }
-    void load(int s, qs::Drone& d) const { d = v[s]; }
-};
-
-qs::PhysRow row_from(const QsParams& P, const double* r) {
-    if (!r) return qs::phys_row_of(P);
-    qs::PhysRow c;
-    c.inv_m = r[0]; c.gravity = r[1]; c.kf = r[2]; c.km = r[3]; c.kx = r[4]; c.ky = r[5];
-    for (int k = 0; k < 3; ++k) { c.j[k] = r[6 + k]; c.j_inv[k] = r[9 + k]; }
-    c.hover_rpm = r[12]; c.max_rpm = r[13];
-    return c;
-}
-
-qs::Drone drone_from(const double* s) {
-    return qs::Drone{s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8], s[9], s[10], s[11], s[12]};
-}
-void drone_to(const qs::Drone& d, double* s) {
-    const double v[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
-    for (int k = 0; k < 13; ++k) s[k] = v[k];
-}
-
 template <int EFF>
 void tick_vjp(const QsParams& P, const qs::PhysRow& c, int S, const double* state, const double* raw, const double* up,
               const double* g_out, double* out, double* g_state, double* g_raw, double* g_up, double* g_row) {
@@ -60,13 +37,11 @@ extern "C" {
 // g_state [n][13], g_raw [n][4], g_up [n][4], g_row [n][16].  effects: 0, GND, DRAG or GND|DRAG.
 void dh_tick_vjp(const QsParams* P, const double* rows, unsigned effects, int S, int n, const double* state, const double* raw,
                  const double* up, const double* g_out, double* out, double* g_state, double* g_raw, double* g_up, double* g_row) {
-    for (int i = 0; i < n; ++i) {
-        const qs::PhysRow c = row_from(*P, rows ? rows + 16 * i : nullptr);
-        auto f = effects == 0 ? tick_vjp<0> : effects == QS_EFFECT_GND ? tick_vjp<QS_EFFECT_GND>
-               : effects == QS_EFFECT_DRAG ? tick_vjp<QS_EFFECT_DRAG> : tick_vjp<3>;
-        f(*P, c, S, state + 13 * i, raw + 4 * i, up + 4 * i, g_out + 13 * i, out + 13 * i, g_state + 13 * i, g_raw + 4 * i,
-          g_up + 4 * i, g_row + 16 * i);
-    }
+    with_effects(effects, [&](auto EFF) {
+        for (int i = 0; i < n; ++i)
+            tick_vjp<decltype(EFF)::value>(*P, row_from(*P, rows ? rows + 16 * i : nullptr), S, state + 13 * i, raw + 4 * i, up + 4 * i,
+                                           g_out + 13 * i, out + 13 * i, g_state + 13 * i, g_raw + 4 * i, g_up + 4 * i, g_row + 16 * i);
+    });
 }
 // half_angle_grad: c, s, dc/dn2, ds/dn2 for n values of n2
 void dh_half_angle_grad(const double* n2, int n, double dt, double* out) {

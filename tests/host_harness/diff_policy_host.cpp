@@ -7,35 +7,16 @@
 #include <cmath>
 #include <vector>
 #include "../../gym_pybullet_drones_b200/csrc/mlp_adjoint.cuh"
+#include "harness.h"
 
 namespace {
-struct HostRec {
-    std::vector<qs::Drone> v;
-    void store(int s, const qs::Drone& d) { v[s] = d; }
-    void load(int s, qs::Drone& d) const { d = v[s]; }
-};
-qs::PhysRow row_from(const double* r) {
-    qs::PhysRow c;
-    c.inv_m = r[0]; c.gravity = r[1]; c.kf = r[2]; c.km = r[3]; c.kx = r[4]; c.ky = r[5];
-    for (int k = 0; k < 3; ++k) { c.j[k] = r[6 + k]; c.j_inv[k] = r[9 + k]; }
-    c.hover_rpm = r[12]; c.max_rpm = r[13];
-    return c;
-}
-qs::Drone drone_from(const double* s) {
-    return qs::Drone{s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8], s[9], s[10], s[11], s[12]};
-}
-void drone_to(const qs::Drone& d, double* s) {
-    const double v[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
-    for (int k = 0; k < 13; ++k) s[k] = v[k];
-}
-
 template <int EFF>
 void tick_vjp(const QsParams& P, int S, int D, int A, int B, int act, int depth, const int* width, const double* const* W,
               const double* const* bias, const double* log_std, const double* noise, const double* row, const double* state,
               const double* Rq, const double* hist, const double* up, const double* g_end, const double* g_raw_out,
               const double* Lang_next, const double* g_hist_next, double* out_state, double* out_raw, double* out_hist,
               double* out_qlast, double* g_state, double* g_Rq, double* g_hist, double* g_up, double* g_row, double* g_raw) {
-    const qs::PhysRow c = row_from(row);
+    const qs::PhysRow c = row_from(P, row);
     const int od = 12 + B * A, in = D * od, out = D * A;
     // ---- forward ----
     std::vector<double> obs(in);
@@ -149,9 +130,10 @@ void dph_tick_vjp(const QsParams* P, unsigned effects, int S, int D, int A, int 
                   const double* g_raw_out, const double* Lang_next, const double* g_hist_next, double* out_state, double* out_raw,
                   double* out_hist, double* out_qlast, double* g_state, double* g_Rq, double* g_hist, double* g_up, double* g_row,
                   double* g_raw) {
-    auto f = effects == 0 ? tick_vjp<0> : effects == QS_EFFECT_GND ? tick_vjp<QS_EFFECT_GND>
-           : effects == QS_EFFECT_DRAG ? tick_vjp<QS_EFFECT_DRAG> : tick_vjp<3>;
-    f(*P, S, D, A, B, act, depth, width, W, bias, log_std, noise, row, state, Rq, hist, up, g_end, g_raw_out, Lang_next, g_hist_next,
-      out_state, out_raw, out_hist, out_qlast, g_state, g_Rq, g_hist, g_up, g_row, g_raw);
+    with_effects(effects, [&](auto EFF) {
+        tick_vjp<decltype(EFF)::value>(*P, S, D, A, B, act, depth, width, W, bias, log_std, noise, row, state, Rq, hist, up, g_end,
+                                       g_raw_out, Lang_next, g_hist_next, out_state, out_raw, out_hist, out_qlast, g_state, g_Rq, g_hist,
+                                       g_up, g_row, g_raw);
+    });
 }
 }

@@ -3,25 +3,9 @@
 // under torch.func.jacfwd) and to the transpose of the host-built adjoint (diff_host.cpp).  A drone is 13 doubles: pos, quat
 // (x, y, z, w), vel, rpy_rates.  Never linked into or imported by the product package.
 #include "../../gym_pybullet_drones_b200/csrc/dyn_tangent.cuh"
+#include "harness.h"
 
 namespace {
-qs::PhysRow row_from(const QsParams& P, const double* r) {
-    if (!r) return qs::phys_row_of(P);
-    qs::PhysRow c;
-    c.inv_m = r[0]; c.gravity = r[1]; c.kf = r[2]; c.km = r[3]; c.kx = r[4]; c.ky = r[5];
-    for (int k = 0; k < 3; ++k) { c.j[k] = r[6 + k]; c.j_inv[k] = r[9 + k]; }
-    c.hover_rpm = r[12]; c.max_rpm = r[13];
-    return c;
-}
-
-qs::Drone drone_from(const double* s) {
-    return qs::Drone{s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8], s[9], s[10], s[11], s[12]};
-}
-void drone_to(const qs::Drone& d, double* s) {
-    const double v[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
-    for (int k = 0; k < 13; ++k) s[k] = v[k];
-}
-
 template <int EFF>
 void tick_jvp(const QsParams& P, const qs::PhysRow& c, const qs::PhysRow& tc, int S, const double* state, const double* raw,
               const double* up, const double* t_state, const double* t_raw, const double* t_up, double* out, double* t_out) {
@@ -42,13 +26,10 @@ extern "C" {
 void jh_tick_jvp(const QsParams* P, const double* rows, unsigned effects, int S, int n, const double* state, const double* raw,
                  const double* up, const double* t_state, const double* t_raw, const double* t_up, const double* t_rows, double* out,
                  double* t_out) {
-    for (int i = 0; i < n; ++i) {
-        const qs::PhysRow c = row_from(*P, rows ? rows + 16 * i : nullptr);
-        qs::PhysRow tc = row_from(*P, t_rows + 16 * i);
-        auto f = effects == 0 ? tick_jvp<0> : effects == QS_EFFECT_GND ? tick_jvp<QS_EFFECT_GND>
-               : effects == QS_EFFECT_DRAG ? tick_jvp<QS_EFFECT_DRAG> : tick_jvp<3>;
-        f(*P, c, tc, S, state + 13 * i, raw + 4 * i, up + 4 * i, t_state + 13 * i, t_raw + 4 * i, t_up + 4 * i, out + 13 * i,
-          t_out + 13 * i);
-    }
+    with_effects(effects, [&](auto EFF) {
+        for (int i = 0; i < n; ++i)
+            tick_jvp<decltype(EFF)::value>(*P, row_from(*P, rows ? rows + 16 * i : nullptr), row_from(*P, t_rows + 16 * i), S, state + 13 * i,
+                                           raw + 4 * i, up + 4 * i, t_state + 13 * i, t_raw + 4 * i, t_up + 4 * i, out + 13 * i, t_out + 13 * i);
+    });
 }
 }

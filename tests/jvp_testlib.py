@@ -2,34 +2,20 @@
 Jacobian kernels, dyn_jvp.cu) and one tick's Jacobian per drone and input block, from that build, from the transpose of the
 host-built adjoint (diff_host.cpp) and from torch.func.jacfwd of the reference tests/diff_ref.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from diff_testlib import ROOT, host_tick_vjp, per_drone_relerr
+from diff_testlib import host_tick_vjp, per_drone_relerr
+from qs_testlib import harness
 
 # input blocks of one tick and their widths: the tick-start state, the raw RPMs, drag's previous clipped RPMs, the 16-column row
 BLOCKS = (("state", 13), ("rpm", 4), ("up", 4), ("row", 16))
 
-_HH = None
-
 
 def jvp_harness():
-    """Builds (g++) and loads tests/host_harness/jvp_host.cpp: the kernels' tick tangent compiled for the host."""
-    global _HH
-    if _HH is not None:
-        return _HH
-    src = os.path.join(ROOT, "tests", "host_harness", "jvp_host.cpp")
-    out = os.path.join(ROOT, "tests", "host_harness", "libjvp_host.so")
-    csrc = os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc")
-    deps = [src, os.path.join(csrc, "dyn_tangent.cuh"), os.path.join(csrc, "dyn_adjoint.cuh"), os.path.join(csrc, "quad_core.cuh"),
-            os.path.join(ROOT, "include", "quadsim.h")]
-    if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
-    L = C.CDLL(out)
+    """tests/host_harness/jvp_host.cpp: the kernels' tick tangent compiled for the host."""
+    L = harness("jvp_host")
     L.jh_tick_jvp.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.c_int, C.c_int] + [C.c_void_p] * 9
-    _HH = L
     return L
 
 

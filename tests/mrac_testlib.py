@@ -1,12 +1,11 @@
 """Shared helpers of the MRAC tests (test infrastructure): the g++ build of mrac_core.cuh, the golden fixture's inputs and the
 comparisons against it, and the free-running horizon derived from the tier-2 oracle."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from qs_testlib import drone_model, harness  # noqa: F401  (drone_model: re-exported for the MRAC tests)
+
 MODELS = ("cf2x", "cf2p", "race")
 DT = 1.0 / 120
 # agreement with the reference's float64 MRAC, |a - b| <= tol * max(|b|, 1) on rpm, Kx, Kr, Xm, pos_e, rpy_e and the state:
@@ -15,31 +14,13 @@ DT = 1.0 / 120
 TOL = 1e-9
 TF_TOL = 1e-12
 
-_HH = None
-
-
 def mrac_harness():
-    """Builds (g++) and loads tests/host_harness/mrac_host.cpp: the kernels' MRAC core compiled for the host."""
-    global _HH
-    if _HH is not None:
-        return _HH
-    src = os.path.join(ROOT, "tests", "host_harness", "mrac_host.cpp")
-    out = os.path.join(ROOT, "tests", "host_harness", "libmrac_host.so")
-    deps = [src, os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc", "mrac_core.cuh"),
-            os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc", "quad_core.cuh"), os.path.join(ROOT, "include", "quadsim.h")]
-    if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
-    L = C.CDLL(out)
+    """tests/host_harness/mrac_host.cpp: the kernels' MRAC core compiled for the host."""
+    L = harness("mrac_host")
     L.hh_mrac.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double] + [C.c_void_p] * 8
     L.hh_mrac_ang_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     L.hh_sizeof_mrac_params.restype = C.c_int
-    _HH = L
     return L
-
-
-def drone_model(name):
-    from gym_pybullet_drones_b200.utils.enums import DroneModel
-    return {"cf2x": DroneModel.CF2X, "cf2p": DroneModel.CF2P, "race": DroneModel.RACE}[name]
 
 
 def gains_of(g, model):

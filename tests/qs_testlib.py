@@ -1,6 +1,7 @@
 """Shared helpers for the parity tests (test infrastructure)."""
 import ctypes as C
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -49,20 +50,42 @@ def unpack_planes(pl):
     return p[0, :, 0:3], p[1], p[2, :, 0:3], w
 
 
-_HH = None
+_INCLUDE = re.compile(r'^\s*#\s*include\s*"([^"]+)"', re.M)
+_HARNESSES = {}
+
+
+def _sources(path, seen=None):
+    """path and every file it reaches through #include "..." lines (resolved against the including file's directory)."""
+    seen = set() if seen is None else seen
+    path = os.path.normpath(path)
+    if path not in seen:
+        seen.add(path)
+        with open(path) as f:
+            for inc in _INCLUDE.findall(f.read()):
+                _sources(os.path.join(os.path.dirname(path), inc), seen)
+    return seen
+
+
+def harness(name):
+    """Builds (g++, when the library is older than tests/host_harness/<name>.cpp or any file it includes) and loads
+    tests/host_harness/lib<name>.so: kernel code compiled for the host."""
+    if name not in _HARNESSES:
+        src = os.path.join(ROOT, "tests", "host_harness", name + ".cpp")
+        out = os.path.join(ROOT, "tests", "host_harness", "lib%s.so" % name)
+        if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in _sources(src)):
+            subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
+        _HARNESSES[name] = C.CDLL(out)
+    return _HARNESSES[name]
+
+
+def drone_model(name):
+    from gym_pybullet_drones_b200.utils.enums import DroneModel
+    return {"cf2x": DroneModel.CF2X, "cf2p": DroneModel.CF2P, "race": DroneModel.RACE}[name]
 
 
 def host_harness():
-    """Builds (g++) and loads tests/host_harness: the CUDA kernels' per-drone core compiled for the host."""
-    global _HH
-    if _HH is not None:
-        return _HH
-    src = os.path.join(ROOT, "tests", "host_harness", "core_host.cpp")
-    out = os.path.join(ROOT, "tests", "host_harness", "libcore_host.so")
-    deps = [src, os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc", "quad_core.cuh"), os.path.join(ROOT, "include", "quadsim.h")]
-    if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
-    L = C.CDLL(out)
+    """tests/host_harness/core_host.cpp: the CUDA kernels' per-drone core compiled for the host."""
+    L = harness("core_host")
     L.hh_downwash_pair.restype = C.c_double
     L.hh_downwash_pair.argtypes = [C.c_void_p, C.c_double, C.c_double]
     L.hh_half_angle.argtypes = [C.c_double, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]
@@ -71,7 +94,6 @@ def host_harness():
     L.hh_quat_to_euler.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     L.hh_upright.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.hh_hover_terms.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_void_p]
-    _HH = L
     return L
 
 

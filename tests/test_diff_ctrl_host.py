@@ -227,10 +227,12 @@ def test_abi_exports_struct_and_refusals():
     assert call(L.qs_dyn_ctrl_traj, io, 1, 1, 1, 0) == -3
     io.control_timestep = 1 / 48
     assert call(L.qs_dyn_ctrl_traj_vjp, io, 1, 1, 1, 0) == -1          # no cotangents, gradient or scratch
+    assert L.qs_last_error().startswith(b"qs_dyn_ctrl_traj_vjp: ")      # a refusal names the entry point that was called
     io.g_states = io.g_state0 = io.scratch = C.addressof(buf)
     assert call(L.qs_dyn_ctrl_traj_vjp, io, 1, 1, 1, N.EFFECT_DW) == -5
     io.T = 0
     assert call(L.qs_dyn_ctrl_traj_vjp, io, 1, 1, 1, 0) == -3
+    assert L.qs_last_error().startswith(b"qs_dyn_ctrl_traj_vjp: ")
     io.T, io.phys = 1, C.addressof(buf) + 8
     assert call(L.qs_dyn_ctrl_traj, io, 1, 1, 1, 0) == -2
     io.phys, io.pid0 = None, None

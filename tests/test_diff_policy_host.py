@@ -2,7 +2,6 @@
 VJP, the code of dyn_policy_traj.cu's kernels) against the torch reference tests/diff_policy_ref.py per input block, with negative
 controls; the reference against its own central differences; the C ABI of qs_dyn_policy_traj (exports, struct size, every
 argument refusal, which returns before any launch) and MlpPolicy.parameters64 / load_parameters on the CPU."""
-import subprocess
 import ctypes as C
 import os
 
@@ -13,6 +12,7 @@ import torch
 import diff_policy_ref as PR
 import diff_ref as R
 from diff_testlib import params_of
+from qs_testlib import harness
 
 
 def _case(activation, A, D, effects, seed):
@@ -90,23 +90,6 @@ def test_parameters64_round_trip_on_the_cpu():
 
 # ---- the g++ build of the aviary tick adjoint ------------------------------------------------------------------------------
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_DPH = None
-
-
-def _harness():
-    global _DPH
-    if _DPH is None:
-        src = os.path.join(ROOT, "tests", "host_harness", "diff_policy_host.cpp")
-        out = os.path.join(ROOT, "tests", "host_harness", "libdiff_policy_host.so")
-        csrc = os.path.join(ROOT, "gym_pybullet_drones_b200", "csrc")
-        deps = [src] + [os.path.join(csrc, h) for h in ("mlp_adjoint.cuh", "dyn_adjoint.cuh", "quad_core.cuh")]
-        if not os.path.isfile(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-            subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-o", out, src], check=True)
-        _DPH = C.CDLL(out)
-    return _DPH
-
-
 def _quat(rpy):
     from diff_testlib import quat_from_rpy
     return torch.tensor(quat_from_rpy(np.asarray(rpy, dtype=np.float64)))
@@ -158,7 +141,7 @@ def _ref_tick(P, L, cot, nth, activation, D, effects, flip=()):
 
 
 def _host_tick(P, L, cot, nth, activation, D, A, effects):
-    lib = _harness()
+    lib = harness("diff_policy_host")
     B = L["hist"].shape[1]
     depth = nth // 2 - 1
     arr = lambda t: np.ascontiguousarray(t.detach().numpy(), dtype=np.float64)
@@ -253,6 +236,7 @@ def test_c_abi_refusals_return_before_any_launch():
         f = lib.qs_dyn_policy_traj_vjp if vjp else lib.qs_dyn_policy_traj
         return f(C.byref(P), C.byref(q), act, E, D, S, eff, None)
     assert rc(io(state0=None)) == -1 and rc(io(w2=None)) == -1 and rc(io(), vjp=True) == -1          # QS_ERR_NULL
+    assert lib.qs_last_error().startswith(b"qs_dyn_policy_traj_vjp: ")      # a refusal names the entry point that was called
     assert rc(io(T=0)) == -3 and rc(io(act_buffer_size=0)) == -3 and rc(io(depth=0)) == -3 and rc(io(depth=5)) == -3
     assert rc(io(width0=257)) == -3 and rc(io(width0=0)) == -3 and rc(io(in_dim=73)) == -3 and rc(io(out_dim=8)) == -3
     assert rc(io(activation=2)) == -4 and rc(io(), eff=8) == -4                                      # QS_ERR_ENUM

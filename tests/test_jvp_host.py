@@ -151,6 +151,7 @@ def test_abi_exports_struct_and_refusals():
         setattr(io, out, C.addressof(buf))
         assert call(io, 1, 1, 1, N.EFFECT_DW) == -5
         assert b"downwash" in L.qs_last_error() and b"pairwise" in L.qs_last_error()
+        assert L.qs_last_error().startswith(f.__name__.encode() + b": ")       # a refusal names the entry point that was called
         assert call(io, 1, 1, 1, N.EFFECT_GND | N.EFFECT_DW) == -5
         assert call(io, 1, 1, 1, 8) == -4
         assert call(io, 0, 1, 1, 0) == -3
