@@ -13,8 +13,9 @@ _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))    # override: A/B builds in tools/
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
-                                             "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
+                                             "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
+                                             "dyn_ctrl_jvp.cu")]
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -156,6 +157,13 @@ class QsDynCtrlTrajIO(C.Structure):
         "g_target_rpy", "g_target_rpy_rates", "g_last_rpm", "g_phys", "g_gains", "scratch")]
 
 
+class QsDynCtrlTrajJvpIO(C.Structure):
+    _fields_ = [("T", C.c_int), ("pad_", C.c_int), ("control_timestep", C.c_double)] + [(n, C.c_void_p) for n in (
+        "state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains",
+        "states", "rpm", "pid_states", "t_state0", "t_pid0", "t_target_pos", "t_target_vel", "t_target_rpy", "t_target_rpy_rates",
+        "t_last_rpm", "t_phys", "t_gains", "t_states", "t_rpm", "jac")]
+
+
 class QsDynPolicyTrajIO(C.Structure):
     _fields_ = [("T", C.c_int), ("act_buffer_size", C.c_int), ("activation", C.c_int), ("depth", C.c_int),
                 ("width", C.c_int * MLP_MAX_HIDDEN), ("in_dim", C.c_int), ("out_dim", C.c_int),
@@ -177,7 +185,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_mrac_control", "qs_mrac_control_state", "qs_ctrl_rollout_mrac", "qs_sizeof_mrac_params", "qs_sizeof_mrac_rollout_io",
            "qs_dyn_traj", "qs_dyn_traj_vjp", "qs_sizeof_dyn_traj_io", "qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp",
            "qs_sizeof_dyn_ctrl_traj_io", "qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp", "qs_sizeof_dyn_policy_traj_io",
-           "qs_dyn_traj_jvp", "qs_dyn_tick_jac", "qs_sizeof_dyn_traj_jvp_io"]
+           "qs_dyn_traj_jvp", "qs_dyn_tick_jac", "qs_sizeof_dyn_traj_jvp_io", "qs_dyn_ctrl_traj_jvp", "qs_dyn_ctrl_tick_jac",
+           "qs_sizeof_dyn_ctrl_traj_jvp_io"]
 MAX_PEERS = 16
 
 
@@ -281,6 +290,11 @@ def lib():
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajIO), C.c_int, C.c_int, C.c_int,
                                   C.c_uint, C.c_void_p]
     L.qs_sizeof_dyn_ctrl_traj_io.restype = C.c_int
+    for n in ("qs_dyn_ctrl_traj_jvp", "qs_dyn_ctrl_tick_jac"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajJvpIO), C.c_int, C.c_int, C.c_int,
+                                  C.c_uint, C.c_void_p]
+    L.qs_sizeof_dyn_ctrl_traj_jvp_io.restype = C.c_int
     for n in ("qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynPolicyTrajIO), C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint,
@@ -342,9 +356,10 @@ def lib():
             L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy) or \
             L.qs_sizeof_mrac_params() != C.sizeof(QsMracParams) or L.qs_sizeof_mrac_rollout_io() != C.sizeof(QsMracRolloutIO) or \
             L.qs_sizeof_dyn_traj_io() != C.sizeof(QsDynTrajIO) or L.qs_sizeof_dyn_ctrl_traj_io() != C.sizeof(QsDynCtrlTrajIO) or \
-            L.qs_sizeof_dyn_policy_traj_io() != C.sizeof(QsDynPolicyTrajIO) or L.qs_sizeof_dyn_traj_jvp_io() != C.sizeof(QsDynTrajJvpIO):
+            L.qs_sizeof_dyn_policy_traj_io() != C.sizeof(QsDynPolicyTrajIO) or L.qs_sizeof_dyn_traj_jvp_io() != C.sizeof(QsDynTrajJvpIO) or \
+            L.qs_sizeof_dyn_ctrl_traj_jvp_io() != C.sizeof(QsDynCtrlTrajJvpIO):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac / "
-                          "dyn traj io / dyn ctrl traj io / dyn policy traj io / dyn traj jvp io): "
+                          "dyn traj io / dyn ctrl traj io / dyn policy traj io / dyn traj jvp io / dyn ctrl traj jvp io): "
                           "rebuild")
     _lib = L
     return L

@@ -4,8 +4,7 @@
 // the backward walks the ticks in reverse, reloading each tick's start state and controller state from the forward's outputs and
 // running dyn_adjoint.cuh's tick adjoint, the two clip adjoints and pid_adjoint.cuh's controller adjoint.
 #include "qs_common.cuh"
-#include "pid_adjoint.cuh"
-#include "traj_io.cuh"
+#include "ctrl_io.cuh"
 
 namespace qsi {
 namespace {
@@ -19,45 +18,6 @@ struct CtrlTrajArgs {
     long long N;
     int D, substeps;
 };
-
-__device__ __forceinline__ qs::PidGains gains_of(const CtrlTrajArgs& a, long long i) {
-    if (!a.io.gains) return qs::pid_gains_of(a.CP);
-    const double* g = a.io.gains + 18 * (i / a.D);
-    qs::PidGains k;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        k.pid_p_for[c] = g[c]; k.pid_i_for[c] = g[3 + c]; k.pid_d_for[c] = g[6 + c];
-        k.pid_p_tor[c] = g[9 + c]; k.pid_i_tor[c] = g[12 + c]; k.pid_d_tor[c] = g[15 + c];
-    }
-    return k;
-}
-__device__ __forceinline__ void ld3(const double* p, long long i, double v[3]) {
-    if (p) { v[0] = p[3 * i]; v[1] = p[3 * i + 1]; v[2] = p[3 * i + 2]; } else { v[0] = v[1] = v[2] = 0.0; }
-}
-// the tick's targets of drone i: target_pos of tick k, the constant target_vel, target yaw and target_rpy_rates
-__device__ __forceinline__ qs::PidTargets targets_of(const QsDynCtrlTrajIO& io, long long N, long long i, int k) {
-    qs::PidTargets t;
-    ld3(io.target_pos, (long long)k * N + i, t.tp);
-    ld3(io.target_vel, i, t.tv);
-    double r[3];
-    ld3(io.target_rpy, i, r);
-    t.tyaw = r[2];
-    ld3(io.target_rpy_rates, i, t.trr);
-    return t;
-}
-
-// computeControlFromEnv + the two clips of the TRACK tick: the raw controller RPMs, the controller's clip u1, the applied u
-__device__ __forceinline__ void control(const CtrlTrajArgs& a, const qs::PidGains& K, qs::PidState& st, const qs::Drone& d,
-                                        const qs::PidTargets& t, double mr, double raw[4], double u1[4], double u[4]) {
-    double pe[3], ye;
-    qs::pid_control_k(a.CP, K, st, a.io.control_timestep, d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz,
-                      t.tp[0], t.tp[1], t.tp[2], t.tyaw, t.tv[0], t.tv[1], t.tv[2], t.trr[0], t.trr[1], t.trr[2], raw, pe, ye);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        u1[j] = qs::clampd(raw[j], 0.0, a.CP.max_rpm);
-        u[j] = qs::clampd(u1[j], 0.0, mr);
-    }
-}
 
 template <int EFF>
 __global__ void __launch_bounds__(kCtrlTrajTPB) dyn_ctrl_traj_kernel(const __grid_constant__ CtrlTrajArgs a) {

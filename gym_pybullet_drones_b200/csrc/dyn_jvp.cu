@@ -19,16 +19,6 @@ struct JvpArgs {
     int D, substeps;
 };
 
-// the tangent of the constants: the aviary's row of t_phys, or zero
-__device__ __forceinline__ qs::PhysRow t_row_of(const JvpArgs& a, long long i) {
-    return aviary_row(a, a.io.t_phys, i, [] {
-        qs::PhysRow z;
-        z.inv_m = z.gravity = z.kf = z.km = z.kx = z.ky = z.hover_rpm = z.max_rpm = 0.0;
-        for (int k = 0; k < 3; ++k) z.j[k] = z.j_inv[k] = 0.0;
-        return z;
-    });
-}
-
 template <int EFF>
 __global__ void __launch_bounds__(kJvpTPB) dyn_traj_jvp_kernel(const __grid_constant__ JvpArgs a) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;

@@ -24,6 +24,27 @@ QS_HD void rpm_clip_jvp(const double raw[4], double max_rpm, const double t_raw[
     for (int i = 0; i < 4; ++i) t_u[i] = raw[i] > max_rpm ? t_max : (raw[i] < 0.0 ? 0.0 : t_raw[i]);
 }
 
+// t_rpy += d rpy / d q  t_q for rpy = quat_to_euler<false>(q), on the forward's branch of the +-0.99999 gimbal guard: the
+// transpose of quat_to_euler_vjp (in the guard roll and pitch are constants and yaw = 2 atan2(x, -y) or 2 atan2(-x, y))
+QS_HD void quat_to_euler_jvp(double qx, double qy, double qz, double qw, const double t_q[4], double t_rpy[3]) {
+    const double sarg = -2.0 * (qx * qz - qw * qy);
+    const double dx = t_q[0], dy = t_q[1], dz = t_q[2], dw = t_q[3];
+    if (sarg <= -0.99999 || sarg >= 0.99999) {
+        const double r2 = qx * qx + qy * qy;
+        t_rpy[2] += (-2.0 * qy / r2) * dx + (2.0 * qx / r2) * dy;
+    } else {
+        const double ra = 2.0 * (qy * qz + qw * qx), rb = qw * qw - qx * qx - qy * qy + qz * qz;
+        const double ya = 2.0 * (qx * qy + qw * qz), yb = qw * qw + qx * qx - qy * qy - qz * qz;
+        const double n_r = ra * ra + rb * rb, n_y = ya * ya + yb * yb;
+        const double dra = 2.0 * (qw * dx + qz * dy + qy * dz + qx * dw), drb = 2.0 * (-qx * dx - qy * dy + qz * dz + qw * dw);
+        const double dsarg = 2.0 * (-qz * dx + qw * dy - qx * dz + qy * dw);
+        const double dya = 2.0 * (qy * dx + qx * dy + qw * dz + qz * dw), dyb = 2.0 * (qx * dx - qy * dy - qz * dz + qw * dw);
+        t_rpy[0] += (rb * dra - ra * drb) / n_r;
+        t_rpy[1] += dsarg / sqrt(1.0 - sarg * sarg);
+        t_rpy[2] += (yb * dya - ya * dyb) / n_y;
+    }
+}
+
 // Tangent of one substep of dyn_tick_k<EFF> from its start state x with (clipped) rpm u and drag sum ds.  t: in, the tangent of
 // x; out, of the substep's end state.  tc / tu / tds: the tangents of the constants, of u and of ds.
 template <int EFF>

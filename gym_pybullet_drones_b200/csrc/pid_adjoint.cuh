@@ -19,7 +19,7 @@
 
 #if defined(__CUDACC__)
 // out of line on the device: the tick adjoint of dyn_adjoint.cuh already holds most of the register file (DESIGN.md 4.5)
-#define QS_HD_NOINLINE __host__ __device__ __noinline__
+#define QS_HD_NOINLINE inline __host__ __device__ __noinline__
 #else
 #define QS_HD_NOINLINE inline
 #endif

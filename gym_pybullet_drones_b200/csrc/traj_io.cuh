@@ -1,5 +1,5 @@
 // traj_io.cuh -- what the differentiable-trajectory translation units (dyn_traj.cu, dyn_ctrl_traj.cu, dyn_policy_traj.cu,
-// dyn_jvp.cu) share: device-side loads and stores of states in the planes layout, the substep record of the tick adjoint, the
+// dyn_jvp.cu, dyn_ctrl_jvp.cu) share: device-side loads and stores of states in the planes layout, the substep record of the tick adjoint, the
 // per-drone inputs and outputs of a tick, and on the host the argument checks and the launch over TrajEffects.
 #pragma once
 #include "qs_common.cuh"
@@ -42,6 +42,16 @@ __device__ __forceinline__ qs::PhysRow aviary_row(const Args& a, const double* p
 template <class Args>
 __device__ __forceinline__ qs::PhysRow row_of(const Args& a, long long i) {
     return aviary_row(a, a.io.phys, i, [&] { return qs::phys_row_of(a.P); });
+}
+// the tangent of the constants (forward mode): the row of a.io.t_phys, or zero
+template <class Args>
+__device__ __forceinline__ qs::PhysRow t_row_of(const Args& a, long long i) {
+    return aviary_row(a, a.io.t_phys, i, [] {
+        qs::PhysRow z;
+        z.inv_m = z.gravity = z.kf = z.km = z.kx = z.ky = z.hover_rpm = z.max_rpm = 0.0;
+        for (int k = 0; k < 3; ++k) z.j[k] = z.j_inv[k] = 0.0;
+        return z;
+    });
 }
 
 __device__ __forceinline__ void clip_rpm(const double raw[4], double max_rpm, double u[4]) {

@@ -118,32 +118,64 @@ class DynTrajectory(torch.autograd.Function):
         return g["g_rpm"], g["g_state0"], g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), None
 
 
+CTRL_INS = ("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains")
+
+
+def _dyn_ctrl_traj(cfg, ins):
+    """{states [T, 13 N], rpm [T, N, 4], pid_states [T, 9, N]} of qs_dyn_ctrl_traj from the dense inputs `ins` (CTRL_INS)."""
+    P, CP, dt, E, D, S, eff = cfg
+    tpos = ins["target_pos"]
+    T, n = tpos.shape[0], E * D
+    f64 = dict(dtype=torch.float64, device=tpos.device)
+    outs = dict(states=torch.empty((T, 13 * n), **f64), rpm=torch.empty((T, n, 4), **f64), pid_states=torch.empty((T, 9, n), **f64))
+    io = _io(N.QsDynCtrlTrajIO, T, dict(ins, **outs), control_timestep=dt)
+    _call("qs_dyn_ctrl_traj", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=tpos.device)
+    return outs
+
+
 class DynCtrlTrajectory(torch.autograd.Function):
     """(states [T, 13 N], rpm [T, N, 4]) = the T ticks of qs_dyn_ctrl_traj from planes0 [13 N] and the controller state pid0
     [9, N], with target_pos [T, N, 3], target_vel / target_rpy / target_rpy_rates [N, 3], last_rpm [N, 4], the per-aviary rows
     [E, 16] and gain sets [E, 18]; backward = qs_dyn_ctrl_traj_vjp, its per-drone row and gain gradients summed over each
-    aviary's drones (torch, deterministic).  `cfg` = (env QsParams, controller QsParams, control_timestep, E, D, substeps,
-    effects).  The inputs may have any strides (the kernels get contiguous copies).  Double backward raises ValueError."""
+    aviary's drones (torch, deterministic); jvp (torch.autograd.forward_ad) = qs_dyn_ctrl_traj_jvp.  `cfg` = (env QsParams,
+    controller QsParams, control_timestep, E, D, substeps, effects).  The inputs may have any strides (the kernels get
+    contiguous copies).  Double backward and tangents that require grad raise ValueError."""
 
     @staticmethod
     def forward(ctx, planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains, cfg):
-        ins = dict(zip(("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains"),
-                       (x.contiguous() for x in (planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains))))
-        P, CP, dt, E, D, S, eff = cfg
-        T, n = tpos.shape[0], E * D
-        f64 = dict(dtype=torch.float64, device=tpos.device)
-        outs = dict(states=torch.empty((T, 13 * n), **f64), rpm=torch.empty((T, n, 4), **f64), pid_states=torch.empty((T, 9, n), **f64))
-        io = _io(N.QsDynCtrlTrajIO, T, dict(ins, **outs), control_timestep=dt)
-        _call("qs_dyn_ctrl_traj", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=tpos.device)
+        ins = dict(zip(CTRL_INS, (x.contiguous() for x in (planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains))))
+        outs = _dyn_ctrl_traj(cfg, ins)
         ctx.save_for_backward(*ins.values(), *outs.values())
+        ctx.save_for_forward(*ins.values(), *outs.values())
         ctx.cfg = cfg
         return outs["states"], outs["rpm"]
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        """Forward mode: the tangents (t_states [T, 13 N], t_rpm [T, N, 4]) along the inputs' tangents (qs_dyn_ctrl_traj_jvp,
+        which linearises each tick at the forward's stored states).  A tangent that requires grad raises ValueError."""
+        tangents = tangents[:9]
+        if any(t is not None and t.requires_grad for t in tangents):
+            raise ValueError("differentiable_rollout: a tangent that requires grad (reverse mode over forward mode) is not supported: "
+                             "the JVP kernel has no derivative of its own")
+        saved = ctx.saved_tensors
+        P, CP, dt, E, D, S, eff = ctx.cfg
+        states = saved[9]
+        dense = [None if t is None else t.to(torch.float64).contiguous() for t in tangents]
+        if dense[7] is not None and dense[7].data_ptr() % 16:          # the kernel reads t_phys rows as 16-byte pairs
+            dense[7] = dense[7].clone()
+        t_states, t_rpm = torch.empty_like(states), torch.empty_like(saved[10])
+        ptrs = dict(zip(CTRL_INS, saved[:9]), **dict(zip(("states", "rpm", "pid_states"), saved[9:])),
+                    **dict(zip(("t_" + k for k in CTRL_INS), dense)), t_states=t_states, t_rpm=t_rpm)
+        io = _io(N.QsDynCtrlTrajJvpIO, states.shape[0], ptrs, control_timestep=dt)
+        _call("qs_dyn_ctrl_traj_jvp", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=states.device)
+        return t_states, t_rpm
 
     @staticmethod
     def backward(ctx, g_states, g_rpm):
         _no_double_backward()
         saved = ctx.saved_tensors
-        ins = dict(zip(("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains"), saved[:9]))
+        ins = dict(zip(CTRL_INS, saved[:9]))
         outs = dict(zip(("states", "rpm", "pid_states"), saved[9:]))
         P, CP, dt, E, D, S, eff = ctx.cfg
         T, n = ins["target_pos"].shape[0], E * D
@@ -378,13 +410,17 @@ def schedule_targets(waypoints, start, offset, T, E, D, dev):
     return tpos
 
 
-def _closed_loop(env, controller, state, last_rpm, phys, waypoints=None, start=None, offset=None, target_rpy=None, target_vel=None,
-                 target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None, pid_state=None):
+def _closed_loop_inputs(env, controller, state, last_rpm, phys, caller, derivative, waypoints=None, start=None, offset=None,
+                        target_rpy=None, target_vel=None, target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None,
+                        pid_state=None):
+    """The checked arguments of a closed-loop call (differentiable_rollout(controller=) or linearise(controller=)): (cfg, T,
+    inputs), inputs = (planes0, pid0, target_pos, target_vel, target_rpy, target_rpy_rates, last_rpm, rows, gains) as
+    DynCtrlTrajectory takes them.  `caller` / `derivative` name the call and its derivative in the MRAC refusal."""
     from .control.DSLPIDControl import DSLPIDControl
     from .control.MRAC import MRAC
     E, D, n, dev = env._E, env._D, env._N, env.device
     if isinstance(controller, MRAC):
-        raise ValueError("differentiable_rollout() has no adjoint of MRAC: pass a DSLPIDControl")
+        raise ValueError("%s has no %s of MRAC: pass a DSLPIDControl" % (caller, derivative))
     if not isinstance(controller, DSLPIDControl):
         raise ValueError("controller must be a DSLPIDControl, got %s" % type(controller).__name__)
     if controller.num_drones != n:
@@ -421,9 +457,15 @@ def _closed_loop(env, controller, state, last_rpm, phys, waypoints=None, start=N
                       else controller._state[3 * j:3 * j + 3].detach().clone() for j, k in enumerate(PID_KEYS)])
     planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
     dt = float(env.CTRL_TIMESTEP if control_timestep is None else control_timestep)
+    cfg = (env._P, CP, dt, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
+    return cfg, T, (planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, table)
+
+
+def _closed_loop(env, controller, state, last_rpm, phys, **schedule):
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    cfg, T, ins = _closed_loop_inputs(env, controller, state, last_rpm, phys, "differentiable_rollout()", "adjoint", **schedule)
     with torch.cuda.device(dev):
-        cfg = (env._P, CP, dt, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
-        states, rpm = DynCtrlTrajectory.apply(planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, table, cfg)
+        states, rpm = DynCtrlTrajectory.apply(*ins, cfg)
     out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
     out["rpm"] = rpm.reshape(T, E, D, 4)
     return out
@@ -491,9 +533,44 @@ def tick_jacobians(cfg, rpm, planes0, last_rpm, rows):
     return states, jac
 
 
-def linearise(env, rpm, state=None, last_rpm=None, phys=None):
+def ctrl_tick_jacobians(cfg, ins):
+    """({states, rpm, pid_states} of qs_dyn_ctrl_traj, jac [T, N, 26, C]) of qs_dyn_ctrl_tick_jac from the dense inputs `ins`
+    (CTRL_INS); `cfg` as DynCtrlTrajectory's, C = 25 or 29 with drag (include/quadsim.h)."""
+    P, CP, dt, E, D, S, eff = cfg
+    outs = _dyn_ctrl_traj(cfg, ins)
+    T, dev = ins["target_pos"].shape[0], ins["target_pos"].device
+    jac = torch.empty((T, E * D, 26, 29 if eff & N.EFFECT_DRAG else 25), dtype=torch.float64, device=dev)
+    io = _io(N.QsDynCtrlTrajJvpIO, T, dict(ins, **outs, jac=jac), control_timestep=dt)
+    _call("qs_dyn_ctrl_tick_jac", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=dev)
+    return outs, jac
+
+
+def _linearise_closed_loop(env, controller, state, last_rpm, phys, **schedule):
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    with torch.no_grad():
+        cfg, T, ins = _closed_loop_inputs(env, controller, state, last_rpm, phys, "linearise()", "tangent", **schedule)
+        with torch.cuda.device(dev):
+            outs, jac = ctrl_tick_jacobians(cfg, dict(zip(CTRL_INS, (x.detach().contiguous() for x in ins))))
+    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(outs["states"], n).items()}
+    out["rpm"] = outs["rpm"].view(T, E, D, 4)
+    out["pid_state"] = outs["pid_states"].transpose(1, 2).reshape(T, E, D, 9)
+    nz = 26 if cfg[6] & N.EFFECT_DRAG else 22
+    jac = jac.view(T, E, D, 26, jac.shape[-1])
+    out["A"], out["B"] = jac[..., :nz, :nz], jac[..., :nz, nz:]
+    out["K"], out["K_target"] = jac[..., 22:26, :nz], jac[..., 22:26, nz:]
+    return out
+
+
+def linearise(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, **schedule):
     """BaseAviary.linearise (see there)."""
     _refuse_downwash(env, "linearise()", "tangent")
+    if (rpm is not None) + (controller is not None) != 1:
+        raise ValueError("linearise() takes exactly one of rpm [T, E, D, 4] (open loop) or controller= (closed loop)")
+    if controller is not None:
+        return _linearise_closed_loop(env, controller, state, last_rpm, phys, **schedule)
+    given = sorted(k for k, v in schedule.items() if v is not None)
+    if given:
+        raise ValueError("%s apply to a controller linearisation only" % ", ".join(given))
     E, D, n = env._E, env._D, env._N
     T = _rpm_ticks(env, rpm)
     with torch.no_grad():

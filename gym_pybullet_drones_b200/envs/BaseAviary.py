@@ -595,7 +595,13 @@ class BaseAviary(Env):
         control_counter stay as they were.  The controller's derivative (DESIGN.md 4.5): every clip as torch.clamp (integral
         clips, torque clip, PWM clip, max_rpm clips), zero where the thrust scalar is <= 0, the forward's branch of the Euler
         angles' gimbal guard, the rate term without angle unwrap.  An MRAC, a controller of the wrong size or device, both rpm
-        and a controller or neither, and unknown keys raise ValueError.
+        and a controller or neither, and unknown keys raise ValueError.  Forward mode: dual tensors (torch.autograd.forward_ad)
+        on any of state, pid_state, waypoints, offset, target_rpy / target_vel / target_rpy_rates, gains, last_rpm and phys give
+        the tangents of the four state entries and rpm (one JVP kernel launch with the same decisions; the primal outputs keep
+        their bits).  The controller reads the stored, unnormalised quaternion, so the closed loop's derivative w.r.t.
+        state["quat"] has a radial part, unlike the open loop's.  linearise(controller=) gives the per-tick Jacobians of the
+        closed loop, rows and columns in the order x (pos, quat x y z w, vel, rpy_rates), controller state (integral_pos_e,
+        last_rpy, integral_rpy_e) and, with drag, the previous tick's applied RPMs.
 
         Policy loop (HoverAviary / MultiHoverAviary with ActionType.RPM or ONE_D_RPM): `policy` is an MlpPolicy mapping
         D * obs_dim inputs to D * A outputs, `params` its float64 parameters as `policy.parameters64()` lays them out ([W1, b1,
@@ -620,14 +626,17 @@ class BaseAviary(Env):
                                       target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps,
                                       gains=gains, pid_state=pid_state)
 
-    def linearise(self, rpm, *, state=None, last_rpm=None, phys=None):
+    def linearise(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None, target_vel=None,
+                  target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None, pid_state=None, state=None,
+                  last_rpm=None, phys=None):
         """The per-tick Jacobians of every drone along the raw-RPM trajectory of differentiable_rollout(rpm, state=,
-        last_rpm=, phys=), in one kernel launch after the forward (DESIGN.md 4.5): what LQR, iLQR / DDP, EKF-style estimators
-        and stability analysis linearise at.  Arguments, checks and defaults are differentiable_rollout(rpm)'s; the result is
-        not differentiable, and the env is not touched.
+        last_rpm=, phys=), or along its closed loop differentiable_rollout(controller=, ...), in one kernel launch after the
+        forward (DESIGN.md 4.5): what LQR, iLQR / DDP, EKF-style estimators and stability analysis linearise at.  Pass exactly
+        one of `rpm` or `controller`.  Arguments, checks and defaults are differentiable_rollout's; the result is not
+        differentiable, and neither the env nor the controller is touched.
 
-        Returns {pos, quat, vel, rpy_rates} of the nominal trajectory ([T, E, D, k], entry k the state after tick k, the same
-        bits as differentiable_rollout) and, for tick k,
+        Open loop (rpm): returns {pos, quat, vel, rpy_rates} of the nominal trajectory ([T, E, D, k], entry k the state after
+        tick k, the same bits as differentiable_rollout) and, for tick k,
           A      [T, E, D, 13, 13]  d x_{k+1} / d x_k,
           B      [T, E, D, 13, 4]   d x_{k+1} / d rpm[k] (the raw command: zero through a clipped rotor),
           B_last [T, E, D, 13, 4]   with drag only: d x_{k+1} / d (the clipped RPMs of tick k-1, last_rpm for k = 0), which drag's
@@ -637,9 +646,27 @@ class BaseAviary(Env):
         the quaternion columns of A act on the stored quaternion and A[..., :, 3:7] @ q_hat = 0.  The derivative decisions are
         differentiable_rollout's (the exponential map everywhere, the RPM clip as torch.clamp, the height clip's predicate, the
         upright switch constant), so the Jacobians are exactly the transposes of its backward's.  A, B and B_last are views of
-        one [T, E, D, 13, 13 + 4 (+ 4)] tensor.  Downwash and bad inputs raise ValueError."""
+        one [T, E, D, 13, 13 + 4 (+ 4)] tensor.
+
+        Closed loop (controller, with differentiable_rollout's schedule arguments): the loop's state is z_k = (x_k, s_k) of
+        n_z = 22 entries, or z_k = (x_k, s_k, u_{k-1}) of n_z = 26 with drag, where x_k is the drone state as above, s_k the
+        controller state tick k starts from (integral_pos_e, last_rpy, integral_rpy_e) and u_{k-1} the applied RPMs of tick k-1
+        (last_rpm for k = 0), which drag reads.  Returns the nominal trajectory (the four state entries and `rpm` as
+        differentiable_rollout(controller=) returns them, and pid_state [T, E, D, 9], s_k) and, for tick k,
+          A        [T, E, D, n_z, n_z]  d z_{k+1} / d z_k,
+          B        [T, E, D, n_z, 3]    d z_{k+1} / d target_pos[k],
+          K        [T, E, D, 4, n_z]    d u_k / d z_k, the PID's local gain (no minus sign),
+          K_target [T, E, D, 4, 3]      d u_k / d target_pos[k].
+        The controller reads the stored, unnormalised quaternion (Bullet's matrix and Euler angles divide by |q|^2 or not at
+        all), so unlike the open loop the closed-loop A has no quaternion null space.  The derivative decisions are
+        differentiable_rollout(controller=)'s, so the Jacobians are exactly the transposes of its backward's.  All four are
+        views of one [T, E, D, 26, n_z + 3] tensor whose rows are x_{k+1}, s_{k+1}, u_k.  Downwash, an MRAC, both rpm and a
+        controller or neither, and bad inputs raise ValueError."""
         from ..diff import linearise
-        return linearise(self, rpm, state=state, last_rpm=last_rpm, phys=phys)
+        return linearise(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, waypoints=waypoints,
+                         start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
+                         target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps, gains=gains,
+                         pid_state=pid_state)
 
     ################################################################################
 

@@ -710,6 +710,54 @@ int qs_dyn_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajI
 int qs_dyn_ctrl_traj_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
                          int substeps, unsigned effects, void* stream);
 
+/* Forward mode of the closed-loop trajectories of qs_dyn_ctrl_traj (DESIGN.md 4.5): the tangents of the T states and applied
+ * RPMs along given tangents of the inputs (JVP), and the dense Jacobians of every closed-loop tick.  Both read the forward's
+ * states, rpm and pid_states and restart tick k from the stored state k-1 (state0 for k = 0) and controller state pid_states[k],
+ * so the loop is linearised at the forward's bits, and both take the derivative decisions of qs_dyn_ctrl_traj_vjp (they are its
+ * exact transpose).  The controller reads the stored, unnormalised quaternion, so the closed-loop Jacobian has no quaternion null
+ * space.  Layouts as in QsDynCtrlTrajIO.  All indices are 64-bit. */
+typedef struct QsDynCtrlTrajJvpIO {
+    int T;                          /* ticks, > 0 */
+    int pad_;
+    double control_timestep;        /* the controller's dt, > 0 */
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* pid0;             /* [9][N] the controller state before tick 0 */
+    const double* target_pos;       /* [T][N][3] */
+    const double* target_vel;       /* [N][3], nullable = zeros */
+    const double* target_rpy;       /* [N][3], nullable = zeros */
+    const double* target_rpy_rates; /* [N][3], nullable = zeros */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows; nullable = the constants of the env's QsParams */
+    const double* gains;            /* [n_envs][18]; nullable = cp's */
+    const double* states;           /* [T][13 N] qs_dyn_ctrl_traj's states for these inputs */
+    const double* rpm;              /* [T][N][4] qs_dyn_ctrl_traj's applied RPMs */
+    const double* pid_states;       /* [T][9][N] qs_dyn_ctrl_traj's controller states */
+    /* qs_dyn_ctrl_traj_jvp: tangents of the inputs, each nullable = zero */
+    const double* t_state0;         /* [13 N] */
+    const double* t_pid0;           /* [9][N] */
+    const double* t_target_pos;     /* [T][N][3] */
+    const double* t_target_vel;     /* [N][3] */
+    const double* t_target_rpy;     /* [N][3] (only component 2, the yaw, is read) */
+    const double* t_target_rpy_rates; /* [N][3] */
+    const double* t_last_rpm;       /* [N][4] */
+    const double* t_phys;           /* [n_envs][16], 16-byte aligned */
+    const double* t_gains;          /* [n_envs][18] */
+    double* t_states;               /* qs_dyn_ctrl_traj_jvp out: [T][13 N] the tangents of the states */
+    double* t_rpm;                  /* qs_dyn_ctrl_traj_jvp out: [T][N][4] the tangents of the applied RPMs */
+    /* qs_dyn_ctrl_tick_jac out: [T][N][26][C], C = 25 (29 with QS_EFFECT_DRAG).  Rows: x_{k+1} (13: pos, quat x y z w, vel,
+     * rpy_rates), the controller state after tick k's call (9: integral_pos_e, last_rpy, integral_rpy_e), the applied RPMs u_k (4).
+     * Columns: the stored x_k (13), the controller state s_k = pid_states[k] (9), with drag u_{k-1} (4, last_rpm for k = 0), then
+     * target_pos[k] (3).  With z_k = (x_k, s_k[, u_{k-1}]) of n_z = 22 (26) entries, jac[..., :n_z, :n_z] is dz_{k+1} / dz_k. */
+    double* jac;
+} QsDynCtrlTrajJvpIO;
+int qs_sizeof_dyn_ctrl_traj_jvp_io(void);
+/* refusals as qs_dyn_ctrl_traj, and NULL outputs, t_phys not 16-byte aligned, QS_ERR_SIZE when T N C / 128 exceeds 2^31-1 CTAs
+ * (qs_dyn_ctrl_tick_jac) */
+int qs_dyn_ctrl_traj_jvp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajJvpIO* io, int n_envs, int drones_per_env,
+                         int substeps, unsigned effects, void* stream);
+int qs_dyn_ctrl_tick_jac(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajJvpIO* io, int n_envs, int drones_per_env,
+                         int substeps, unsigned effects, void* stream);
+
 /* Differentiable policy trajectories (DESIGN.md 4.5): T control ticks of an MLP actor driving Physics.DYN (+ GND and/or DRAG, no
  * downwash) through the RPM or ONE_D_RPM action decode, and their VJP.  Tick k: the aviary's float64 observation
  * [D][12 + B A] (pos, rpy, vel, ang_v = R_last w, then the B buffered clipped actions, oldest first) of the state after tick
