@@ -15,7 +15,7 @@ _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
                                              "dyn_ctrl_jvp.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"), os.path.join(_CSRC, "rollout_kernel_body.inc"),
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)

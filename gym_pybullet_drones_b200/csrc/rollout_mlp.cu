@@ -1,5 +1,6 @@
 // rollout_mlp.cu -- qs_rollout_mlp: the policy rollout with a general network (QsMlpPolicy; DESIGN.md 4.1b): the rollout kernel's
-// body with warp_mlp in place of warp_net, in a translation unit of its own so that it compiles in parallel with rollout.cu.
+// kNetMlp instantiations (warp_mlp in place of warp_net), in a translation unit of their own so that they compile in parallel
+// with rollout.cu.
 #include "rollout_kernel.cuh"
 
 using namespace qsi;
@@ -41,19 +42,6 @@ int check_net(const QsMlpNet& n, const char* which, bool critic) {
     return 0;
 }
 
-template <int EFF, bool PIDACT, bool PHYS, int MODE>
-void launch_mlp(const MlpRolloutArgs& a, int blocks, cudaStream_t s) {
-    auto* k = rollout_mlp_kernel<EFF, PIDACT, PHYS, MODE>;
-    const size_t sm = (size_t)a.stage_off + mlp_stage_bytes(a.stage_ks * 16);
-    if (sm > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    // carve-out: the resident CTAs (as many as the staging leaves room for, at most the register limit), the rest is L1
-    int ctas = (int)((228 * 1024) / (sm + 1024));
-    if (ctas > policy_ctas(EFF)) ctas = policy_ctas(EFF);
-    if (ctas < 1) ctas = 1;
-    set_policy_carveout(k, ctas, sm);
-    k<<<blocks, 64, sm, s>>>(a);
-}
-
 }  // namespace
 
 extern "C" {
@@ -81,9 +69,10 @@ int qs_rollout_mlp(const QsParams* p, const QsState* st, const QsRolloutIO* io, 
     MlpRolloutArgs a;
     memset(&a, 0, sizeof(a));
     bool pid_act = false;
-    if (int rc = prepare_rollout(p, st, io, act_type, task, n_envs, drones_per_env, substeps, effects, flags, q.critic.depth > 0, a, pid_act))
+    if (int rc = prepare_rollout("qs_rollout_mlp", p, st, io, act_type, task, n_envs, drones_per_env, substeps, effects, flags,
+                                 q.critic.depth > 0, a, pid_act))
         return rc;
-    if (int rc = check_policy_config(a, io)) return rc;
+    if (int rc = check_policy_config("qs_rollout_mlp", a, io)) return rc;
     if (q.activation != QS_MLP_TANH && q.activation != QS_MLP_RELU) return fail(QS_ERR_ENUM, "qs_rollout_mlp: activation must be QS_MLP_TANH or QS_MLP_RELU");
     if (int rc = check_net(q.actor, "actor", false)) return rc;
     if (q.critic.depth != 0)
@@ -102,21 +91,14 @@ int qs_rollout_mlp(const QsParams* p, const QsState* st, const QsRolloutIO* io, 
     const size_t sm_var = policy_smem_var(a.tpb, a.obs_dim, io->T, a.A, drones_per_env, q.actor.out_tiles);
     a.stage_off = (int)((policy_smem_fixed(a.effects & 7u) + sm_var + 15) / 16 * 16);
     a.stage_ks = wmax / 16;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int mode = (flags & QS_FLAG_AUTORESET_NEXT_STEP) ? kRolloutNext : (io->final_obs || io->final_values) ? kRolloutFin : kRolloutNone;
-    const int blocks = (int)((a.N + a.tpb - 1) / a.tpb);
-    // check_policy_config has rejected every effect set outside PolicyEffects
-    with_int(PolicyEffects{}, (int)(a.effects & 7u), [&](auto EFF) {
-        with_bool(pid_act, [&](auto PIDACT) {
-            with_bool(a.st.phys != nullptr, [&](auto PHYS) {
-                with_int(IntList<kRolloutNone, kRolloutFin, kRolloutNext>{}, mode, [&](auto MODE) {
-                    launch_mlp<decltype(EFF)::value, decltype(PIDACT)::value, decltype(PHYS)::value, decltype(MODE)::value>(a, blocks, s);
-                });
-            });
+    const size_t sm = (size_t)a.stage_off + mlp_stage_bytes(wmax);
+    int rc = 0;
+    with_bool(a.st.phys != nullptr, [&](auto PHYS) {
+        with_int(IntList<kRolloutNone, kRolloutFin, kRolloutNext>{}, rollout_mode(io, flags), [&](auto MODE) {
+            rc = launch_policy<kNetMlp, decltype(PHYS)::value, decltype(MODE)::value>(a, sm, pid_act, (cudaStream_t)stream);
         });
     });
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, "qs_rollout_mlp launch");
+    return rc;
 }
 
 }  // extern "C"

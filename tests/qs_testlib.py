@@ -102,7 +102,7 @@ def ptr(a):
 
 
 class PolicyRef:
-    """Float64 NumPy restatement of the on-device policy (`MlpPolicy` evaluated by rollout_kernel<.,.,true>): actor mean,
+    """Float64 NumPy restatement of the on-device policy (`MlpPolicy` evaluated by rollout_kernel<.,.,kNetClassic>): actor mean,
     sampled action, log-probability and critic value from the fp32 weights the policy holds, plus the accuracy criterion the
     kernel is held to.
 

@@ -133,6 +133,7 @@ def test_round2_entry_points_validate_arguments_without_a_gpu():
     rio.T, rio.act_buffer_size = 4, 15
     rio.policy = C.addressof(pol)
     assert lib.qs_rollout(C.byref(P), C.byref(st), C.byref(rio), 0, 1, 4, 2, 8, 0, 0, None) == -1 and b"policy" in lib.qs_last_error()
+    assert lib.qs_last_error().startswith(b"qs_rollout: ")
 
 
 def test_fused_publish_entry_point_validates_arguments_without_a_gpu():

@@ -1,4 +1,4 @@
-"""The on-device policy of qs_rollout (rollout_kernel<0, false, true>: SB3-MlpPolicy-shaped actor and critic on the tensor cores
+"""The on-device policy of qs_rollout (rollout_kernel<0, false, kNetClassic>: SB3-MlpPolicy-shaped actor and critic on the tensor cores
 with a two-term fp16 split of both operands) against the float64 reference tests/qs_testlib.PolicyRef, at every shape the
 kernel accepts.
 

@@ -1,5 +1,5 @@
 """The on-device policy of qs_rollout with the embedded DSLPID controller (PID, VEL, ONE_D_PID actions) and with the DYN+ effects
-(ground effect, drag, downwash): rollout_kernel<EFF, PIDACT, true, PHYS>.
+(ground effect, drag, downwash): rollout_kernel<EFF, PIDACT, kNetClassic, PHYS>.
 
 Every case runs the two checks of test_gpu_policy.py, with episodes started near their time limit so that same-step autoresets
 happen inside the rollout:
@@ -282,7 +282,7 @@ def test_policy_refuses_effect_sets_the_envs_cannot_produce(effects, what):
     buf = (C.c_char * 256)()
     pol = _complete_policy(2 * 57, 2 * 3, buf)
     rc, msg = _rollout_call(lib, N.ACT_PID, 2, effects, pol)
-    assert rc == -5 and what in msg and "policy" in msg, (rc, msg)
+    assert rc == -5 and what in msg and "policy" in msg and msg.startswith("qs_rollout: "), (rc, msg)
 
 
 def test_policy_refusals_before_launch():
@@ -292,12 +292,12 @@ def test_policy_refusals_before_launch():
     buf = (C.c_char * 256)()
     # PID, D = 2: obs 12 + 15 * 3 = 57
     rc, msg = _rollout_call(lib, N.ACT_PID, 2, 7, _complete_policy(2 * 57, 2 * 4, buf))
-    assert rc == -3 and "in_dim/out_dim" in msg, (rc, msg)
+    assert rc == -3 and "in_dim/out_dim" in msg and msg.startswith("qs_rollout: "), (rc, msg)
     rc, msg = _rollout_call(lib, N.ACT_ONE_D_PID, 65, 0, _complete_policy(65 * 27, 65, buf))
-    assert rc == -5 and "drones_per_env <= 64" in msg, (rc, msg)
+    assert rc == -5 and "drones_per_env <= 64" in msg and msg.startswith("qs_rollout: "), (rc, msg)
     pol = N.QsPolicy()                                   # empty: NULL weights
     rc, msg = _rollout_call(lib, N.ACT_VEL, 2, 4, pol)
-    assert rc == -1 and "policy" in msg, (rc, msg)
+    assert rc == -1 and "policy" in msg and msg.startswith("qs_rollout: "), (rc, msg)
 
 
 @pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""The on-device policy with any supported SB3 net_arch (qs_rollout_mlp: rollout_mlp_kernel<EFF, PIDACT, PHYS, MODE>).
+"""The on-device policy with any supported SB3 net_arch (qs_rollout_mlp: rollout_kernel<EFF, PIDACT, kNetMlp, PHYS, MODE>).
 
 Every case runs the two checks of test_gpu_policy_actions.py, with same-step autoresets inside the rollout:
 * network, teacher-forced per tick against the float64 tests/mlp_ref.MlpRef (PolicyRef's criterion generalised to any depth and

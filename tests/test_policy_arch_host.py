@@ -274,11 +274,11 @@ def _set(field, value, net="actor"):
 ])
 def test_mlp_entry_argument_errors_without_a_gpu(mutate, kw, code, match):
     rc, msg = _mlp_call(N.lib(), mutate, **kw)
-    assert rc == code and match in msg, (rc, msg)
+    assert rc == code and match in msg and msg.startswith("qs_rollout_mlp: "), (rc, msg)
 
 
 def test_mlp_entry_null_policy_and_drones_per_env():
     lib = N.lib()
     assert lib.qs_rollout_mlp(None, None, None, None, 0, 1, 4, 2, 8, 0, 0, None) == -1
     rc, msg = _mlp_call(lib, lambda q: setattr(q, "in_dim", 65 * 27) or setattr(q, "out_dim", 65), act_type=N.ACT_ONE_D_RPM, D=65)
-    assert rc == -5 and "drones_per_env <= 64" in msg, (rc, msg)
+    assert rc == -5 and "drones_per_env <= 64" in msg and msg.startswith("qs_rollout_mlp: "), (rc, msg)
