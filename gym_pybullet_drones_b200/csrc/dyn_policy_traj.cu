@@ -1,24 +1,15 @@
 // dyn_policy_traj.cu -- qs_dyn_policy_traj / qs_dyn_policy_traj_vjp: differentiable trajectories of an MLP actor driving
 // Physics.DYN through the RPM / ONE_D_RPM decode (include/quadsim.h, DESIGN.md 4.5).  A CTA owns M whole aviaries for all T ticks:
 // their observation rows live in shared memory (the action history is shifted in place), the actor runs as a float64 GEMM chain
-// over the M rows on the FP64 tensor cores (cta_gemm), and
-// one thread per drone runs the decode and the physics.  The backward walks the ticks in reverse: it reloads the tick's
+// over the M rows on the FP64 tensor cores (cta_gemm, policy_actor.cuh), and one thread per drone runs the decode and the physics.  The backward walks the ticks in reverse: it reloads the tick's
 // observation and start state from the forward's outputs, recomputes the hidden activations with the forward's own
 // actor_forward, runs mlp_adjoint.cuh's tick adjoint, collects the action's cotangent (physics + the returned action + what later
 // observations sent back through the history, a ring of B cotangents per drone in shared memory), and pushes it through the
 // transposed actor to the observation's cotangent.
-#include "qs_common.cuh"
-#include "mlp_adjoint.cuh"
-#include "traj_io.cuh"
+#include "policy_actor.cuh"
 
 namespace qsi {
 namespace {
-
-constexpr int kPolTPB = 256;
-constexpr int kPolMG = 8;            // aviaries per CTA come in m-tiles of 8 rows (mma.m8n8k4)
-constexpr int kPolMaxM = 16;         // aviaries per CTA at most
-constexpr int kPolNT = 4;            // n-tiles a warp carries per pass: one A fragment per m-tile feeds kPolNT products
-constexpr size_t kPolSmemMax = 227 * 1024;
 
 struct PolArgs {
     QsParams P;
@@ -28,92 +19,6 @@ struct PolArgs {
     int M;                          // aviaries per CTA, a multiple of kPolMG with M * D <= kPolTPB
     int maxw, cw;                   // widest hidden layer; max(maxw, in_dim): the row stride of the cotangent buffers
 };
-
-// C[r][n] = sum_k X[r][k] Bm(k, n) for the CTA's M rows (X in shared memory, row stride ldx) and n < Nn, with
-// Bm(k, n) = W[k * sk + n * sn] read from global memory: (sk, sn) = (Nout, 1) is a layer, (1, Nout) its transpose.  epi(r, n, c)
-// receives every element once.  Every thread of the CTA calls it; no barrier inside.
-//
-// The product runs on the FP64 tensor cores (mma.sync.aligned.m8n8k4.row.col.f64): lane 4 g + t holds A[g][t], B[t][g] and
-// C[g][2 t], C[g][2 t + 1].  A warp owns kPolNT n-tiles at a time for all M / 8 m-tiles, so each weight is loaded exactly once
-// per CTA and layer (no other warp needs it: staging it through shared memory would add a copy and no reuse) and each A fragment
-// feeds kPolNT products.  Built with -DQS_POLICY_GEMM_FMA the same interface runs mlp_adjoint.cuh's plain FMA loop (what the
-// host build uses), four rows per thread: the A/B partner of DESIGN.md 4.5's measurement, not a run-time option.
-template <class Epi>
-__device__ __forceinline__ void cta_gemm(int M, const double* X, int ldx, const double* W, int sk, int sn, int K, int Nn, Epi epi) {
-#if defined(QS_POLICY_GEMM_FMA)
-    for (int it = threadIdx.x; it < Nn * (M / 4); it += blockDim.x) {
-        const int n = it % Nn, g = it / Nn;
-        double acc[4] = {0.0, 0.0, 0.0, 0.0};
-        for (int k = 0; k < K; ++k) {
-            const double w = W[(long long)k * sk + (long long)n * sn];
-#pragma unroll
-            for (int m = 0; m < 4; ++m) acc[m] = qs::fmad(X[(size_t)(g * 4 + m) * ldx + k], w, acc[m]);
-        }
-#pragma unroll
-        for (int m = 0; m < 4; ++m) epi(g * 4 + m, n, acc[m]);
-    }
-#else
-    const int warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const int MT = M / kPolMG;                                   // 1 or 2
-    for (int nt0 = warp * kPolNT; nt0 * 8 < Nn; nt0 += nwarps * kPolNT) {
-        double c[kPolNT][2][2];
-#pragma unroll
-        for (int j = 0; j < kPolNT; ++j) c[j][0][0] = c[j][0][1] = c[j][1][0] = c[j][1][1] = 0.0;
-        for (int k0 = 0; k0 < K; k0 += 4) {
-            const int kk = k0 + t;
-            const bool kin = kk < K;
-            const double a0 = kin ? X[(size_t)g * ldx + kk] : 0.0;
-            const double a1 = (kin && MT > 1) ? X[(size_t)(8 + g) * ldx + kk] : 0.0;
-            double bfr[kPolNT];
-#pragma unroll
-            for (int j = 0; j < kPolNT; ++j) {
-                const int n = (nt0 + j) * 8 + g;
-                bfr[j] = (kin && n < Nn) ? W[(long long)kk * sk + (long long)n * sn] : 0.0;
-            }
-#pragma unroll
-            for (int j = 0; j < kPolNT; ++j) {
-                asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                             : "+d"(c[j][0][0]), "+d"(c[j][0][1]) : "d"(a0), "d"(bfr[j]));
-                if (MT > 1)
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                                 : "+d"(c[j][1][0]), "+d"(c[j][1][1]) : "d"(a1), "d"(bfr[j]));
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < kPolNT; ++j)
-#pragma unroll
-            for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int n = (nt0 + j) * 8 + 2 * t + h;
-                    if (mt < MT && n < Nn) epi(mt * 8 + g, n, c[j][mt][h]);
-                }
-    }
-#endif
-}
-
-// The actor's hidden layers (and, with `mean`, its output layer) over the CTA's M observation rows.  Layer l's activations go
-// to act + (keep ? l : l & 1) * M * maxw, row stride maxw.  Every thread of the CTA calls it; it ends on a barrier.
-__device__ void actor_forward(const PolArgs& a, const double* obs, double* act, bool keep, double* mean) {
-    const QsDynPolicyTrajIO& io = a.io;
-    const int layers = io.depth + (mean ? 1 : 0);
-    const double* x = obs;
-    int K = io.in_dim, ldx = io.in_dim;
-    for (int l = 0; l < layers; ++l) {
-        const bool last = l == io.depth;
-        const int Nout = last ? io.out_dim : io.width[l];
-        double* dst = last ? mean : act + (size_t)(keep ? l : (l & 1)) * a.M * a.maxw;
-        const int ldd = last ? io.out_dim : a.maxw;
-        const double* bias = io.b[l];
-        const int kind = io.activation;
-        cta_gemm(a.M, x, ldx, io.w[l], Nout, 1, K, Nout, [&](int r, int n, double v) {
-            v = v + bias[n];
-            dst[(size_t)r * ldd + n] = last ? v : qs::mlp_act(kind, v);
-        });
-        __syncthreads();
-        x = dst; K = Nout; ldx = ldd;
-    }
-}
 
 // The transposed actor: gz [M][out_dim] (the cotangent of the mean action) down to the observation's cotangent, which it
 // returns: [M] rows of stride cw in one of the two buffers.  `act` holds every hidden layer (actor_forward, keep).  Ends on a barrier.
@@ -189,18 +94,6 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_kernel(const __grid_c
             for (int j = 0; j < 4; ++j) up[j] = u[j];
         }
     }
-}
-
-// the applied RPMs of tick k, from the saved raw action
-__device__ __forceinline__ void applied_rpm(const PolArgs& a, const qs::PhysRow& c, long long i, int k, double raw_a[4], double aa[4],
-                                            double raw[4], double u[4]) {
-    aa[0] = aa[1] = aa[2] = aa[3] = 0.0;
-    for (int j = 0; j < a.A; ++j) {
-        raw_a[j] = a.io.actions[((long long)k * a.N + i) * a.A + j];
-        aa[j] = qs::clampd(raw_a[j], -1.0, 1.0);
-    }
-    qs::policy_rpm(a.A, c, aa, raw);
-    clip_rpm(raw, c.max_rpm, u);
 }
 
 template <int EFF>
@@ -293,31 +186,12 @@ __global__ void __launch_bounds__(kPolTPB) dyn_policy_traj_vjp_kernel(const __gr
 template <bool VJP>
 int launch_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env, int substeps,
                        unsigned effects, void* stream, const char* what) {
-    if (!p || !io) return fail(QS_ERR_NULL, what, "NULL params / io");
-    if (!io->state0 || !io->action_buffer || !io->log_std || !io->states || !io->actions || !io->obs)
-        return fail(QS_ERR_NULL, what, "NULL state0 / action_buffer / log_std / states / actions / obs");
+    if (int rc = policy_check_inputs(p, io, what)) return rc;
     if (VJP && (!io->g_states || !io->g_raw || !io->g_state0 || !io->scratch))
         return fail(QS_ERR_NULL, what, "NULL g_states / g_raw / g_state0 / scratch");
-    if (int rc = traj_check_sizes(what, n_envs, drones_per_env, substeps, io->T)) return rc;
-    if (act_type != QS_ACT_RPM && act_type != QS_ACT_ONE_D_RPM)
-        return fail(QS_ERR_UNSUPPORTED, what, "only the RPM and ONE_D_RPM actions have an adjoint (PID, VEL and ONE_D_PID run the embedded "
-                                              "controller)");
-    const int A = act_width(act_type), D = drones_per_env;
-    if (io->act_buffer_size <= 0) return fail(QS_ERR_SIZE, what, "act_buffer_size must be > 0");
-    if (io->activation != QS_MLP_TANH && io->activation != QS_MLP_RELU) return fail(QS_ERR_ENUM, what, "bad activation");
-    if (io->depth < 1 || io->depth > QS_MLP_MAX_HIDDEN) return fail(QS_ERR_SIZE, what, "1 to 4 hidden layers");
     int maxw = 0;
-    for (int l = 0; l <= io->depth; ++l) {
-        if (!io->w[l] || !io->b[l]) return fail(QS_ERR_NULL, what, "NULL weight / bias");
-        if (l < io->depth) {
-            if (io->width[l] < 1 || io->width[l] > QS_MLP_MAX_WIDTH) return fail(QS_ERR_SIZE, what, "hidden widths must be 1 .. 256");
-            maxw = io->width[l] > maxw ? io->width[l] : maxw;
-        }
-    }
-    if (D * A > 32 || D > kPolTPB / kPolMG) return fail(QS_ERR_UNSUPPORTED, what, "up to 32 action outputs (D * A) and 32 drones per aviary");
-    if (io->in_dim != D * (12 + io->act_buffer_size * A) || io->out_dim != D * A)
-        return fail(QS_ERR_SIZE, what, "in_dim must be D (12 + B A) and out_dim D A");
-    if (int rc = traj_check_effects(what, effects, io->phys, nullptr)) return rc;
+    if (int rc = policy_check_shape(io, act_type, n_envs, drones_per_env, substeps, effects, nullptr, what, maxw)) return rc;
+    const int A = act_width(act_type), D = drones_per_env;
     PolArgs a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.io = *io;
@@ -328,17 +202,9 @@ int launch_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_t
     // doubles of shared memory per aviary: the observation row, the hidden activations (two buffers forward, every layer
     // backward), the mean action / its cotangent, and backward the two cotangent buffers and the history ring
     // The forward is refused where its VJP would be: a trajectory that cannot be differentiated must not come back with a grad_fn.
-    const size_t per_vjp = (size_t)io->in_dim + (size_t)io->depth * maxw + io->out_dim + 2 * (size_t)a.cw + (size_t)D * io->act_buffer_size * A;
-    const size_t per = VJP ? per_vjp : (size_t)io->in_dim + 2 * (size_t)maxw + io->out_dim;
-    int M = (int)(kPolSmemMax / (per * sizeof(double)));
-    if (kPolSmemMax / (per_vjp * sizeof(double)) < (size_t)kPolMG) M = 0;
-    M = M < kPolTPB / D ? M : kPolTPB / D;
-    M = M < kPolMaxM ? M : kPolMaxM;
-    M -= M % kPolMG;
-    if (M < kPolMG)
-        return fail(QS_ERR_UNSUPPORTED, what, "the observation rows, hidden activations and cotangents of 8 aviaries exceed the 227 KB of "
-                                              "shared memory of a CTA (shorten the action buffer with a lower ctrl_freq, or use fewer drones "
-                                              "per aviary)");
+    const size_t per = VJP ? policy_vjp_doubles(io, D, A, maxw) : (size_t)io->in_dim + 2 * (size_t)maxw + io->out_dim;
+    int M = 0;
+    if (int rc = policy_ctas(io, D, A, maxw, per, what, M)) return rc;
     a.M = M;
     const size_t smem = per * M * sizeof(double);
     const unsigned blocks = (unsigned)((n_envs + M - 1) / M);

@@ -1,7 +1,7 @@
 // mlp_adjoint.cuh -- the per-element math of the differentiable policy trajectories (dyn_policy_traj.cu, DESIGN.md 4.5): the
 // float64 MLP actor and its transpose, the observation head and its adjoint, the RPM / ONE_D_RPM decode and its adjoint, and the
 // tick adjoint that also takes the cotangent of the next observation's ang_v.  Compiled for the sm_90a kernels and for the host
-// harness (tests/host_harness/diff_policy_host.cpp); the kernels' GEMMs run on the tensor cores (dyn_policy_traj.cu, cta_gemm), the
+// harness (tests/host_harness/diff_policy_host.cpp); the kernels' GEMMs run on the tensor cores (policy_actor.cuh, cta_gemm), the
 // host build and the FMA comparison build use mlp_col / mlp_row_t.
 //
 // Which derivative (DESIGN.md 4.5):

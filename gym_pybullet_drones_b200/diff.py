@@ -1,7 +1,8 @@
 """Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs),
 qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop) and qs_dyn_policy_traj / qs_dyn_policy_traj_vjp (an
-MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5), and the forward mode of the raw-RPM trajectories: DynTrajectory.jvp
-(qs_dyn_traj_jvp) and the per-tick Jacobians of linearise (qs_dyn_tick_jac).
+MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5), and their forward mode: the jvp of each Function (qs_dyn_traj_jvp,
+qs_dyn_ctrl_traj_jvp, qs_dyn_policy_traj_jvp) and the per-tick Jacobians of linearise (qs_dyn_tick_jac, qs_dyn_ctrl_tick_jac,
+qs_dyn_policy_tick_jac).
 BaseAviary.differentiable_rollout is the public entry point; this module packs the state into the kernels' planes layout, runs
 the forward and backward kernels and unpacks the result."""
 import ctypes as C
@@ -204,10 +205,31 @@ def actor64(params, activation, obs, noise=None):
     return raw if noise is None else raw + torch.exp(params[-1]) * noise
 
 
-def _policy_io(cfg, T, theta, ptrs):
-    """The QsDynPolicyTrajIO of PolicyTrajectory: the actor's layers from the float64 parameters theta, the tensors of `ptrs`."""
+def actor64_jvp(params, t_params, activation, obs, noise=None, t_noise=None):
+    """The tangent of actor64(params, activation, obs, noise) along t_params (None: zero) and t_noise (None: zero), obs held
+    constant: one batched forward-mode pass written out (forward-mode AD cannot nest inside the jvp of an autograd.Function).
+    ReLU passes the tangent where the unit is positive, as torch.relu's derivative does."""
+    z = lambda t, x: torch.zeros_like(x) if t is None else t
+    h, th = obs, None
+    for k in range(0, len(params) - 3, 2):
+        W, b = params[k], params[k + 1]
+        pre = h @ W + b
+        tz = h @ z(t_params[k], W) + z(t_params[k + 1], b) + (0.0 if th is None else th @ W)
+        h = torch.tanh(pre) if activation == "tanh" else torch.relu(pre)
+        th = tz * (1.0 - h * h) if activation == "tanh" else torch.where(h > 0, tz, torch.zeros_like(tz))
+    W, b = params[-3], params[-2]
+    t_raw = h @ z(t_params[-3], W) + z(t_params[-2], b) + th @ W
+    if noise is not None:
+        scale = torch.exp(params[-1])
+        t_raw = t_raw + scale * (z(t_params[-1], params[-1]) * noise + z(t_noise, noise))
+    return t_raw
+
+
+def _policy_io(cls, cfg, T, theta, ptrs):
+    """The QsDynPolicyTrajIO (or QsDynPolicyTrajJvpIO: `cls`) of PolicyTrajectory: the actor's layers from the float64
+    parameters theta, the tensors of `ptrs`."""
     activation, B = cfg[2], cfg[3]
-    io = _io(N.QsDynPolicyTrajIO, T, dict(ptrs, log_std=theta[-1]), act_buffer_size=B, depth=len(theta) // 2 - 1,
+    io = _io(cls, T, dict(ptrs, log_std=theta[-1]), act_buffer_size=B, depth=len(theta) // 2 - 1,
              activation=N.MLP_TANH if activation == "tanh" else N.MLP_RELU, in_dim=theta[0].shape[0], out_dim=theta[-3].shape[1])
     for l in range(io.depth + 1):
         io.w[l], io.b[l] = theta[2 * l].data_ptr(), theta[2 * l + 1].data_ptr()
@@ -221,8 +243,20 @@ class PolicyTrajectory(torch.autograd.Function):
     action buffer abuf [N, B, A], with last_rpm [N, 4], the per-aviary rows [E, 16], noise [T, E, out] (or None) and the actor's
     float64 parameters `theta` ([W1, b1, ..., Wout, bout, log_std]).  backward = qs_dyn_policy_traj_vjp, which carries the
     sequential dependency and returns g_raw, the cotangent of every raw action; the gradients of theta and noise are then one
-    batched autograd pass of the actor over the T * E saved observation rows (deterministic, any architecture).  obs is not
-    differentiable.  `cfg` = (QsParams, act_type, activation, B, E, D, A, substeps, effects, T)."""
+    batched autograd pass of the actor over the T * E saved observation rows (deterministic, any architecture).  jvp
+    (torch.autograd.forward_ad) = one batched forward-mode pass of the actor over the same rows for the tangent that theta and
+    the noise add to each raw action (actor64_jvp), then qs_dyn_policy_traj_jvp.  obs is not differentiable.  `cfg` = (QsParams, act_type,
+    activation, B, E, D, A, substeps, effects, T).  Double backward and tangents that require grad raise ValueError."""
+
+    @staticmethod
+    def _saved(ctx):
+        """({state0, last_rpm, phys, action_buffer, noise (or None)}, {states, actions, obs}, theta) of the forward"""
+        saved = list(ctx.saved_tensors)
+        keys = ["state0", "last_rpm", "phys", "action_buffer"] + (["noise"] if ctx.has_noise else [])
+        ins = dict(zip(keys, saved[:len(keys)]))
+        ins.setdefault("noise", None)
+        outs = dict(zip(("states", "actions", "obs"), saved[len(keys):len(keys) + 3]))
+        return ins, outs, saved[len(keys) + 3:]
 
     @staticmethod
     def forward(ctx, planes0, last_rpm, rows, abuf, noise, cfg, *theta):
@@ -234,22 +268,47 @@ class PolicyTrajectory(torch.autograd.Function):
         f64 = dict(dtype=torch.float64, device=planes0.device)
         outs = dict(states=torch.empty((T, 13 * n), **f64), actions=torch.empty((T, n, A), **f64),
                     obs=torch.empty((T, E, theta[0].shape[0]), **f64))
-        io = _policy_io(cfg, T, theta, dict(ins, **outs))
+        io = _policy_io(N.QsDynPolicyTrajIO, cfg, T, theta, dict(ins, **outs))
         _call("qs_dyn_policy_traj", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=planes0.device)
         ctx.save_for_backward(*(x for x in ins.values() if x is not None), *outs.values(), *theta)
+        ctx.save_for_forward(*(x for x in ins.values() if x is not None), *outs.values(), *theta)
         ctx.cfg, ctx.has_noise = cfg, noise is not None
         ctx.mark_non_differentiable(outs["obs"])
         return outs["states"], outs["actions"], outs["obs"]
 
     @staticmethod
+    def jvp(ctx, t_planes0, t_last_rpm, t_rows, t_abuf, t_noise, _t_cfg, *t_theta):
+        """Forward mode: the tangents (t_states [T, 13 N], t_actions [T, N, A]) along the inputs' tangents; obs has none.  The
+        tangent theta and the noise add to raw action k, t_raw_in = J_theta t_theta + exp(log_std) (t_log_std noise + t_noise),
+        is one batched forward-mode pass of the actor over the saved observations (actor64_jvp); qs_dyn_policy_traj_jvp carries
+        the rest, linearising each tick at the forward's stored states.  A tangent that requires grad raises ValueError."""
+        tangents = (t_planes0, t_last_rpm, t_rows, t_abuf, t_noise) + tuple(t_theta)
+        if any(t is not None and t.requires_grad for t in tangents):
+            raise ValueError("differentiable_rollout: a tangent that requires grad (reverse mode over forward mode) is not supported: "
+                             "the JVP kernel has no derivative of its own")
+        ins, outs, theta = PolicyTrajectory._saved(ctx)
+        cfg = ctx.cfg
+        P, act_type, activation, B, E, D, A, S, eff, T = cfg
+        n = E * D
+        f64 = lambda t: None if t is None else t.to(torch.float64).contiguous()
+        t_raw_in = None
+        t_eps = f64(t_noise) if ctx.has_noise else None
+        if t_eps is not None or any(t is not None for t in t_theta):
+            t_raw_in = actor64_jvp(theta, [f64(t) for t in t_theta], activation, outs["obs"], ins["noise"], t_eps).reshape(T, n, A).contiguous()
+        t_phys = f64(t_rows)
+        if t_phys is not None and t_phys.data_ptr() % 16:          # the kernel reads t_phys rows as 16-byte pairs
+            t_phys = t_phys.clone()
+        t_states, t_actions = torch.empty_like(outs["states"]), torch.empty_like(outs["actions"])
+        ptrs = dict(ins, **outs, t_state0=f64(t_planes0), t_last_rpm=f64(t_last_rpm), t_phys=t_phys, t_action_buffer=f64(t_abuf),
+                    t_raw_in=t_raw_in, t_states=t_states, t_actions=t_actions)
+        io = _policy_io(N.QsDynPolicyTrajJvpIO, cfg, T, theta, ptrs)
+        _call("qs_dyn_policy_traj_jvp", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=t_states.device)
+        return t_states, t_actions, None
+
+    @staticmethod
     def backward(ctx, g_states, g_actions, _g_obs):
         _no_double_backward()
-        saved = list(ctx.saved_tensors)
-        keys = ["state0", "last_rpm", "phys", "action_buffer"] + (["noise"] if ctx.has_noise else [])
-        ins = dict(zip(keys, saved[:len(keys)]))
-        ins.setdefault("noise", None)
-        outs = dict(zip(("states", "actions", "obs"), saved[len(keys):len(keys) + 3]))
-        theta = saved[len(keys) + 3:]
+        ins, outs, theta = PolicyTrajectory._saved(ctx)
         cfg = ctx.cfg
         P, act_type, activation, B, E, D, A, S, eff, T = cfg
         n = E * D
@@ -258,7 +317,7 @@ class PolicyTrajectory(torch.autograd.Function):
                      g_phys=torch.empty((n, 16), **f64), g_action_buffer=torch.empty((n, B, A), **f64))
         outs.update(g_states=g_states.to(torch.float64).contiguous(), g_actions=g_actions.to(torch.float64).contiguous(),
                     scratch=torch.empty((S, 13, n), **f64))
-        io = _policy_io(cfg, T, theta, dict(ins, **outs, **grads))
+        io = _policy_io(N.QsDynPolicyTrajIO, cfg, T, theta, dict(ins, **outs, **grads))
         _call("qs_dyn_policy_traj_vjp", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=outs["states"].device)
         # the parameters' (and the noise's) gradients: raw[k, e] = actor(obs[k, e]) + exp(log_std) noise[k, e] with cotangent g_raw
         g_raw = grads["g_raw"].view(T, E, D * A)
@@ -471,18 +530,20 @@ def _closed_loop(env, controller, state, last_rpm, phys, **schedule):
     return out
 
 
-def _policy_loop(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys):
+def _policy_inputs(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys, caller):
+    """The checked arguments of a policy-loop call (differentiable_rollout(policy=) or linearise(policy=), named by `caller`):
+    (cfg, inputs, theta), inputs = (planes0, last_rpm, rows, action_buffer, noise) as PolicyTrajectory takes them."""
     from .policy import MlpPolicy
     E, D, n, dev = env._E, env._D, env._N, env.device
     if not isinstance(policy, MlpPolicy):
         raise ValueError("policy must be an MlpPolicy, got %s" % type(policy).__name__)
     act_type = env._act_type()
     if act_type not in (N.ACT_RPM, N.ACT_ONE_D_RPM):
-        raise ValueError("differentiable_rollout(policy=) supports ActionType.RPM and ONE_D_RPM: PID, VEL and ONE_D_PID run the embedded "
-                         "DSLPID controller inside the policy loop, which has no adjoint yet")
+        raise ValueError("%s supports ActionType.RPM and ONE_D_RPM: PID, VEL and ONE_D_PID run the embedded "
+                         "DSLPID controller inside the policy loop, which has no adjoint yet" % caller)
     A, B, od = env._A, env._B, env._obs_dim
     if B == 0:
-        raise ValueError("differentiable_rollout(policy=) needs an action buffer: ctrl_freq=%d gives ACTION_BUFFER_SIZE = 0" % env.CTRL_FREQ)
+        raise ValueError("%s needs an action buffer: ctrl_freq=%d gives ACTION_BUFFER_SIZE = 0" % (caller, env.CTRL_FREQ))
     if policy.in_dim != D * od or policy.out_dim != D * A:
         raise ValueError("policy must map %d inputs to %d outputs, not %d to %d" % (D * od, D * A, policy.in_dim, policy.out_dim))
     if torch.device(policy.device) != dev:
@@ -513,13 +574,26 @@ def _policy_loop(env, policy, params, noise, action_buffer, num_steps, state, la
     else:
         action_buffer = _tensor(action_buffer, "action_buffer", (E, D, B, A), dev).reshape(n, B, A)
     planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
-    with torch.cuda.device(dev):
-        cfg = (env._P, act_type, policy.activation, B, E, D, A, env.PYB_STEPS_PER_CTRL, env._effects, T)
-        states, actions, obs = PolicyTrajectory.apply(planes0, last_rpm, rows, action_buffer, noise, cfg, *theta)
+    cfg = (env._P, act_type, policy.activation, B, E, D, A, env.PYB_STEPS_PER_CTRL, env._effects, T)
+    return cfg, (planes0, last_rpm, rows, action_buffer, noise), theta
+
+
+def _policy_out(env, cfg, states, actions, obs):
+    """{pos, quat, vel, rpy_rates, actions, obs} of a policy loop as differentiable_rollout(policy=) returns them"""
+    E, D, n = env._E, env._D, env._N
+    T, A, od = cfg[9], cfg[6], env._obs_dim
     out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
     out["actions"] = actions.reshape(T, E, D, A)
     out["obs"] = obs.reshape(T, E, D, od)
     return out
+
+
+def _policy_loop(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys):
+    cfg, ins, theta = _policy_inputs(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys,
+                                     "differentiable_rollout(policy=)")
+    with torch.cuda.device(env.device):
+        states, actions, obs = PolicyTrajectory.apply(*ins, cfg, *theta)
+    return _policy_out(env, cfg, states, actions, obs)
 
 
 def tick_jacobians(cfg, rpm, planes0, last_rpm, rows):
@@ -561,9 +635,52 @@ def _linearise_closed_loop(env, controller, state, last_rpm, phys, **schedule):
     return out
 
 
-def linearise(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, **schedule):
+def policy_tick_jacobians(cfg, ins, theta):
+    """({states, actions, obs} of qs_dyn_policy_traj, jac [T, E, R, R]) of qs_dyn_policy_tick_jac from the dense inputs `ins`
+    (planes0, last_rpm, rows, action_buffer, noise) and the float64 parameters theta; `cfg` as PolicyTrajectory's, R = n_z + D A
+    (include/quadsim.h)."""
+    P, act_type, activation, B, E, D, A, S, eff, T = cfg
+    planes0 = ins[0]
+    n, dev = E * D, planes0.device
+    f64 = dict(dtype=torch.float64, device=dev)
+    outs = dict(states=torch.empty((T, 13 * n), **f64), actions=torch.empty((T, n, A), **f64), obs=torch.empty((T, E, theta[0].shape[0]), **f64))
+    ptrs = dict(zip(("state0", "last_rpm", "phys", "action_buffer", "noise"), ins), **outs)
+    io = _policy_io(N.QsDynPolicyTrajIO, cfg, T, theta, ptrs)
+    _call("qs_dyn_policy_traj", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=dev)
+    R = D * (16 + B * A + (4 if eff & N.EFFECT_DRAG else 0)) + D * A
+    jac = torch.empty((T, E, R, R), **f64)
+    io = _policy_io(N.QsDynPolicyTrajJvpIO, cfg, T, theta, dict(ptrs, jac=jac))
+    _call("qs_dyn_policy_tick_jac", C.byref(P), C.byref(io), act_type, E, D, S, eff, device=dev)
+    return outs, jac
+
+
+def _linearise_policy(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys):
+    with torch.no_grad():
+        cfg, ins, theta = _policy_inputs(env, policy, params, noise, action_buffer, num_steps, state, last_rpm, phys, "linearise(policy=)")
+        dense = lambda x: None if x is None else x.detach().contiguous()
+        with torch.cuda.device(env.device):
+            outs, jac = policy_tick_jacobians(cfg, [dense(x) for x in ins], [dense(t) for t in theta])
+    out = _policy_out(env, cfg, outs["states"], outs["actions"], outs["obs"])
+    nz = jac.shape[-1] - env._D * env._A
+    out["A"], out["B"], out["K"] = jac[..., :nz, :nz], jac[..., :nz, nz:], jac[..., nz:, :nz]
+    return out
+
+
+def linearise(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
+              action_buffer=None, **schedule):
     """BaseAviary.linearise (see there)."""
     _refuse_downwash(env, "linearise()", "tangent")
+    if policy is not None:
+        if rpm is not None or controller is not None:
+            raise ValueError("linearise() takes exactly one of rpm [T, E, D, 4] (open loop), controller= (closed loop) or policy= (an "
+                             "MlpPolicy in the loop)")
+        given = sorted(k for k, v in schedule.items() if v is not None and k != "num_steps")
+        if given:
+            raise ValueError("%s apply to a controller linearisation only" % ", ".join(given))
+        return _linearise_policy(env, policy, params, noise, action_buffer, schedule.get("num_steps"), state, last_rpm, phys)
+    given = sorted(k for k, v in (("params", params), ("noise", noise), ("action_buffer", action_buffer)) if v is not None)
+    if given:
+        raise ValueError("%s apply to a policy linearisation only" % ", ".join(given))
     if (rpm is not None) + (controller is not None) != 1:
         raise ValueError("linearise() takes exactly one of rpm [T, E, D, 4] (open loop) or controller= (closed loop)")
     if controller is not None:

@@ -618,7 +618,11 @@ class BaseAviary(Env):
         which evaluates the actor at float32 accuracy on the tensor cores and decodes float32 actions: the two agree to
         float32 level over short horizons (tests/test_gpu_diff_policy.py holds the bound).  No reward, flags or autoreset.
         PID / VEL / ONE_D_PID actions, a policy of the wrong size or device, ctrl_freq with an empty action buffer and an
-        observation too wide for a CTA's shared memory raise ValueError."""
+        observation too wide for a CTA's shared memory raise ValueError.  Forward mode: dual tensors (torch.autograd.forward_ad)
+        on any tensor of params, state, last_rpm, phys, action_buffer and noise give the tangents of the four state entries and
+        `actions` (one batched forward-mode actor pass over the saved observations for the parameters' and the noise's part,
+        then one JVP kernel launch with the same decisions; the primal outputs keep their bits; `obs` has no tangent).
+        linearise(policy=) gives the per-tick Jacobians of the policy loop."""
         from ..diff import differentiable_rollout
         return differentiable_rollout(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, policy=policy,
                                       params=params, noise=noise, action_buffer=action_buffer, waypoints=waypoints,
@@ -628,12 +632,13 @@ class BaseAviary(Env):
 
     def linearise(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None, target_vel=None,
                   target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None, pid_state=None, state=None,
-                  last_rpm=None, phys=None):
+                  last_rpm=None, phys=None, policy=None, params=None, noise=None, action_buffer=None):
         """The per-tick Jacobians of every drone along the raw-RPM trajectory of differentiable_rollout(rpm, state=,
-        last_rpm=, phys=), or along its closed loop differentiable_rollout(controller=, ...), in one kernel launch after the
-        forward (DESIGN.md 4.5): what LQR, iLQR / DDP, EKF-style estimators and stability analysis linearise at.  Pass exactly
-        one of `rpm` or `controller`.  Arguments, checks and defaults are differentiable_rollout's; the result is not
-        differentiable, and neither the env nor the controller is touched.
+        last_rpm=, phys=), along its closed loop differentiable_rollout(controller=, ...), or of every aviary along its policy
+        loop differentiable_rollout(policy=, ...), in one kernel launch after the forward (DESIGN.md 4.5): what LQR, iLQR / DDP,
+        EKF-style estimators and stability analysis linearise at.  Pass exactly one of `rpm`, `controller` or `policy`.
+        Arguments, checks and defaults are differentiable_rollout's; the result is not differentiable, and neither the env nor
+        the controller or policy is touched.
 
         Open loop (rpm): returns {pos, quat, vel, rpy_rates} of the nominal trajectory ([T, E, D, k], entry k the state after
         tick k, the same bits as differentiable_rollout) and, for tick k,
@@ -660,10 +665,29 @@ class BaseAviary(Env):
         The controller reads the stored, unnormalised quaternion (Bullet's matrix and Euler angles divide by |q|^2 or not at
         all), so unlike the open loop the closed-loop A has no quaternion null space.  The derivative decisions are
         differentiable_rollout(controller=)'s, so the Jacobians are exactly the transposes of its backward's.  All four are
-        views of one [T, E, D, 26, n_z + 3] tensor whose rows are x_{k+1}, s_{k+1}, u_k.  Downwash, an MRAC, both rpm and a
-        controller or neither, and bad inputs raise ValueError."""
+        views of one [T, E, D, 26, n_z + 3] tensor whose rows are x_{k+1}, s_{k+1}, u_k.
+
+        Policy loop (policy, with differentiable_rollout's params, noise, num_steps and action_buffer): the actor couples the
+        drones of an aviary, so the Jacobians are per aviary.  The loop state z_k is drone-major; per drone it is pos (3), quat
+        x y z w (4), vel (3), rpy_rates (3), the observation's ang_v (3: R_last w, the body rates seen through the attitude at
+        the start of the previous tick's last substep, which is neither an input nor an output of the rollout), the B buffered
+        clipped actions (B A, oldest first) and, with drag, the applied RPMs of the previous tick (4): n_z = D (16 + B A), or
+        D (20 + B A) with drag.  Returns the nominal trajectory (the four state entries, `actions` and `obs`, the bits of
+        differentiable_rollout(policy=)) and, for tick k,
+          A [T, E, n_z, n_z]    d z_{k+1} / d z_k,
+          B [T, E, n_z, D A]    d z_{k+1} / d delta_k, delta_k an additive perturbation of the raw action raw_k (the noise's
+                                direction is delta's times exp(log_std)),
+          K [T, E, D A, n_z]    d raw_k / d z_k, the policy's local gain (d raw_k / d delta_k is the identity).
+        All three are views of one [T, E, n_z + D A, n_z + D A] tensor whose rows are z_{k+1}, raw_k.  Indices are drone ids,
+        also after reorder_by_morton().  The derivative decisions are differentiable_rollout(policy=)'s (the action clip as
+        torch.clamp, ReLU where the unit is positive, the Euler angles on the forward's side of the gimbal guard), so the
+        Jacobians are exactly the transposes of its backward's.  For tick 0, ang_v is R(q0 / |q0|) w0 of the initial state.
+
+        Downwash, an MRAC, not exactly one of rpm, controller and policy, arguments of another loop, and bad inputs raise
+        ValueError."""
         from ..diff import linearise
-        return linearise(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, waypoints=waypoints,
+        return linearise(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, policy=policy, params=params,
+                         noise=noise, action_buffer=action_buffer, waypoints=waypoints,
                          start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
                          target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps, gains=gains,
                          pid_state=pid_state)

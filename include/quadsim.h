@@ -805,6 +805,55 @@ int qs_dyn_policy_traj(const QsParams* p, const QsDynPolicyTrajIO* io, int act_t
 int qs_dyn_policy_traj_vjp(const QsParams* p, const QsDynPolicyTrajIO* io, int act_type, int n_envs, int drones_per_env,
                            int substeps, unsigned effects, void* stream);
 
+/* Forward mode of the policy trajectories of qs_dyn_policy_traj (DESIGN.md 4.5): the tangents of the T states and raw actions
+ * along given tangents of the inputs (JVP), and the dense Jacobians of every tick of every aviary.  Both read the forward's
+ * states, actions and obs and restart tick k from the stored state k-1 (state0 for k = 0), the saved observation obs[k] and the
+ * stored raw actions, so the loop is linearised at the forward's bits, and both take the derivative decisions of
+ * qs_dyn_policy_traj_vjp (they are its exact transpose).  The actor's parameters and the noise enter through t_raw_in, the tangent
+ * they add to each raw action (J_theta t_theta + exp(log_std) (t_log_std noise + t_noise), formed by the caller over the saved
+ * observations).  The fields up to obs are QsDynPolicyTrajIO's.  All indices are 64-bit.
+ *
+ * The loop state z_k of an aviary is drone-major; per drone: pos (3), quat x y z w (4), vel (3), rpy_rates (3), the observation's
+ * ang_v (3: R_last w, which is neither an input nor an output of the trajectory), the B buffered clipped actions (B A, oldest
+ * first) and with QS_EFFECT_DRAG the applied RPMs of the previous tick (4): n_z = D (16 + B A), or D (20 + B A) with drag. */
+typedef struct QsDynPolicyTrajJvpIO {
+    int T;                          /* ticks, > 0 */
+    int act_buffer_size;            /* B > 0 */
+    int activation;                 /* QS_MLP_TANH or QS_MLP_RELU */
+    int depth;                      /* hidden layers, 1 .. QS_MLP_MAX_HIDDEN */
+    int width[QS_MLP_MAX_HIDDEN];   /* hidden widths, 1 .. QS_MLP_MAX_WIDTH (unpadded) */
+    int in_dim, out_dim;            /* D (12 + B A) and D A <= 32 */
+    const double* w[QS_MLP_MAX_HIDDEN + 1];   /* [in][out] row-major per layer */
+    const double* b[QS_MLP_MAX_HIDDEN + 1];   /* [out] */
+    const double* log_std;          /* [out_dim] */
+    const double* noise;            /* [T][n_envs][out_dim], nullable */
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* last_rpm;         /* [N][4] (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16]; nullable = the constants of QsParams */
+    const double* action_buffer;    /* [N][B][A] */
+    const double* states;           /* [T][13 N] qs_dyn_policy_traj's states for these inputs */
+    const double* actions;          /* [T][N][A] qs_dyn_policy_traj's raw actions */
+    const double* obs;              /* [T][n_envs][in_dim] qs_dyn_policy_traj's observations */
+    /* qs_dyn_policy_traj_jvp: tangents of the inputs, each nullable = zero */
+    const double* t_state0;         /* [13 N] */
+    const double* t_last_rpm;       /* [N][4] */
+    const double* t_phys;           /* [n_envs][16], 16-byte aligned (HOVER_RPM enters through the decode, MAX_RPM the clip) */
+    const double* t_action_buffer;  /* [N][B][A] */
+    const double* t_raw_in;         /* [T][N][A] the tangent the actor's parameters and the noise add to raw action k */
+    double* t_states;               /* qs_dyn_policy_traj_jvp out: [T][13 N] the tangents of the states */
+    double* t_actions;              /* qs_dyn_policy_traj_jvp out: [T][N][A] the tangents of the raw actions */
+    /* qs_dyn_policy_tick_jac out: [T][n_envs][R][R], R = n_z + D A.  Rows: z_{k+1}, then raw_k (D A, drone-major).  Columns: z_k,
+     * then delta_k, an additive perturbation of raw_k (the noise's columns are delta's times exp(log_std)); the raw_k x delta_k
+     * block is the identity.  The tangents are NULL here. */
+    double* jac;
+} QsDynPolicyTrajJvpIO;
+int qs_sizeof_dyn_policy_traj_jvp_io(void);
+/* refusals as qs_dyn_policy_traj, and NULL outputs, t_phys not 16-byte aligned, QS_ERR_SIZE when the grid exceeds 2^31-1 CTAs */
+int qs_dyn_policy_traj_jvp(const QsParams* p, const QsDynPolicyTrajJvpIO* io, int act_type, int n_envs, int drones_per_env,
+                           int substeps, unsigned effects, void* stream);
+int qs_dyn_policy_tick_jac(const QsParams* p, const QsDynPolicyTrajJvpIO* io, int act_type, int n_envs, int drones_per_env,
+                           int substeps, unsigned effects, void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
