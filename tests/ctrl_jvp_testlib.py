@@ -70,11 +70,12 @@ def vjp_ctrl_tick_jac(P, CP, effects, S, dt, rows, gains, state, pid, tg, up):
     return {blk: np.stack([x[blk] for x in per_row], axis=1) for blk, _ in BLOCKS}
 
 
-def ref_ctrl_tick_jac(P, CP, effects, S, dt, rows, gains, state, pid, tg, up, flip=()):
-    """{block: [n, 26, width]}: torch.func.jacfwd of diff_pid_ref.pid + diff_ref.tick, the diagonal (per-drone) blocks.  flip:
-    diff_pid_ref's decisions to turn the other way (the negative controls)."""
-    K, Cc = R.model_constants(P), PR.controller_constants(CP)
-    t = lambda v: torch.tensor(np.asarray(v, dtype=np.float64))
+def ref_ctrl_tick_jac(P, CP, effects, S, dt, rows, gains, state, pid, tg, up, flip=(), device=None):
+    """{block: [n, 26, width]}: torch.func.jacfwd of diff_pid_ref.pid + diff_ref.tick, the diagonal (per-drone) blocks, as NumPy
+    arrays; evaluated on `device` (the inputs may be arrays or tensors).  flip: diff_pid_ref's decisions to turn the other way
+    (the negative controls)."""
+    K, Cc = R.model_constants(P, device), PR.controller_constants(CP, device)
+    t = lambda v: torch.as_tensor(v, dtype=torch.float64, device=device)
     args = tuple(t(v) for v in (state, pid, tg, up, rows, gains))
 
     def f(x, st, tgt, u_prev, rw, gn):
@@ -83,4 +84,4 @@ def ref_ctrl_tick_jac(P, CP, effects, S, dt, rows, gains, state, pid, tg, up, fl
         return torch.cat([out, st1, u], dim=1)
 
     J = torch.func.jacfwd(f, argnums=tuple(range(6)))(*args)
-    return {blk: torch.diagonal(j, dim1=0, dim2=2).permute(2, 0, 1).numpy() for (blk, _), j in zip(BLOCKS, J)}
+    return {blk: torch.diagonal(j, dim1=0, dim2=2).permute(2, 0, 1).cpu().numpy() for (blk, _), j in zip(BLOCKS, J)}

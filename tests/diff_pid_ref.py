@@ -63,9 +63,11 @@ def quat_to_euler(q, branch_free=False):
     return torch.stack([roll, pitch, yaw], dim=1)
 
 
-def pid(Cc, gains, st, dt, x, tp, tyaw, tv, trr, flip=()):
+def pid(Cc, gains, st, dt, x, tp, tyaw, tv, trr, flip=(), probe=None):
     """One computeControl for B drones: x [B, 13] (pos, quat, vel, rates), st [B, 9], targets tp / tv / trr [B, 3] and tyaw [B],
-    gains [B, 18] -> (raw rpm [B, 4], the updated state [B, 9], pos_e [B, 3], yaw_e [B])."""
+    gains [B, 18] -> (raw rpm [B, 4], the updated state [B, 9], pos_e [B, 3], yaw_e [B]).  probe: a dict that receives the inputs
+    of the decisions (scalar [B], sarg [B], the torques and PWMs before their clips [B, 3] / [B, 4]), for tests that show a
+    decision is taken."""
     pos, q, vel = x[:, 0:3], x[:, 3:7], x[:, 7:10]
     Kp, Ki, Kd, Tp, Ti, Td = (gains[:, 3 * j:3 * j + 3] for j in range(6))
     Rm = quat_to_matrix(q)
@@ -98,6 +100,9 @@ def pid(Cc, gains, st, dt, x, tp, tyaw, tv, trr, flip=()):
     tq = _clip(-Tp * re + Td * rr + Ti * ir, -3200.0, 3200.0, "torque" in flip)
     pwm = _clip(thrust[:, None] + tq @ Cc["mixer"].T, Cc["min_pwm"], Cc["max_pwm"], "pwm" in flip)
     rpm = Cc["scale"] * pwm + Cc["const"]
+    if probe is not None:
+        probe.update(scalar=scalar, sarg=-2.0 * (q[:, 0] * q[:, 2] - q[:, 3] * q[:, 1]), torque=-Tp * re + Td * rr + Ti * ir,
+                     pwm=thrust[:, None] + tq @ Cc["mixer"].T)
     ec = torch.atan2(-Rd[:, 0, 1], Rd[:, 0, 0])
     return rpm, torch.cat([ip, rpy, ir], dim=1), e, ec - rpy[:, 2]
 

@@ -96,6 +96,16 @@ def per_drone_relerr(got, want):
     return np.where(n > 0, d / np.where(n > 0, n, 1.0), np.where(np.any(got != 0, axis=1), np.inf, 0.0))
 
 
+def batched_jvp(f, primals, directions):
+    """torch.func.jvp of f({key: tensor}) -> {key: tensor} at `primals` along each of `directions` ({key: tangent}; a missing key
+    carries none), in one pass batched with torch.func.vmap: {key: [len(directions), ...]}"""
+    import torch
+    keys = list(primals)
+    stacked = tuple(torch.stack([d[k] if k in d else torch.zeros_like(primals[k]) for d in directions]) for k in keys)
+    g = lambda *xs: f(dict(zip(keys, xs)))
+    return torch.func.vmap(lambda *v: torch.func.jvp(g, tuple(primals[k] for k in keys), v)[1])(*stacked)
+
+
 BLOCKS = ("rpm", "pos", "quat", "vel", "rpy_rates", "last_rpm", "row")
 
 

@@ -105,13 +105,39 @@ def ref_tick(P, effects, S, activation, theta, noise, flip=(), device=None):
     return f
 
 
-def ref_tick_jac(P, effects, S, activation, theta, noise, x, flip=()):
-    """{block: [rows, width]}: torch.func.jacfwd of ref_tick"""
+def ref_tick_jac(P, effects, S, activation, theta, noise, x, flip=(), device=None):
+    """{block: [rows, width]}: torch.func.jacfwd of ref_tick on `device` (x's entries may be arrays or tensors), as NumPy arrays"""
     D = x["state"].shape[0]
-    args = tuple(torch.as_tensor(_arr(x[k])) for k in ("state", "ang", "hist", "up", "row")) + (torch.zeros(D * x["hist"].shape[2],
-                                                                                                         dtype=torch.float64),)
-    J = torch.func.jacfwd(ref_tick(P, effects, S, activation, theta, noise, flip), argnums=tuple(range(6)))(*args)
-    return {blk: j.reshape(j.shape[0], -1).numpy() for blk, j in zip(BLOCKS, J)}
+    t = lambda v: torch.as_tensor(v, dtype=torch.float64, device=device)
+    args = tuple(t(x[k]) for k in ("state", "ang", "hist", "up", "row")) + (torch.zeros(D * x["hist"].shape[2], dtype=torch.float64,
+                                                                                        device=device),)
+    J = torch.func.jacfwd(ref_tick(P, effects, S, activation, theta, noise, flip, device), argnums=tuple(range(6)))(*args)
+    return {blk: j.reshape(j.shape[0], -1).cpu().numpy() for blk, j in zip(BLOCKS, J)}
+
+
+def kernel_layout(D, A, B, drag):
+    """Where linearise(policy=)'s [R, R] tick Jacobian of one aviary sits in ref_tick_jac's blocks: (rows, cols, groups) with
+    rows [R] the reference row of each kernel row, cols [R] the column of each kernel column in the reference blocks laid side by
+    side in BLOCKS order, and groups {block: kernel columns} (state, ang, hist, up with drag, delta = raw_in).  The loop state is
+    drone-major in the kernel (quadsim.h: pos, quat, vel, rpy_rates, ang_v, history, drag's previous rpm per drone) and
+    block-major in the reference."""
+    iw, ow = widths(D, A, B)
+    BA, nzd = B * A, 16 + B * A + (4 if drag else 0)
+    z = []
+    for d in range(D):
+        z += [13 * d + j for j in range(13)] + [13 * D + 3 * d + j for j in range(3)]
+        z += [16 * D + d * BA + j for j in range(BA)] + ([16 * D + D * BA + 4 * d + j for j in range(4)] if drag else [])
+    raw_row = ow["state"] + ow["ang"] + ow["hist"] + ow["u"]
+    raw_col = iw["state"] + iw["ang"] + iw["hist"] + iw["up"] + iw["row"]
+    rows = np.array(z + [raw_row + i for i in range(D * A)])
+    cols = np.array(z + [raw_col + i for i in range(D * A)])
+    entry = np.array([j for d in range(D) for j in range(nzd)])
+    groups = dict(state=np.flatnonzero(entry < 13), ang=np.flatnonzero((entry >= 13) & (entry < 16)),
+                  hist=np.flatnonzero((entry >= 16) & (entry < 16 + BA)))
+    if drag:
+        groups["up"] = np.flatnonzero(entry >= 16 + BA)
+    groups["delta"] = np.arange(D * nzd, D * nzd + D * A)
+    return rows, cols, groups
 
 
 def vjp_tick_jac(P, effects, S, activation, theta, noise, x, ql):

@@ -85,7 +85,7 @@ def _edge(c, bound):
 
 def _lattice(model, rng):
     """Drones one ulp below, at and above the controller's decisions: the integral clips (x at +-2, z at +-0.15, roll at +-1),
-    the thrust scalar at 0 and the gimbal guard at +-0.99999.  (P, CP, rows, gains, state, pid, targets, up, label); CP has a
+    the thrust scalar at 0 (the last e_z below 0, the first at or above, the first above) and the gimbal guard at +-0.99999.  (P, CP, rows, gains, state, pid, targets, up, label); CP has a
     MIN_PWM low enough that the thrust is not saturated at scalar = 0."""
     P, CP, rows, gains, state, pid, tg, up = _case(model, "flight", rng, copy.copy(_ctrl_params(model)))
     CP.pid_min_pwm = -1e5
@@ -128,8 +128,10 @@ def _lattice(model, rng):
             break
         ez = _ulps(ez, -1)
     b[2][:, 2] = 0.0                        # e_z = target_z - 0 exactly
-    for j, k in enumerate((-1, 0, 1)):
-        b[4][j, 2] = _ulps(ez, k)
+    live = _ulps(ez, 1)
+    while kp * live + g <= 0:               # kp e_z + g can round to 0 at more than one e_z: the first drone with scalar > 0
+        live = _ulps(live, 1)
+    b[4][:, 2] = [_ulps(ez, -1), ez, live]
     add(b, "scalar")
     # the gimbal guard: sarg = -2 (x z - w y) at 0.99999, one ulp either side (w moved)
     b = take(range(3))
