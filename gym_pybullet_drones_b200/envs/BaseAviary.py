@@ -692,6 +692,40 @@ class BaseAviary(Env):
                          target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps, gains=gains,
                          pid_state=pid_state)
 
+    def ilqr(self, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None, last_rpm=None,
+             phys=None):
+        """Optimal raw-RPM trajectories of every drone by iLQR (Gauss-Newton DDP) on the device, one independent problem per
+        drone, solved in lockstep with its own regularisation, step size and convergence flag (DESIGN.md 4.5.1).  Drone i
+        minimises
+            J = 1/2 sum_k (x_k - r_k)' W_k (x_k - r_k) + 1/2 sum_k (u_k - u_ref)' diag(R / HOVER_RPM^2) (u_k - u_ref)
+        over its raw commands u_k = rpm[k], where x_k is the state after tick k (entry k of differentiable_rollout), r_k the
+        target of tick k, W_k = diag(Q) for k < T - 1 and diag(Q_final) for the last tick, and HOVER_RPM the aviary's.  The clip
+        to [0, MAX_RPM] stays inside the dynamics, as in linearise(rpm).  The state cost is taken on the stored components (pos,
+        quat x y z w, vel, rpy_rates), the quaternion as a 4-vector.
+
+        target: {"pos": [3], [E, D, 3] or [T, E, D, 3]} and optionally "quat", "vel", "rpy_rates" in the same shapes (default
+        hover: the identity quaternion, zero velocity and rates).  T comes from num_steps, the target's time axis or rpm, which
+        must agree where given.  rpm: the initial guess [T, E, D, 4] (default each aviary's HOVER_RPM).  Q, Q_final: 13 diagonal
+        weights, [13] or [E, 13] (default Q = 1 on pos and quat, 0.1 on vel, 0.01 on rpy_rates; Q_final = 100 Q).  R: 4
+        diagonal weights on the command relative to HOVER_RPM, [4] or [E, 4] (default 1e-2).  rpm_ref: [4] or [E, D, 4] (default
+        each aviary's HOVER_RPM).  iters: iterations (>= 0).  state, last_rpm and phys as in differentiable_rollout.  The
+        weights are checked once (one synchronisation); nothing in the iterations synchronises with the host.
+
+        Returns (indices are drone ids, also after reorder_by_morton()):
+          pos, quat, vel, rpy_rates [T, E, D, k]  the final nominal trajectory, bit for bit differentiable_rollout(rpm=rpm)
+          rpm        [T, E, D, 4]
+          K          [T, E, D, 4, n_z], k [T, E, D, 4]  the feedback and feed-forward gains of a backward pass at the returned
+                     trajectory: u_k = rpm[k] + k_k + K_k (z_k - z_nom,k) is its time-varying LQR tracker, z_k the state
+                     before tick k (n_z = 13), with drag followed by the clipped RPMs of tick k - 1 (n_z = 17)
+          cost       [iters + 1, E, D]  J per iteration, row 0 the initial guess (non-increasing)
+          mu         [E, D]  the final regularisation
+          converged  [E, D]  bool: an accepted step decreased J by less than 1e-9 relative; the drone stopped there
+        The env is not touched and the result is not differentiable.  Downwash, T <= 0, iters < 0, negative or non-finite
+        weights, R <= 0 and bad shapes, dtypes or devices raise ValueError."""
+        from ..ilqr import ilqr
+        return ilqr(self, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, iters=iters, state=state,
+                    last_rpm=last_rpm, phys=phys)
+
     ################################################################################
 
     def _stream(self):

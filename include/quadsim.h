@@ -854,6 +854,56 @@ int qs_dyn_policy_traj_jvp(const QsParams* p, const QsDynPolicyTrajJvpIO* io, in
 int qs_dyn_policy_tick_jac(const QsParams* p, const QsDynPolicyTrajJvpIO* io, int act_type, int n_envs, int drones_per_env,
                            int substeps, unsigned effects, void* stream);
 
+/* Batched iLQR of raw-RPM trajectories (DESIGN.md 4.5.1): Gauss-Newton DDP, one independent problem per drone (no downwash).
+ * Drone i minimises J = 1/2 sum_k (x_k - r_k)' W_k (x_k - r_k) + 1/2 sum_k (u_k - u_ref)' Rt (u_k - u_ref) over its raw commands
+ * u_k = rpm[k], where x_k is the state after tick k (qs_dyn_traj's states[k]), W_k = diag(Q) for k < T-1 and diag(Q_final) for
+ * k = T-1, and Rt = diag(R) / HOVER_RPM^2 with the drone's row constants.  The loop state is z_k = x_{k-1} (state0 for k = 0),
+ * n_z = 13, or with drag z_k = (x_{k-1}, the clipped u_{k-1}), n_z = 17.  One iteration is qs_dyn_tick_jac at the nominal,
+ * qs_ilqr_backward, qs_ilqr_line_search and qs_ilqr_commit; none of them reads anything back to the host.  The rollouts of the
+ * line search and the commit are qs_dyn_traj's ticks, so a committed trajectory is qs_dyn_traj's output for the committed rpm. */
+typedef struct QsIlqrIO {
+    int T;                          /* ticks, > 0 */
+    int n_alpha;                    /* qs_ilqr_line_search / qs_ilqr_commit: step sizes in alpha, 1..16 */
+    const double* jac;              /* [T][N][13][C] qs_dyn_tick_jac's output at the nominal (qs_ilqr_backward) */
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows; nullable = the constants of QsParams */
+    const double* targets;          /* [T][13 N] r_k in the planes layout of the states */
+    const double* weights;          /* [n_envs][30]: Q (13), Q_final (13), R (4), all >= 0 and R > 0 (not checked here) */
+    const double* rpm_ref;          /* [N][4] u_ref */
+    const double* alpha;            /* [n_alpha] step sizes */
+    double* states;                 /* [T][13 N] the nominal trajectory; qs_ilqr_commit: in/out */
+    double* rpm;                    /* [T][N][4] the nominal raw commands; qs_ilqr_commit: in/out */
+    double* mu;                     /* [N] the regularisation; qs_ilqr_backward and qs_ilqr_commit: in/out */
+    double* K;                      /* [T][N][4][n_z] feedback gains (qs_ilqr_backward out); line search / commit: nullable = 0 */
+    double* k;                      /* [T][N][4] feed-forward gains (qs_ilqr_backward out); line search / commit: nullable = 0 */
+    double* dV;                     /* [N][2] sum k'Qu and 1/2 sum k'Quu k of the backward pass (qs_ilqr_backward out) */
+    double* J;                      /* [n_alpha][N] J(alpha) (qs_ilqr_line_search out, qs_ilqr_commit in) */
+    int* status;                    /* [N] 0, or 1 when Quu stayed indefinite through 8 raised regularisations (qs_ilqr_backward
+                                     * out); line search: nullable = 0 */
+    unsigned char* converged;       /* [N] 0 / 1 (qs_ilqr_commit in/out); line search: nullable = 0 */
+    const double* cost_in;          /* [N] the nominal's J (qs_ilqr_commit) */
+    double* cost_out;               /* [N] the committed J (qs_ilqr_commit out) */
+} QsIlqrIO;
+int qs_sizeof_ilqr_io(void);
+/* Backward pass (Riccati recursion) at the nominal, for k = T-1 .. 0: V += the stage cost of x_k; Qx = A'V_x,
+ * Qu = Rt (u_k - u_ref) + B'V_x, Qxx = A'V_xx A, Quu = Rt + B'V_xx B, Qux = B'V_xx A; Quu_mu = Quu + mu diag(Quu) by a 4x4
+ * Cholesky; k = -Quu_mu^-1 Qu, K = -Quu_mu^-1 Qux; V_x = Qx + K'Quu k + K'Qu + Qux'k, V_xx = Qxx + K'Quu K + K'Qux + Qux'K,
+ * symmetrised.  A failed Cholesky sets mu = max(1e-6, 10 mu) and restarts the drone's pass, at most 8 times.  With drag
+ * A = [[A_x, B_last], [0, 0]] and B = [[B_x], [diag(clip'(u_k))]].  One warp per drone. */
+int qs_ilqr_backward(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                     void* stream);
+/* J(alpha_a) of the rollout u_k = rpm[k] + alpha_a k_k + K_k (z_k - z_nom,k) from z_nom,0, for every drone and step size; no state
+ * is stored.  A drone with status != 0 or converged gets +inf. */
+int qs_ilqr_line_search(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                        void* stream);
+/* Per drone: the largest alpha with J(alpha) < cost_in and cost_in - J(alpha) >= 1e-4 (-(alpha dV1 + alpha^2 dV2)).  If there is
+ * one, its rollout overwrites states and rpm, cost_out = its J (the line search's bits), mu = mu / 10 (0 below 1e-6), and a
+ * relative decrease below 1e-9 sets converged; otherwise cost_out = cost_in and mu = max(1e-6, 10 mu).  A converged drone is
+ * left as it is. */
+int qs_ilqr_commit(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                   void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
