@@ -1,7 +1,9 @@
 """CPU tests of the iLQR backward pass (csrc/riccati.cuh, built for the host by tests/host_harness/ilqr_host.cpp; DESIGN.md 4.5.1):
 one tick against the float64 restatement tests/ilqr_ref.py for n_z = 13 and 17, a long pass with constant (A, B) from the hover
 Jacobian of the reference dynamics against the discrete algebraic Riccati equation, the stage cost, a Cholesky failure, and the
-C ABI's refusals of qs_ilqr_backward / qs_ilqr_line_search / qs_ilqr_commit without a GPU."""
+C ABI's refusals of qs_ilqr_backward / qs_ilqr_line_search / qs_ilqr_commit without a GPU.  Also the restatements the device tests
+use (ilqr_ref.commit, mu_ladder, rollout_cost, tick_jac) on hand-worked cases, and the host build on adversarial inputs: a
+subnormal and a zero pivot, an overflowing Quu, every rotor clipped."""
 import ctypes as C
 
 import numpy as np
@@ -184,3 +186,204 @@ def test_abi_exports_struct_and_refusals():
             io.n_alpha = 1
         io.phys = a + 8
         assert call(io, 1, 1, 1, 0) == -2
+
+
+# ---- H4: the commit rule, the restart ladder and J(alpha) of the restatement --------------------------------------------------
+
+def test_commit_rule_by_hand():
+    nan, inf = float("nan"), float("inf")
+    al = [1.0, 0.5, 0.25]
+    # the largest accepted alpha wins, not the first; unsorted alpha
+    assert IR.commit([0.25, 1.0, 0.5], [9.0, 9.5, 8.0], 10.0, -1.0, 0.0, 0.0, 0, False)[0] == 1
+    assert IR.commit([0.25, 1.0, 0.5], [9.0, 9.5, 8.0], 10.0, -1.0, 0.0, 0.0, 0, False, first_accepted=True)[0] == 0
+    # a tie between equal alpha: the first index
+    assert IR.commit([0.5, 0.5, 0.25], [9.0, 8.0, 7.0], 10.0, -1.0, 0.0, 0.0, 0, False)[0] == 0
+    # NaN and +inf J are never accepted; with Jn = +inf only a finite J passes Ja < Jn
+    assert IR.commit(al, [nan, inf, 9.0], 10.0, -1.0, 0.0, 0.0, 0, False)[0] == 2
+    assert IR.commit(al, [nan, inf, nan], 10.0, -1.0, 0.0, 0.0, 0, False) == (-1, 1e-6, False)
+    assert IR.commit(al, [inf, inf, inf], inf, -1.0, 0.0, 0.0, 0, False)[0] == -1
+    assert IR.commit(al, [inf, 5.0, inf], inf, -1.0, 0.0, 0.0, 0, False)[0] == 1
+    # Ja == Jn is rejected; Armijo at equality is accepted, one ulp short is not
+    assert IR.commit([1.0], [10.0], 10.0, 0.0, 0.0, 0.0, 0, False)[0] == -1
+    exp = 1e-4 * -(1.0 * -1e4 + 1.0 * 1.0 * 0.0)                 # 1.0 exactly
+    assert IR.commit([1.0], [10.0 - exp], 10.0, -1e4, 0.0, 0.0, 0, False)[0] == 0
+    assert IR.commit([1.0], [np.nextafter(10.0 - exp, inf)], 10.0, -1e4, 0.0, 0.0, 0, False)[0] == -1
+    # a negative dV2 raises the bar: the expected decrease of alpha = 1 is -(dV1 + dV2)
+    assert IR.commit([1.0], [9.99], 10.0, -1.0, -100.0, 0.0, 0, False)[0] == -1
+    # mu: /10 and 0 below 1e-6 on acceptance, max(1e-6, 10 mu) on rejection
+    acc = lambda mu: IR.commit([1.0], [5.0], 10.0, -1.0, 0.0, mu, 0, False)[1]
+    rej = lambda mu: IR.commit([1.0], [11.0], 10.0, -1.0, 0.0, mu, 0, False)[1]
+    assert acc(1e-5) == 1.0000000000000002e-06 and acc(9.999999999999999e-06) == 1e-6 and acc(1e-6) == 0.0 and acc(0.0) == 0.0
+    assert acc(9.99999999999999e-06) == 0.0                       # 9.99999999999999e-07 < 1e-6
+    assert rej(0.0) == 1e-6 and rej(1e-5) == 1e-4 and rej(9.999999999999999e-06) == 9.999999999999999e-05 and rej(1e-8) == 1e-6
+    # converged: Jn - Jc < 1e-9 Jn, strictly
+    Jn = 1.0
+    Jc = IR.converged_boundary(Jn)
+    assert Jn - Jc == 1e-9 * Jn or Jn - Jc > 1e-9 * Jn > Jn - np.nextafter(Jc, inf)
+    assert IR.commit([1.0], [Jc], Jn, 0.0, 0.0, 0.0, 0, False) == (0, 0.0, False)
+    assert IR.commit([1.0], [np.nextafter(Jc, inf)], Jn, 0.0, 0.0, 0.0, 0, False) == (0, 0.0, True)
+    # status 1 and converged drones are never accepted; a converged drone keeps its mu
+    assert IR.commit([1.0], [5.0], 10.0, -1.0, 0.0, 0.5, 1, False) == (-1, 5.0, False)
+    assert IR.commit([1.0], [5.0], 10.0, -1.0, 0.0, 0.5, 0, True) == (-1, 0.5, True)
+
+
+def test_mu_ladder():
+    assert IR.mu_ladder(0.0, 0.0) == (0.0, 0)
+    assert IR.mu_ladder(0.0, 5e-6) == (9.999999999999999e-06, 0)
+    assert IR.mu_ladder(0.0, 5e-4) == (0.001, 0)
+    assert IR.mu_ladder(0.0, lambda m: False) == (100.0, 1)
+    assert IR.mu_ladder(0.37, 2.0) == (3.7, 0)
+    assert IR.mu_ladder(0.37, lambda m: False)[1] == 1
+
+
+def _drag_problem(T=12, B=6, seed=0, model="cf2x"):
+    """A drag rollout whose nominal clips rotors at 0 and at MAX_RPM on some drones and ticks."""
+    import diff_ref as DR
+    from diff_testlib import aviary_rows
+    P, c = params_of(model, 240, 48)
+    rng = np.random.default_rng(seed)
+    _, rows = aviary_rows(model, B, rng)
+    hover, mx = rows[:, 12:13], rows[:, 13:14]
+    rpm = hover * (1 + 0.05 * torch.as_tensor(rng.uniform(-1, 1, (T, B, 4))))
+    rpm[3, 0, 1] = -50.0                                          # drone 0: a rotor below 0
+    rpm[5, 1, 2] = mx[1, 0] * 1.01                               # drone 1: a rotor beyond MAX_RPM
+    x0 = torch.zeros((B, 13), dtype=torch.float64)
+    x0[:, 2], x0[:, 6] = 1.0, 1.0
+    last = hover.expand(B, 4).clone()
+    K_dyn = DR.model_constants(P)
+    eff = DR.EFFECT_DRAG
+    S = 5
+    states = DR.rollout(K_dyn, rows, x0, rpm, last, S, eff)
+    W = torch.as_tensor(rng.uniform(0.1, 2.0, (T, B, 13)))
+    tg = torch.as_tensor(rng.normal(size=(T, B, 13))) * 0.1
+    Rt = torch.as_tensor(rng.uniform(0.5, 2.0, (B, 4))) * 1e-2 / hover ** 2
+    uref = hover.expand(B, 4) * 1.001
+    return dict(K_dyn=K_dyn, rows=rows, x0=x0, last_rpm=last, rpm_nom=rpm, states_nom=states, targets=tg, W=W, Rt=Rt, uref=uref, S=S,
+                effects=eff), rng
+
+
+def test_rollout_cost_at_alpha_zero_is_the_nominal_cost():
+    import diff_ref as DR
+    a, rng = _drag_problem()
+    T, B = a["rpm_nom"].shape[:2]
+    want = IR.cost(a["states_nom"], a["targets"], a["W"], a["rpm_nom"], a["uref"], a["Rt"])
+    for eff in (0, DR.EFFECT_DRAG):
+        b = dict(a, effects=eff, states_nom=DR.rollout(a["K_dyn"], a["rows"], a["x0"], a["rpm_nom"], a["last_rpm"], a["S"], eff))
+        r = IR.rollout_cost(Kfb=None, kff=None, alpha=0.0, **b)
+        assert torch.equal(r["x"], b["states_nom"]) and torch.equal(r["u"], b["rpm_nom"])
+        w = IR.cost(b["states_nom"], b["targets"], b["W"], b["rpm_nom"], b["uref"], b["Rt"])
+        assert torch.equal(r["J"], w)
+    # with gains at alpha = 0 the rollout reproduces the nominal (dz = 0 exactly) ...
+    Kfb = torch.as_tensor(rng.normal(size=(T, B, 4, 17))) * 1e2
+    kff = torch.as_tensor(rng.normal(size=(T, B, 4)))
+    r = IR.rollout_cost(Kfb=Kfb, kff=kff, alpha=0.0, **a)
+    assert torch.equal(r["J"], want)
+    # ... unless the nominal's previous RPMs are taken unclipped: that changes J only on the drones whose nominal clips a rotor
+    # (drones 0 and 1) before the last tick
+    bad = IR.rollout_cost(Kfb=Kfb, kff=kff, alpha=0.0, drag_prev_raw=True, **a)
+    changed = bad["J"] != want
+    print("drag_prev_raw at alpha = 0: relative change %s" % ((bad["J"] - want).abs() / want).tolist())
+    assert changed.tolist() == [True, True] + [False] * (B - 2)
+    assert ((bad["J"] - want).abs() / want)[:2].min() > 1e-6
+    # alpha moves J, and a per-drone alpha is the same as one alpha at a time
+    al = torch.tensor([1.0, 0.5, 0.25, 0.0, 1.0, 0.125], dtype=torch.float64)
+    rb = IR.rollout_cost(Kfb=Kfb, kff=kff, alpha=al, **a)
+    for i in (0, 2, 3):
+        one = IR.rollout_cost(Kfb=Kfb, kff=kff, alpha=float(al[i]), **a)
+        assert torch.equal(one["J"][i], rb["J"][i])
+    assert torch.equal(rb["J"][3], want[3]) and (rb["J"][0] != want[0])
+
+
+# ---- H5: the host build of the backward pass on adversarial inputs ------------------------------------------------------------
+
+def _adversarial(nz, seed, T=3, clipped=2):
+    rng = np.random.default_rng(seed)
+    F = np.concatenate([_random_tick(nz, rng, clipped) for _ in range(T)])
+    F[:, :, nz + clipped] = 0.0                                   # the clipped rotor's B column is 0 (with drag too)
+    dx, W = rng.normal(size=(T, 13)), rng.uniform(0.5, 2.0, (T, 13))
+    Rt, du = rng.uniform(0.5, 2.0, 4), rng.normal(size=(T, 4))
+    return F, dx, W, Rt, du
+
+
+def _ref_pass(F, dx, W, Rt, du, mu):
+    t = lambda x: torch.as_tensor(np.ascontiguousarray(x), dtype=torch.float64)
+    return IR.backward_pass(t(F), t(dx), t(W), t(Rt), t(du), mu)
+
+
+@pytest.mark.parametrize("nz", [13, 17])
+def test_backward_subnormal_and_zero_pivot(nz):
+    F, dx, W, Rt, du = _adversarial(nz, 20 + nz)
+    zero = np.zeros((nz, nz)), np.zeros(nz)
+    # the smallest subnormal Rt on the clipped rotor (its B column is 0): the pivot is positive, the pass goes through
+    Rt[2] = 5e-324
+    rc, K, k, V, vx, dV = host_pass(F, dx, W, Rt, du, 0.0, *zero)
+    r = _ref_pass(F, dx, W, Rt, du, 0.0)
+    assert rc == 0 and bool(r["ok"])
+    eK, ek = rel(K, r["K"]), rel(k, r["k"])
+    print("subnormal Rt nz=%d: K %.1e k %.1e, k of the clipped rotor %s" % (nz, eK, ek, k[:, 2]))
+    assert eK <= 1e-12 and ek <= 1e-12 and np.all(K[:, 2] == 0.0)
+    # Rt = 0 there: a pivot exactly 0 at the one tick whose B column is 0; the return code names that tick
+    Rt[2] = 0.0
+    F2 = F.copy()
+    for t in (0, 2):                                              # ticks 0 and 2 drive rotor 2 ...
+        F2[t, :13, nz + 2] = np.random.default_rng(t).normal(size=13)
+        if nz == 17:
+            F2[t, 15, nz + 2] = 1.0
+    rc = host_pass(F2, dx, W, Rt, du, 0.0, *zero)[0]
+    r = _ref_pass(F2, dx, W, Rt, du, 0.0)
+    assert rc == 2 and not bool(r["ok"])                          # ... tick 1 does not: 1 + 1
+    assert host_pass(F2, dx, W, Rt, du, 0.5, *zero)[0] == 2        # mu diag(Quu) scales a zero pivot to zero
+
+
+@pytest.mark.parametrize("nz", [13, 17])
+def test_backward_overflowing_quu_is_rejected(nz):
+    F, dx, W, Rt, du = _adversarial(nz, 30 + nz)
+    zero = np.zeros((nz, nz)), np.zeros(nz)
+    W[:] = 1e300
+    F[:, :13, nz + 1] *= 1e5                                      # rotor 1: Quu_11 = +inf, every other entry finite
+    rc = host_pass(F, dx, W, Rt, du, 0.0, *zero)[0]
+    t = lambda x: torch.as_tensor(x, dtype=torch.float64)
+    V, vx = IR.stage(t(zero[0]), t(zero[1]), t(dx[2]), t(W[2]))
+    r = IR.backward_tick(t(F[2]), V, vx, t(Rt), t(du[2]), 0.0)
+    B = t(F[2])[:, nz:]
+    Quu = torch.diag(t(Rt)) + B.T @ V @ B
+    print("overflow nz=%d: Quu diagonal %s" % (nz, torch.diagonal(Quu).tolist()))
+    assert torch.isinf(Quu[1, 1]) and torch.isfinite(Quu[0]).all() and torch.isfinite(Quu[2:, 2:]).all()
+    assert rc == 3 and not bool(r["ok"])                          # s = +inf fails s < INFINITY at t = T - 1
+    F[:, :13, nz + 1] /= 1e5
+    assert host_pass(F, dx, W, Rt, du, 0.0, *zero)[0] == 0
+
+
+@pytest.mark.parametrize("nz", [13, 17])
+def test_backward_all_rotors_clipped(nz):
+    F, dx, W, Rt, du = _adversarial(nz, 40 + nz)
+    F[:, :, nz:] = 0.0                                            # B = 0: no rotor reaches the state
+    zero = np.zeros((nz, nz)), np.zeros(nz)
+    rc, K, k, V, vx, dV = host_pass(F, dx, W, Rt, du, 0.3, *zero)
+    r = _ref_pass(F, dx, W, Rt, du, 0.3)
+    assert rc == 0 and bool(r["ok"])
+    assert np.all(K == 0.0)
+    ek, eV = rel(k, r["k"]), rel(V, r["V"])
+    print("all rotors clipped nz=%d: k %.1e V %.1e" % (nz, ek, eV))
+    assert ek <= 1e-15 and eV <= 1e-12
+    assert rel(k, -du / 1.3) <= 1e-15                            # Quu = diag(Rt), Quu_mu = 1.3 Quu, Qu = Rt du
+
+
+def test_tick_jac_is_jacfwd():
+    import diff_ref as DR
+    from diff_testlib import aviary_rows
+    P, _ = params_of("cf2p", 240, 48)
+    rng = np.random.default_rng(5)
+    _, rows = aviary_rows("cf2p", 3, rng)
+    x = torch.as_tensor(rng.normal(size=(3, 13))) * 0.1
+    x[:, 2] += 0.05
+    x[:, 6] += 1.0
+    raw = rows[:, 12:13] * (1 + 0.2 * torch.as_tensor(rng.uniform(-1, 1, (3, 4))))
+    raw[0, 1], raw[1, 2] = -1.0, rows[1, 13] * 1.5                # a rotor clipped at 0 and one at MAX_RPM
+    up = raw.clamp(min=0.0) * 0.9
+    for eff in (0, DR.EFFECT_GND | DR.EFFECT_DRAG):
+        got = IR.tick_jac(DR.model_constants(P), rows, x, raw, up, 5, eff)
+        want = ref_tick_jac(P, eff, 5, x.numpy(), raw.numpy(), up.numpy(), rows.numpy())
+        w = np.concatenate([want["state"], want["rpm"]] + ([want["up"]] if eff & DR.EFFECT_DRAG else []), axis=-1)
+        assert rel(got.numpy(), w) <= 1e-15
+        assert np.all(got[0, :, 14].numpy() == 0.0) and np.all(got[1, :, 15].numpy() == 0.0)
