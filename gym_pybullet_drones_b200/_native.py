@@ -186,6 +186,11 @@ class QsIlqrIO(C.Structure):
         "status", "converged", "cost_in", "cost_out")]
 
 
+class QsIlqrBoxIO(C.Structure):
+    _fields_ = [("base", QsIlqrIO), ("rpm_lo", C.c_void_p), ("rpm_hi", C.c_void_p), ("per_tick", C.c_int), ("pad_", C.c_int),
+                ("active", C.c_void_p)]
+
+
 class QsStepCall(C.Structure):
     _fields_ = [("p", C.c_void_p), ("st", C.c_void_p), ("io", C.c_void_p),
                 ("act_type", C.c_int), ("task", C.c_int), ("n_envs", C.c_int), ("drones_per_env", C.c_int), ("substeps", C.c_int),
@@ -201,7 +206,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_sizeof_dyn_ctrl_traj_io", "qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp", "qs_sizeof_dyn_policy_traj_io",
            "qs_dyn_traj_jvp", "qs_dyn_tick_jac", "qs_sizeof_dyn_traj_jvp_io", "qs_dyn_ctrl_traj_jvp", "qs_dyn_ctrl_tick_jac",
            "qs_sizeof_dyn_ctrl_traj_jvp_io", "qs_dyn_policy_traj_jvp", "qs_dyn_policy_tick_jac", "qs_sizeof_dyn_policy_traj_jvp_io",
-           "qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit", "qs_sizeof_ilqr_io"]
+           "qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit", "qs_sizeof_ilqr_io", "qs_ilqr_box_backward",
+           "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io"]
 MAX_PEERS = 16
 
 
@@ -324,6 +330,10 @@ def lib():
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
     L.qs_sizeof_ilqr_io.restype = C.c_int
+    for n in ("qs_ilqr_box_backward", "qs_ilqr_box_line_search", "qs_ilqr_box_commit"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrBoxIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
+    L.qs_sizeof_ilqr_box_io.restype = C.c_int
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -386,8 +396,8 @@ def lib():
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac / "
                           "dyn traj io / dyn ctrl traj io / dyn policy traj io / dyn traj jvp io / dyn ctrl traj jvp io / "
                           "dyn policy traj jvp io): rebuild")
-    if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io): rebuild")
+    if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO) or L.qs_sizeof_ilqr_box_io() != C.sizeof(QsIlqrBoxIO):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io / ilqr box io): rebuild")
     _lib = L
     return L
 

@@ -1,13 +1,16 @@
 // ilqr.cu -- qs_ilqr_backward / qs_ilqr_line_search / qs_ilqr_commit: batched iLQR of raw-RPM trajectories of Physics.DYN
 // (include/quadsim.h, DESIGN.md 4.5.1), one independent problem per drone, on qs_dyn_tick_jac's per-tick Jacobians.
-//   ilqr_backward_kernel<EFF>:    one warp per drone for all T ticks; lane j runs column j of riccati.cuh's phases on the
-//                                 drone's workspace in shared memory.  The tick's Jacobian block is one contiguous 13 C-double
-//                                 read per warp.
-//   ilqr_line_search_kernel<EFF>: one thread per (drone, step size), the step sizes of a drone in neighbouring lanes so that
-//                                 they read its K and k rows together.
-//   ilqr_commit_kernel<EFF>:      one thread per drone.
+//   ilqr_backward_kernel<EFF, BOX>:    one warp per drone for all T ticks; lane j runs column j of riccati.cuh's phases on
+//                                      the drone's workspace in shared memory.  The tick's Jacobian block is one contiguous
+//                                      13 C-double read per warp.
+//   ilqr_line_search_kernel<EFF, BOX>: one thread per (drone, step size), the step sizes of a drone in neighbouring lanes so
+//                                      that they read its K and k rows together.
+//   ilqr_commit_kernel<EFF, BOX>:      one thread per drone.
 // The rollouts of the last two are ilqr_rollout, whose tick is dyn_traj_kernel's (clip_rpm, dyn_tick_k, round_to_planes), so a
 // committed trajectory is qs_dyn_traj's output for the committed rpm and the commit's J is the line search's J bit for bit.
+// BOX = true is the control-limited variant (qs_ilqr_box_*): the backward solves riccati.cuh's box QP per tick and writes the
+// held rotors, the rollouts clamp each command to [rpm_lo, rpm_hi] before the tick, the stage cost and the commit's store.
+#include <type_traits>
 #include "qs_common.cuh"
 #include "dyn_tangent.cuh"
 #include "riccati.cuh"
@@ -28,6 +31,21 @@ struct IlqrArgs {
     long long N;
     int D, substeps;
 };
+struct IlqrBoxArgs : IlqrArgs {
+    const double* lo;               // [N][4], or [T][N][4] with per_tick
+    const double* hi;
+    signed char* active;            // [T][N][4], nullable
+    int per_tick;
+};
+template <bool BOX>
+using IlqrArgsOf = std::conditional_t<BOX, IlqrBoxArgs, IlqrArgs>;
+
+// the box [lo, hi] of the raw command of drone i at tick k
+__device__ __forceinline__ void box_at(const IlqrBoxArgs& a, int k, long long i, double lo[4], double hi[4]) {
+    const long long at = a.per_tick ? (long long)k * a.N + i : i;
+    ld4(a.lo, at, lo);
+    ld4(a.hi, at, hi);
+}
 
 // index of state component j (pos, quat x y z w, vel, rpy_rates) of drone i in a [13 N] planes state
 __device__ __forceinline__ long long plane_at(long long N, long long i, int j) {
@@ -49,8 +67,11 @@ __device__ __forceinline__ void rel_weights(const double* wt, const qs::PhysRow&
     for (int j = 0; j < 4; ++j) Rt[j] = wt[26 + j] / h2;
 }
 
-template <int EFF>
-__global__ void __launch_bounds__(32 * kBwdWarps) ilqr_backward_kernel(const __grid_constant__ IlqrArgs a) {
+// BOX: at least 3 CTAs (12 warps) per SM, as the unconstrained kernel runs.  Left free, the drag variant takes 196 registers
+// and 8 warps per SM, and its backward pass ran 37% longer than with the 24 spilled bytes this bound costs (DESIGN.md 4.5.1).
+// 0 leaves the unconstrained kernels as they were.
+template <int EFF, bool BOX>
+__global__ void __launch_bounds__(32 * kBwdWarps, BOX ? 3 : 0) ilqr_backward_kernel(const __grid_constant__ IlqrArgsOf<BOX> a) {
     constexpr int NZ = (EFF & QS_EFFECT_DRAG) ? 17 : 13, M = NZ + 4, C = (EFF & QS_EFFECT_DRAG) ? 21 : 17;
     __shared__ double sm[kBwdWarps][qs::RicWs<NZ>::DOUBLES];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -97,17 +118,35 @@ __global__ void __launch_bounds__(32 * kBwdWarps) ilqr_backward_kernel(const __g
             __syncwarp();
             if (lane < M) qs::ric_col_H(w, lane);
             __syncwarp();
-            qs::RicGains G;
-            if (!qs::ric_gains(w, Rt, du, mu, G, dV1, dV2)) {          // the same bits in every lane: a uniform branch
-                ok = false;
-                break;
+            std::conditional_t<BOX, qs::RicBoxGains, qs::RicGains> G;
+            if constexpr (BOX) {
+                double lo[4], hi[4];                                  // the box of k: the command's box minus u_nom
+                box_at(a, k, i, lo, hi);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    lo[j] -= raw[j];
+                    hi[j] -= raw[j];
+                }
+                if (!qs::ric_gains_box(w, Rt, du, lo, hi, mu, G, dV1, dV2)) {   // the same bits in every lane: uniform
+                    ok = false;
+                    break;
+                }
+                if (lane < NZ) qs::ric_col_K_box(w, lane, G);
+            } else {
+                if (!qs::ric_gains(w, Rt, du, mu, G, dV1, dV2)) {      // the same bits in every lane: a uniform branch
+                    ok = false;
+                    break;
+                }
+                if (lane < NZ) qs::ric_col_K(w, lane, G);
             }
-            if (lane < NZ) qs::ric_col_K(w, lane, G);
             __syncwarp();
             if (lane < NZ) qs::ric_col_V(w, lane, G);
             double* Ko = io.K + ki * 4 * NZ;
             for (int idx = lane; idx < 4 * NZ; idx += 32) Ko[idx] = w.K[idx];
             if (lane < 4) io.k[4 * ki + lane] = G.k[lane];
+            if constexpr (BOX) {
+                if (a.active && lane < 4) a.active[4 * ki + lane] = (signed char)G.act[lane];
+            }
             __syncwarp();
             if (lane < NZ) qs::ric_col_sym(w, lane);
         }
@@ -129,8 +168,8 @@ __global__ void __launch_bounds__(32 * kBwdWarps) ilqr_backward_kernel(const __g
 
 // J of the rollout u_k = rpm[k] + alpha k_k + K_k (z_k - z_nom,k) from z_nom,0 (K, k NULL: zero).  With `commit` the rollout
 // overwrites tick k's nominal rpm and state after reading them.
-template <int EFF>
-__device__ __forceinline__ double ilqr_rollout(const IlqrArgs& a, long long i, double alpha, bool commit) {
+template <int EFF, bool BOX>
+__device__ __forceinline__ double ilqr_rollout(const IlqrArgsOf<BOX>& a, long long i, double alpha, bool commit) {
     constexpr int NZ = (EFF & QS_EFFECT_DRAG) ? 17 : 13;
     const QsIlqrIO& io = a.io;
     const long long N = a.N;
@@ -174,6 +213,12 @@ __device__ __forceinline__ double ilqr_rollout(const IlqrArgs& a, long long i, d
             }
             u[j] = v;
         }
+        if constexpr (BOX) {
+            double lo[4], hi[4];
+            box_at(a, k, i, lo, hi);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) u[j] = qs::clampd(u[j], lo[j], hi[j]);
+        }
         if (commit) {
             double* o = io.rpm + 4 * ki;
             o[0] = u[0]; o[1] = u[1]; o[2] = u[2]; o[3] = u[3];
@@ -198,8 +243,8 @@ __device__ __forceinline__ double ilqr_rollout(const IlqrArgs& a, long long i, d
     return J;
 }
 
-template <int EFF>
-__global__ void __launch_bounds__(kIlqrTPB) ilqr_line_search_kernel(const __grid_constant__ IlqrArgs a) {
+template <int EFF, bool BOX>
+__global__ void __launch_bounds__(kIlqrTPB) ilqr_line_search_kernel(const __grid_constant__ IlqrArgsOf<BOX> a) {
     const QsIlqrIO& io = a.io;
     const int na = io.n_alpha;
     const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -207,12 +252,12 @@ __global__ void __launch_bounds__(kIlqrTPB) ilqr_line_search_kernel(const __grid
     const long long i = g / na;
     const int s = (int)(g - i * na);
     double J = INFINITY;
-    if (!(io.status && io.status[i]) && !(io.converged && io.converged[i])) J = ilqr_rollout<EFF>(a, i, io.alpha[s], false);
+    if (!(io.status && io.status[i]) && !(io.converged && io.converged[i])) J = ilqr_rollout<EFF, BOX>(a, i, io.alpha[s], false);
     io.J[(long long)s * a.N + i] = J;
 }
 
-template <int EFF>
-__global__ void __launch_bounds__(kIlqrTPB) ilqr_commit_kernel(const __grid_constant__ IlqrArgs a) {
+template <int EFF, bool BOX>
+__global__ void __launch_bounds__(kIlqrTPB) ilqr_commit_kernel(const __grid_constant__ IlqrArgsOf<BOX> a) {
     const QsIlqrIO& io = a.io;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long N = a.N;
@@ -223,6 +268,15 @@ __global__ void __launch_bounds__(kIlqrTPB) ilqr_commit_kernel(const __grid_cons
         return;
     }
     const double dV1 = io.dV[2 * i], dV2 = io.dV[2 * i + 1];
+    if constexpr (BOX) {
+        // k = 0 at every tick (dV2 = 1/2 sum k'Quu k = 0): the nominal is the box QPs' fixed point, typically every rotor held
+        // at a bound.  No step can lower J there, so without this the drone would only raise mu until it overflows.
+        if (io.status[i] == 0 && dV1 == 0.0 && dV2 == 0.0) {
+            io.cost_out[i] = Jn;
+            io.converged[i] = 1;
+            return;
+        }
+    }
     int best = -1;
     if (io.status[i] == 0) {
         for (int s = 0; s < io.n_alpha; ++s) {
@@ -233,7 +287,7 @@ __global__ void __launch_bounds__(kIlqrTPB) ilqr_commit_kernel(const __grid_cons
     }
     double mu = io.mu[i];
     if (best >= 0) {
-        const double Jc = ilqr_rollout<EFF>(a, i, io.alpha[best], true);
+        const double Jc = ilqr_rollout<EFF, BOX>(a, i, io.alpha[best], true);
         io.cost_out[i] = Jc;
         mu = mu / 10.0;
         if (mu < 1e-6) mu = 0.0;
@@ -247,10 +301,13 @@ __global__ void __launch_bounds__(kIlqrTPB) ilqr_commit_kernel(const __grid_cons
 
 enum IlqrEntry { kBackward, kLineSearch, kCommit };
 
-template <IlqrEntry WHICH>
-int launch_ilqr(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects, void* stream,
-                const char* what) {
+// BOX: io = &box->base (both NULL when box is)
+template <IlqrEntry WHICH, bool BOX>
+int launch_ilqr(const QsParams* p, const QsIlqrIO* io, const QsIlqrBoxIO* box, int n_envs, int drones_per_env, int substeps,
+                unsigned effects, void* stream, const char* what) {
     if (!p || !io) return fail(QS_ERR_NULL, what, "NULL params / io");
+    if (BOX && (!box->rpm_lo || !box->rpm_hi)) return fail(QS_ERR_NULL, what, "NULL rpm_lo / rpm_hi");
+    if (BOX && box->per_tick != 0 && box->per_tick != 1) return fail(QS_ERR_SIZE, what, "per_tick must be 0 or 1");
     if (!io->state0 || !io->rpm || !io->states || !io->targets || !io->weights || !io->rpm_ref)
         return fail(QS_ERR_NULL, what, "NULL state0 / rpm / states / targets / weights / rpm_ref");
     if (WHICH == kBackward && (!io->jac || !io->mu || !io->K || !io->k || !io->dV || !io->status))
@@ -266,14 +323,20 @@ int launch_ilqr(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_pe
     const long long blocks = WHICH == kBackward ? (N + kBwdWarps - 1) / kBwdWarps
                              : WHICH == kLineSearch ? (N * io->n_alpha + kIlqrTPB - 1) / kIlqrTPB : (N + kIlqrTPB - 1) / kIlqrTPB;
     if (blocks > 0x7fffffffLL) return fail(QS_ERR_SIZE, what, "the grid exceeds 2^31-1 CTAs");
-    IlqrArgs a;
+    IlqrArgsOf<BOX> a;
     memset(&a, 0, sizeof(a));
     a.P = *p; a.io = *io;
     a.N = N;
     a.D = drones_per_env; a.substeps = substeps;
+    if constexpr (BOX) {
+        a.lo = box->rpm_lo; a.hi = box->rpm_hi;
+        a.active = box->active;
+        a.per_tick = box->per_tick;
+    }
     return traj_launch(what, effects, [](auto EFF) {
         constexpr int E = decltype(EFF)::value;
-        return WHICH == kBackward ? ilqr_backward_kernel<E> : WHICH == kLineSearch ? ilqr_line_search_kernel<E> : ilqr_commit_kernel<E>;
+        return WHICH == kBackward ? ilqr_backward_kernel<E, BOX>
+                                  : WHICH == kLineSearch ? ilqr_line_search_kernel<E, BOX> : ilqr_commit_kernel<E, BOX>;
     }, (unsigned)blocks, WHICH == kBackward ? 32 * kBwdWarps : kIlqrTPB, 0, (cudaStream_t)stream, a);
 }
 
@@ -288,17 +351,38 @@ int qs_sizeof_ilqr_io(void) { return (int)sizeof(QsIlqrIO); }
 
 int qs_ilqr_backward(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                      void* stream) {
-    return launch_ilqr<kBackward>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_ilqr_backward");
+    return launch_ilqr<kBackward, false>(p, io, nullptr, n_envs, drones_per_env, substeps, effects, stream, "qs_ilqr_backward");
 }
 
 int qs_ilqr_line_search(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                         void* stream) {
-    return launch_ilqr<kLineSearch>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_ilqr_line_search");
+    return launch_ilqr<kLineSearch, false>(p, io, nullptr, n_envs, drones_per_env, substeps, effects, stream,
+                                           "qs_ilqr_line_search");
 }
 
 int qs_ilqr_commit(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                    void* stream) {
-    return launch_ilqr<kCommit>(p, io, n_envs, drones_per_env, substeps, effects, stream, "qs_ilqr_commit");
+    return launch_ilqr<kCommit, false>(p, io, nullptr, n_envs, drones_per_env, substeps, effects, stream, "qs_ilqr_commit");
+}
+
+int qs_sizeof_ilqr_box_io(void) { return (int)sizeof(QsIlqrBoxIO); }
+
+int qs_ilqr_box_backward(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                         void* stream) {
+    return launch_ilqr<kBackward, true>(p, io ? &io->base : nullptr, io, n_envs, drones_per_env, substeps, effects, stream,
+                                        "qs_ilqr_box_backward");
+}
+
+int qs_ilqr_box_line_search(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps,
+                            unsigned effects, void* stream) {
+    return launch_ilqr<kLineSearch, true>(p, io ? &io->base : nullptr, io, n_envs, drones_per_env, substeps, effects, stream,
+                                          "qs_ilqr_box_line_search");
+}
+
+int qs_ilqr_box_commit(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                       void* stream) {
+    return launch_ilqr<kCommit, true>(p, io ? &io->base : nullptr, io, n_envs, drones_per_env, substeps, effects, stream,
+                                      "qs_ilqr_box_commit");
 }
 
 }  // extern "C"

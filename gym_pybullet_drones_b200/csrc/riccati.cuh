@@ -210,6 +210,187 @@ QS_HD void ric_col_sym(const RicWs<NZ>& w, int j) {
     for (int i = 0; i < NZ; ++i) w.V[i * NZ + j] = 0.5 * (w.H[i * M + j] + w.H[j * M + i]);
 }
 
+// ---- Control limits (qs_ilqr_box_backward): the tick's k solves min 1/2 k'Quu_mu k + Qu'k subject to lo <= k <= hi, where
+// lo, hi = the box of the raw command minus u_nom.  The unconstrained k of ric_gains is kept when it lies in the box (with
+// today's K: a problem whose bounds never bind gives ric_gains' bits); otherwise a projected-Newton box QP (Tassa, Mansard &
+// Todorov, ICRA 2014) runs from clamp(0).  Its constants:
+constexpr int kBoxMaxIter = 100;        // projected-Newton iterations
+constexpr double kBoxArmijo = 0.1;      // a step is accepted when (f(x_new) - f(x)) / (step s'grad) >= kBoxArmijo
+constexpr double kBoxStepDec = 0.6;     // the line search's step factor
+constexpr double kBoxMinStep = 1e-22;   // the line search gives up below this step
+constexpr double kBoxGradTol = 1e-12;   // converged when every free |grad_j| <= kBoxGradTol (|g_j| + sum_q |a_jq x_q|)
+
+// true when lo <= x <= hi (false for a NaN entry)
+QS_HD bool box_inside(const double x[4], const double lo[4], const double hi[4]) {
+    bool in = true;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) in = in && lo[j] <= x[j] && x[j] <= hi[j];
+    return in;
+}
+
+// 1/2 x'a x + g'x
+QS_HD double box_value(const double a[16], const double g[4], const double x[4]) {
+    double f = 0.0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        double ax = 0.0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) ax += a[i * 4 + j] * x[j];
+        f += x[i] * (g[i] + 0.5 * ax);
+    }
+    return f;
+}
+
+// The projected-Newton box QP: x = argmin 1/2 x'a x + g'x subject to lo <= x <= hi, a symmetric positive definite, lo <= hi.
+// act[j] = -1 / +1 where x_j is held at lo_j / hi_j (x at the bound with the gradient pointing out of the box), 0 free.  Lf =
+// the Cholesky factor of a's free block embedded in a 4x4 with identity rows and columns on the held dimensions, so that
+// chol4_neg_solve with a right-hand side that is 0 on them solves the free block alone.  Returns the iterations taken, or -1
+// when the free block has no factor.
+QS_HD int box_qp(const double a[16], const double g[4], const double lo[4], const double hi[4], double x[4], double Lf[16],
+                 int act[4]) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        x[j] = clampd(0.0, lo[j], hi[j]);
+        act[j] = 0;
+    }
+    double f = box_value(a, g, x);
+    bool factored = false;
+    int it = 0;
+    for (; it < kBoxMaxIter; ++it) {
+        double gr[4];
+        bool changed = !factored, held = true, small = true;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            double s = g[i], sc = fabs(g[i]);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                s += a[i * 4 + j] * x[j];
+                sc += fabs(a[i * 4 + j] * x[j]);
+            }
+            gr[i] = s;
+            const int na = (x[i] == lo[i] && s > 0.0) ? -1 : ((x[i] == hi[i] && s < 0.0) ? 1 : 0);
+            changed = changed || na != act[i];
+            act[i] = na;
+            held = held && na != 0;
+            small = small && (na != 0 || fabs(s) <= kBoxGradTol * sc);
+        }
+        if (held) {
+#pragma unroll
+            for (int q = 0; q < 16; ++q) Lf[q] = (q % 5 == 0) ? 1.0 : 0.0;
+            return it;
+        }
+        if (changed) {
+            double e[16];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) e[i * 4 + j] = (act[i] == 0 && act[j] == 0) ? a[i * 4 + j] : (i == j ? 1.0 : 0.0);
+            }
+            if (!chol4(e, Lf)) return -1;
+            factored = true;
+        }
+        if (small) return it;
+        // the Newton step of the free block with the held entries fixed: x_f + s_f = -a_ff^-1 (g_f + a_fh x_h)
+        double r[4], s[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            double v = g[i];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) v += act[j] != 0 ? a[i * 4 + j] * x[j] : 0.0;
+            r[i] = act[i] != 0 ? 0.0 : v;
+        }
+        chol4_neg_solve(Lf, r, s);
+        double sg = 0.0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            s[j] = act[j] != 0 ? 0.0 : s[j] - x[j];
+            sg += s[j] * gr[j];
+        }
+        if (!(sg < 0.0)) return it;                                   // no descent left: rounding
+        double step = 1.0, xc[4], fc;
+        for (;;) {                                                    // Armijo backtracking along the projected arc
+#pragma unroll
+            for (int j = 0; j < 4; ++j) xc[j] = clampd(x[j] + step * s[j], lo[j], hi[j]);
+            fc = box_value(a, g, xc);
+            if ((fc - f) / (step * sg) >= kBoxArmijo) break;
+            step *= kBoxStepDec;
+            if (step < kBoxMinStep) return it;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) x[j] = xc[j];
+        f = fc;
+    }
+    return it;
+}
+
+// What every column needs after phase G of the box backward: RicGains with k the box QP's, the factor Lf that K is solved
+// with (L on the fast path) and the held rotors
+struct RicBoxGains : RicGains {
+    double Lf[16];
+    int act[4];
+};
+
+// Phase G of the box backward (every lane, the same bits): ric_gains, then k as above for the box [lo, hi] of k, and dV1 +=
+// k'Qu, dV2 += 1/2 k'Quu k with that k.  false when Quu_mu or its free block is not positive definite.
+template <int NZ>
+QS_HD bool ric_gains_box(const RicWs<NZ>& w, const double Rt[4], const double du[4], const double lo[4], const double hi[4],
+                         double mu, RicBoxGains& G, double& dV1, double& dV2) {
+    double d1 = 0.0, d2 = 0.0;
+    if (!ric_gains(w, Rt, du, mu, G, d1, d2)) return false;
+    if (box_inside(G.k, lo, hi)) {                                    // the fast path: ric_gains' k, K from its factor
+#pragma unroll
+        for (int q = 0; q < 16; ++q) G.Lf[q] = G.L[q];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) G.act[j] = 0;
+        dV1 += d1;
+        dV2 += d2;
+        return true;
+    }
+    double a[16];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) a[i * 4 + j] = i == j ? G.Quu[i * 4 + j] + mu * G.Quu[i * 4 + j] : G.Quu[i * 4 + j];
+    }
+    if (box_qp(a, G.Qu, lo, hi, G.k, G.Lf, G.act) < 0) return false;
+    d1 = d2 = 0.0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        double qk = 0.0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) qk += G.Quu[i * 4 + j] * G.k[j];
+        d1 += G.k[i] * G.Qu[i];
+        d2 += G.k[i] * qk;
+    }
+    dV1 += d1;
+    dV2 += 0.5 * d2;
+    return true;
+}
+
+// Phase K of the box backward (j < NZ): ric_col_K with K's free rows -(Quu_mu,ff)^-1 Qux,f from Lf and its held rows 0
+template <int NZ>
+QS_HD void ric_col_K_box(const RicWs<NZ>& w, int j, const RicBoxGains& G) {
+    constexpr int M = NZ + 4;
+    double qux[4], rhs[4], kj[4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        qux[a] = w.H[(NZ + a) * M + j];
+        rhs[a] = G.act[a] != 0 ? 0.0 : qux[a];
+    }
+    chol4_neg_solve(G.Lf, rhs, kj);
+    double v = w.g[j];
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        if (G.act[a] != 0) kj[a] = 0.0;
+        double qk = 0.0;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) qk += G.Quu[a * 4 + b] * G.k[b];
+        v += kj[a] * qk + kj[a] * G.Qu[a] + qux[a] * G.k[a];
+        w.K[a * NZ + j] = kj[a];
+    }
+    w.vx[j] = v;
+}
+
 // 1/2 (sum_r W_r (x_r - ref_r)^2 + sum_j Rt_j (u_j - uref_j)^2): the cost of one tick, x and ref in the order pos, quat, vel,
 // rpy_rates
 QS_HD double stage_cost(const double x[13], const double ref[13], const double W[13], const double u[4], const double uref[4],

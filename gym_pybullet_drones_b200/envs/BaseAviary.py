@@ -693,7 +693,7 @@ class BaseAviary(Env):
                          pid_state=pid_state)
 
     def ilqr(self, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None, last_rpm=None,
-             phys=None):
+             phys=None, rpm_bounds=None):
         """Optimal raw-RPM trajectories of every drone by iLQR (Gauss-Newton DDP) on the device, one independent problem per
         drone, solved in lockstep with its own regularisation, step size and convergence flag (DESIGN.md 4.5.1).  Drone i
         minimises
@@ -711,6 +711,16 @@ class BaseAviary(Env):
         each aviary's HOVER_RPM).  iters: iterations (>= 0).  state, last_rpm and phys as in differentiable_rollout.  The
         weights are checked once (one synchronisation); nothing in the iterations synchronises with the host.
 
+        rpm_bounds: None (default: the clip inside the dynamics is the only motor limit, the solver does not see it), "motor"
+        for (0, MAX_RPM) of each aviary's row (phys included), or a pair (lo, hi) of float64 CUDA tensors in raw RPM, each [4],
+        [E, D, 4] or [T, E, D, 4] (a time axis lets a limit change mid-horizon).  With bounds the solve is control-limited DDP:
+        each tick of the backward pass solves a box-constrained QP for k, the guess is projected into the box before the first
+        rollout (rpm_ref may lie outside it), and the line search and the commit clamp every command into the box, so every
+        returned rpm lies in [lo, hi] and the clip inside the dynamics never binds.  The tracker is then
+        u = clamp(rpm[k] + K_k (z_k - z_nom,k), lo_k, hi_k), where the rows of K on clamped rotors are zero.  The bounds are
+        checked in the same synchronisation as the weights: NaN, lo > hi, lo < 0 or hi > MAX_RPM of the drone's row raise
+        ValueError, as do a time axis other than T and bad shapes, dtypes or devices.
+
         Returns (indices are drone ids, also after reorder_by_morton()):
           pos, quat, vel, rpy_rates [T, E, D, k]  the final nominal trajectory, bit for bit differentiable_rollout(rpm=rpm)
           rpm        [T, E, D, 4]
@@ -720,11 +730,12 @@ class BaseAviary(Env):
           cost       [iters + 1, E, D]  J per iteration, row 0 the initial guess (non-increasing)
           mu         [E, D]  the final regularisation
           converged  [E, D]  bool: an accepted step decreased J by less than 1e-9 relative; the drone stopped there
+          active     [T, E, D, 4] int8, with rpm_bounds only: the rotors the last backward pass held, -1 at lo, +1 at hi, 0 free
         The env is not touched and the result is not differentiable.  Downwash, T <= 0, iters < 0, negative or non-finite
         weights, R <= 0 and bad shapes, dtypes or devices raise ValueError."""
         from ..ilqr import ilqr
         return ilqr(self, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, iters=iters, state=state,
-                    last_rpm=last_rpm, phys=phys)
+                    last_rpm=last_rpm, phys=phys, rpm_bounds=rpm_bounds)
 
     ################################################################################
 

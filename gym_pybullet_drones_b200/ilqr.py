@@ -1,7 +1,8 @@
 """Batched iLQR of raw-RPM trajectories of Physics.DYN (DESIGN.md 4.5.1): Gauss-Newton DDP for every drone at once, one
 independent problem per drone, on the per-tick Jacobians of qs_dyn_tick_jac and the kernels qs_ilqr_backward,
-qs_ilqr_line_search and qs_ilqr_commit (include/quadsim.h).  BaseAviary.ilqr is the public entry point; Problem holds one
-solve's device buffers and runs its steps, so that each step can also be called on its own."""
+qs_ilqr_line_search and qs_ilqr_commit (include/quadsim.h), or with rpm_bounds their control-limited variants qs_ilqr_box_*.
+BaseAviary.ilqr is the public entry point; Problem holds one solve's device buffers and runs its steps, so that each step can
+also be called on its own."""
 import ctypes as C
 
 import torch
@@ -39,6 +40,39 @@ def _target_part(x, name, width, T, E, D, dev):
     return _tensor(x, name, (T, E, D, width), dev).reshape(T, E * D, width)
 
 
+def _bound(x, name, T, E, D, dev):
+    """One side of rpm_bounds as ([E * D, 4] or [T, E * D, 4], has a time axis): from [4], [E, D, 4] or [T, E, D, 4]."""
+    if not isinstance(x, torch.Tensor) or x.dim() not in (1, 3, 4):
+        raise ValueError("%s must be a float64 CUDA tensor [4], [%d, %d, 4] or [%d, %d, %d, 4]" % (name, E, D, T, E, D))
+    if x.dim() == 1:
+        return _tensor(x, name, (4,), dev).expand(E * D, 4), False
+    if x.dim() == 3:
+        return _tensor(x, name, (E, D, 4), dev).reshape(E * D, 4), False
+    if x.shape[0] != T:
+        raise ValueError("ilqr(): %s has %d ticks but the horizon is T = %d" % (name, x.shape[0], T))
+    return _tensor(x, name, (T, E, D, 4), dev).reshape(T, E * D, 4), True
+
+
+def _rpm_box(rpm_bounds, rows, T, E, D, dev):
+    """rpm_bounds as (lo, hi, per_tick, ok): lo and hi [N, 4] (per_tick False) or [T, N, 4] (True), contiguous, and ok a 0-dim
+    bool tensor (not read here) that is true when no bound is NaN, lo <= hi and 0 <= lo, hi <= MAX_RPM of each drone's row."""
+    n = E * D
+    max_rpm = rows[:, 13].reshape(E, 1, 1).expand(E, D, 4).reshape(n, 4)
+    if isinstance(rpm_bounds, str) and rpm_bounds == "motor":
+        lo = torch.zeros((n, 4), dtype=torch.float64, device=dev)
+        return lo, max_rpm.contiguous(), False, torch.ones((), dtype=torch.bool, device=dev)
+    if not isinstance(rpm_bounds, (tuple, list)) or len(rpm_bounds) != 2:
+        raise ValueError("rpm_bounds must be None, 'motor' or a pair (lo, hi) of float64 CUDA tensors in raw RPM")
+    lo, lo_t = _bound(rpm_bounds[0], "rpm_bounds[0] (lo)", T, E, D, dev)
+    hi, hi_t = _bound(rpm_bounds[1], "rpm_bounds[1] (hi)", T, E, D, dev)
+    per_tick = lo_t or hi_t
+    if per_tick:
+        lo, hi = lo.expand(T, n, 4), hi.expand(T, n, 4)
+    lo, hi = lo.detach().contiguous(), hi.detach().contiguous()
+    ok = ~(torch.isnan(lo).any() | torch.isnan(hi).any()) & (lo <= hi).all() & (lo >= 0).all() & (hi <= max_rpm).all()
+    return lo, hi, per_tick, ok
+
+
 def _weight(x, name, default, E, dev):
     """A weight vector as [E, width]: from [width] or [E, width]; None -> `default`."""
     width = len(default)
@@ -52,10 +86,11 @@ def _weight(x, name, default, E, dev):
 class Problem:
     """The device buffers of one batched iLQR solve and its steps.  Arguments as BaseAviary.ilqr; `alphas` are the line
     search's step sizes (1 to 16).  `feedback = False` runs the line search and the commit with K = 0 (an open-loop line
-    search along k)."""
+    search along k).  With `rpm_bounds` every step runs the control-limited kernels qs_ilqr_box_*, the guess is projected into
+    the box before the first nominal, and `active` holds the held rotors of the last backward pass."""
 
     def __init__(self, env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, state=None, last_rpm=None,
-                 phys=None, alphas=ALPHAS):
+                 phys=None, alphas=ALPHAS, rpm_bounds=None):
         _refuse_downwash(env, "ilqr()", "Jacobian")
         E, D, n, dev = env._E, env._D, env._N, env.device
         if not isinstance(target, dict) or "pos" not in target:
@@ -96,9 +131,22 @@ class Problem:
             qf = FINAL_SCALE * q if Q_final is None else _weight(Q_final, "Q_final", DEFAULT_Q, E, dev)
             r = _weight(R, "R", DEFAULT_R, E, dev)
             self.weights = torch.cat([q, qf, r], dim=1).contiguous()
-            # the one synchronisation of a solve: the weights' values
-            if not bool((torch.isfinite(self.weights).all() & (self.weights >= 0).all() & (r > 0).all()).item()):
-                raise ValueError("ilqr(): Q and Q_final must be finite and >= 0, R finite and > 0")
+            w_ok = torch.isfinite(self.weights).all() & (self.weights >= 0).all() & (r > 0).all()
+            if rpm_bounds is None:
+                # the one synchronisation of a solve: the weights' values
+                if not bool(w_ok.item()):
+                    raise ValueError("ilqr(): Q and Q_final must be finite and >= 0, R finite and > 0")
+                self.box = None
+            else:
+                lo, hi, per_tick, b_ok = _rpm_box(rpm_bounds, rows, T, E, D, dev)
+                # the one synchronisation of a solve: the weights' and the bounds' values
+                w_ok, b_ok = torch.stack([w_ok, b_ok]).tolist()
+                if not w_ok:
+                    raise ValueError("ilqr(): Q and Q_final must be finite and >= 0, R finite and > 0")
+                if not b_ok:
+                    raise ValueError("ilqr(): rpm_bounds must not be NaN and must satisfy 0 <= lo <= hi <= MAX_RPM of each "
+                                     "drone's row")
+                self.box = (lo, hi, per_tick)
             hover = rows[:, 12].reshape(E, 1, 1).expand(E, D, 4)
             if rpm_ref is None:
                 ref = hover.reshape(n, 4)
@@ -112,6 +160,9 @@ class Problem:
             else:
                 rpm = _tensor(rpm, "rpm", (T, E, D, 4), dev).reshape(T, n, 4)
             self.rpm = rpm.detach().clone().contiguous()
+            if self.box is not None:                             # the guess projected into the box
+                lo, hi, per_tick = self.box
+                torch.minimum(torch.maximum(self.rpm, lo), hi, out=self.rpm)
         self.env_shape = (E, D)
         self.planes0, self.last_rpm, self.rows = planes0.contiguous(), last_rpm.detach().contiguous(), rows.contiguous()
         self.cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
@@ -128,6 +179,7 @@ class Problem:
         self.mu = torch.zeros((n,), **f64)
         self.status = torch.zeros((n,), dtype=torch.int32, device=dev)
         self.converged = torch.zeros((n,), dtype=torch.uint8, device=dev)
+        self.active = None if self.box is None else torch.zeros((T, n, 4), dtype=torch.int8, device=dev)
         self.feedback = True
 
     def _ilqr(self, name, alpha=None, **ptrs):
@@ -139,6 +191,11 @@ class Problem:
                     converged=self.converged)
         base.update(ptrs)
         io = _io(N.QsIlqrIO, self.T, base, n_alpha=alpha.numel())
+        if self.box is not None:
+            lo, hi, per_tick = self.box
+            io = N.QsIlqrBoxIO(base=io, rpm_lo=lo.data_ptr(), rpm_hi=hi.data_ptr(), per_tick=int(per_tick),
+                               active=None if self.active is None else self.active.data_ptr())
+            name = name.replace("qs_ilqr_", "qs_ilqr_box_")
         _call(name, C.byref(P), C.byref(io), E, D, S, eff, device=self.dev)
 
     def nominal(self):
@@ -181,6 +238,8 @@ class Problem:
         out["cost"] = cost.view(cost.shape[0], E, D)
         out["mu"] = self.mu.view(E, D)
         out["converged"] = self.converged.view(E, D).bool()
+        if self.active is not None:
+            out["active"] = self.active.view(T, E, D, 4)
         return out
 
 
@@ -203,10 +262,11 @@ def solve(p, iters):
     return p.result(cost)
 
 
-def ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None, last_rpm=None, phys=None):
+def ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None, last_rpm=None, phys=None,
+         rpm_bounds=None):
     """BaseAviary.ilqr (see there)."""
     if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
         raise ValueError("iters must be an integer >= 0, got %r" % (iters,))
     p = Problem(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, state=state, last_rpm=last_rpm,
-                phys=phys)
+                phys=phys, rpm_bounds=rpm_bounds)
     return solve(p, iters)

@@ -904,6 +904,34 @@ int qs_ilqr_line_search(const QsParams* p, const QsIlqrIO* io, int n_envs, int d
 int qs_ilqr_commit(const QsParams* p, const QsIlqrIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                    void* stream);
 
+/* Control-limited iLQR (DESIGN.md 4.5.1): the problem of QsIlqrIO with every raw command held to the box
+ * rpm_lo <= u_k <= rpm_hi.  The bounds must satisfy 0 <= rpm_lo <= rpm_hi <= MAX_RPM of the drone's row (not checked here), and
+ * the nominal rpm must lie in the box: the clip to [0, MAX_RPM] in the dynamics then never binds. */
+typedef struct QsIlqrBoxIO {
+    QsIlqrIO base;                  /* as for qs_ilqr_backward / qs_ilqr_line_search / qs_ilqr_commit */
+    const double* rpm_lo;           /* [N][4] raw RPM, or [T][N][4] with per_tick */
+    const double* rpm_hi;           /* [N][4] raw RPM, or [T][N][4] with per_tick */
+    int per_tick;                   /* 0: one box per drone; 1: one per tick and drone */
+    int pad_;
+    signed char* active;            /* [T][N][4] qs_ilqr_box_backward out: -1 where k_k holds a rotor at rpm_lo, +1 at rpm_hi,
+                                     * 0 free; nullable */
+} QsIlqrBoxIO;
+int qs_sizeof_ilqr_box_io(void);
+/* qs_ilqr_backward with k_k = argmin 1/2 k'Quu_mu k + Qu'k subject to rpm_lo,k - u_k <= k <= rpm_hi,k - u_k: the unconstrained k
+ * when it lies in the box (then K, k and dV are qs_ilqr_backward's bits), otherwise a projected-Newton box QP from clamp(0) on
+ * Quu_mu.  Rows of K on held rotors are 0, free rows -(Quu_mu,ff)^-1 Qux,f; dV and the value update take this k and K.  A free
+ * block without a Cholesky factor restarts the pass as a failed Quu_mu does.  Refusals as qs_ilqr_backward, and NULL
+ * rpm_lo / rpm_hi, per_tick not 0 or 1. */
+int qs_ilqr_box_backward(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                         void* stream);
+/* qs_ilqr_line_search with u_k clamped to [rpm_lo,k, rpm_hi,k] before the tick and the stage cost */
+int qs_ilqr_box_line_search(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps,
+                            unsigned effects, void* stream);
+/* qs_ilqr_commit with u_k clamped as in the line search; the clamped u_k is stored.  A drone with status 0 and dV1 = dV2 = 0
+ * (k = 0 at every tick, e.g. every rotor held at a bound) is set converged with cost_out = cost_in and mu unchanged. */
+int qs_ilqr_box_commit(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                       void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]

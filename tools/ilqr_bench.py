@@ -6,7 +6,11 @@ events around its launch, [min, median, max] ms over --reps iterations after --w
   * backward: qs_ilqr_backward, with the bytes it must move computed from the shapes (the Jacobian read, K and k written, the
               states, targets and rpm read once) over its time, and that rate as a share of the H100 SXM data sheet's 3.35 TB/s;
   * line:     qs_ilqr_line_search over the 10 step sizes;
-  * commit:   qs_ilqr_commit."""
+  * commit:   qs_ilqr_commit.
+--rpm-bounds motor times the control-limited kernels (qs_ilqr_box_*) with the box (0, MAX_RPM), and reports the share of
+rotor-ticks the last backward pass held.  --task picks the targets: spread (within 0.5 m of (0, 0, 1), the default), hover
+(within 2 mm of each drone's start: no bound binds, the backward takes the fast path at every tick) or climb (1 m straight up:
+rotors saturate)."""
 import argparse
 import json
 import os
@@ -29,7 +33,7 @@ def stats(ts):
     return [round(ts[0], 3), round(ts[len(ts) // 2], 3), round(ts[-1], 3)]
 
 
-def run(physics, E, D, T, reps, warmup):
+def run(physics, E, D, T, reps, warmup, task="spread", rpm_bounds=None):
     from gym_pybullet_drones_b200.envs import CtrlAviary
     from gym_pybullet_drones_b200.ilqr import Problem
     from gym_pybullet_drones_b200.utils.enums import Physics
@@ -37,8 +41,16 @@ def run(physics, E, D, T, reps, warmup):
     xyz = np.stack([rng.uniform(-1, 1, D), rng.uniform(-1, 1, D), rng.uniform(0.5, 1.5, D)], 1)
     env = CtrlAviary(num_drones=D, physics=getattr(Physics, physics), pyb_freq=240, ctrl_freq=48, initial_xyzs=xyz, num_envs=E)
     env.reset()
-    target = {"pos": torch.tensor(rng.uniform(-0.5, 0.5, (E, D, 3)) + np.array([0.0, 0.0, 1.0]), device=env.device)}
-    p = Problem(env, target, num_steps=T)
+    if task == "spread":
+        target = {"pos": torch.tensor(rng.uniform(-0.5, 0.5, (E, D, 3)) + np.array([0.0, 0.0, 1.0]), device=env.device)}
+    else:
+        pos = env.pos.to(torch.float64).clone()
+        if task == "climb":
+            pos[..., 2] += 1.0
+        else:
+            pos += torch.as_tensor(rng.uniform(-2e-3, 2e-3, tuple(pos.shape)), dtype=torch.float64, device=env.device)
+        target = {"pos": pos}
+    p = Problem(env, target, num_steps=T, rpm_bounds=rpm_bounds)
     n = p.n
     cost = torch.empty((2, n), dtype=torch.float64, device=env.device)
     p.nominal()
@@ -62,7 +74,9 @@ def run(physics, E, D, T, reps, warmup):
     # the backward's compulsory traffic: the Jacobian, the nominal states, targets and rpm read, K and k written
     bwd_bytes = 8 * T * n * (13 * C + 13 + 13 + 4 + 4 * nz + 4)
     med = {k: stats(v)[1] for k, v in times.items()}
-    return {"physics": physics, "drones": n, "T": T, "nz": nz, "ms": {k: stats(v) for k, v in times.items()},
+    held = None if p.active is None else round(float((p.active != 0).float().mean()), 4)
+    return {"physics": physics, "task": task, "rpm_bounds": rpm_bounds, "held_share": held, "drones": n, "T": T, "nz": nz,
+            "ms": {k: stats(v) for k, v in times.items()},
             "iteration_ms": round(sum(med.values()), 3), "backward_GB": round(bwd_bytes / 1e9, 3),
             "backward_TB_per_s": round(bwd_bytes / (med["backward"] * 1e-3) / 1e12, 3),
             "backward_share_of_3.35TB_per_s": round(bwd_bytes / (med["backward"] * 1e-3) / HBM_BYTES_PER_S, 3),
@@ -77,12 +91,14 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--physics", default="DYN,PYB_DRAG")
+    ap.add_argument("--task", default="spread", choices=["spread", "hover", "climb"])
+    ap.add_argument("--rpm-bounds", default=None, choices=["motor"])
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("ilqr_bench: no CUDA device")
     name = card()
     for physics in a.physics.split(","):
-        r = run(physics, a.envs, a.drones, a.T, a.reps, a.warmup)
+        r = run(physics, a.envs, a.drones, a.T, a.reps, a.warmup, a.task, a.rpm_bounds)
         r["card"] = name
         print(json.dumps(r))
         torch.cuda.empty_cache()
