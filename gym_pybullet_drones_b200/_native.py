@@ -15,7 +15,7 @@ _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
                                              "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "lqr_law.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -35,6 +35,7 @@ FLAG_OBS_STATE20 = 32
 FLAG_SKIP_EPILOGUE, FLAG_RPM_FROM_LAST, FLAG_ACTION_F64 = 0x100, 0x200, 0x400
 CTRL_RAW, CTRL_VEL, CTRL_TRACK = 0, 1, 2          # qs_ctrl_rollout modes
 CTRL_MRAC = 3                                     # qs_ctrl_rollout_mrac
+CTRL_LQR = 4                                      # qs_ctrl_rollout_lqr
 MRAC_STATE = 76                                   # doubles of one MRAC's adaptive state (Kx 48, Kr 16, Xm 12)
 ABI_VERSION = 4
 MLP_TANH, MLP_RELU = 0, 1                         # QsMlpPolicy.activation
@@ -140,6 +141,11 @@ class QsMracRolloutIO(C.Structure):
     _fields_ = [("params", C.c_void_p), ("state", C.c_void_p), ("init", C.c_int), ("pad_", C.c_int), ("rpy_e", C.c_void_p)]
 
 
+class QsLqrRolloutIO(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("K", "z_nom", "rpm_nom", "lo", "hi")] + [
+        ("per_tick", C.c_int), ("n_z", C.c_int), ("T_plan", C.c_int), ("tick0", C.c_int)]
+
+
 class QsDynTrajIO(C.Structure):
     _fields_ = [("T", C.c_int), ("pad_", C.c_int)] + [(n, C.c_void_p) for n in (
         "state0", "rpm", "last_rpm", "phys", "states", "g_states", "g_rpm", "g_state0", "g_last_rpm", "g_phys", "scratch")]
@@ -207,7 +213,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_dyn_traj_jvp", "qs_dyn_tick_jac", "qs_sizeof_dyn_traj_jvp_io", "qs_dyn_ctrl_traj_jvp", "qs_dyn_ctrl_tick_jac",
            "qs_sizeof_dyn_ctrl_traj_jvp_io", "qs_dyn_policy_traj_jvp", "qs_dyn_policy_tick_jac", "qs_sizeof_dyn_policy_traj_jvp_io",
            "qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit", "qs_sizeof_ilqr_io", "qs_ilqr_box_backward",
-           "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io"]
+           "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io", "qs_ctrl_rollout_lqr",
+           "qs_sizeof_lqr_rollout_io"]
 MAX_PEERS = 16
 
 
@@ -298,6 +305,10 @@ def lib():
         [C.c_void_p] * 8
     L.qs_sizeof_mrac_params.restype = C.c_int
     L.qs_sizeof_mrac_rollout_io.restype = C.c_int
+    L.qs_ctrl_rollout_lqr.restype = C.c_int
+    L.qs_ctrl_rollout_lqr.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.POINTER(QsLqrRolloutIO),
+                                      C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
+    L.qs_sizeof_lqr_rollout_io.restype = C.c_int
     for n in ("qs_dyn_traj", "qs_dyn_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
@@ -398,6 +409,8 @@ def lib():
                           "dyn policy traj jvp io): rebuild")
     if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO) or L.qs_sizeof_ilqr_box_io() != C.sizeof(QsIlqrBoxIO):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io / ilqr box io): rebuild")
+    if L.qs_sizeof_lqr_rollout_io() != C.sizeof(QsLqrRolloutIO):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (lqr rollout io): rebuild")
     _lib = L
     return L
 

@@ -13,6 +13,7 @@
 #include <type_traits>
 #include "qs_common.cuh"
 #include "dyn_tangent.cuh"
+#include "lqr_law.cuh"
 #include "riccati.cuh"
 #include "traj_io.cuh"
 
@@ -205,12 +206,7 @@ __device__ __forceinline__ double ilqr_rollout(const IlqrArgsOf<BOX>& a, long lo
         for (int j = 0; j < 4; ++j) {
             double v = raw[j];
             if (io.k) v += alpha * io.k[4 * ki + j];
-            if (Kk) {
-                double s = 0.0;
-#pragma unroll
-                for (int q = 0; q < NZ; ++q) s += Kk[j * NZ + q] * dz[q];
-                v += s;
-            }
+            if (Kk) v += lqr_feedback<NZ>([&](int q) { return Kk[j * NZ + q]; }, dz);
             u[j] = v;
         }
         if constexpr (BOX) {

@@ -2,8 +2,9 @@
 // (RAW), VelocityAviary (VEL, the embedded controller on QsState.pid) and CtrlAviary driven by a DSLPIDControl that tracks a
 // waypoint schedule (TRACK: the pid.py / downwash.py loop, computeControlFromEnv + step, inside the kernel).  Unlike qs_rollout there
 // is no action history: the state vector rows are written from registers through a small shared-memory stage, so this is a
-// translation unit of its own and leaves every rollout_kernel entry as it was.
+// translation unit of its own and leaves every rollout_kernel entry as it was.  QS_CTRL_LQR flies an iLQR plan with its LQR tracker.
 #include "qs_common.cuh"
+#include "lqr_law.cuh"
 #include "mrac_core.cuh"
 
 namespace qsi {
@@ -28,14 +29,21 @@ struct CtrlMracArgs : CtrlRolloutArgs {
     QsMracParams M;
     QsMracRolloutIO mio;
 };
+// QS_CTRL_LQR: the plan travels with the launch
+struct CtrlLqrArgs : CtrlRolloutArgs {
+    QsLqrRolloutIO lio;
+};
 template <int MODE> struct CtrlArgsOf { using type = CtrlRolloutArgs; };
 template <> struct CtrlArgsOf<QS_CTRL_MRAC> { using type = CtrlMracArgs; };
+template <> struct CtrlArgsOf<QS_CTRL_LQR> { using type = CtrlLqrArgs; };
 
 // MRAC: threads per CTA (each keeps its controller's 76 doubles in shared memory, [76][tpb]: 86 KB per CTA with the row stage)
 // and CTAs per SM.  64-thread CTAs (43 KB, up to 5 per SM) ran as fast within the spread on the H100 (DESIGN.md 4.1e).
 constexpr int kMracTPB = 128;
 constexpr int kMracMinBlocks = 2;
 constexpr size_t mrac_smem(int tpb) { return (size_t)tpb * QS_MRAC_STATE * 8; }
+// LQR: CTAs per SM (DESIGN.md 4.1e)
+constexpr int kLqrMinBlocks = 4;
 
 // the state stored back at the end of the rollout: the quaternion is already renormalised (round_to_planes after every tick), so
 // it is stored as it is -- store_drone would renormalise a second time and could move the last bit
@@ -69,8 +77,11 @@ __device__ __forceinline__ void const_target(const double* p, long long i, doubl
 // QS_CTRL_MRAC: the same loop with mrac_control in place of pid_control; the adaptive state (76 doubles per drone) cannot share the
 // register file with the drone, so it lives in dynamic shared memory as [76][tpb] (consecutive threads, consecutive words), loaded
 // once at the start and stored once at the end.
+// QS_CTRL_LQR: the RAW loop with the tracker's RPMs.  The plan stays in ilqr()'s layout, K [T][N][4][n_z] and z_nom [T][N][n_z]:
+// each drone reads its own contiguous span; the plane-major transpose ([T][4 n_z][N], coalesced per warp) was 17% slower with
+// DYN and 5-8% faster with all three effects on the H100 (DESIGN.md 4.1e).
 template <int EFF, int MODE, bool PHYS>
-__global__ void __launch_bounds__(kCtrlTPB, MODE == QS_CTRL_MRAC ? kMracMinBlocks : 4)
+__global__ void __launch_bounds__(kCtrlTPB, MODE == QS_CTRL_MRAC ? kMracMinBlocks : MODE == QS_CTRL_LQR ? kLqrMinBlocks : 4)
 ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const QsParams& P = a.P;
@@ -94,7 +105,7 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
     long long lj = -1, head0 = 0;                // the Logger ring: my entry column, the ring head before the first tick
     if (live) {
         load_drone(a.st.planes, N, i, d);
-        if ((EFF & QS_EFFECT_DRAG) && a.st.last_rpm) load_rpm(a.st.last_rpm, i, rpm_prev);
+        if (((EFF & QS_EFFECT_DRAG) || MODE == QS_CTRL_LQR) && a.st.last_rpm) load_rpm(a.st.last_rpm, i, rpm_prev);
         if (MODE == QS_CTRL_VEL) load_pid(a.st.pid, N, i, pst);
         if (MODE == QS_CTRL_TRACK) load_pid(io.pid_state, N, i, pst);
         if constexpr (MODE == QS_CTRL_MRAC) {
@@ -145,6 +156,38 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
                 const double mr = PHYS ? load_phys_rpm(a.st.phys, e).max_rpm : P.max_rpm;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) rpm[j] = qs::clampd(qs::clampd(rpm[j], 0.0, a.CP.max_rpm), 0.0, mr);
+            } else if constexpr (MODE == QS_CTRL_LQR) {
+                // u = rpm_nom + K (z - z_nom) (lqr_law.cuh), the optional box, then the env's clip as in RAW
+                const QsLqrRolloutIO& L = a.lio;
+                const int nz = L.n_z;
+                const long long p = (long long)L.tick0 + k;
+                const double* zn = L.z_nom + (p * N + i) * nz;
+                double dz[17];
+                const double x[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
+#pragma unroll
+                for (int q = 0; q < 13; ++q) dz[q] = x[q] - __ldg(zn + q);
+                if (nz == 17) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) dz[13 + j] = rpm_prev[j] - __ldg(zn + 13 + j);
+                }
+                const D4 un = ld256_nc(L.rpm_nom, p * N + i);
+                double u[4] = {un.x, un.y, un.z, un.w};
+                const double* Kp = L.K + (p * N + i) * 4 * nz;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const double* Kj = Kp + j * nz;
+                    u[j] += nz == 17 ? lqr_feedback<17>([&](int q) { return __ldg(Kj + q); }, dz)
+                                     : lqr_feedback<13>([&](int q) { return __ldg(Kj + q); }, dz);
+                }
+                if (L.lo) {
+                    const long long at = L.per_tick ? p * N + i : i;
+                    const D4 lo = ld256_nc(L.lo, at), hi = ld256_nc(L.hi, at);
+                    u[0] = qs::clampd(u[0], lo.x, hi.x); u[1] = qs::clampd(u[1], lo.y, hi.y);
+                    u[2] = qs::clampd(u[2], lo.z, hi.z); u[3] = qs::clampd(u[3], lo.w, hi.w);
+                }
+                const double mr = PHYS ? load_phys_rpm(a.st.phys, e).max_rpm : P.max_rpm;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) rpm[j] = qs::clampd(u[j], 0.0, mr);                       // CtrlAviary.py:140
             } else {
                 // MRAC.computeControlFromEnv (mrac_kernel on the planes): the tick's targets, ang_v rebuilt from the state, the
                 // controller's max_rpm clip, then the env's
@@ -291,14 +334,15 @@ int qs_sizeof_ctrl_rollout_io(void) { return (int)sizeof(QsCtrlRolloutIO); }
 }  // extern "C"
 
 namespace {
-// qs_ctrl_rollout (mio == NULL) and qs_ctrl_rollout_mrac (mode QS_CTRL_MRAC, mio != NULL)
-int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int mode, int n_envs,
-                 int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
+// qs_ctrl_rollout (mio == lio == NULL), qs_ctrl_rollout_mrac (mode QS_CTRL_MRAC, mio != NULL) and qs_ctrl_rollout_lqr (mode
+// QS_CTRL_LQR, lio != NULL)
+int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, const QsLqrRolloutIO* lio,
+                 int mode, int n_envs, int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
     if (!p || !io) return fail(QS_ERR_NULL, "qs_ctrl_rollout: NULL params/io");
     if (int rc = check_state(st, 0)) return rc;
     if (n_envs <= 0 || drones_per_env <= 0 || substeps <= 0 || io->T <= 0) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: n_envs, drones_per_env, substeps and T must be > 0");
     if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: n_envs * drones_per_env exceeds 2^31-1");
-    if (mio ? mode != QS_CTRL_MRAC : (mode != QS_CTRL_RAW && mode != QS_CTRL_VEL && mode != QS_CTRL_TRACK))
+    if (mio ? mode != QS_CTRL_MRAC : lio ? mode != QS_CTRL_LQR : (mode != QS_CTRL_RAW && mode != QS_CTRL_VEL && mode != QS_CTRL_TRACK))
         return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad mode (QS_CTRL_RAW, QS_CTRL_VEL or QS_CTRL_TRACK; QS_CTRL_MRAC is qs_ctrl_rollout_mrac)");
     if (effects & ~7u) return fail(QS_ERR_ENUM, "qs_ctrl_rollout: bad effects");
     const unsigned eff = effects & 7u;
@@ -323,6 +367,18 @@ int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io
         if (io->W <= 0) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: W (waypoint rows) must be > 0");
         if (io->M != 1 && (long long)io->M != (long long)n_envs * drones_per_env) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: M (waypoint columns) must be 1 or N");
         if (!(io->control_timestep > 0.0)) return fail(QS_ERR_SIZE, "qs_ctrl_rollout: control_timestep must be > 0");
+    } else if (mode == QS_CTRL_LQR) {
+        if (io->actions) return fail(QS_ERR_UNSUPPORTED, "qs_ctrl_rollout_lqr: takes a plan, not actions");
+        if (!lio->K || !lio->z_nom || !lio->rpm_nom) return fail(QS_ERR_NULL, "qs_ctrl_rollout_lqr: NULL K / z_nom / rpm_nom");
+        if (lio->n_z != 13 && lio->n_z != 17) return fail(QS_ERR_SIZE, "qs_ctrl_rollout_lqr: n_z must be 13 or 17");
+        if (lio->T_plan <= 0) return fail(QS_ERR_SIZE, "qs_ctrl_rollout_lqr: T_plan must be > 0");
+        if (lio->tick0 < 0 || (long long)lio->tick0 + io->T > lio->T_plan)
+            return fail(QS_ERR_SIZE, "qs_ctrl_rollout_lqr: the ticks [tick0, tick0 + T) must lie in the plan [0, T_plan)");
+        if (!lio->lo != !lio->hi) return fail(QS_ERR_NULL, "qs_ctrl_rollout_lqr: lo and hi are both given or both NULL");
+        if (lio->per_tick != 0 && lio->per_tick != 1) return fail(QS_ERR_SIZE, "qs_ctrl_rollout_lqr: per_tick must be 0 or 1");
+        if (!aligned32(lio->rpm_nom) || (lio->lo && (!aligned32(lio->lo) || !aligned32(lio->hi))))
+            return fail(QS_ERR_ALIGN, "qs_ctrl_rollout_lqr: rpm_nom, lo and hi must be 32-byte aligned");
+        if (lio->n_z == 17 && !st->last_rpm) return fail(QS_ERR_NULL, "qs_ctrl_rollout_lqr: an n_z = 17 plan needs QsState.last_rpm");
     } else {
         if (!io->actions) return fail(QS_ERR_NULL, "qs_ctrl_rollout: actions is NULL");
         if (f64 ? !aligned32(io->actions) : !aligned16(io->actions))
@@ -342,10 +398,13 @@ int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io
         a0.rg = r;
         a0.has_log = 1;
     }
-    CtrlMracArgs ma;                         // MRAC: the derived arguments, of which `a` is the base
-    CtrlRolloutArgs& a = mio ? static_cast<CtrlRolloutArgs&>(ma) : a0;
+    CtrlMracArgs ma;                         // MRAC / LQR: the derived arguments, of which `a` is the base
+    CtrlLqrArgs la;
+    CtrlRolloutArgs& a = mio ? static_cast<CtrlRolloutArgs&>(ma) : lio ? static_cast<CtrlRolloutArgs&>(la) : a0;
     memset(&ma, 0, sizeof(ma));
+    memset(&la, 0, sizeof(la));
     if (mio) { a = a0; ma.M = *mio->params; ma.mio = *mio; }
+    if (lio) { a = a0; la.lio = *lio; }
     a.P = *p;
     if (mode == QS_CTRL_TRACK) a.CP = *io->ctrl_params;
     a.st = *st; a.io = *io;
@@ -361,9 +420,9 @@ int ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io
     size_t sm = (size_t)a.tpb * 20 * 4 + ((eff & QS_EFFECT_DW) ? (size_t)a.tpb * 3 * 8 : 0);
     if (mode == QS_CTRL_MRAC) sm += mrac_smem(a.tpb);
     cudaStream_t s = (cudaStream_t)stream;
-    // eff is one of PolicyEffects and mode one of the four (both checked above)
+    // eff is one of PolicyEffects and mode one of the five (both checked above)
     with_int(PolicyEffects{}, (int)eff, [&](auto EFF) {
-        with_int(IntList<QS_CTRL_RAW, QS_CTRL_VEL, QS_CTRL_TRACK, QS_CTRL_MRAC>{}, mode, [&](auto MODE) {
+        with_int(IntList<QS_CTRL_RAW, QS_CTRL_VEL, QS_CTRL_TRACK, QS_CTRL_MRAC, QS_CTRL_LQR>{}, mode, [&](auto MODE) {
             with_bool(st->phys != nullptr, [&](auto PHYS) {
                 using Args = typename CtrlArgsOf<decltype(MODE)::value>::type;
                 void (*k)(Args) = ctrl_rollout_kernel<decltype(EFF)::value, decltype(MODE)::value, decltype(PHYS)::value>;
@@ -386,7 +445,7 @@ extern "C" {
 
 int qs_ctrl_rollout(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, int mode, int n_envs, int drones_per_env,
                     int substeps, unsigned effects, unsigned flags, void* stream) {
-    return ctrl_rollout(p, st, io, nullptr, mode, n_envs, drones_per_env, substeps, effects, flags, stream);
+    return ctrl_rollout(p, st, io, nullptr, nullptr, mode, n_envs, drones_per_env, substeps, effects, flags, stream);
 }
 
 int qs_sizeof_mrac_rollout_io(void) { return (int)sizeof(QsMracRolloutIO); }
@@ -394,7 +453,15 @@ int qs_sizeof_mrac_rollout_io(void) { return (int)sizeof(QsMracRolloutIO); }
 int qs_ctrl_rollout_mrac(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int n_envs,
                          int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
     if (!mio) return fail(QS_ERR_NULL, "qs_ctrl_rollout_mrac: NULL mio");
-    return ctrl_rollout(p, st, io, mio, QS_CTRL_MRAC, n_envs, drones_per_env, substeps, effects, flags, stream);
+    return ctrl_rollout(p, st, io, mio, nullptr, QS_CTRL_MRAC, n_envs, drones_per_env, substeps, effects, flags, stream);
+}
+
+int qs_sizeof_lqr_rollout_io(void) { return (int)sizeof(QsLqrRolloutIO); }
+
+int qs_ctrl_rollout_lqr(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsLqrRolloutIO* lio, int n_envs,
+                        int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream) {
+    if (!lio) return fail(QS_ERR_NULL, "qs_ctrl_rollout_lqr: NULL lio");
+    return ctrl_rollout(p, st, io, nullptr, lio, QS_CTRL_LQR, n_envs, drones_per_env, substeps, effects, flags, stream);
 }
 
 }  // extern "C"

@@ -725,8 +725,13 @@ class BaseAviary(Env):
           pos, quat, vel, rpy_rates [T, E, D, k]  the final nominal trajectory, bit for bit differentiable_rollout(rpm=rpm)
           rpm        [T, E, D, 4]
           K          [T, E, D, 4, n_z], k [T, E, D, 4]  the feedback and feed-forward gains of a backward pass at the returned
-                     trajectory: u_k = rpm[k] + k_k + K_k (z_k - z_nom,k) is its time-varying LQR tracker, z_k the state
-                     before tick k (n_z = 13), with drag followed by the clipped RPMs of tick k - 1 (n_z = 17)
+                     trajectory.  Its time-varying LQR tracker is u_k = rpm[k] + K_k (z_k - z[k]) (clamped to the box with
+                     rpm_bounds); rpm[k] + k_k + K_k (z_k - z[k]) is the next iteration's full step.  ilqr.Tracker(sol) flies
+                     it in CtrlAviary.rollout()
+          z          [T, E, D, n_z] float64  the loop state the gains act on, z_nom: the nominal state before tick k in the
+                     order px py pz qx qy qz qw vx vy vz wx wy wz (tick 0 the solve's start, tick k >= 1 the returned state
+                     k - 1), with drag (n_z = 17) followed by clip(rpm[k - 1], 0, MAX_RPM of the drone's row), the solve's
+                     last_rpm at tick 0
           cost       [iters + 1, E, D]  J per iteration, row 0 the initial guess (non-increasing)
           mu         [E, D]  the final regularisation
           converged  [E, D]  bool: an accepted step decreased J by less than 1e-9 relative; the drone stopped there
@@ -831,7 +836,8 @@ class BaseAviary(Env):
                       target_rpy=None, target_vel=None, target_rpy_rates=None, control_timestep=None, record=True, errors=False,
                       out=None, log_targets=False):
         """rollout() of the state-vector envs (CtrlAviary, VelocityAviary): one qs_ctrl_rollout launch of T ticks in `mode`
-        (N.CTRL_RAW / CTRL_VEL / CTRL_TRACK), or of qs_ctrl_rollout_mrac (N.CTRL_MRAC); see CtrlAviary.rollout."""
+        (N.CTRL_RAW / CTRL_VEL / CTRL_TRACK), or of qs_ctrl_rollout_mrac (N.CTRL_MRAC) or qs_ctrl_rollout_lqr (N.CTRL_LQR, an
+        ilqr.Tracker); see CtrlAviary.rollout."""
         if not self.VECTORIZED:
             raise ValueError("rollout() needs the vector API (num_envs=...)")
         if self._py_hooks:
@@ -855,8 +861,26 @@ class BaseAviary(Env):
             t = t.reshape(n, 3).contiguous()
             keep.append(t)
             return t.data_ptr()
-        mio = None
-        if mode in (N.CTRL_TRACK, N.CTRL_MRAC):
+        mio = lio = None
+        if mode == N.CTRL_LQR:
+            if actions is not None:
+                raise ValueError("pass either actions or a controller")
+            trk = controller
+            if trk.env_shape != (E, D):
+                raise ValueError("the Tracker's plan is for %d x %d drones, the env has %d x %d" % (*trk.env_shape, E, D))
+            if trk.device != dev:
+                raise ValueError("the Tracker's plan is on %s, the env's state on %s" % (trk.device, dev))
+            if isinstance(trk.tick, bool) or not isinstance(trk.tick, int) or trk.tick < 0:
+                raise ValueError("Tracker.tick must be an integer >= 0, got %r" % (trk.tick,))
+            T = trk.T - trk.tick if num_steps is None else int(num_steps)
+            if T <= 0 or trk.tick + T > trk.T:
+                raise ValueError("the Tracker's plan has %d ticks: ticks [%d, %d) do not fit" % (trk.T, trk.tick, trk.tick + T))
+            if self._order is not None:
+                raise ValueError("a Tracker indexes drones by id: not available on a formation reordered by reorder_by_morton()")
+            if trk.nz == 17 and not self._track_last_action:
+                raise ValueError("an n_z = 17 plan (solved with drag) needs the env's last_clipped_action, which this env does not keep")
+            lio = trk._io(trk.tick)
+        elif mode in (N.CTRL_TRACK, N.CTRL_MRAC):
             if actions is not None:
                 raise ValueError("pass either actions or a controller")
             if controller is None:
@@ -952,12 +976,17 @@ class BaseAviary(Env):
             if mio is not None:
                 rc = self._lib.qs_ctrl_rollout_mrac(C.byref(self._P), C.byref(self._st), C.byref(io), C.byref(mio), E, D,
                                                     self.PYB_STEPS_PER_CTRL, self._effects, flags, self._stream())
+            elif lio is not None:
+                rc = self._lib.qs_ctrl_rollout_lqr(C.byref(self._P), C.byref(self._st), C.byref(io), C.byref(lio), E, D,
+                                                   self.PYB_STEPS_PER_CTRL, self._effects, flags, self._stream())
             else:
                 rc = self._lib.qs_ctrl_rollout(C.byref(self._P), C.byref(self._st), C.byref(io), mode, E, D, self.PYB_STEPS_PER_CTRL,
                                                self._effects, flags, self._stream())
-        N.check(rc, "qs_ctrl_rollout" if mio is None else "qs_ctrl_rollout_mrac")
+        N.check(rc, "qs_ctrl_rollout_mrac" if mio is not None else "qs_ctrl_rollout_lqr" if lio is not None else "qs_ctrl_rollout")
         self._cur = tgt
-        if controller is not None:
+        if lio is not None:
+            controller.tick += T
+        elif controller is not None:
             controller.control_counter += T
         return res
 

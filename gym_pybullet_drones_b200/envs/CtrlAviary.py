@@ -76,8 +76,23 @@ class CtrlAviary(BaseAviary):
           reference model Xm when `controller.control_counter` is 0.  With `errors=True` the result holds `pos_e` and `rpy_e`
           [T, E, D, 3] (float32) instead of `yaw_e`.
 
+        * `controller`: an `ilqr.Tracker(sol)` of a solution of `ilqr()` on this env's E x D drones: T ticks of the plan's LQR
+          tracker (see Tracker), from plan tick `controller.tick`, which then advances by T.  `num_steps` defaults to the ticks
+          left in the plan.  `record`, `out` and the result are those of `actions`; the schedule arguments, `errors=True` and
+          `log_targets=True` are refused.  Refused too (ValueError): another E, D or device than the plan's, a negative tick, a
+          tick range past the plan's end, and an n_z = 17 plan (planned with drag) on an env that keeps no last_clipped_action.
+          Indices are drone ids: a formation reordered by reorder_by_morton() is refused (its storage order is not the plan's;
+          such a formation has more than 128 downwash drones per aviary, which rollout() refuses in any mode).
+
         What the kernel refuses (downwash with more than 128 drones per aviary, a controller of the wrong size or device, both
         actions and a controller, the single-env API, external downwash) raises ValueError."""
+        from ..ilqr import Tracker
+        if isinstance(controller, Tracker):
+            if any(x is not None for x in (waypoints, start, offset, target_rpy, target_vel, target_rpy_rates, control_timestep)):
+                raise ValueError("a Tracker flies its plan: it takes no waypoints, start, offset, targets or control_timestep")
+            if errors or log_targets:
+                raise ValueError("a Tracker has no targets: errors=True and log_targets=True are for DSLPIDControl and MRAC")
+            return self._ctrl_rollout(N.CTRL_LQR, actions=actions, controller=controller, num_steps=num_steps, record=record, out=out)
         if controller is not None or actions is None:
             from ..control.MRAC import MRAC
             mode = N.CTRL_MRAC if isinstance(controller, MRAC) else N.CTRL_TRACK

@@ -2,7 +2,7 @@
 independent problem per drone, on the per-tick Jacobians of qs_dyn_tick_jac and the kernels qs_ilqr_backward,
 qs_ilqr_line_search and qs_ilqr_commit (include/quadsim.h), or with rpm_bounds their control-limited variants qs_ilqr_box_*.
 BaseAviary.ilqr is the public entry point; Problem holds one solve's device buffers and runs its steps, so that each step can
-also be called on its own."""
+also be called on its own.  Tracker flies a solution's LQR tracker in CtrlAviary.rollout() (qs_ctrl_rollout_lqr)."""
 import ctypes as C
 
 import torch
@@ -71,6 +71,11 @@ def _rpm_box(rpm_bounds, rows, T, E, D, dev):
     lo, hi = lo.detach().contiguous(), hi.detach().contiguous()
     ok = ~(torch.isnan(lo).any() | torch.isnan(hi).any()) & (lo <= hi).all() & (lo >= 0).all() & (hi <= max_rpm).all()
     return lo, hi, per_tick, ok
+
+
+def _clampd(v, lo, hi):
+    """qs::clampd elementwise: v < lo ? lo : (v > hi ? hi : v)"""
+    return torch.where(v < lo, lo, torch.where(v > hi, hi, v))
 
 
 def _weight(x, name, default, E, dev):
@@ -234,6 +239,7 @@ class Problem:
         out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(self.states, n).items()}
         out["rpm"] = self.rpm.view(T, E, D, 4)
         out["K"] = self.K.view(T, E, D, 4, self.nz)
+        out["z"] = self.loop_states().view(T, E, D, self.nz)
         out["k"] = self.k.view(T, E, D, 4)
         out["cost"] = cost.view(cost.shape[0], E, D)
         out["mu"] = self.mu.view(E, D)
@@ -241,6 +247,19 @@ class Problem:
         if self.active is not None:
             out["active"] = self.active.view(T, E, D, 4)
         return out
+
+
+    def loop_states(self):
+        """z_nom [T, N, n_z]: the state before each tick in drone_vec's order (px py pz qx qy qz qw vx vy vz wx wy wz), tick 0 the
+        start, and with drag the clipped RPMs of the tick before (last_rpm at tick 0): what the rollouts difference against"""
+        T, n = self.T, self.n
+        x = unpack_states(torch.cat([self.planes0.view(1, -1), self.states[:-1]]), n)
+        z = [x[k] for k, _ in STATE_KEYS]
+        if self.nz == 17:
+            E, D = self.env_shape
+            mr = self.rows[:, 13].reshape(E, 1, 1).expand(E, D, 4).reshape(1, n, 4)
+            z.append(torch.cat([self.last_rpm.view(1, n, 4), _clampd(self.rpm[:-1], torch.zeros_like(mr), mr)]))
+        return torch.cat(z, dim=-1)
 
 
 def solve(p, iters):
@@ -270,3 +289,81 @@ def ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rp
     p = Problem(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, state=state, last_rpm=last_rpm,
                 phys=phys, rpm_bounds=rpm_bounds)
     return solve(p, iters)
+
+
+class Tracker:
+    """The time-varying LQR tracker of an ilqr() solution, flown by CtrlAviary.rollout(controller=Tracker(sol)) in one launch
+    (qs_ctrl_rollout_lqr, DESIGN.md 4.1e).  Plan tick p of drone i applies
+        u = rpm[p] + K[p] (z - z[p]),   then clamp(u, lo[p], hi[p]) with rpm_bounds,   then the env's clip to [0, MAX_RPM]
+    where z is the drone's state before the tick in drone_vec's order, with n_z = 17 followed by the RPMs the env applied at the tick
+    before (its last_clipped_action), and z[p], rpm[p], K[p] are sol's.  From the solve's own start, on the plant it planned on,
+    every tick reproduces sol's trajectory bit for bit (z - z[p] = 0).  The plant may differ from the plan: any Physics mode
+    (downwash up to 128 drones per aviary) and any set_physical_params table; the tracker runs the plan's n_z whatever the
+    plant's effects.  The result of ilqr() does not record the control rate: flying a plan at a rate other than the env's
+    CTRL_FREQ it was solved at is the caller's error and is not detected.
+
+    sol: the result of BaseAviary.ilqr (its rpm, K and z; float64 CUDA tensors of one device).  The plan is copied once (ilqr's
+    layout is the kernel's), so later changes to sol do not reach the tracker.  rpm_bounds: None (default) or "motor" (the env's own
+    clip only), or the pair (lo, hi) the plan was solved with, each [4], [E, D, 4] or [T, E, D, 4] float64 on sol's device
+    (NaN or lo > hi raise ValueError).
+
+    tick: the plan tick of the next rollout's first tick, 0 at construction.  Each rollout of R ticks advances it by R, so calls
+    of R and T - R ticks fly the plan as one call of T ticks, bit for bit; the caller may set it.
+
+    sol's K is the gain of the solve's last backward pass at each drone's final regularisation: K = -(Quu + mu diag(Quu))^-1 Qux,
+    about 1 / (1 + mu) of the unregularised gain.  A drone whose last steps were rejected ends with a large mu (1e3 to 1e5 is
+    common after 30 iterations) and its tracker barely acts.  To fly with the unregularised gains at the returned trajectory,
+    solve through Problem and recompute them at mu = 0 (Quu is positive definite for R > 0):
+        p = Problem(env, target, ...); sol = solve(p, iters); p.mu.zero_(); p.backward(); sol = p.result(sol["cost"])
+
+    Gains are not screened on the device (that would synchronise every call).  For a drone whose last backward pass failed
+    (an exhausted restart ladder, e.g. mu = +inf), K at tick t holds the gains of the last attempt that factorised tick t: the
+    pass runs from tick T - 1 down and every attempt, the failing ones included, writes the ticks above the one where its
+    factorisation failed, at its own (largest) mu.  A tick that no attempt of any pass reached holds 0 (sol's K starts at zero);
+    with mu = +inf no attempt factorises any tick, so K is what earlier passes left.  The tracker applies those gains as they
+    are.  A non-finite gain gives a NaN command, which the clip does not
+    remove: that drone's state becomes NaN, the others are unaffected."""
+
+    def __init__(self, sol, rpm_bounds=None):
+        if not isinstance(sol, dict) or not all(isinstance(sol.get(k), torch.Tensor) for k in ("rpm", "K", "z")):
+            raise ValueError("Tracker(sol): sol must be the result of ilqr(), with tensors rpm, K and z")
+        rpm, K, z = sol["rpm"], sol["K"], sol["z"]
+        if rpm.dim() != 4 or rpm.shape[-1] != 4 or rpm.shape[0] <= 0 or not rpm.is_cuda:
+            raise ValueError("Tracker(sol): sol['rpm'] must be a [T, E, D, 4] float64 CUDA tensor")
+        T, E, D = rpm.shape[:3]
+        dev = rpm.device
+        nz = K.shape[-1] if K.dim() == 5 else -1
+        if nz not in (13, 17):
+            raise ValueError("Tracker(sol): sol['K'] must be [%d, %d, %d, 4, n_z] with n_z 13 or 17" % (T, E, D))
+        _tensor(rpm, "sol['rpm']", (T, E, D, 4), dev)
+        _tensor(K, "sol['K']", (T, E, D, 4, nz), dev)
+        _tensor(z, "sol['z']", (T, E, D, nz), dev)
+        n = E * D
+        with torch.no_grad():
+            # owned, C-contiguous copies whatever sol's strides (clone alone keeps a permuted tensor's strides)
+            dense = dict(memory_format=torch.contiguous_format)
+            self.K = K.detach().reshape(T, n, 4, nz).clone(**dense)                     # [T][N][4][n_z]
+            self.z_nom = z.detach().reshape(T, n, nz).clone(**dense)                    # [T][N][n_z]
+            self.rpm_nom = rpm.detach().reshape(T, n, 4).clone(**dense)                 # [T][N][4]: one 32-byte load per drone
+            self.box = None
+            if not (rpm_bounds is None or (isinstance(rpm_bounds, str) and rpm_bounds == "motor")):
+                if not isinstance(rpm_bounds, (tuple, list)) or len(rpm_bounds) != 2:
+                    raise ValueError("rpm_bounds must be None, 'motor' or a pair (lo, hi) of float64 CUDA tensors in raw RPM")
+                lo, lo_t = _bound(rpm_bounds[0], "rpm_bounds[0] (lo)", T, E, D, dev)
+                hi, hi_t = _bound(rpm_bounds[1], "rpm_bounds[1] (hi)", T, E, D, dev)
+                per_tick = lo_t or hi_t
+                if per_tick:
+                    lo, hi = lo.expand(T, n, 4), hi.expand(T, n, 4)
+                lo, hi = lo.detach().clone().contiguous(), hi.detach().clone().contiguous()      # owned, 32-byte aligned
+                if not bool((~(torch.isnan(lo).any() | torch.isnan(hi).any()) & (lo <= hi).all()).item()):
+                    raise ValueError("Tracker: rpm_bounds must not be NaN and must satisfy lo <= hi")
+                self.box = (lo, hi, per_tick)
+        self.T, self.env_shape, self.nz, self.device = T, (E, D), nz, dev
+        self.tick = 0
+
+    def _io(self, tick):
+        """The QsLqrRolloutIO of a launch from plan tick `tick`"""
+        lo, hi, per_tick = self.box if self.box is not None else (None, None, False)
+        return N.QsLqrRolloutIO(K=self.K.data_ptr(), z_nom=self.z_nom.data_ptr(), rpm_nom=self.rpm_nom.data_ptr(),
+                                lo=None if lo is None else lo.data_ptr(), hi=None if hi is None else hi.data_ptr(),
+                                per_tick=int(per_tick), n_z=self.nz, T_plan=self.T, tick0=tick)

@@ -605,6 +605,32 @@ int qs_sizeof_mrac_rollout_io(void);
 int qs_ctrl_rollout_mrac(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsMracRolloutIO* mio, int n_envs,
                          int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
 
+/* qs_ctrl_rollout with the time-varying LQR tracker of an iLQR plan in the loop (mode QS_CTRL_LQR, DESIGN.md 4.1e): io->T ticks
+ * from plan tick tick0.  Tick k of the launch (plan tick p = tick0 + k), drone i:
+ *   dz   = (x - z_nom[p][0:13], and with n_z = 17 rpm_prev - z_nom[p][13:17]), x the float64 state in drone_vec's order
+ *          (px py pz qx qy qz qw vx vy vz wx wy wz), rpm_prev the applied RPMs of the tick before (QsState.last_rpm at k = 0);
+ *   u_j  = rpm_nom[p][i][j] + s_j,  s_j = sum_{q=0}^{n_z-1} K[p][j][q] dz_q summed in that order from 0.0 (qs_ilqr_line_search's
+ *          feedback term, without the feed-forward);
+ *   with lo / hi: u_j = min(max(u_j, lo_j), hi_j) (qs::clampd); then the env's clip to [0, MAX_RPM of the aviary's row] and the
+ *   substeps of qs_dyn_substeps(QS_FLAG_ACTION_F64) for any effect set qs_ctrl_rollout accepts.
+ * QsCtrlRolloutIO.actions must be NULL; T, obs, rpm, obs_last, log and log_controls act as for QS_CTRL_RAW, and so do the env
+ * state, last_rpm and the step counters.  Non-finite gains are not screened: they reach the RPMs and the clip. */
+enum { QS_CTRL_LQR = 4 };
+typedef struct QsLqrRolloutIO {
+    const double* K;                /* [T_plan][N][4][n_z] (ilqr's layout) */
+    const double* z_nom;            /* [T_plan][N][n_z] the nominal loop state before each tick */
+    const double* rpm_nom;          /* [T_plan][N][4] the nominal raw commands (32-byte aligned) */
+    const double* lo;               /* [N][4], or [T_plan][N][4] with per_tick (32-byte aligned); nullable together with hi */
+    const double* hi;
+    int per_tick;                   /* 0 or 1 */
+    int n_z;                        /* 13, or 17 (the plan's loop state carries the previous clipped RPMs: needs QsState.last_rpm) */
+    int T_plan;                     /* ticks of the plan, > 0 */
+    int tick0;                      /* the plan tick of this launch's tick 0: 0 <= tick0, tick0 + T <= T_plan */
+} QsLqrRolloutIO;
+int qs_sizeof_lqr_rollout_io(void);
+int qs_ctrl_rollout_lqr(const QsParams* p, const QsState* st, const QsCtrlRolloutIO* io, const QsLqrRolloutIO* lio, int n_envs,
+                        int drones_per_env, int substeps, unsigned effects, unsigned flags, void* stream);
+
 /* Differentiable raw-RPM trajectories (DESIGN.md 4.5): T control ticks of Physics.DYN (+ GND and/or DRAG, no downwash) from a
  * given state, and the reverse-mode product (VJP) of that trajectory with cotangents of its T states.  The env is not touched:
  * every input and output is a caller-owned float64 device array.  A "state" is 13 N doubles in QsState.planes' layout
