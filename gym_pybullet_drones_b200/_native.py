@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
-                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu")]
+                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu")]
 HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "lqr_law.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
@@ -151,6 +151,12 @@ class QsDynTrajIO(C.Structure):
         "state0", "rpm", "last_rpm", "phys", "states", "g_states", "g_rpm", "g_state0", "g_last_rpm", "g_phys", "scratch")]
 
 
+class QsDynLqrTrajIO(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("T", "n_z", "T_plan", "tick0", "per_tick", "pad_")] + [(n, C.c_void_p) for n in (
+        "state0", "last_rpm", "phys", "K", "z_nom", "rpm_nom", "lo", "hi", "states", "rpm", "g_states", "g_rpm", "g_state0",
+        "g_last_rpm", "g_phys", "g_K", "g_z_nom", "g_rpm_nom", "scratch")]
+
+
 class QsDynTrajJvpIO(C.Structure):
     _fields_ = [("T", C.c_int), ("pad_", C.c_int)] + [(n, C.c_void_p) for n in (
         "state0", "rpm", "last_rpm", "phys", "states", "t_state0", "t_rpm", "t_last_rpm", "t_phys", "t_states", "jac")]
@@ -214,7 +220,7 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_sizeof_dyn_ctrl_traj_jvp_io", "qs_dyn_policy_traj_jvp", "qs_dyn_policy_tick_jac", "qs_sizeof_dyn_policy_traj_jvp_io",
            "qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit", "qs_sizeof_ilqr_io", "qs_ilqr_box_backward",
            "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io", "qs_ctrl_rollout_lqr",
-           "qs_sizeof_lqr_rollout_io"]
+           "qs_sizeof_lqr_rollout_io", "qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp", "qs_sizeof_dyn_lqr_traj_io"]
 MAX_PEERS = 16
 
 
@@ -313,6 +319,10 @@ def lib():
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
     L.qs_sizeof_dyn_traj_io.restype = C.c_int
+    for n in ("qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynLqrTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
+    L.qs_sizeof_dyn_lqr_traj_io.restype = C.c_int
     for n in ("qs_dyn_traj_jvp", "qs_dyn_tick_jac"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajJvpIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
@@ -409,8 +419,8 @@ def lib():
                           "dyn policy traj jvp io): rebuild")
     if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO) or L.qs_sizeof_ilqr_box_io() != C.sizeof(QsIlqrBoxIO):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io / ilqr box io): rebuild")
-    if L.qs_sizeof_lqr_rollout_io() != C.sizeof(QsLqrRolloutIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (lqr rollout io): rebuild")
+    if L.qs_sizeof_lqr_rollout_io() != C.sizeof(QsLqrRolloutIO) or L.qs_sizeof_dyn_lqr_traj_io() != C.sizeof(QsDynLqrTrajIO):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (lqr rollout io / dyn lqr traj io): rebuild")
     _lib = L
     return L
 

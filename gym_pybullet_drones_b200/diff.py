@@ -1,6 +1,6 @@
 """Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs),
-qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop) and qs_dyn_policy_traj / qs_dyn_policy_traj_vjp (an
-MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5), and their forward mode: the jvp of each Function (qs_dyn_traj_jvp,
+qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop), qs_dyn_lqr_traj / qs_dyn_lqr_traj_vjp (an iLQR plan's
+LQR tracker in the loop) and qs_dyn_policy_traj / qs_dyn_policy_traj_vjp (an MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5), and their forward mode: the jvp of each Function (qs_dyn_traj_jvp,
 qs_dyn_ctrl_traj_jvp, qs_dyn_policy_traj_jvp) and the per-tick Jacobians of linearise (qs_dyn_tick_jac, qs_dyn_ctrl_tick_jac,
 qs_dyn_policy_tick_jac).
 BaseAviary.differentiable_rollout is the public entry point; this module packs the state into the kernels' planes layout, runs
@@ -192,6 +192,114 @@ class DynCtrlTrajectory(torch.autograd.Function):
         g = grads
         return (g["g_state0"], g["g_pid0"], g["g_target_pos"], g["g_target_vel"], g["g_target_rpy"], g["g_target_rpy_rates"],
                 g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), g["g_gains"].view(E, D, 18).sum(dim=1), None)
+
+
+LQR_INS = ("state0", "last_rpm", "phys", "rpm_nom", "K", "z_nom")
+PLAN_KEYS = ("rpm", "K", "z")                                                          # plan= keys, in sol's names
+
+
+class DynLqrTrajectory(torch.autograd.Function):
+    """(states [T, 13 N], rpm [T, N, 4]) = the T ticks of qs_dyn_lqr_traj from planes0 [13 N], with last_rpm [N, 4], the
+    per-aviary rows [E, 16] and the plan rpm_nom [T_plan, N, 4], K [T_plan, N, 4, n_z], z_nom [T_plan, N, n_z], flown from plan
+    tick tick0; backward = qs_dyn_lqr_traj_vjp, its per-drone row gradients summed over each aviary's drones (torch,
+    deterministic), the plan's gradients zero on the ticks not flown.  `cfg` = (QsParams, E, D, substeps, effects, tick0, box),
+    box = (lo, hi, per_tick) of the tracker (constants) or None.  The inputs may have any strides (the kernels get contiguous
+    copies).  Double backward and forward mode (dual tensors) raise ValueError: the tracker loop has reverse mode only."""
+
+    @staticmethod
+    def _lqr_io(cfg, T, ptrs):
+        """The QsDynLqrTrajIO of T ticks with the tensors of `ptrs` and the tracker's box"""
+        P, E, D, S, eff, tick0, box = cfg
+        lo, hi, per_tick = box if box is not None else (None, None, False)
+        K = ptrs["K"]
+        return _io(N.QsDynLqrTrajIO, T, dict(ptrs, lo=lo, hi=hi), n_z=K.shape[-1], T_plan=K.shape[0], tick0=tick0,
+                   per_tick=int(per_tick))
+
+    @staticmethod
+    def forward(ctx, planes0, last_rpm, rows, rpm_nom, K, z_nom, cfg, T):
+        ins = dict(zip(LQR_INS, (x.contiguous() for x in (planes0, last_rpm, rows, rpm_nom, K, z_nom))))
+        if ins["rpm_nom"].data_ptr() % 32:                  # the kernel reads a drone's 4 nominal RPMs as one 32-byte access
+            ins["rpm_nom"] = ins["rpm_nom"].clone()
+        P, E, D, S, eff, tick0, box = cfg
+        n = E * D
+        f64 = dict(dtype=torch.float64, device=planes0.device)
+        outs = dict(states=torch.empty((T, 13 * n), **f64), rpm=torch.empty((T, n, 4), **f64))
+        _call("qs_dyn_lqr_traj", C.byref(P), C.byref(DynLqrTrajectory._lqr_io(cfg, T, dict(ins, **outs))), E, D, S, eff,
+              device=planes0.device)
+        ctx.save_for_backward(*ins.values(), *outs.values())
+        ctx.cfg = cfg
+        return outs["states"], outs["rpm"]
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise ValueError("differentiable_rollout(controller=Tracker): the tracker loop has reverse mode only; forward-mode "
+                         "(dual tensor) derivatives are not implemented for it")
+
+    @staticmethod
+    def backward(ctx, g_states, g_rpm):
+        _no_double_backward()
+        saved = ctx.saved_tensors
+        ins = dict(zip(LQR_INS, saved[:6]))
+        outs = dict(zip(("states", "rpm"), saved[6:]))
+        P, E, D, S, eff, tick0, box = ctx.cfg
+        T, n = outs["rpm"].shape[0], E * D
+        f64 = dict(dtype=torch.float64, device=outs["rpm"].device)
+        grads = dict(g_state0=torch.empty((13 * n,), **f64), g_last_rpm=torch.empty((n, 4), **f64), g_phys=torch.empty((n, 16), **f64),
+                     g_rpm_nom=torch.zeros_like(ins["rpm_nom"]) if ctx.needs_input_grad[3] else None,
+                     g_K=torch.zeros_like(ins["K"]) if ctx.needs_input_grad[4] else None,
+                     g_z_nom=torch.zeros_like(ins["z_nom"]) if ctx.needs_input_grad[5] else None)
+        ptrs = dict(ins, **outs, **grads, g_states=g_states.to(torch.float64).contiguous(),
+                    g_rpm=None if g_rpm is None else g_rpm.to(torch.float64).contiguous(), scratch=torch.empty((S, 13, n), **f64))
+        _call("qs_dyn_lqr_traj_vjp", C.byref(P), C.byref(DynLqrTrajectory._lqr_io(ctx.cfg, T, ptrs)), E, D, S, eff, device=outs["rpm"].device)
+        g = grads
+        return (g["g_state0"], g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), g["g_rpm_nom"], g["g_K"], g["g_z_nom"], None,
+                None)
+
+
+def _tracker_inputs(env, trk, plan, state, last_rpm, phys, num_steps=None, **schedule):
+    """The checked arguments of differentiable_rollout(controller=Tracker, plan=): (cfg, T, inputs), inputs = (planes0,
+    last_rpm, rows, rpm_nom, K, z_nom) as DynLqrTrajectory takes them."""
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    given = sorted(k for k, v in schedule.items() if v is not None)
+    if given:
+        raise ValueError("a Tracker flies its plan: %s do not apply (no waypoints, start, offset, targets, gains, pid_state or "
+                         "control_timestep)" % ", ".join(given))
+    if trk.env_shape != (E, D):
+        raise ValueError("the Tracker's plan is for %d x %d drones, the env has %d x %d" % (*trk.env_shape, E, D))
+    if trk.device != dev:
+        raise ValueError("the Tracker's plan is on %s, the env's state on %s" % (trk.device, dev))
+    if isinstance(trk.tick, bool) or not isinstance(trk.tick, int) or trk.tick < 0:
+        raise ValueError("Tracker.tick must be an integer >= 0, got %r" % (trk.tick,))
+    T = trk.T - trk.tick if num_steps is None else int(num_steps)
+    if T <= 0:
+        raise ValueError("num_steps must be > 0")
+    if trk.tick + T > trk.T:
+        raise ValueError("the Tracker's plan has %d ticks: ticks [%d, %d) do not fit" % (trk.T, trk.tick, trk.tick + T))
+    if env._order is not None:
+        raise ValueError("a Tracker indexes drones by id: not available on a formation reordered by reorder_by_morton()")
+    if trk.nz == 17 and last_rpm is None and not env._track_last_action:
+        raise ValueError("an n_z = 17 plan (solved with drag) needs the RPMs applied before tick 0: pass last_rpm= (this env does "
+                         "not keep last_clipped_action)")
+    plan = dict(plan or {})
+    bad = set(plan) - set(PLAN_KEYS)
+    if bad:
+        raise ValueError("unknown plan keys %s (expected some of rpm, K, z)" % sorted(bad))
+    shapes = dict(rpm=(trk.T, E, D, 4), K=(trk.T, E, D, 4, trk.nz), z=(trk.T, E, D, trk.nz))
+    own = dict(rpm=trk.rpm_nom, K=trk.K, z=trk.z_nom)
+    tens = [_tensor(plan[k], "plan[%r]" % k, shapes[k], dev).reshape(own[k].shape) if k in plan else own[k] for k in PLAN_KEYS]
+    planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
+    cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects, trk.tick, trk.box)
+    return cfg, T, (planes0, last_rpm, rows, *tens)
+
+
+def _tracker_loop(env, trk, plan, state, last_rpm, phys, **schedule):
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    cfg, T, ins = _tracker_inputs(env, trk, plan, state, last_rpm, phys, **schedule)
+    with torch.cuda.device(dev):
+        states, rpm = DynLqrTrajectory.apply(*ins, cfg, T)
+    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out["rpm"] = rpm.reshape(T, E, D, 4)
+    return out
 
 
 def actor64(params, activation, obs, noise=None):
@@ -402,12 +510,17 @@ def _rpm_ticks(env, rpm):
 
 
 def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
-                           action_buffer=None, **schedule):
+                           action_buffer=None, plan=None, **schedule):
     """BaseAviary.differentiable_rollout (see there)."""
+    from .ilqr import Tracker
     _refuse_downwash(env, "differentiable_rollout()", "adjoint")
     if (rpm is not None) + (controller is not None) + (policy is not None) != 1:
         raise ValueError("differentiable_rollout() takes exactly one of rpm [T, E, D, 4] (open loop), controller= (closed loop) or "
                          "policy= (an MlpPolicy in the loop)")
+    if plan is not None and not isinstance(controller, Tracker):
+        raise ValueError("plan= is the plan of a tracker loop: it needs controller=ilqr.Tracker(sol), got %s"
+                         % ("controller=%s" % type(controller).__name__ if controller is not None else
+                            "policy=" if policy is not None else "rpm="))
     if policy is not None:
         given = sorted(k for k, v in schedule.items() if v is not None and k != "num_steps")
         if given:
@@ -416,6 +529,8 @@ def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=
     given = sorted(k for k, v in (("params", params), ("noise", noise), ("action_buffer", action_buffer)) if v is not None)
     if given:
         raise ValueError("%s apply to a policy rollout only" % ", ".join(given))
+    if isinstance(controller, Tracker):
+        return _tracker_loop(env, controller, plan, state, last_rpm, phys, **schedule)
     if controller is not None:
         return _closed_loop(env, controller, state, last_rpm, phys, **schedule)
     given = sorted(k for k, v in schedule.items() if v is not None)

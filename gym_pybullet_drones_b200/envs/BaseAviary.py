@@ -556,7 +556,7 @@ class BaseAviary(Env):
     def differentiable_rollout(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None,
                                target_vel=None, target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None,
                                pid_state=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
-                               action_buffer=None):
+                               action_buffer=None, plan=None):
         """T control ticks of raw RPMs, of a DSLPIDControl tracking a waypoint schedule, or of an MlpPolicy acting on the
         aviary's observations, as a differentiable function (torch.autograd), without changing the env.  Pass exactly one of
         `rpm` (open loop), `controller` (closed loop) or `policy` (policy loop, at the end of this text).
@@ -603,6 +603,23 @@ class BaseAviary(Env):
         closed loop, rows and columns in the order x (pos, quat x y z w, vel, rpy_rates), controller state (integral_pos_e,
         last_rpy, integral_rpy_e) and, with drag, the previous tick's applied RPMs.
 
+        Tracker loop: `controller` is an ilqr.Tracker(sol, rpm_bounds=...) of this env's E x D drones, and the call flies plan
+        ticks trk.tick .. trk.tick + T - 1 (num_steps defaults to trk.T - trk.tick) as CtrlAviary.rollout(controller=trk) does:
+        u = rpm[p] + K[p] (z - z[p]), the tracker's box, the env's clip; the forward is that rollout's bits, states and applied
+        RPMs.  Unlike rollout(), trk.tick does not advance and neither the tracker nor the env changes.  plan: optional dict of
+        some of rpm [T_plan, E, D, 4], K [T_plan, E, D, 4, n_z] and z [T_plan, E, D, n_z] (sol's shapes, float64 CUDA tensors of any
+        strides; a missing key is the tracker's own detached copy); any of them, state, last_rpm and phys may require grad, and a
+        plan tick the call does not fly gets exactly zero gradient.  The box's bounds are constants.  Returns the four state
+        entries and `rpm` [T, E, D, 4], the applied RPMs.  The derivative (DESIGN.md 4.5): the law is linear (the cotangent
+        lambda of u gives rpm[p] lambda, K[p] lambda dz^T, z[p] -K[p]^T lambda, and K[p]^T lambda joins the state's); the box as
+        torch.clamp (the gradient passes for lo <= u <= hi); the env's clip as in the open loop; z reads the stored,
+        unnormalised quaternion, so the derivative w.r.t. state["quat"] has a radial part; with n_z = 17 dz reads the RPMs
+        applied at the tick before, so that tick's command (through its clip) gets a second cotangent, last_rpm at k = 0.
+        plan= without a Tracker, unknown plan keys or bad plan tensors, schedule (waypoints, start, offset, targets, gains,
+        pid_state, control_timestep) or policy arguments with a Tracker, a tracker of another size or device, ticks past the
+        plan, a reorder_by_morton() formation, an n_z = 17 plan on an env without last_clipped_action and no last_rpm=, double
+        backward and forward mode (dual tensors: the tracker loop has reverse mode only) raise ValueError.
+
         Policy loop (HoverAviary / MultiHoverAviary with ActionType.RPM or ONE_D_RPM): `policy` is an MlpPolicy mapping
         D * obs_dim inputs to D * A outputs, `params` its float64 parameters as `policy.parameters64()` lays them out ([W1, b1,
         ..., Wout, bout, log_std]; None: detached copies of the policy's weights), `num_steps` the tick count, `noise`
@@ -628,7 +645,7 @@ class BaseAviary(Env):
                                       params=params, noise=noise, action_buffer=action_buffer, waypoints=waypoints,
                                       start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
                                       target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps,
-                                      gains=gains, pid_state=pid_state)
+                                      gains=gains, pid_state=pid_state, plan=plan)
 
     def linearise(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None, target_vel=None,
                   target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None, pid_state=None, state=None,

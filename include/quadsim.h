@@ -958,6 +958,51 @@ int qs_ilqr_box_line_search(const QsParams* p, const QsIlqrBoxIO* io, int n_envs
 int qs_ilqr_box_commit(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                        void* stream);
 
+/* Differentiable tracker loops (DESIGN.md 4.5): T control ticks of an iLQR plan's time-varying LQR tracker around Physics.DYN
+ * (+ GND and/or DRAG, no downwash), and their VJP.  Tick k (plan tick p = tick0 + k) is the QS_CTRL_LQR tick of
+ * qs_ctrl_rollout_lqr, in the same order: dz from the state and the RPMs applied at the tick before (last_rpm at k = 0),
+ * u = rpm_nom[p] + K[p] dz, the optional box clampd(u, lo, hi), the env's clip to [0, MAX_RPM of the row], `substeps` substeps.
+ * States as in QsDynTrajIO, the plan in ilqr's layout as in QsLqrRolloutIO.  The VJP follows QsDynTrajIO's decisions for the
+ * physics and the env's clip; the box is torch.clamp with constant bounds (the gradient passes for lo <= u <= hi); the law is
+ * linear: g_rpm_nom[p] = lambda, g_K[p] = lambda dz^T, g_z_nom[p] = -K[p]^T lambda, and K[p]^T lambda joins the cotangent of the
+ * stored state (its quaternion unnormalised) and, with n_z = 17, of the RPMs applied at the tick before.  One thread per drone;
+ * deterministic (per-drone gradients of per-aviary rows, no atomics). */
+typedef struct QsDynLqrTrajIO {
+    int T;                          /* ticks, > 0 */
+    int n_z;                        /* 13, or 17 (dz carries the RPMs applied at the tick before) */
+    int T_plan;                     /* ticks of the plan */
+    int tick0;                      /* the plan tick of tick 0: 0 <= tick0, tick0 + T <= T_plan */
+    int per_tick;                   /* 0: lo / hi are [N][4]; 1: [T_plan][N][4] */
+    int pad_;
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* last_rpm;         /* [N][4] the RPMs applied at the tick before tick 0 (drag, n_z = 17); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows (16-byte aligned); nullable = the constants of QsParams */
+    const double* K;                /* [T_plan][N][4][n_z] */
+    const double* z_nom;            /* [T_plan][N][n_z] */
+    const double* rpm_nom;          /* [T_plan][N][4] (32-byte aligned) */
+    const double* lo;               /* the box (32-byte aligned); nullable together with hi = no box */
+    const double* hi;
+    double* states;                 /* qs_dyn_lqr_traj out: [T][13 N], entry k = the state after tick k */
+    double* rpm;                    /* qs_dyn_lqr_traj out: [T][N][4] the applied (clipped) RPMs */
+    /* qs_dyn_lqr_traj_vjp: states and rpm are read (the forward's outputs), and */
+    const double* g_states;         /* [T][13 N] cotangents of the states */
+    const double* g_rpm;            /* [T][N][4] cotangents of rpm, nullable = zeros */
+    double* g_state0;               /* out [13 N] */
+    double* g_last_rpm;             /* out [N][4], nullable */
+    double* g_phys;                 /* out [N][16]: PER DRONE (sum the drones of an aviary for its row); nullable */
+    double* g_K;                    /* out [T_plan][N][4][n_z]: the flown plan ticks only are written; nullable */
+    double* g_z_nom;                /* out [T_plan][N][n_z]: the flown plan ticks only are written; nullable */
+    double* g_rpm_nom;              /* out [T_plan][N][4]: the flown plan ticks only are written; nullable */
+    double* scratch;                /* [substeps][13][N] workspace */
+} QsDynLqrTrajIO;
+int qs_sizeof_dyn_lqr_traj_io(void);
+/* effects as qs_dyn_traj.  Refusals, in this order: NULL pointers, sizes, effects (QS_ERR_ENUM, QS_ERR_UNSUPPORTED for downwash),
+ * n_z not 13 or 17, ticks outside the plan, only one of lo and hi, per_tick not 0 or 1, alignment. */
+int qs_dyn_lqr_traj(const QsParams* p, const QsDynLqrTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                    void* stream);
+int qs_dyn_lqr_traj_vjp(const QsParams* p, const QsDynLqrTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                        void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
