@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
-                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu")]
+                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu", "ilqr_adjoint.cu")]
 HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "lqr_law.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
@@ -203,6 +203,11 @@ class QsIlqrBoxIO(C.Structure):
                 ("active", C.c_void_p)]
 
 
+class QsIlqrAdjointIO(C.Structure):
+    _fields_ = [("T", C.c_int), ("pad_", C.c_int)] + [(n, C.c_void_p) for n in (
+        "jac", "rpm", "phys", "weights", "active", "g_states", "g_rpm", "K", "k", "status", "w", "dx")]
+
+
 class QsStepCall(C.Structure):
     _fields_ = [("p", C.c_void_p), ("st", C.c_void_p), ("io", C.c_void_p),
                 ("act_type", C.c_int), ("task", C.c_int), ("n_envs", C.c_int), ("drones_per_env", C.c_int), ("substeps", C.c_int),
@@ -220,7 +225,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_sizeof_dyn_ctrl_traj_jvp_io", "qs_dyn_policy_traj_jvp", "qs_dyn_policy_tick_jac", "qs_sizeof_dyn_policy_traj_jvp_io",
            "qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit", "qs_sizeof_ilqr_io", "qs_ilqr_box_backward",
            "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io", "qs_ctrl_rollout_lqr",
-           "qs_sizeof_lqr_rollout_io", "qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp", "qs_sizeof_dyn_lqr_traj_io"]
+           "qs_sizeof_lqr_rollout_io", "qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp", "qs_sizeof_dyn_lqr_traj_io",
+           "qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout", "qs_sizeof_ilqr_adjoint_io"]
 MAX_PEERS = 16
 
 
@@ -355,6 +361,10 @@ def lib():
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrBoxIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
     L.qs_sizeof_ilqr_box_io.restype = C.c_int
+    for n in ("qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrAdjointIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
+    L.qs_sizeof_ilqr_adjoint_io.restype = C.c_int
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -417,8 +427,10 @@ def lib():
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac / "
                           "dyn traj io / dyn ctrl traj io / dyn policy traj io / dyn traj jvp io / dyn ctrl traj jvp io / "
                           "dyn policy traj jvp io): rebuild")
-    if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO) or L.qs_sizeof_ilqr_box_io() != C.sizeof(QsIlqrBoxIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io / ilqr box io): rebuild")
+    if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO) or L.qs_sizeof_ilqr_box_io() != C.sizeof(QsIlqrBoxIO) or \
+            L.qs_sizeof_ilqr_adjoint_io() != C.sizeof(QsIlqrAdjointIO):
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io / ilqr box io / ilqr adjoint io): "
+                          "rebuild")
     if L.qs_sizeof_lqr_rollout_io() != C.sizeof(QsLqrRolloutIO) or L.qs_sizeof_dyn_lqr_traj_io() != C.sizeof(QsDynLqrTrajIO):
         raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (lqr rollout io / dyn lqr traj io): rebuild")
     _lib = L

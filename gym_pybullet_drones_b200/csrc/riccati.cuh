@@ -391,6 +391,67 @@ QS_HD void ric_col_K_box(const RicWs<NZ>& w, int j, const RicBoxGains& G) {
     w.vx[j] = v;
 }
 
+// ---- The adjoint LQR of the solution's derivative (qs_ilqr_adjoint, ilqr_adjoint.cu; DESIGN.md 4.5.1): the solve's stage
+// Hessians at mu = 0 with the linear terms -g_X (state) and -g_U (command), on the free rotors only.  Its phases S and G are
+// below; phases H, K, V and Y are the solve's (ric_col_H, ric_col_K / ric_col_K_box, ric_col_V, ric_col_sym).
+
+// Phase S of the adjoint (j < 13): the stage 1/2 wj dx_j^2 - gx dx_j of z_{k+1}'s state component j
+template <int NZ>
+QS_HD void ric_stage_adj(const RicWs<NZ>& w, int j, double wj, double gx) {
+    w.V[j * NZ + j] += wj;
+    w.vx[j] -= gx;
+}
+
+// Phase G of the adjoint (every lane, the same bits): Quu = Rt + B'V_xx B as ric_gains takes it, Qu = -gu + B'V_x, and the
+// factor of Quu's free block embedded in a 4x4 with identity rows and columns on the held rotors (act[j] != 0; all free: Quu's
+// own factor, bit for bit ric_gains' at mu = 0); k = -Quu_ff^-1 Qu_f, 0 on held rotors.  G.L = G.Lf.  false when the free
+// block is not positive definite.
+template <int NZ>
+QS_HD bool ric_gains_adj(const RicWs<NZ>& w, const double Rt[4], const double gu[4], const int act[4], RicBoxGains& G) {
+    constexpr int M = NZ + 4;
+    double e[16], rhs[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            double q = 0.5 * (w.H[(NZ + i) * M + NZ + j] + w.H[(NZ + j) * M + NZ + i]);
+            if (i == j) q += Rt[i];
+            G.Quu[i * 4 + j] = q;
+            e[i * 4 + j] = (act[i] == 0 && act[j] == 0) ? q : (i == j ? 1.0 : 0.0);
+        }
+        G.Qu[i] = w.g[NZ + i] - gu[i];
+        G.act[i] = act[i];
+        rhs[i] = act[i] != 0 ? 0.0 : G.Qu[i];
+    }
+    if (!chol4(e, G.Lf)) return false;
+    chol4_neg_solve(G.Lf, rhs, G.k);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        if (act[i] != 0) G.k[i] = 0.0;
+    }
+#pragma unroll
+    for (int q = 0; q < 16; ++q) G.L[q] = G.Lf[q];
+    return true;
+}
+
+// The adjoint's linear rollout, one tick: w_j = k_j + K_j dz (0 on held rotors), K_j dz summed in q order from 0.0
+template <int NZ>
+QS_HD double ric_adj_w(const double* Kj, double kj, const double* dz, bool held) {
+    double s = 0.0;
+#pragma unroll
+    for (int q = 0; q < NZ; ++q) s += Kj[q] * dz[q];
+    return held ? 0.0 : kj + s;
+}
+// Row r (< NZ) of dz_{k+1} = F [dz; w]: y = [dz | w] (M entries), summed in column order from 0.0
+template <int NZ>
+QS_HD double ric_adj_next(const RicWs<NZ>& w, int r, const double* y) {
+    constexpr int M = NZ + 4;
+    double s = 0.0;
+#pragma unroll
+    for (int c = 0; c < M; ++c) s += w.F[r * M + c] * y[c];
+    return s;
+}
+
 // 1/2 (sum_r W_r (x_r - ref_r)^2 + sum_j Rt_j (u_j - uref_j)^2): the cost of one tick, x and ref in the order pos, quat, vel,
 // rpy_rates
 QS_HD double stage_cost(const double x[13], const double ref[13], const double W[13], const double u[4], const double uref[4],

@@ -106,17 +106,23 @@ class DynTrajectory(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_states):
         _no_double_backward()
-        rpm = ctx.saved_tensors[0]
-        P, E, D, S, eff = ctx.cfg
-        T, n = rpm.shape[0], E * D
-        f64 = dict(dtype=torch.float64, device=rpm.device)
-        g = dict(g_rpm=torch.empty((T, n, 4), **f64), g_state0=torch.empty((13 * n,), **f64), g_last_rpm=torch.empty((n, 4), **f64),
-                 g_phys=torch.empty((n, 16), **f64))
-        ptrs = dict(_traj_ptrs(*ctx.saved_tensors), g_states=g_states.to(torch.float64).contiguous(), scratch=torch.empty((S, 13, n), **f64),
-                    **g)
-        io = _io(N.QsDynTrajIO, T, ptrs)
-        _call("qs_dyn_traj_vjp", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
-        return g["g_rpm"], g["g_state0"], g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), None
+        return (*_dyn_traj_vjp(ctx.cfg, *ctx.saved_tensors, g_states), None)
+
+
+def _dyn_traj_vjp(cfg, rpm, planes0, last_rpm, rows, states, g_states):
+    """qs_dyn_traj_vjp of the trajectory `states` (qs_dyn_traj's output for the other inputs) for the cotangent g_states
+    [T, 13 N]: (g_rpm [T, N, 4], g_planes0 [13 N], g_last_rpm [N, 4], g_rows [E, 16]), the per-drone row gradients summed over
+    each aviary's drones (torch, deterministic)."""
+    P, E, D, S, eff = cfg
+    T, n = rpm.shape[0], E * D
+    f64 = dict(dtype=torch.float64, device=rpm.device)
+    g = dict(g_rpm=torch.empty((T, n, 4), **f64), g_state0=torch.empty((13 * n,), **f64), g_last_rpm=torch.empty((n, 4), **f64),
+             g_phys=torch.empty((n, 16), **f64))
+    ptrs = dict(_traj_ptrs(rpm, planes0, last_rpm, rows, states), g_states=g_states.to(torch.float64).contiguous(),
+                scratch=torch.empty((S, 13, n), **f64), **g)
+    io = _io(N.QsDynTrajIO, T, ptrs)
+    _call("qs_dyn_traj_vjp", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
+    return g["g_rpm"], g["g_state0"], g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1)
 
 
 CTRL_INS = ("state0", "pid0", "target_pos", "target_vel", "target_rpy", "target_rpy_rates", "last_rpm", "phys", "gains")

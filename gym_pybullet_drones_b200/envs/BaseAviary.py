@@ -759,6 +759,41 @@ class BaseAviary(Env):
         return ilqr(self, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, iters=iters, state=state,
                     last_rpm=last_rpm, phys=phys, rpm_bounds=rpm_bounds)
 
+    def differentiable_ilqr(self, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None,
+                            last_rpm=None, phys=None, rpm_bounds=None):
+        """ilqr() with gradients of the solution (DESIGN.md 4.5.1 "Gradients of the solution"): the same arguments and the same
+        result, every output bit for bit ilqr()'s, with pos, quat, vel, rpy_rates and rpm differentiable (torch autograd, reverse
+        mode) w.r.t. every target entry, Q, Q_final, R, rpm_ref, the state entries, last_rpm and the phys entries, in every shape
+        they accept.  K, k, z, cost, mu, converged and active are returned detached.  The initial guess rpm gets no gradient (the
+        solution does not depend on it locally), and the bounds are constants ("motor" takes MAX_RPM detached).
+
+        The derivative.  Per drone the solve minimises J(u; theta) = 1/2 sum_k (x_k - r_k)' W_k (x_k - r_k)
+        + 1/2 sum_k (u_k - u_ref)' Rt (u_k - u_ref), x = X(u; x0, last_rpm, rows), Rt = diag(R) / HOVER_RPM^2.  For cotangents g_X
+        of the states and g_U of rpm, the backward solves the adjoint LQR
+            min_w 1/2 sum dx_k' W_k dx_k + 1/2 sum w_k' Rt w_k - sum g_X,k . dx_k - sum g_U,k . w_k,  dx = J w,
+        i.e. w_S = H_SS^-1 (g_U + J' g_X)_S with H = J'WJ + Rt the Gauss-Newton Hessian the solve itself uses, J = dX/du, and S the
+        free rotor-ticks: all of them without bounds, those with active == 0 (the last backward pass, at the returned trajectory)
+        with bounds; held rotors are constants with zero derivative.  It is one Riccati pass at mu = 0 and one linear rollout on
+        the device (qs_ilqr_adjoint, qs_ilqr_adjoint_rollout), whatever the drone's final mu.  The cost-side inputs get the
+        gradient of -sum_k [W_k (X*_k - r_k) . dx_k + Rt (U*_k - u_ref) . w_k] (so dl/dr_k = W_k dx_k, dl/du_ref = sum_k Rt w_k),
+        the dynamics-side inputs (state, last_rpm, phys) qs_dyn_traj_vjp at the solution with the cotangent g_X - W dx; the rows
+        get both parts.
+
+        This is the exact derivative of the LQR model at the returned trajectory: the model the whole solver is built on.  It is
+        the derivative of the true solution map where the dynamics' curvature term sum_k lambda_{k+1} . d2f vanishes (e.g. a
+        solution with zero residual, such as hovering at the target), and an approximation elsewhere (DESIGN.md 4.5.1 measures
+        the gap).  On a drone that has not converged (see `converged`) it is the derivative of the model at the returned
+        trajectory, not of a solution.  A drone whose adjoint has no Cholesky factor gets NaN gradients (Quu is positive definite
+        for R > 0, so this needs non-finite inputs), and the NaN reaches every input it shares with other drones: the per-aviary
+        Q, Q_final, R and phys rows of its aviary, and a [13], [4] or [k] entry shared by every drone.  The forward synchronises once, as ilqr() does; the backward does not
+        synchronise, and holds no Jacobian buffer between forward and backward (it recomputes the Jacobians once).
+
+        Raises ValueError as ilqr() does, and for a bound tensor that requires grad, double backward (create_graph=True) and
+        forward-mode AD."""
+        from ..ilqr import differentiable_ilqr
+        return differentiable_ilqr(self, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, iters=iters,
+                                   state=state, last_rpm=last_rpm, phys=phys, rpm_bounds=rpm_bounds)
+
     ################################################################################
 
     def _stream(self):

@@ -2,13 +2,16 @@
 independent problem per drone, on the per-tick Jacobians of qs_dyn_tick_jac and the kernels qs_ilqr_backward,
 qs_ilqr_line_search and qs_ilqr_commit (include/quadsim.h), or with rpm_bounds their control-limited variants qs_ilqr_box_*.
 BaseAviary.ilqr is the public entry point; Problem holds one solve's device buffers and runs its steps, so that each step can
-also be called on its own.  Tracker flies a solution's LQR tracker in CtrlAviary.rollout() (qs_ctrl_rollout_lqr)."""
+also be called on its own.  Tracker flies a solution's LQR tracker in CtrlAviary.rollout() (qs_ctrl_rollout_lqr).
+differentiable_ilqr (BaseAviary.differentiable_ilqr) is the same solve with gradients of the solution: IlqrSolution, whose
+backward is one adjoint LQR pass on the device (qs_ilqr_adjoint, qs_ilqr_adjoint_rollout)."""
+import contextlib
 import ctypes as C
 
 import torch
 
 from . import _native as N
-from .diff import STATE_KEYS, _call, _io, _refuse_downwash, _start_state, _tensor, _traj_ptrs, unpack_states
+from .diff import STATE_KEYS, _call, _dyn_traj_vjp, _io, _refuse_downwash, _start_state, _tensor, _traj_ptrs, pack_state, unpack_states
 
 ALPHAS = tuple(2.0 ** -j for j in range(10))               # the line search's step sizes, largest first
 DEFAULT_Q = (1.0,) * 3 + (1.0,) * 4 + (0.1,) * 3 + (0.01,) * 3   # pos, quat, vel, rpy_rates
@@ -92,10 +95,12 @@ class Problem:
     """The device buffers of one batched iLQR solve and its steps.  Arguments as BaseAviary.ilqr; `alphas` are the line
     search's step sizes (1 to 16).  `feedback = False` runs the line search and the commit with K = 0 (an open-loop line
     search along k).  With `rpm_bounds` every step runs the control-limited kernels qs_ilqr_box_*, the guess is projected into
-    the box before the first nominal, and `active` holds the held rotors of the last backward pass."""
+    the box before the first nominal, and `active` holds the held rotors of the last backward pass.  With `graph` the inputs
+    are packed with autograd recording (the solve's buffers stay detached) and `graph` holds the recorded packed (targets, weights,
+    rpm_ref, planes0, last_rpm, rows): the inputs of IlqrSolution."""
 
     def __init__(self, env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, state=None, last_rpm=None,
-                 phys=None, alphas=ALPHAS, rpm_bounds=None):
+                 phys=None, alphas=ALPHAS, rpm_bounds=None, graph=False):
         _refuse_downwash(env, "ilqr()", "Jacobian")
         E, D, n, dev = env._E, env._D, env._N, env.device
         if not isinstance(target, dict) or "pos" not in target:
@@ -126,16 +131,18 @@ class Problem:
         alphas = tuple(float(a) for a in alphas)
         if not 1 <= len(alphas) <= 16:
             raise ValueError("alphas must hold 1 to 16 step sizes")
-        with torch.no_grad():
+        with contextlib.nullcontext() if graph else torch.no_grad():
             planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
             parts = [_target_part(target[k], "target[%r]" % k, w, T, E, D, dev) if k in target
                      else _target_part(torch.tensor(HOVER_TARGET[k], dtype=torch.float64, device=dev), k, w, T, E, D, dev)
                      for k, w in STATE_KEYS]
-            self.targets = pack_traj(*parts).contiguous()
+            targets = pack_traj(*parts)
+            self.targets = targets.detach().contiguous()
             q = _weight(Q, "Q", DEFAULT_Q, E, dev)
             qf = FINAL_SCALE * q if Q_final is None else _weight(Q_final, "Q_final", DEFAULT_Q, E, dev)
             r = _weight(R, "R", DEFAULT_R, E, dev)
-            self.weights = torch.cat([q, qf, r], dim=1).contiguous()
+            weights = torch.cat([q, qf, r], dim=1)
+            self.weights = weights.detach().contiguous()
             w_ok = torch.isfinite(self.weights).all() & (self.weights >= 0).all() & (r > 0).all()
             if rpm_bounds is None:
                 # the one synchronisation of a solve: the weights' values
@@ -151,7 +158,7 @@ class Problem:
                 if not b_ok:
                     raise ValueError("ilqr(): rpm_bounds must not be NaN and must satisfy 0 <= lo <= hi <= MAX_RPM of each "
                                      "drone's row")
-                self.box = (lo, hi, per_tick)
+                self.box = (lo.detach(), hi.detach(), per_tick)      # "motor": MAX_RPM is a constant
             hover = rows[:, 12].reshape(E, 1, 1).expand(E, D, 4)
             if rpm_ref is None:
                 ref = hover.reshape(n, 4)
@@ -169,7 +176,8 @@ class Problem:
                 lo, hi, per_tick = self.box
                 torch.minimum(torch.maximum(self.rpm, lo), hi, out=self.rpm)
         self.env_shape = (E, D)
-        self.planes0, self.last_rpm, self.rows = planes0.contiguous(), last_rpm.detach().contiguous(), rows.contiguous()
+        self.graph = (targets, weights, ref, planes0, last_rpm, rows) if graph else None
+        self.planes0, self.last_rpm, self.rows = planes0.detach().contiguous(), last_rpm.detach().contiguous(), rows.detach().contiguous()
         self.cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
         self.T, self.n, self.dev = T, n, dev
         self.nz = 17 if env._effects & N.EFFECT_DRAG else 13
@@ -289,6 +297,134 @@ def ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rp
     p = Problem(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, state=state, last_rpm=last_rpm,
                 phys=phys, rpm_bounds=rpm_bounds)
     return solve(p, iters)
+
+
+def adjoint(p, g_states, g_rpm):
+    """The adjoint LQR of Problem p's solution (DESIGN.md 4.5.1 "Gradients of the solution") for the cotangents g_states
+    [T, 13 N] and g_rpm [T, N, 4] (either None: zeros): qs_dyn_tick_jac at (p.rpm, p.states) into a buffer freed on return, then
+    qs_ilqr_adjoint and qs_ilqr_adjoint_rollout, with p.active as the held set when p has bounds.  Returns (w [T, N, 4],
+    dx [T, 13 N], K [T, N, 4, n_z], k [T, N, 4], status [N] int32); w and dx are NaN on drones with status 1."""
+    P, E, D, S, eff = p.cfg
+    T, n, dev = p.T, p.n, p.dev
+    f64 = dict(dtype=torch.float64, device=dev)
+    with torch.no_grad(), torch.cuda.device(dev):
+        p.jac = torch.empty((T, n, 13, 21 if p.nz == 17 else 17), **f64)
+        try:
+            p.jacobians()
+            out = dict(K=torch.empty((T, n, 4, p.nz), **f64), k=torch.empty((T, n, 4), **f64),
+                       status=torch.empty((n,), dtype=torch.int32, device=dev), w=torch.empty((T, n, 4), **f64),
+                       dx=torch.empty((T, 13 * n), **f64))
+            g_states = torch.zeros((T, 13 * n), **f64) if g_states is None else g_states.to(torch.float64).contiguous()
+            g_rpm = None if g_rpm is None else g_rpm.to(torch.float64).reshape(T, n, 4).contiguous()
+            io = _io(N.QsIlqrAdjointIO, T, dict(jac=p.jac, rpm=p.rpm, phys=p.rows, weights=p.weights, active=p.active,
+                                                g_states=g_states, g_rpm=g_rpm, **out))
+            for name in ("qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout"):
+                _call(name, C.byref(P), C.byref(io), E, D, S, eff, device=dev)
+        finally:
+            p.jac = None
+    return out["w"], out["dx"], out["K"], out["k"], out["status"]
+
+
+def state_weights(weights, E, D, T):
+    """W [T, 13 N] in the planes layout of the states: each aviary's Q for ticks < T - 1 and Q_final for the last, from the
+    packed weights [E, 30]."""
+    n = E * D
+    planes = lambda q: pack_state(q[:, 0:3], q[:, 3:7], q[:, 7:10], q[:, 10:13])
+    q = weights[:, 0:13].repeat_interleave(D, dim=0)
+    qf = weights[:, 13:26].repeat_interleave(D, dim=0)
+    return torch.cat([planes(q).reshape(1, 13 * n).expand(T - 1, 13 * n), planes(qf).reshape(1, 13 * n)])
+
+
+def _refuse_forward_ad(xs):
+    from torch.autograd import forward_ad
+    if any(x is not None and forward_ad.unpack_dual(x).tangent is not None for x in xs):
+        raise ValueError("differentiable_ilqr() is reverse mode only: forward-mode AD (dual tensors) is not supported")
+
+
+class IlqrSolution(torch.autograd.Function):
+    """(states [T, 13 N], rpm [T, N, 4]) of solve(p, iters) as a function of the packed inputs of Problem p built with
+    graph=True: targets [T, 13 N], weights [E, 30], rpm_ref [N, 4], planes0 [13 N], last_rpm [N, 4] and rows [E, 16] (p's own
+    detached buffers are what the kernels read).  `out` receives the whole result of solve().  The forward frees p's Jacobian
+    buffer; the backward recomputes it once at the solution (adjoint()), so nothing of size T N 13 C is held in between.
+
+    Backward, with w and dx the adjoint LQR's solution for the cotangents: the cost-side inputs (targets, weights, rpm_ref, the
+    rows through HOVER_RPM) get the gradient of the surrogate
+        s = -sum_k [W_k (X*_k - r_k) . dx_k + Rt (U*_k - u_ref) . w_k]
+    (X*, U*, dx and w constant) by torch autograd, and the dynamics-side inputs (planes0, last_rpm, rows) qs_dyn_traj_vjp at the
+    solution with the cotangent g_X - W dx.  Double backward and forward-mode AD raise ValueError."""
+
+    @staticmethod
+    def forward(ctx, targets, weights, rpm_ref, planes0, last_rpm, rows, p, iters, out):
+        out.update(solve(p, iters))
+        states, rpm = p.states, p.rpm
+        # the outputs live on ctx through save_for_backward only: p keeps no reference to them (no cycle through the graph)
+        p.states = p.rpm = p.jac = None
+        ctx.save_for_backward(states, rpm)
+        ctx.p = p
+        return states, rpm
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise ValueError("differentiable_ilqr() is reverse mode only: forward-mode AD (dual tensors) is not supported")
+
+    @staticmethod
+    def backward(ctx, g_states, g_rpm):
+        if torch.is_grad_enabled():
+            raise ValueError("differentiable_ilqr(): double backward (create_graph=True) is not supported: the adjoint LQR has no "
+                             "derivative of its own")
+        p = ctx.p
+        states, rpm = ctx.saved_tensors
+        E, D = p.env_shape
+        T, n = p.T, p.n
+        p.states, p.rpm = states, rpm
+        try:
+            w, dx, _, _, _ = adjoint(p, g_states, g_rpm)
+        finally:
+            p.states = p.rpm = None
+        need = ctx.needs_input_grad
+        W = state_weights(p.weights, E, D, T)
+        grads = [None] * 6
+        # cost side: the surrogate s(theta), by autograd over detached leaves
+        cost_ins = [j for j in (0, 1, 2, 5) if need[j]]
+        if cost_ins:
+            tg, wt, ref, rows = (x.detach().requires_grad_(j in cost_ins)
+                                 for j, x in ((0, p.targets), (1, p.weights), (2, p.rpm_ref), (5, p.rows)))
+            with torch.enable_grad():
+                Rt = (wt[:, 26:30] / (rows[:, 12:13] * rows[:, 12:13])).repeat_interleave(D, dim=0)
+                s = -((state_weights(wt, E, D, T) * (states - tg) * dx).sum() + (Rt * (rpm - ref) * w).sum())
+                got = torch.autograd.grad(s, [x for j, x in zip((0, 1, 2, 5), (tg, wt, ref, rows)) if j in cost_ins])
+            for j, g in zip(cost_ins, got):
+                grads[j] = g
+        # dynamics side: one VJP with the direct cotangent g_X and the Gauss-Newton implicit term -W dx
+        if need[3] or need[4] or need[5]:
+            cot = -(W * dx) if g_states is None else g_states - W * dx
+            _, g0, glast, grows = _dyn_traj_vjp(p.cfg, rpm, p.planes0, p.last_rpm, p.rows, states, cot)
+            grads[3], grads[4] = g0, glast
+            grads[5] = grows if grads[5] is None else grads[5] + grows
+        return (*grads, None, None, None)
+
+
+def differentiable_ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None,
+                        last_rpm=None, phys=None, rpm_bounds=None):
+    """BaseAviary.differentiable_ilqr (see there)."""
+    _refuse_downwash(env, "differentiable_ilqr()", "Jacobian")
+    if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
+        raise ValueError("iters must be an integer >= 0, got %r" % (iters,))
+    if isinstance(rpm_bounds, (tuple, list)) and any(isinstance(b, torch.Tensor) and b.requires_grad for b in rpm_bounds):
+        raise ValueError("differentiable_ilqr(): rpm_bounds are constants: a bound tensor must not require grad (detach it)")
+    p = Problem(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, state=state, last_rpm=last_rpm,
+                phys=phys, rpm_bounds=rpm_bounds, graph=True)
+    _refuse_forward_ad(p.graph)
+    out = {}
+    states, rpm_out = IlqrSolution.apply(*p.graph, p, iters, out)
+    E, D = p.env_shape
+    T, n = p.T, p.n
+    sol = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    sol["rpm"] = rpm_out.view(T, E, D, 4)
+    for k in ("K", "z", "k", "cost", "mu", "converged", "active"):
+        if k in out:
+            sol[k] = out[k]
+    return sol
 
 
 class Tracker:

@@ -958,6 +958,44 @@ int qs_ilqr_box_line_search(const QsParams* p, const QsIlqrBoxIO* io, int n_envs
 int qs_ilqr_box_commit(const QsParams* p, const QsIlqrBoxIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                        void* stream);
 
+/* The derivative of an iLQR solution (DESIGN.md 4.5.1 "Gradients of the solution"): given the cotangents g_X of the solution's
+ * states and g_U of its rpm, the adjoint LQR  min_w 1/2 sum dx_k' W_k dx_k + 1/2 sum w_k' Rt w_k - sum g_X,k . dx_k
+ * - sum g_U,k . w_k  with dz_0 = 0, dz_{k+1} = F_k [dz_k; w_k] and w = 0 on held rotors, where F_k = [A | B] is the solve's (from
+ * qs_dyn_tick_jac at the solution, with drag's rows of the clipped RPMs) and W_k, Rt are QsIlqrIO's.  Its solution
+ * w_S = H_SS^-1 G_S (H = J'W J + Rt the Gauss-Newton Hessian, G = g_U + J'g_X, J = dX/dU, S the free rotor-ticks) gives the
+ * solution's gradients (ilqr.IlqrSolution).  One warp per drone in both entry points. */
+typedef struct QsIlqrAdjointIO {
+    int T;                          /* ticks, > 0 */
+    int pad_;
+    const double* jac;              /* [T][N][13][C] qs_dyn_tick_jac's output at the solution */
+    const double* rpm;              /* [T][N][4] the solution's raw commands (drag: the clip's derivative) */
+    const double* phys;             /* [n_envs][16] QsState.phys rows (16-byte aligned); nullable = the constants of QsParams */
+    const double* weights;          /* [n_envs][30]: Q (13), Q_final (13), R (4), as QsIlqrIO */
+    const signed char* active;      /* [T][N][4] the held rotors (nonzero) of the solve's last backward pass; nullable = none held
+                                     * (then the unconstrained kernels run) */
+    const double* g_states;         /* [T][13 N] g_X in the planes layout of the states (qs_ilqr_adjoint) */
+    const double* g_rpm;            /* [T][N][4] g_U; nullable = zeros (qs_ilqr_adjoint) */
+    double* K;                      /* [T][N][4][n_z] the adjoint's feedback gains: qs_ilqr_adjoint out, rollout in */
+    double* k;                      /* [T][N][4] its feed-forward: qs_ilqr_adjoint out, rollout in */
+    int* status;                    /* [N] 0, or 1 when a tick's free block of Quu has no Cholesky factor: qs_ilqr_adjoint out,
+                                     * rollout in */
+    double* w;                      /* [T][N][4] qs_ilqr_adjoint_rollout out: w_k, 0 on held rotors; NaN where status != 0 */
+    double* dx;                     /* [T][13 N] qs_ilqr_adjoint_rollout out: the state part of dz_{k+1}; NaN where status != 0 */
+} QsIlqrAdjointIO;
+int qs_sizeof_ilqr_adjoint_io(void);
+/* The adjoint's Riccati pass, k = T-1 .. 0: qs_ilqr_backward's recursion at mu = 0 with the stage's linear term -g_X,k (V_x),
+ * Qu = -g_U,k + B'V_x, and the held rotors of `active` fixed at 0: Quu's free block is factored (held rows and columns replaced
+ * by the identity), k = -Quu_ff^-1 Qu_f and K = -Quu_ff^-1 Qux_f on free rotors, 0 on held ones.  Without `active` K is
+ * qs_ilqr_backward's K at mu = 0 bit for bit.  No regularisation ladder: a failed factor sets status = 1 and leaves the ticks
+ * below it unwritten.  Refusals, in this order: NULL params / io, NULL jac / rpm / weights / K / k / status, NULL g_states,
+ * sizes, effects (QS_ERR_UNSUPPORTED for downwash), phys alignment. */
+int qs_ilqr_adjoint(const QsParams* p, const QsIlqrAdjointIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                    void* stream);
+/* The adjoint's linear forward pass: w_k = k_k + K_k dz_k (0 on held rotors), dz_{k+1} = F_k [dz_k; w_k] from dz_0 = 0, each sum
+ * in index order from 0.0.  Refusals as qs_ilqr_adjoint, with NULL w / dx in place of NULL g_states. */
+int qs_ilqr_adjoint_rollout(const QsParams* p, const QsIlqrAdjointIO* io, int n_envs, int drones_per_env, int substeps,
+                            unsigned effects, void* stream);
+
 /* Differentiable tracker loops (DESIGN.md 4.5): T control ticks of an iLQR plan's time-varying LQR tracker around Physics.DYN
  * (+ GND and/or DRAG, no downwash), and their VJP.  Tick k (plan tick p = tick0 + k) is the QS_CTRL_LQR tick of
  * qs_ctrl_rollout_lqr, in the same order: dz from the state and the RPMs applied at the tick before (last_rpm at k = 0),
