@@ -267,6 +267,16 @@ def build(force=False, verbose=False):
 _lib = None
 
 
+# qs_sizeof_<name> of include/quadsim.h and the ctypes mirror of that struct: lib() refuses a library whose layouts differ
+_MIRRORS = (("params", QsParams), ("state", QsState), ("step_io", QsStepIO), ("rollout_io", QsRolloutIO), ("host_io", QsHostIO),
+            ("log_ring", QsLogRing), ("mlp_policy", QsMlpPolicy), ("ctrl_rollout_io", QsCtrlRolloutIO), ("mrac_params", QsMracParams),
+            ("mrac_rollout_io", QsMracRolloutIO), ("lqr_rollout_io", QsLqrRolloutIO), ("dyn_traj_io", QsDynTrajIO),
+            ("dyn_ctrl_traj_io", QsDynCtrlTrajIO), ("dyn_policy_traj_io", QsDynPolicyTrajIO), ("dyn_lqr_traj_io", QsDynLqrTrajIO),
+            ("dyn_traj_jvp_io", QsDynTrajJvpIO), ("dyn_ctrl_traj_jvp_io", QsDynCtrlTrajJvpIO),
+            ("dyn_policy_traj_jvp_io", QsDynPolicyTrajJvpIO), ("ilqr_io", QsIlqrIO), ("ilqr_box_io", QsIlqrBoxIO),
+            ("ilqr_adjoint_io", QsIlqrAdjointIO))
+
+
 def lib():
     """Loads (once) and returns the CUDA library.  Raises if it is not built: no fallback."""
     global _lib
@@ -278,8 +288,8 @@ def lib():
     L = C.CDLL(LIB_PATH)
     L.qs_abi_version.restype = C.c_int
     L.qs_last_error.restype = C.c_char_p
-    for n in ("qs_sizeof_params", "qs_sizeof_state", "qs_sizeof_step_io", "qs_sizeof_rollout_io"):
-        getattr(L, n).restype = C.c_int
+    for name, _ in _MIRRORS:
+        getattr(L, "qs_sizeof_" + name).restype = C.c_int
     L.qs_step.restype = C.c_int
     L.qs_step.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsStepIO), C.c_int, C.c_int,
                           C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -288,7 +298,6 @@ def lib():
     L.qs_step_host.restype = C.c_int
     L.qs_step_host.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsStepIO), C.POINTER(QsHostIO), C.c_int, C.c_int,
                                C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
-    L.qs_sizeof_host_io.restype = C.c_int
     L.qs_host_is_pinned.restype = C.c_int
     L.qs_host_is_pinned.argtypes = [C.c_void_p]
     L.qs_rollout.restype = C.c_int
@@ -301,11 +310,9 @@ def lib():
                                  C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
     L.qs_rollout_mlp_max_ticks.restype = C.c_int
     L.qs_rollout_mlp_max_ticks.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
-    L.qs_sizeof_mlp_policy.restype = C.c_int
     L.qs_ctrl_rollout.restype = C.c_int
     L.qs_ctrl_rollout.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_uint, C.c_uint, C.c_void_p]
-    L.qs_sizeof_ctrl_rollout_io.restype = C.c_int
     L.qs_ctrl_rollout_mrac.restype = C.c_int
     L.qs_ctrl_rollout_mrac.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.POINTER(QsMracRolloutIO),
                                        C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -315,56 +322,43 @@ def lib():
     L.qs_mrac_control_state.restype = C.c_int
     L.qs_mrac_control_state.argtypes = [C.POINTER(QsMracParams), C.c_void_p, C.c_int, C.c_double, C.POINTER(QsState), C.c_int] + \
         [C.c_void_p] * 8
-    L.qs_sizeof_mrac_params.restype = C.c_int
-    L.qs_sizeof_mrac_rollout_io.restype = C.c_int
     L.qs_ctrl_rollout_lqr.restype = C.c_int
     L.qs_ctrl_rollout_lqr.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.POINTER(QsLqrRolloutIO),
                                       C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
-    L.qs_sizeof_lqr_rollout_io.restype = C.c_int
     for n in ("qs_dyn_traj", "qs_dyn_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    L.qs_sizeof_dyn_traj_io.restype = C.c_int
     for n in ("qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynLqrTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    L.qs_sizeof_dyn_lqr_traj_io.restype = C.c_int
     for n in ("qs_dyn_traj_jvp", "qs_dyn_tick_jac"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajJvpIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    L.qs_sizeof_dyn_traj_jvp_io.restype = C.c_int
     for n in ("qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajIO), C.c_int, C.c_int, C.c_int,
                                   C.c_uint, C.c_void_p]
-    L.qs_sizeof_dyn_ctrl_traj_io.restype = C.c_int
     for n in ("qs_dyn_ctrl_traj_jvp", "qs_dyn_ctrl_tick_jac"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajJvpIO), C.c_int, C.c_int, C.c_int,
                                   C.c_uint, C.c_void_p]
-    L.qs_sizeof_dyn_ctrl_traj_jvp_io.restype = C.c_int
     for n in ("qs_dyn_policy_traj", "qs_dyn_policy_traj_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynPolicyTrajIO), C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint,
                                   C.c_void_p]
-    L.qs_sizeof_dyn_policy_traj_io.restype = C.c_int
     for n in ("qs_dyn_policy_traj_jvp", "qs_dyn_policy_tick_jac"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynPolicyTrajJvpIO), C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint,
                                   C.c_void_p]
-    L.qs_sizeof_dyn_policy_traj_jvp_io.restype = C.c_int
     for n in ("qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    L.qs_sizeof_ilqr_io.restype = C.c_int
     for n in ("qs_ilqr_box_backward", "qs_ilqr_box_line_search", "qs_ilqr_box_commit"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrBoxIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    L.qs_sizeof_ilqr_box_io.restype = C.c_int
     for n in ("qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrAdjointIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    L.qs_sizeof_ilqr_adjoint_io.restype = C.c_int
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
@@ -408,31 +402,14 @@ def lib():
     L.qs_log_append.restype = C.c_int
     L.qs_log_append.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_int, C.c_void_p, C.POINTER(QsLogRing),
                                 C.c_int, C.c_int, C.c_void_p]
-    L.qs_sizeof_log_ring.restype = C.c_int
     L.qs_reset.restype = C.c_int
     L.qs_reset.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_int, C.c_int,
                            C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     if L.qs_abi_version() != ABI_VERSION:
         raise ImportError("libquadsim.so ABI %d != binding ABI %d: rebuild" % (L.qs_abi_version(), ABI_VERSION))
-    if (L.qs_sizeof_params(), L.qs_sizeof_state(), L.qs_sizeof_step_io(), L.qs_sizeof_rollout_io()) != \
-            (C.sizeof(QsParams), C.sizeof(QsState), C.sizeof(QsStepIO), C.sizeof(QsRolloutIO)):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror: rebuild")
-    if L.qs_sizeof_log_ring() != C.sizeof(QsLogRing) or L.qs_sizeof_host_io() != C.sizeof(QsHostIO) or \
-            L.qs_sizeof_ctrl_rollout_io() != C.sizeof(QsCtrlRolloutIO) or L.qs_sizeof_mlp_policy() != C.sizeof(QsMlpPolicy) or \
-            L.qs_sizeof_mrac_params() != C.sizeof(QsMracParams) or L.qs_sizeof_mrac_rollout_io() != C.sizeof(QsMracRolloutIO) or \
-            L.qs_sizeof_dyn_traj_io() != C.sizeof(QsDynTrajIO) or L.qs_sizeof_dyn_ctrl_traj_io() != C.sizeof(QsDynCtrlTrajIO) or \
-            L.qs_sizeof_dyn_policy_traj_io() != C.sizeof(QsDynPolicyTrajIO) or L.qs_sizeof_dyn_traj_jvp_io() != C.sizeof(QsDynTrajJvpIO) or \
-            L.qs_sizeof_dyn_ctrl_traj_jvp_io() != C.sizeof(QsDynCtrlTrajJvpIO) or \
-            L.qs_sizeof_dyn_policy_traj_jvp_io() != C.sizeof(QsDynPolicyTrajJvpIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (log ring / host io / ctrl rollout io / mlp policy / mrac / "
-                          "dyn traj io / dyn ctrl traj io / dyn policy traj io / dyn traj jvp io / dyn ctrl traj jvp io / "
-                          "dyn policy traj jvp io): rebuild")
-    if L.qs_sizeof_ilqr_io() != C.sizeof(QsIlqrIO) or L.qs_sizeof_ilqr_box_io() != C.sizeof(QsIlqrBoxIO) or \
-            L.qs_sizeof_ilqr_adjoint_io() != C.sizeof(QsIlqrAdjointIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (ilqr io / ilqr box io / ilqr adjoint io): "
-                          "rebuild")
-    if L.qs_sizeof_lqr_rollout_io() != C.sizeof(QsLqrRolloutIO) or L.qs_sizeof_dyn_lqr_traj_io() != C.sizeof(QsDynLqrTrajIO):
-        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (lqr rollout io / dyn lqr traj io): rebuild")
+    bad = [mirror.__name__ for name, mirror in _MIRRORS if getattr(L, "qs_sizeof_" + name)() != C.sizeof(mirror)]
+    if bad:
+        raise ImportError("libquadsim.so struct layout differs from the ctypes mirror (%s): rebuild" % ", ".join(bad))
     _lib = L
     return L
 

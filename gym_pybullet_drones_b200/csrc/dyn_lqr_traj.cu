@@ -1,6 +1,6 @@
 // dyn_lqr_traj.cu -- qs_dyn_lqr_traj / qs_dyn_lqr_traj_vjp: differentiable trajectories of an iLQR plan's time-varying LQR tracker
 // around Physics.DYN (include/quadsim.h, DESIGN.md 4.5).  One thread per drone for all T ticks.  The forward is the QS_CTRL_LQR tick
-// of ctrl_rollout_kernel (the law of lqr_law.cuh, the optional box, the env's clip, dyn_tick_k, round_to_planes) in the same order;
+// of ctrl_rollout_kernel (lqr_law.cuh's tracker_command, the env's clip, dyn_tick_k, round_to_planes) in the same order;
 // the backward walks the ticks in reverse, reloading each tick's start state and the applied RPMs of the tick before from the
 // forward's outputs, and runs dyn_adjoint.cuh's tick adjoint, the two clip adjoints and the law's adjoint.  n_z is a template
 // parameter, so dz, the K rows and K^T lambda are registers, never runtime-indexed local arrays.
@@ -21,10 +21,10 @@ struct LqrTrajArgs {
     int D, substeps;
 };
 
-// dz of drone i at plan tick p: the state x in drone_vec's order minus z_nom[p][0:13], and with NZ = 17 the RPMs applied at the
-// tick before minus z_nom[p][13:17]
+// lqr_law.cuh's tracker_dz and tracker_command, written out for dyn_lqr_traj_vjp_kernel: through the plan view that kernel, at
+// the register cap, took other registers.  The forward kernel calls tracker_command.
 template <int NZ>
-__device__ __forceinline__ void loop_dz(const QsDynLqrTrajIO& io, long long N, long long i, long long p, const qs::Drone& d,
+__device__ __forceinline__ void vjp_dz(const QsDynLqrTrajIO& io, long long N, long long i, long long p, const qs::Drone& d,
                                         const double up[4], double dz[NZ]) {
     const double* zn = io.z_nom + (p * N + i) * NZ;
     const double x[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
@@ -36,13 +36,11 @@ __device__ __forceinline__ void loop_dz(const QsDynLqrTrajIO& io, long long N, l
     }
 }
 
-// The tracker's command of drone i at plan tick p (qs_ctrl_rollout_lqr's arithmetic): b = rpm_nom + K dz, clamped to the box when
-// there is one (keep[j]: torch.clamp's gradient passes, lo_j <= b_j <= hi_j before the clamp), and the applied u = clip(b, 0, max_rpm)
 template <int NZ>
-__device__ __forceinline__ void tracker_command(const QsDynLqrTrajIO& io, long long N, long long i, long long p, const qs::Drone& d,
+__device__ __forceinline__ void vjp_command(const QsDynLqrTrajIO& io, long long N, long long i, long long p, const qs::Drone& d,
                                                 const double up[4], double max_rpm, double b[4], bool keep[4], double u[4]) {
     double dz[NZ];
-    loop_dz<NZ>(io, N, i, p, d, up, dz);
+    vjp_dz<NZ>(io, N, i, p, d, up, dz);
     const D4 un = ld256_nc(io.rpm_nom, p * N + i);
     b[0] = un.x; b[1] = un.y; b[2] = un.z; b[3] = un.w;
     const double* Kp = io.K + (p * N + i) * 4 * NZ;
@@ -78,7 +76,8 @@ __global__ void __launch_bounds__(kLqrTrajTPB) dyn_lqr_traj_kernel(const __grid_
     bool keep[4];
     if (((EFF & QS_EFFECT_DRAG) || NZ == 17) && io.last_rpm) ld4(io.last_rpm, i, up);
     for (int k = 0; k < io.T; ++k) {
-        tracker_command<NZ>(io, N, i, (long long)io.tick0 + k, d, up, c.max_rpm, b, keep, u);
+        tracker_command<NZ>(device_plan<NZ>(io, N, i, (long long)io.tick0 + k), d, up, b, keep);
+        clip_rpm(b, c.max_rpm, u);                                                    // CtrlAviary.py:140
         double R_last[9];
         qs::dyn_tick_k<EFF>(a.P, c, d, u, up, 0.0, a.substeps, R_last);
         round_to_planes(d);
@@ -112,7 +111,7 @@ __global__ void __launch_bounds__(kLqrTrajTPB) dyn_lqr_traj_vjp_kernel(const __g
         const long long p = (long long)io.tick0 + k;
         double b[4], u[4];
         bool keep[4];
-        tracker_command<NZ>(io, N, i, p, d0, up, c.max_rpm, b, keep, u);
+        vjp_command<NZ>(io, N, i, p, d0, up, c.max_rpm, b, keep, u);
         double Lu[4] = {Lup_next[0], Lup_next[1], Lup_next[2], Lup_next[3]}, Lup[4] = {0, 0, 0, 0};
         if (io.g_rpm) {
             double gr[4];
@@ -128,7 +127,7 @@ __global__ void __launch_bounds__(kLqrTrajTPB) dyn_lqr_traj_vjp_kernel(const __g
         for (int j = 0; j < 4; ++j) lam[j] = keep[j] ? lam[j] : 0.0;
         // the law's adjoint at plan tick p: dz recomputed here rather than held across the tick's adjoint
         double dz[NZ], Ktl[NZ];
-        loop_dz<NZ>(io, N, i, p, d0, up, dz);
+        vjp_dz<NZ>(io, N, i, p, d0, up, dz);
         const long long pi = p * N + i;
         const double* Kp = io.K + pi * 4 * NZ;
         double* gK = io.g_K ? io.g_K + pi * 4 * NZ : nullptr;

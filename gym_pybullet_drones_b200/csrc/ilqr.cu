@@ -22,7 +22,6 @@ namespace {
 
 constexpr int kBwdWarps = 4;          // drones (warps) per backward CTA
 constexpr int kIlqrTPB = 128;         // line search and commit
-constexpr int kWeights = 30;          // doubles of one aviary's weights: Q, Q_final, R
 constexpr int kMaxAlpha = 16;
 constexpr int kMaxRestarts = 8;
 
@@ -43,29 +42,9 @@ using IlqrArgsOf = std::conditional_t<BOX, IlqrBoxArgs, IlqrArgs>;
 
 // the box [lo, hi] of the raw command of drone i at tick k
 __device__ __forceinline__ void box_at(const IlqrBoxArgs& a, int k, long long i, double lo[4], double hi[4]) {
-    const long long at = a.per_tick ? (long long)k * a.N + i : i;
+    const long long at = a.per_tick ? (long long)k * a.N + i : i;                    // lqr_law.cuh's box_row
     ld4(a.lo, at, lo);
     ld4(a.hi, at, hi);
-}
-
-// index of state component j (pos, quat x y z w, vel, rpy_rates) of drone i in a [13 N] planes state
-__device__ __forceinline__ long long plane_at(long long N, long long i, int j) {
-    if (j < 3) return 4 * i + j;
-    if (j < 7) return 4 * (N + i) + (j - 3);
-    if (j < 10) return 4 * (2 * N + i) + (j - 7);
-    if (j == 10) return 4 * i + 3;
-    if (j == 11) return 4 * (2 * N + i) + 3;
-    return 12 * N + i;
-}
-__device__ __forceinline__ void drone_vec(const qs::Drone& d, double x[13]) {
-    x[0] = d.px; x[1] = d.py; x[2] = d.pz; x[3] = d.qx; x[4] = d.qy; x[5] = d.qz; x[6] = d.qw;
-    x[7] = d.vx; x[8] = d.vy; x[9] = d.vz; x[10] = d.wx; x[11] = d.wy; x[12] = d.wz;
-}
-// Rt = R / HOVER_RPM^2 of the drone's row
-__device__ __forceinline__ void rel_weights(const double* wt, const qs::PhysRow& c, double Rt[4]) {
-    const double h2 = c.hover_rpm * c.hover_rpm;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) Rt[j] = wt[26 + j] / h2;
 }
 
 // BOX: at least 3 CTAs (12 warps) per SM, as the unconstrained kernel runs.  Left free, the drag variant takes 196 registers
@@ -82,9 +61,9 @@ __global__ void __launch_bounds__(32 * kBwdWarps, BOX ? 3 : 0) ilqr_backward_ker
     const QsIlqrIO& io = a.io;
     const qs::RicWs<NZ> w = qs::ric_ws<NZ>(sm[wid]);
     const qs::PhysRow c = row_of(a, i);
-    const double* wt = io.weights + (long long)kWeights * (i / a.D);
+    const double* wt = io.weights + (long long)qs::kWeightsRow * (i / a.D);
     double Rt[4], uref[4];
-    rel_weights(wt, c, Rt);
+    qs::rel_weights(wt, c, Rt);
     ld4(io.rpm_ref, i, uref);
     const int T = io.T;
     double mu = io.mu[i], dV1 = 0.0, dV2 = 0.0;
@@ -99,7 +78,7 @@ __global__ void __launch_bounds__(32 * kBwdWarps, BOX ? 3 : 0) ilqr_backward_ker
             __syncwarp();
             if (lane < 13) {                                          // phase S: the cost of the state after tick k
                 const long long at = (long long)k * 13 * N + plane_at(N, i, lane);
-                qs::ric_stage(w, lane, io.states[at] - io.targets[at], wt[(k == T - 1 ? 13 : 0) + lane]);
+                qs::ric_stage(w, lane, io.states[at] - io.targets[at], wt[qs::stage_weights(k, T) + lane]);
             }
             const double* jb = io.jac + ki * 13 * C;
             for (int idx = lane; idx < 13 * C; idx += 32) {
@@ -175,9 +154,9 @@ __device__ __forceinline__ double ilqr_rollout(const IlqrArgsOf<BOX>& a, long lo
     const QsIlqrIO& io = a.io;
     const long long N = a.N;
     const qs::PhysRow c = row_of(a, i);
-    const double* wt = io.weights + (long long)kWeights * (i / a.D);
+    const double* wt = io.weights + (long long)qs::kWeightsRow * (i / a.D);
     double Rt[4], uref[4];
-    rel_weights(wt, c, Rt);
+    qs::rel_weights(wt, c, Rt);
     ld4(io.rpm_ref, i, uref);
     qs::Drone d, dn;                                                  // the rollout's and the nominal's state before tick k
     ld_state(io.state0, N, i, d);
@@ -231,7 +210,7 @@ __device__ __forceinline__ double ilqr_rollout(const IlqrArgsOf<BOX>& a, long lo
         ld_state(io.targets + (long long)k * 13 * N, N, i, rd);
         drone_vec(rd, ref);
         drone_vec(d, x);
-        J += qs::stage_cost(x, ref, wt + (k == io.T - 1 ? 13 : 0), u, uref, Rt);
+        J += qs::stage_cost(x, ref, wt + (k == io.T - 1 ? qs::kWeightsQFinal : qs::kWeightsQ), u, uref, Rt);   // stage_weights
         clip_rpm(raw, c.max_rpm, upn);
 #pragma unroll
         for (int j = 0; j < 4; ++j) up[j] = uc[j];

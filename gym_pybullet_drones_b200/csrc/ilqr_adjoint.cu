@@ -19,7 +19,6 @@ namespace qsi {
 namespace {
 
 constexpr int kAdjWarps = 4;          // drones (warps) per CTA, both kernels
-constexpr int kAdjWeights = 30;       // doubles of one aviary's weights: Q, Q_final, R
 
 struct IlqrAdjArgs {
     QsParams P;
@@ -27,16 +26,6 @@ struct IlqrAdjArgs {
     long long N;
     int D;
 };
-
-// index of state component j (pos, quat x y z w, vel, rpy_rates) of drone i in a [13 N] planes state
-__device__ __forceinline__ long long adj_plane_at(long long N, long long i, int j) {
-    if (j < 3) return 4 * i + j;
-    if (j < 7) return 4 * (N + i) + (j - 3);
-    if (j < 10) return 4 * (2 * N + i) + (j - 7);
-    if (j == 10) return 4 * i + 3;
-    if (j == 11) return 4 * (2 * N + i) + 3;
-    return 12 * N + i;
-}
 
 // F = [A | B] of tick k of drone i in the workspace: qs_dyn_tick_jac's block (one coalesced warp read) and with drag the rows
 // of the clipped RPMs, as ilqr_backward_kernel builds it
@@ -70,11 +59,9 @@ __global__ void __launch_bounds__(32 * kAdjWarps, 3) ilqr_adjoint_kernel(const _
     const QsIlqrAdjointIO& io = a.io;
     const qs::RicWs<NZ> w = qs::ric_ws<NZ>(sm[wid]);
     const qs::PhysRow c = row_of(a, i);
-    const double* wt = io.weights + (long long)kAdjWeights * (i / a.D);
+    const double* wt = io.weights + (long long)qs::kWeightsRow * (i / a.D);
     double Rt[4];
-    const double h2 = c.hover_rpm * c.hover_rpm;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) Rt[j] = wt[26 + j] / h2;
+    qs::rel_weights(wt, c, Rt);
     const int T = io.T;
     for (int idx = lane; idx < NZ * NZ; idx += 32) w.V[idx] = 0.0;
     if (lane < NZ) w.vx[lane] = 0.0;
@@ -83,7 +70,7 @@ __global__ void __launch_bounds__(32 * kAdjWarps, 3) ilqr_adjoint_kernel(const _
         const long long ki = (long long)k * N + i;
         __syncwarp();
         if (lane < 13)                                                // phase S: the state after tick k
-            qs::ric_stage_adj(w, lane, wt[(k == T - 1 ? 13 : 0) + lane], io.g_states[(long long)k * 13 * N + adj_plane_at(N, i, lane)]);
+            qs::ric_stage_adj(w, lane, wt[qs::stage_weights(k, T) + lane], io.g_states[(long long)k * 13 * N + plane_at(N, i, lane)]);
         adj_load_f<EFF, NZ>(io, w, c, ki, lane);
         double gu[4] = {0.0, 0.0, 0.0, 0.0};
         if (io.g_rpm) ld4(io.g_rpm, ki, gu);
@@ -128,7 +115,7 @@ __global__ void __launch_bounds__(32 * kAdjWarps, 3) ilqr_adjoint_rollout_kernel
     if (io.status[i] != 0) {                                          // the adjoint had no factor: NaN gradients
         for (int k = 0; k < T; ++k) {
             if (lane < 4) io.w[4 * ((long long)k * N + i) + lane] = NAN;
-            if (lane < 13) io.dx[(long long)k * 13 * N + adj_plane_at(N, i, lane)] = NAN;
+            if (lane < 13) io.dx[(long long)k * 13 * N + plane_at(N, i, lane)] = NAN;
         }
         return;
     }
@@ -159,7 +146,7 @@ __global__ void __launch_bounds__(32 * kAdjWarps, 3) ilqr_adjoint_rollout_kernel
         if (lane < NZ) v = qs::ric_adj_next(w, lane, y);
         __syncwarp();
         if (lane < NZ) y[lane] = v;
-        if (lane < 13) io.dx[(long long)k * 13 * N + adj_plane_at(N, i, lane)] = v;
+        if (lane < 13) io.dx[(long long)k * 13 * N + plane_at(N, i, lane)] = v;
     }
 }
 

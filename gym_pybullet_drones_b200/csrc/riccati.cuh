@@ -12,6 +12,17 @@
 
 namespace qs {
 
+// One aviary's row of QsIlqrIO.weights: [Q 13 | Q_final 13 | R 4]
+constexpr int kWeightsQ = 0, kWeightsQFinal = 13, kWeightsR = 26, kWeightsRow = 30;
+// the offset in the row of the state weights of the state after tick k of T: Q, or Q_final after the last tick
+QS_HD int stage_weights(int k, int T) { return k == T - 1 ? kWeightsQFinal : kWeightsQ; }
+// Rt = R / HOVER_RPM^2 of the drone's row
+QS_HD void rel_weights(const double* wt, const PhysRow& c, double Rt[4]) {
+    const double h2 = c.hover_rpm * c.hover_rpm;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) Rt[j] = wt[kWeightsR + j] / h2;
+}
+
 template <int NZ>
 struct RicWs {
     static constexpr int M = NZ + 4;

@@ -157,13 +157,14 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
 #pragma unroll
                 for (int j = 0; j < 4; ++j) rpm[j] = qs::clampd(qs::clampd(rpm[j], 0.0, a.CP.max_rpm), 0.0, mr);
             } else if constexpr (MODE == QS_CTRL_LQR) {
-                // u = rpm_nom + K (z - z_nom) (lqr_law.cuh), the optional box, then the env's clip as in RAW
+                // u = rpm_nom + K (z - z_nom), the optional box, then the env's clip as in RAW.  The command mirrors lqr_law.cuh's
+                // tracker_command with n_z read at run time: routed through it, these kernels' SASS changed.
                 const QsLqrRolloutIO& L = a.lio;
                 const int nz = L.n_z;
                 const long long p = (long long)L.tick0 + k;
                 const double* zn = L.z_nom + (p * N + i) * nz;
-                double dz[17];
-                const double x[13] = {d.px, d.py, d.pz, d.qx, d.qy, d.qz, d.qw, d.vx, d.vy, d.vz, d.wx, d.wy, d.wz};
+                double dz[17], x[13];
+                drone_vec(d, x);
 #pragma unroll
                 for (int q = 0; q < 13; ++q) dz[q] = x[q] - __ldg(zn + q);
                 if (nz == 17) {
@@ -180,7 +181,7 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
                                      : lqr_feedback<13>([&](int q) { return __ldg(Kj + q); }, dz);
                 }
                 if (L.lo) {
-                    const long long at = L.per_tick ? p * N + i : i;
+                    const long long at = box_row(L.per_tick, p, N, i);
                     const D4 lo = ld256_nc(L.lo, at), hi = ld256_nc(L.hi, at);
                     u[0] = qs::clampd(u[0], lo.x, hi.x); u[1] = qs::clampd(u[1], lo.y, hi.y);
                     u[2] = qs::clampd(u[2], lo.z, hi.z); u[3] = qs::clampd(u[3], lo.w, hi.w);

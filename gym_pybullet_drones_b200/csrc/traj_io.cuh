@@ -21,6 +21,15 @@ __device__ __forceinline__ void st_state(double* s, long long N, long long i, co
     s[4 * (2 * N + i)] = d.vx; s[4 * (2 * N + i) + 1] = d.vy; s[4 * (2 * N + i) + 2] = d.vz; s[4 * (2 * N + i) + 3] = d.wy;
     s[12 * N + i] = d.wz;
 }
+// the index of state component j (drone_vec's order: pos, quat x y z w, vel, rpy_rates) of drone i in a state of 13 N doubles
+__device__ __forceinline__ long long plane_at(long long N, long long i, int j) {
+    if (j < 3) return 4 * i + j;
+    if (j < 7) return 4 * (N + i) + (j - 3);
+    if (j < 10) return 4 * (2 * N + i) + (j - 7);
+    if (j == 10) return 4 * i + 3;
+    if (j == 11) return 4 * (2 * N + i) + 3;
+    return 12 * N + i;
+}
 // L += entry i of a stored [13 N] cotangent
 __device__ __forceinline__ void add_state(const double* s, long long N, long long i, qs::Drone& L) {
     qs::Drone g;

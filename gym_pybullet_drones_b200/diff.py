@@ -29,6 +29,16 @@ def unpack_states(planes, n):
     return {"pos": p0[..., 0:3], "quat": q, "vel": p2[..., 0:3], "rpy_rates": w}
 
 
+def unpack_traj(states, T, E, D):
+    """[T, 13 N] planes -> {pos, quat, vel, rpy_rates} as [T, E, D, k]."""
+    return {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, E * D).items()}
+
+
+def dyn_cfg(env):
+    """The launch configuration of the DYN kernels for `env`: (QsParams, E, D, substeps per control tick, effects)."""
+    return env._P, env._E, env._D, env.PYB_STEPS_PER_CTRL, env._effects
+
+
 def _call(name, *args, device):
     """N.lib().<name>(*args, stream) on `device` and its current stream; a refusal or launch error raises (N.check)."""
     with torch.cuda.device(device):
@@ -265,27 +275,12 @@ class DynLqrTrajectory(torch.autograd.Function):
 def _tracker_inputs(env, trk, plan, state, last_rpm, phys, num_steps=None, **schedule):
     """The checked arguments of differentiable_rollout(controller=Tracker, plan=): (cfg, T, inputs), inputs = (planes0,
     last_rpm, rows, rpm_nom, K, z_nom) as DynLqrTrajectory takes them."""
-    E, D, n, dev = env._E, env._D, env._N, env.device
+    E, D, dev = env._E, env._D, env.device
     given = sorted(k for k, v in schedule.items() if v is not None)
     if given:
         raise ValueError("a Tracker flies its plan: %s do not apply (no waypoints, start, offset, targets, gains, pid_state or "
                          "control_timestep)" % ", ".join(given))
-    if trk.env_shape != (E, D):
-        raise ValueError("the Tracker's plan is for %d x %d drones, the env has %d x %d" % (*trk.env_shape, E, D))
-    if trk.device != dev:
-        raise ValueError("the Tracker's plan is on %s, the env's state on %s" % (trk.device, dev))
-    if isinstance(trk.tick, bool) or not isinstance(trk.tick, int) or trk.tick < 0:
-        raise ValueError("Tracker.tick must be an integer >= 0, got %r" % (trk.tick,))
-    T = trk.T - trk.tick if num_steps is None else int(num_steps)
-    if T <= 0:
-        raise ValueError("num_steps must be > 0")
-    if trk.tick + T > trk.T:
-        raise ValueError("the Tracker's plan has %d ticks: ticks [%d, %d) do not fit" % (trk.T, trk.tick, trk.tick + T))
-    if env._order is not None:
-        raise ValueError("a Tracker indexes drones by id: not available on a formation reordered by reorder_by_morton()")
-    if trk.nz == 17 and last_rpm is None and not env._track_last_action:
-        raise ValueError("an n_z = 17 plan (solved with drag) needs the RPMs applied before tick 0: pass last_rpm= (this env does "
-                         "not keep last_clipped_action)")
+    T = trk.ticks(env, num_steps, last_rpm)
     plan = dict(plan or {})
     bad = set(plan) - set(PLAN_KEYS)
     if bad:
@@ -294,16 +289,16 @@ def _tracker_inputs(env, trk, plan, state, last_rpm, phys, num_steps=None, **sch
     own = dict(rpm=trk.rpm_nom, K=trk.K, z=trk.z_nom)
     tens = [_tensor(plan[k], "plan[%r]" % k, shapes[k], dev).reshape(own[k].shape) if k in plan else own[k] for k in PLAN_KEYS]
     planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
-    cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects, trk.tick, trk.box)
+    cfg = (*dyn_cfg(env), trk.tick, trk.box)
     return cfg, T, (planes0, last_rpm, rows, *tens)
 
 
 def _tracker_loop(env, trk, plan, state, last_rpm, phys, **schedule):
-    E, D, n, dev = env._E, env._D, env._N, env.device
+    E, D, dev = env._E, env._D, env.device
     cfg, T, ins = _tracker_inputs(env, trk, plan, state, last_rpm, phys, **schedule)
     with torch.cuda.device(dev):
         states, rpm = DynLqrTrajectory.apply(*ins, cfg, T)
-    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out = unpack_traj(states, T, E, D)
     out["rpm"] = rpm.reshape(T, E, D, 4)
     return out
 
@@ -464,6 +459,18 @@ def _tensor(x, name, shape, device):
     return x
 
 
+def _per_drone(x, name, width, E, D, dev, T=None):
+    """An input of `width` values per drone as [E * D, width]: from [width] (every drone) or [E, D, width], and where T is given
+    from [T, E, D, width] too, as [T, E * D, width].  Anything else raises ValueError naming `name`."""
+    if isinstance(x, torch.Tensor) and x.dim() == 1:
+        return _tensor(x, name, (width,), dev).expand(E * D, width)
+    if T is not None and isinstance(x, torch.Tensor) and x.dim() == 4:
+        if x.shape[0] != T:
+            raise ValueError("%s has %d ticks but the horizon is T = %d" % (name, x.shape[0], T))
+        return _tensor(x, name, (T, E, D, width), dev).reshape(T, E * D, width)
+    return _tensor(x, name, (E, D, width), dev).reshape(E * D, width)
+
+
 def _start_state(env, state, last_rpm, phys):
     """The planes [13 N] of the initial state, last_rpm [N, 4] and the per-aviary rows [E, 16] of differentiable_rollout."""
     from .params import PHYS_KEYS, physical_rows
@@ -546,19 +553,8 @@ def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=
     T = _rpm_ticks(env, rpm)
     planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
     with torch.cuda.device(dev):
-        cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
-        states = DynTrajectory.apply(rpm.reshape(T, n, 4).contiguous(), planes0, last_rpm.contiguous(), rows.contiguous(), cfg)
-    return {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
-
-
-def _rows3(x, name, E, D, dev):
-    """[E, D, 3] or [3] float64 tensor -> [E * D, 3]; None -> zeros."""
-    n = E * D
-    if x is None:
-        return torch.zeros((n, 3), dtype=torch.float64, device=dev)
-    if isinstance(x, torch.Tensor) and x.dim() == 1:
-        return _tensor(x, name, (3,), dev).expand(n, 3)
-    return _tensor(x, name, (E, D, 3), dev).reshape(n, 3)
+        states = DynTrajectory.apply(rpm.reshape(T, n, 4).contiguous(), planes0, last_rpm.contiguous(), rows.contiguous(), dyn_cfg(env))
+    return unpack_traj(states, T, E, D)
 
 
 def schedule_targets(waypoints, start, offset, T, E, D, dev):
@@ -586,7 +582,7 @@ def schedule_targets(waypoints, start, offset, T, E, D, dev):
     rot = torch.gather(wp, 0, idx[:, :, None].expand(W, n, 3))                               # [W, n, 3]: tick k' (k' < W)
     tpos = rot[:T] if T <= W else rot.repeat((T + W - 1) // W, 1, 1)[:T]
     if offset is not None:                  # no zero offset when there is none: -0.0 + 0.0 would change the sign of a zero target
-        tpos = tpos + _rows3(offset, "offset", E, D, dev)
+        tpos = tpos + _per_drone(offset, "offset", 3, E, D, dev)
     return tpos
 
 
@@ -613,8 +609,8 @@ def _closed_loop_inputs(env, controller, state, last_rpm, phys, caller, derivati
     if T <= 0:
         raise ValueError("num_steps must be > 0")
     tpos = schedule_targets(waypoints, start, offset, T, E, D, dev)
-    tvel, trpy, trr = (_rows3(x, k, E, D, dev) for x, k in ((target_vel, "target_vel"), (target_rpy, "target_rpy"),
-                                                             (target_rpy_rates, "target_rpy_rates")))
+    tvel, trpy, trr = (torch.zeros((n, 3), dtype=torch.float64, device=dev) if x is None else _per_drone(x, k, 3, E, D, dev)
+                       for x, k in ((target_vel, "target_vel"), (target_rpy, "target_rpy"), (target_rpy_rates, "target_rpy_rates")))
     CP = controller._P
     gains = dict(gains or {})
     bad = set(gains) - set(GAIN_KEYS)
@@ -642,11 +638,11 @@ def _closed_loop_inputs(env, controller, state, last_rpm, phys, caller, derivati
 
 
 def _closed_loop(env, controller, state, last_rpm, phys, **schedule):
-    E, D, n, dev = env._E, env._D, env._N, env.device
+    E, D, dev = env._E, env._D, env.device
     cfg, T, ins = _closed_loop_inputs(env, controller, state, last_rpm, phys, "differentiable_rollout()", "adjoint", **schedule)
     with torch.cuda.device(dev):
         states, rpm = DynCtrlTrajectory.apply(*ins, cfg)
-    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out = unpack_traj(states, T, E, D)
     out["rpm"] = rpm.reshape(T, E, D, 4)
     return out
 
@@ -701,9 +697,9 @@ def _policy_inputs(env, policy, params, noise, action_buffer, num_steps, state, 
 
 def _policy_out(env, cfg, states, actions, obs):
     """{pos, quat, vel, rpy_rates, actions, obs} of a policy loop as differentiable_rollout(policy=) returns them"""
-    E, D, n = env._E, env._D, env._N
+    E, D = env._E, env._D
     T, A, od = cfg[9], cfg[6], env._obs_dim
-    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out = unpack_traj(states, T, E, D)
     out["actions"] = actions.reshape(T, E, D, A)
     out["obs"] = obs.reshape(T, E, D, od)
     return out
@@ -741,12 +737,12 @@ def ctrl_tick_jacobians(cfg, ins):
 
 
 def _linearise_closed_loop(env, controller, state, last_rpm, phys, **schedule):
-    E, D, n, dev = env._E, env._D, env._N, env.device
+    E, D, dev = env._E, env._D, env.device
     with torch.no_grad():
         cfg, T, ins = _closed_loop_inputs(env, controller, state, last_rpm, phys, "linearise()", "tangent", **schedule)
         with torch.cuda.device(dev):
             outs, jac = ctrl_tick_jacobians(cfg, dict(zip(CTRL_INS, (x.detach().contiguous() for x in ins))))
-    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(outs["states"], n).items()}
+    out = unpack_traj(outs["states"], T, E, D)
     out["rpm"] = outs["rpm"].view(T, E, D, 4)
     out["pid_state"] = outs["pid_states"].transpose(1, 2).reshape(T, E, D, 9)
     nz = 26 if cfg[6] & N.EFFECT_DRAG else 22
@@ -813,10 +809,9 @@ def linearise(env, rpm=None, controller=None, state=None, last_rpm=None, phys=No
     T = _rpm_ticks(env, rpm)
     with torch.no_grad():
         planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
-        cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
-        states, jac = tick_jacobians(cfg, *(x.detach().contiguous() for x in (rpm.reshape(T, n, 4), planes0, last_rpm, rows)))
+        states, jac = tick_jacobians(dyn_cfg(env), *(x.detach().contiguous() for x in (rpm.reshape(T, n, 4), planes0, last_rpm, rows)))
     cols = jac.shape[-1]
-    out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
+    out = unpack_traj(states, T, E, D)
     jac = jac.view(T, E, D, 13, cols)
     out["A"], out["B"] = jac[..., :13], jac[..., 13:17]
     if cols == 21:

@@ -918,19 +918,7 @@ class BaseAviary(Env):
             if actions is not None:
                 raise ValueError("pass either actions or a controller")
             trk = controller
-            if trk.env_shape != (E, D):
-                raise ValueError("the Tracker's plan is for %d x %d drones, the env has %d x %d" % (*trk.env_shape, E, D))
-            if trk.device != dev:
-                raise ValueError("the Tracker's plan is on %s, the env's state on %s" % (trk.device, dev))
-            if isinstance(trk.tick, bool) or not isinstance(trk.tick, int) or trk.tick < 0:
-                raise ValueError("Tracker.tick must be an integer >= 0, got %r" % (trk.tick,))
-            T = trk.T - trk.tick if num_steps is None else int(num_steps)
-            if T <= 0 or trk.tick + T > trk.T:
-                raise ValueError("the Tracker's plan has %d ticks: ticks [%d, %d) do not fit" % (trk.T, trk.tick, trk.tick + T))
-            if self._order is not None:
-                raise ValueError("a Tracker indexes drones by id: not available on a formation reordered by reorder_by_morton()")
-            if trk.nz == 17 and not self._track_last_action:
-                raise ValueError("an n_z = 17 plan (solved with drag) needs the env's last_clipped_action, which this env does not keep")
+            T = trk.ticks(self, num_steps)
             lio = trk._io(trk.tick)
         elif mode in (N.CTRL_TRACK, N.CTRL_MRAC):
             if actions is not None:

@@ -11,13 +11,16 @@ import ctypes as C
 import torch
 
 from . import _native as N
-from .diff import STATE_KEYS, _call, _dyn_traj_vjp, _io, _refuse_downwash, _start_state, _tensor, _traj_ptrs, pack_state, unpack_states
+from .diff import (STATE_KEYS, _call, _dyn_traj_vjp, _io, _per_drone, _refuse_downwash, _start_state, _tensor, _traj_ptrs, dyn_cfg,
+                   pack_state, unpack_states, unpack_traj)
 
 ALPHAS = tuple(2.0 ** -j for j in range(10))               # the line search's step sizes, largest first
 DEFAULT_Q = (1.0,) * 3 + (1.0,) * 4 + (0.1,) * 3 + (0.01,) * 3   # pos, quat, vel, rpy_rates
 DEFAULT_R = (1e-2,) * 4                                    # on the command relative to HOVER_RPM
 FINAL_SCALE = 100.0                                        # Q_final = FINAL_SCALE * Q by default
 HOVER_TARGET = {"quat": (0.0, 0.0, 0.0, 1.0), "vel": (0.0, 0.0, 0.0), "rpy_rates": (0.0, 0.0, 0.0)}
+# one aviary's row of the packed weights [E, 30] (QsIlqrIO.weights): [Q | Q_final | R]
+W_Q, W_Q_FINAL, W_R = slice(0, 13), slice(13, 26), slice(26, 30)
 
 
 def pack_traj(pos, quat, vel, w):
@@ -32,47 +35,25 @@ def _target_ticks(target):
     return {x.shape[0] for x in target.values() if isinstance(x, torch.Tensor) and x.dim() == 4}
 
 
-def _target_part(x, name, width, T, E, D, dev):
-    """target[name] as [T, E * D, width]: from [width], [E, D, width] or [T, E, D, width]."""
-    if not isinstance(x, torch.Tensor):
-        raise ValueError("%s must be a float64 tensor [%d], [%d, %d, %d] or [%d, %d, %d, %d]" % (name, width, E, D, width, T, E, D, width))
-    if x.dim() == 1:
-        return _tensor(x, name, (width,), dev).expand(T, E * D, width)
-    if x.dim() == 3:
-        return _tensor(x, name, (E, D, width), dev).reshape(1, E * D, width).expand(T, E * D, width)
-    return _tensor(x, name, (T, E, D, width), dev).reshape(T, E * D, width)
-
-
-def _bound(x, name, T, E, D, dev):
-    """One side of rpm_bounds as ([E * D, 4] or [T, E * D, 4], has a time axis): from [4], [E, D, 4] or [T, E, D, 4]."""
-    if not isinstance(x, torch.Tensor) or x.dim() not in (1, 3, 4):
-        raise ValueError("%s must be a float64 CUDA tensor [4], [%d, %d, 4] or [%d, %d, %d, 4]" % (name, E, D, T, E, D))
-    if x.dim() == 1:
-        return _tensor(x, name, (4,), dev).expand(E * D, 4), False
-    if x.dim() == 3:
-        return _tensor(x, name, (E, D, 4), dev).reshape(E * D, 4), False
-    if x.shape[0] != T:
-        raise ValueError("ilqr(): %s has %d ticks but the horizon is T = %d" % (name, x.shape[0], T))
-    return _tensor(x, name, (T, E, D, 4), dev).reshape(T, E * D, 4), True
-
-
-def _rpm_box(rpm_bounds, rows, T, E, D, dev):
-    """rpm_bounds as (lo, hi, per_tick, ok): lo and hi [N, 4] (per_tick False) or [T, N, 4] (True), contiguous, and ok a 0-dim
-    bool tensor (not read here) that is true when no bound is NaN, lo <= hi and 0 <= lo, hi <= MAX_RPM of each drone's row."""
-    n = E * D
-    max_rpm = rows[:, 13].reshape(E, 1, 1).expand(E, D, 4).reshape(n, 4)
+def _rpm_box(rpm_bounds, T, E, D, dev, max_rpm=None):
+    """rpm_bounds (None, "motor" or a pair (lo, hi) of [4], [E, D, 4] or [T, E, D, 4]) as None or (lo, hi, per_tick, ok): owned
+    contiguous lo, hi [N, 4] or, per tick, [T, N, 4], and a 0-dim bool ok (not read here): no NaN, lo <= hi and, with each drone's
+    max_rpm [N, 4], 0 <= lo, hi <= max_rpm.  "motor" is the box [0, max_rpm], or None (the env's clip only) without max_rpm."""
+    if rpm_bounds is None or (isinstance(rpm_bounds, str) and rpm_bounds == "motor" and max_rpm is None):
+        return None
     if isinstance(rpm_bounds, str) and rpm_bounds == "motor":
-        lo = torch.zeros((n, 4), dtype=torch.float64, device=dev)
-        return lo, max_rpm.contiguous(), False, torch.ones((), dtype=torch.bool, device=dev)
+        return torch.zeros_like(max_rpm), max_rpm.clone(), False, torch.ones((), dtype=torch.bool, device=dev)
     if not isinstance(rpm_bounds, (tuple, list)) or len(rpm_bounds) != 2:
         raise ValueError("rpm_bounds must be None, 'motor' or a pair (lo, hi) of float64 CUDA tensors in raw RPM")
-    lo, lo_t = _bound(rpm_bounds[0], "rpm_bounds[0] (lo)", T, E, D, dev)
-    hi, hi_t = _bound(rpm_bounds[1], "rpm_bounds[1] (hi)", T, E, D, dev)
-    per_tick = lo_t or hi_t
+    lo = _per_drone(rpm_bounds[0], "rpm_bounds[0] (lo)", 4, E, D, dev, T)
+    hi = _per_drone(rpm_bounds[1], "rpm_bounds[1] (hi)", 4, E, D, dev, T)
+    per_tick = lo.dim() == 3 or hi.dim() == 3
     if per_tick:
-        lo, hi = lo.expand(T, n, 4), hi.expand(T, n, 4)
-    lo, hi = lo.detach().contiguous(), hi.detach().contiguous()
-    ok = ~(torch.isnan(lo).any() | torch.isnan(hi).any()) & (lo <= hi).all() & (lo >= 0).all() & (hi <= max_rpm).all()
+        lo, hi = lo.expand(T, E * D, 4), hi.expand(T, E * D, 4)
+    lo, hi = lo.detach().clone(memory_format=torch.contiguous_format), hi.detach().clone(memory_format=torch.contiguous_format)
+    ok = ~(torch.isnan(lo).any() | torch.isnan(hi).any()) & (lo <= hi).all()
+    if max_rpm is not None:
+        ok = ok & (lo >= 0).all() & (hi <= max_rpm).all()
     return lo, hi, per_tick, ok
 
 
@@ -133,24 +114,27 @@ class Problem:
             raise ValueError("alphas must hold 1 to 16 step sizes")
         with contextlib.nullcontext() if graph else torch.no_grad():
             planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
-            parts = [_target_part(target[k], "target[%r]" % k, w, T, E, D, dev) if k in target
-                     else _target_part(torch.tensor(HOVER_TARGET[k], dtype=torch.float64, device=dev), k, w, T, E, D, dev)
+            parts = [_per_drone(target[k], "target[%r]" % k, w, E, D, dev, T) if k in target
+                     else _per_drone(torch.tensor(HOVER_TARGET[k], dtype=torch.float64, device=dev), k, w, E, D, dev)
                      for k, w in STATE_KEYS]
+            parts = [x if x.dim() == 3 else x.expand(T, n, x.shape[-1]) for x in parts]
             targets = pack_traj(*parts)
             self.targets = targets.detach().contiguous()
             q = _weight(Q, "Q", DEFAULT_Q, E, dev)
             qf = FINAL_SCALE * q if Q_final is None else _weight(Q_final, "Q_final", DEFAULT_Q, E, dev)
             r = _weight(R, "R", DEFAULT_R, E, dev)
-            weights = torch.cat([q, qf, r], dim=1)
+            weights = torch.cat([q, qf, r], dim=1)                 # W_Q, W_Q_FINAL, W_R
             self.weights = weights.detach().contiguous()
             w_ok = torch.isfinite(self.weights).all() & (self.weights >= 0).all() & (r > 0).all()
-            if rpm_bounds is None:
+            max_rpm = rows[:, 13].reshape(E, 1, 1).expand(E, D, 4).reshape(n, 4)
+            box = _rpm_box(rpm_bounds, T, E, D, dev, max_rpm)
+            if box is None:
                 # the one synchronisation of a solve: the weights' values
                 if not bool(w_ok.item()):
                     raise ValueError("ilqr(): Q and Q_final must be finite and >= 0, R finite and > 0")
                 self.box = None
             else:
-                lo, hi, per_tick, b_ok = _rpm_box(rpm_bounds, rows, T, E, D, dev)
+                lo, hi, per_tick, b_ok = box
                 # the one synchronisation of a solve: the weights' and the bounds' values
                 w_ok, b_ok = torch.stack([w_ok, b_ok]).tolist()
                 if not w_ok:
@@ -158,14 +142,9 @@ class Problem:
                 if not b_ok:
                     raise ValueError("ilqr(): rpm_bounds must not be NaN and must satisfy 0 <= lo <= hi <= MAX_RPM of each "
                                      "drone's row")
-                self.box = (lo.detach(), hi.detach(), per_tick)      # "motor": MAX_RPM is a constant
+                self.box = (lo, hi, per_tick)                        # "motor": MAX_RPM is a constant
             hover = rows[:, 12].reshape(E, 1, 1).expand(E, D, 4)
-            if rpm_ref is None:
-                ref = hover.reshape(n, 4)
-            elif isinstance(rpm_ref, torch.Tensor) and rpm_ref.dim() == 1:
-                ref = _tensor(rpm_ref, "rpm_ref", (4,), dev).expand(n, 4)
-            else:
-                ref = _tensor(rpm_ref, "rpm_ref", (E, D, 4), dev).reshape(n, 4)
+            ref = hover.reshape(n, 4) if rpm_ref is None else _per_drone(rpm_ref, "rpm_ref", 4, E, D, dev)
             self.rpm_ref = ref.detach().contiguous()
             if rpm is None:
                 rpm = hover.reshape(1, n, 4).expand(T, n, 4)
@@ -178,7 +157,7 @@ class Problem:
         self.env_shape = (E, D)
         self.graph = (targets, weights, ref, planes0, last_rpm, rows) if graph else None
         self.planes0, self.last_rpm, self.rows = planes0.detach().contiguous(), last_rpm.detach().contiguous(), rows.detach().contiguous()
-        self.cfg = (env._P, E, D, env.PYB_STEPS_PER_CTRL, env._effects)
+        self.cfg = dyn_cfg(env)
         self.T, self.n, self.dev = T, n, dev
         self.nz = 17 if env._effects & N.EFFECT_DRAG else 13
         f64 = dict(dtype=torch.float64, device=dev)
@@ -243,8 +222,8 @@ class Problem:
 
     def result(self, cost):
         E, D = self.env_shape
-        T, n = self.T, self.n
-        out = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(self.states, n).items()}
+        T = self.T
+        out = unpack_traj(self.states, T, E, D)
         out["rpm"] = self.rpm.view(T, E, D, 4)
         out["K"] = self.K.view(T, E, D, 4, self.nz)
         out["z"] = self.loop_states().view(T, E, D, self.nz)
@@ -330,8 +309,8 @@ def state_weights(weights, E, D, T):
     packed weights [E, 30]."""
     n = E * D
     planes = lambda q: pack_state(q[:, 0:3], q[:, 3:7], q[:, 7:10], q[:, 10:13])
-    q = weights[:, 0:13].repeat_interleave(D, dim=0)
-    qf = weights[:, 13:26].repeat_interleave(D, dim=0)
+    q = weights[:, W_Q].repeat_interleave(D, dim=0)
+    qf = weights[:, W_Q_FINAL].repeat_interleave(D, dim=0)
     return torch.cat([planes(q).reshape(1, 13 * n).expand(T - 1, 13 * n), planes(qf).reshape(1, 13 * n)])
 
 
@@ -390,7 +369,7 @@ class IlqrSolution(torch.autograd.Function):
             tg, wt, ref, rows = (x.detach().requires_grad_(j in cost_ins)
                                  for j, x in ((0, p.targets), (1, p.weights), (2, p.rpm_ref), (5, p.rows)))
             with torch.enable_grad():
-                Rt = (wt[:, 26:30] / (rows[:, 12:13] * rows[:, 12:13])).repeat_interleave(D, dim=0)
+                Rt = (wt[:, W_R] / (rows[:, 12:13] * rows[:, 12:13])).repeat_interleave(D, dim=0)
                 s = -((state_weights(wt, E, D, T) * (states - tg) * dx).sum() + (Rt * (rpm - ref) * w).sum())
                 got = torch.autograd.grad(s, [x for j, x in zip((0, 1, 2, 5), (tg, wt, ref, rows)) if j in cost_ins])
             for j, g in zip(cost_ins, got):
@@ -418,9 +397,8 @@ def differentiable_ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q
     out = {}
     states, rpm_out = IlqrSolution.apply(*p.graph, p, iters, out)
     E, D = p.env_shape
-    T, n = p.T, p.n
-    sol = {k: v.reshape(T, E, D, v.shape[-1]) for k, v in unpack_states(states, n).items()}
-    sol["rpm"] = rpm_out.view(T, E, D, 4)
+    sol = unpack_traj(states, p.T, E, D)
+    sol["rpm"] = rpm_out.view(p.T, E, D, 4)
     for k in ("K", "z", "k", "cost", "mu", "converged", "active"):
         if k in out:
             sol[k] = out[k]
@@ -481,19 +459,10 @@ class Tracker:
             self.K = K.detach().reshape(T, n, 4, nz).clone(**dense)                     # [T][N][4][n_z]
             self.z_nom = z.detach().reshape(T, n, nz).clone(**dense)                    # [T][N][n_z]
             self.rpm_nom = rpm.detach().reshape(T, n, 4).clone(**dense)                 # [T][N][4]: one 32-byte load per drone
-            self.box = None
-            if not (rpm_bounds is None or (isinstance(rpm_bounds, str) and rpm_bounds == "motor")):
-                if not isinstance(rpm_bounds, (tuple, list)) or len(rpm_bounds) != 2:
-                    raise ValueError("rpm_bounds must be None, 'motor' or a pair (lo, hi) of float64 CUDA tensors in raw RPM")
-                lo, lo_t = _bound(rpm_bounds[0], "rpm_bounds[0] (lo)", T, E, D, dev)
-                hi, hi_t = _bound(rpm_bounds[1], "rpm_bounds[1] (hi)", T, E, D, dev)
-                per_tick = lo_t or hi_t
-                if per_tick:
-                    lo, hi = lo.expand(T, n, 4), hi.expand(T, n, 4)
-                lo, hi = lo.detach().clone().contiguous(), hi.detach().clone().contiguous()      # owned, 32-byte aligned
-                if not bool((~(torch.isnan(lo).any() | torch.isnan(hi).any()) & (lo <= hi).all()).item()):
-                    raise ValueError("Tracker: rpm_bounds must not be NaN and must satisfy lo <= hi")
-                self.box = (lo, hi, per_tick)
+            box = _rpm_box(rpm_bounds, T, E, D, dev)                                  # owned, 32-byte aligned
+            if box is not None and not bool(box[3].item()):
+                raise ValueError("Tracker: rpm_bounds must not be NaN and must satisfy lo <= hi")
+            self.box = None if box is None else box[:3]
         self.T, self.env_shape, self.nz, self.device = T, (E, D), nz, dev
         self.tick = 0
 
@@ -503,3 +472,25 @@ class Tracker:
         return N.QsLqrRolloutIO(K=self.K.data_ptr(), z_nom=self.z_nom.data_ptr(), rpm_nom=self.rpm_nom.data_ptr(),
                                 lo=None if lo is None else lo.data_ptr(), hi=None if hi is None else hi.data_ptr(),
                                 per_tick=int(per_tick), n_z=self.nz, T_plan=self.T, tick0=tick)
+
+    def ticks(self, env, num_steps=None, last_rpm=None):
+        """The ticks of a rollout of `env` from plan tick self.tick (num_steps, or the rest of the plan), after checking this plan
+        against env; `last_rpm` (differentiable_rollout()'s) stands in for env's last_clipped_action for an n_z = 17 plan."""
+        E, D = env._E, env._D
+        if self.env_shape != (E, D):
+            raise ValueError("the Tracker's plan is for %d x %d drones, the env has %d x %d" % (*self.env_shape, E, D))
+        if self.device != env.device:
+            raise ValueError("the Tracker's plan is on %s, the env's state on %s" % (self.device, env.device))
+        if isinstance(self.tick, bool) or not isinstance(self.tick, int) or self.tick < 0:
+            raise ValueError("Tracker.tick must be an integer >= 0, got %r" % (self.tick,))
+        T = self.T - self.tick if num_steps is None else int(num_steps)
+        if num_steps is not None and T <= 0:
+            raise ValueError("num_steps must be > 0")
+        if T <= 0 or self.tick + T > self.T:
+            raise ValueError("the Tracker's plan has %d ticks: ticks [%d, %d) do not fit" % (self.T, self.tick, self.tick + T))
+        if env._order is not None:
+            raise ValueError("a Tracker indexes drones by id: not available on a formation reordered by reorder_by_morton()")
+        if self.nz == 17 and last_rpm is None and not env._track_last_action:
+            raise ValueError("an n_z = 17 plan (solved with drag) needs the RPMs applied before tick 0: the env's last_clipped_action, "
+                             "which this env does not keep (differentiable_rollout() also takes last_rpm=)")
+        return T

@@ -7,6 +7,22 @@
 #include "harness.h"
 
 namespace {
+// one drone's plan tick in host arrays, as lqr_law.cuh's tracker reads it
+template <int NZ>
+struct HostPlan {
+    const double *z_nom, *k, *rpm_nom, *lo, *hi;
+    double zn(int q) const { return z_nom[q]; }
+    double K(int j, int q) const { return k[j * NZ + q]; }
+    void nom(double b[4]) const {
+        for (int j = 0; j < 4; ++j) b[j] = rpm_nom[j];
+    }
+    bool box(double l[4], double h[4]) const {
+        if (!lo) return false;
+        for (int j = 0; j < 4; ++j) { l[j] = lo[j]; h[j] = hi[j]; }
+        return true;
+    }
+};
+
 template <int EFF, int NZ>
 void lqr_tick_vjp(const QsParams& P, const double* row, int S, const double* state, const double* up, const double* rpm_nom,
                   const double* K, const double* z_nom, const double* lo, const double* hi, const double* g_out, const double* g_rpm,
@@ -14,21 +30,12 @@ void lqr_tick_vjp(const QsParams& P, const double* row, int S, const double* sta
                   double* g_z_nom) {
     const qs::PhysRow c = row_from(P, row);
     const qs::Drone d0 = drone_from(state);
-    // forward, as tracker_command + one tick of dyn_lqr_traj_kernel
-    double dz[NZ];
-    for (int q = 0; q < 13; ++q) dz[q] = state[q] - z_nom[q];
-    for (int q = 13; q < NZ; ++q) dz[q] = up[q - 13] - z_nom[q];
+    // forward, as one tick of dyn_lqr_traj_kernel: the shared tracker_command, then the env's clip
+    const HostPlan<NZ> pl = {z_nom, K, rpm_nom, lo, hi};
     double b[4], u[4];
     bool keep[4];
-    for (int j = 0; j < 4; ++j) {
-        b[j] = rpm_nom[j] + qsi::lqr_feedback<NZ>([&](int q) { return K[j * NZ + q]; }, dz);
-        keep[j] = true;
-        if (lo) {
-            keep[j] = !(b[j] < lo[j]) && !(b[j] > hi[j]);
-            b[j] = qs::clampd(b[j], lo[j], hi[j]);
-        }
-        u[j] = qs::clampd(b[j], 0.0, c.max_rpm);
-    }
+    qsi::tracker_command<NZ>(pl, d0, up, b, keep);
+    for (int j = 0; j < 4; ++j) u[j] = qs::clampd(b[j], 0.0, c.max_rpm);
     qs::Drone d = d0;
     double R_last[9];
     qs::dyn_tick_k<EFF>(P, c, d, u, up, 0.0, S, R_last);
@@ -42,10 +49,11 @@ void lqr_tick_vjp(const QsParams& P, const double* row, int S, const double* sta
     qs::PhysGrad G;
     for (int j = 0; j < 16; ++j) G.g[j] = 0.0;
     qs::dyn_tick_vjp<EFF>(P, c, d0, u, up, S, rec, L, Lu, Lup, G);
-    double lam[4], Ktl[NZ];
+    double lam[4], dz[NZ], Ktl[NZ];
+    qsi::tracker_dz<NZ>(pl, d0, up, dz);
     qs::rpm_clip_vjp(b, c.max_rpm, Lu, lam, G.g[13]);
     for (int j = 0; j < 4; ++j) lam[j] = keep[j] ? lam[j] : 0.0;
-    qsi::lqr_feedback_vjp<NZ>([&](int j, int q) { return K[j * NZ + q]; }, dz, lam, [&](int j, int q, double g) { g_K[j * NZ + q] = g; },
+    qsi::lqr_feedback_vjp<NZ>([&](int j, int q) { return pl.K(j, q); }, dz, lam, [&](int j, int q, double g) { g_K[j * NZ + q] = g; },
                               Ktl);
     double gs[13];
     drone_to(L, gs);
