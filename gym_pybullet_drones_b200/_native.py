@@ -14,8 +14,8 @@ LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
-                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu", "ilqr_adjoint.cu")]
-HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "lqr_law.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
+                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu", "ilqr_adjoint.cu", "mppi.cu")]
+HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "lqr_law.cuh"), os.path.join(_CSRC, "philox.cuh"), os.path.join(_CSRC, "mppi.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
@@ -208,6 +208,12 @@ class QsIlqrAdjointIO(C.Structure):
         "jac", "rpm", "phys", "weights", "active", "g_states", "g_rpm", "K", "k", "status", "w", "dx")]
 
 
+class QsMppiIO(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("T", "K", "iteration", "per_tick")] + [("seed", C.c_ulonglong), ("temperature", _d)] + [
+        (n, C.c_void_p) for n in ("state0", "last_rpm", "phys", "targets", "weights", "rpm_ref", "sigma", "rpm_lo", "rpm_hi", "rpm",
+                                  "states", "J", "cand", "cost_out", "pick", "noise")]
+
+
 class QsStepCall(C.Structure):
     _fields_ = [("p", C.c_void_p), ("st", C.c_void_p), ("io", C.c_void_p),
                 ("act_type", C.c_int), ("task", C.c_int), ("n_envs", C.c_int), ("drones_per_env", C.c_int), ("substeps", C.c_int),
@@ -226,7 +232,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_ilqr_backward", "qs_ilqr_line_search", "qs_ilqr_commit", "qs_sizeof_ilqr_io", "qs_ilqr_box_backward",
            "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io", "qs_ctrl_rollout_lqr",
            "qs_sizeof_lqr_rollout_io", "qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp", "qs_sizeof_dyn_lqr_traj_io",
-           "qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout", "qs_sizeof_ilqr_adjoint_io"]
+           "qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout", "qs_sizeof_ilqr_adjoint_io", "qs_mppi_sample", "qs_mppi_update",
+           "qs_mppi_commit", "qs_mppi_noise", "qs_sizeof_mppi_io"]
 MAX_PEERS = 16
 
 
@@ -274,7 +281,7 @@ _MIRRORS = (("params", QsParams), ("state", QsState), ("step_io", QsStepIO), ("r
             ("dyn_ctrl_traj_io", QsDynCtrlTrajIO), ("dyn_policy_traj_io", QsDynPolicyTrajIO), ("dyn_lqr_traj_io", QsDynLqrTrajIO),
             ("dyn_traj_jvp_io", QsDynTrajJvpIO), ("dyn_ctrl_traj_jvp_io", QsDynCtrlTrajJvpIO),
             ("dyn_policy_traj_jvp_io", QsDynPolicyTrajJvpIO), ("ilqr_io", QsIlqrIO), ("ilqr_box_io", QsIlqrBoxIO),
-            ("ilqr_adjoint_io", QsIlqrAdjointIO))
+            ("ilqr_adjoint_io", QsIlqrAdjointIO), ("mppi_io", QsMppiIO))
 
 
 def lib():
@@ -359,6 +366,11 @@ def lib():
     for n in ("qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsIlqrAdjointIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
+    for n in ("qs_mppi_sample", "qs_mppi_update", "qs_mppi_commit"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsMppiIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
+    L.qs_mppi_noise.restype = C.c_int
+    L.qs_mppi_noise.argtypes = [C.POINTER(QsMppiIO), C.c_int, C.c_int, C.c_void_p]
     L.qs_dyn_substeps.restype = C.c_int
     L.qs_dyn_substeps.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]

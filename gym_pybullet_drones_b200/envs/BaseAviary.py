@@ -759,6 +759,37 @@ class BaseAviary(Env):
         return ilqr(self, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, iters=iters, state=state,
                     last_rpm=last_rpm, phys=phys, rpm_bounds=rpm_bounds)
 
+    def mppi(self, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=30, samples=64, sigma=0.02,
+             temperature=0.1, seed=0, state=None, last_rpm=None, phys=None, rpm_bounds=None):
+        """Raw-RPM trajectories by MPPI (model predictive path integral) on the device (DESIGN.md 4.5.2): the problem and the cost
+        J of ilqr(), minimised by importance-weighted averages of random perturbations of the nominal plan.  It needs only the
+        forward tick, so it runs on every Physics mode of the DYN family, downwash included (PYB_DW, PYB_GND_DRAG_DW), which
+        ilqr() refuses.  Without downwash every drone is its own problem; with downwash the unit is the aviary (at most 128
+        drones): one sample perturbs all its drones together and the decisions use the sum of their J in drone order.
+
+        target, num_steps, rpm (the initial guess), Q, R, Q_final, rpm_ref, state, last_rpm, phys and rpm_bounds: as ilqr(), with
+        the same shapes, defaults and checks, in one synchronisation with sigma's.  samples: K in [2, 1024]; sample 0 is always
+        the nominal.  sigma: the noise scale relative to each aviary's HOVER_RPM, a number or a float64 tensor [] or [E],
+        finite and > 0.  temperature: finite and > 0.  seed: an integer in [0, 2^64).
+
+        Iteration j: sample s applies v_k = rpm[k] + sigma HOVER_RPM eps (clamped to the box with rpm_bounds), eps the standard
+        normals of Philox4x32-10 at counter (k, s, drone id, 2 j + h); J_min and the mean over the finite J_s give
+        lambda = temperature (mean - J_min) and w_s = exp(-(J_s - J_min) / lambda); the candidate rpm + sum w_s delta_s / sum w_s
+        is kept when its J is no worse than the best sample's, otherwise the best sample is.  So a unit's cost never increases.
+        The same seed gives the same bits.
+
+        Returns (indices are drone ids, also after reorder_by_morton() without downwash):
+          pos, quat, vel, rpy_rates [T, E, D, k]  the final nominal trajectory: differentiable_rollout(rpm=rpm) bit for bit, with
+                     downwash CtrlAviary.rollout(actions=rpm)'s
+          rpm        [T, E, D, 4]
+          cost       [iters + 1, E, D]  each drone's J per iteration, row 0 the initial guess
+        The env is not touched, the result is not differentiable and nothing is read back to the host after the checks.
+        ilqr()'s refusals but downwash, samples, sigma, temperature or seed out of range, more than 128 drones per aviary with
+        downwash and a formation reordered by reorder_by_morton() with downwash raise ValueError."""
+        from ..mppi import mppi
+        return mppi(self, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, iters=iters, samples=samples,
+                    sigma=sigma, temperature=temperature, seed=seed, state=state, last_rpm=last_rpm, phys=phys, rpm_bounds=rpm_bounds)
+
     def differentiable_ilqr(self, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None,
                             last_rpm=None, phys=None, rpm_bounds=None):
         """ilqr() with gradients of the solution (DESIGN.md 4.5.1 "Gradients of the solution"): the same arguments and the same

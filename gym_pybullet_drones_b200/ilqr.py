@@ -72,6 +72,87 @@ def _weight(x, name, default, E, dev):
     return _tensor(x, name, (E, width), dev)
 
 
+def horizon(env, target, num_steps, rpm, what):
+    """T of a planner's call (ilqr(), mppi()) from num_steps, the target's time axis and rpm, every one that is given agreeing,
+    after checking the target's keys; anything else raises ValueError naming `what`."""
+    E, D = env._E, env._D
+    if not isinstance(target, dict) or "pos" not in target:
+        raise ValueError("target must be a dict with 'pos' ([3], [%d, %d, 3] or [T, %d, %d, 3]) and optionally quat, vel and "
+                         "rpy_rates" % (E, D, E, D))
+    bad = set(target) - {k for k, _ in STATE_KEYS}
+    if bad:
+        raise ValueError("unknown target keys %s (expected pos, quat, vel, rpy_rates)" % sorted(bad))
+    given = {}
+    if num_steps is not None:
+        given["num_steps"] = {int(num_steps)}
+    if _target_ticks(target):
+        given["target"] = _target_ticks(target)
+    if rpm is not None:
+        if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
+            raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
+        given["rpm"] = {rpm.shape[0]}
+    if not given:
+        raise ValueError("%s needs the horizon: num_steps, a target with a time axis [T, %d, %d, k] or rpm [T, %d, %d, 4]"
+                         % (what, E, D, E, D))
+    ticks = set().union(*given.values())
+    if len(ticks) != 1:
+        raise ValueError("%s: the horizons of %s disagree (%s)" % (what, ", ".join(sorted(given)), sorted(ticks)))
+    T = ticks.pop()
+    if T <= 0:
+        raise ValueError("%s: the horizon T must be > 0, got %d" % (what, T))
+    return T
+
+
+def pack_inputs(env, target, T, rpm, Q, R, Q_final, rpm_ref, state, last_rpm, phys, rpm_bounds, what, checks=(), graph=False):
+    """The packed inputs of a planner's problem over T ticks (arguments as BaseAviary.ilqr), as a dict: targets [T, 13 N],
+    weights [E, 30], rpm_ref [N, 4], the guess rpm [T, N, 4] (owned, projected into the box), box None or (lo, hi, per_tick),
+    planes0 [13 N], last_rpm [N, 4], rows [E, 16] and graph (with `graph`: the recorded (targets, weights, rpm_ref, planes0,
+    last_rpm, rows), else None).  The values of the weights, of the bounds and of every (ok, message) of `checks` (0-dim bool
+    tensors) are read in one synchronisation; the first that fails raises ValueError."""
+    E, D, n, dev = env._E, env._D, env._N, env.device
+    out = {}
+    with contextlib.nullcontext() if graph else torch.no_grad():
+        planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
+        parts = [_per_drone(target[k], "target[%r]" % k, w, E, D, dev, T) if k in target
+                 else _per_drone(torch.tensor(HOVER_TARGET[k], dtype=torch.float64, device=dev), k, w, E, D, dev)
+                 for k, w in STATE_KEYS]
+        parts = [x if x.dim() == 3 else x.expand(T, n, x.shape[-1]) for x in parts]
+        targets = pack_traj(*parts)
+        out["targets"] = targets.detach().contiguous()
+        q = _weight(Q, "Q", DEFAULT_Q, E, dev)
+        qf = FINAL_SCALE * q if Q_final is None else _weight(Q_final, "Q_final", DEFAULT_Q, E, dev)
+        r = _weight(R, "R", DEFAULT_R, E, dev)
+        weights = torch.cat([q, qf, r], dim=1)                 # W_Q, W_Q_FINAL, W_R
+        out["weights"] = weights.detach().contiguous()
+        oks = [(torch.isfinite(out["weights"]).all() & (out["weights"] >= 0).all() & (r > 0).all(),
+                "%s: Q and Q_final must be finite and >= 0, R finite and > 0" % what)]
+        max_rpm = rows[:, 13].reshape(E, 1, 1).expand(E, D, 4).reshape(n, 4)
+        box = _rpm_box(rpm_bounds, T, E, D, dev, max_rpm)
+        if box is not None:
+            oks.append((box[3], "%s: rpm_bounds must not be NaN and must satisfy 0 <= lo <= hi <= MAX_RPM of each drone's row" % what))
+        oks += list(checks)
+        # the one synchronisation of a solve: the weights', the bounds' and the checks' values
+        vals = [bool(oks[0][0].item())] if len(oks) == 1 else torch.stack([ok for ok, _ in oks]).tolist()
+        for v, (_, msg) in zip(vals, oks):
+            if not v:
+                raise ValueError(msg)
+        out["box"] = None if box is None else box[:3]                # "motor": MAX_RPM is a constant
+        hover = rows[:, 12].reshape(E, 1, 1).expand(E, D, 4)
+        ref = hover.reshape(n, 4) if rpm_ref is None else _per_drone(rpm_ref, "rpm_ref", 4, E, D, dev)
+        out["rpm_ref"] = ref.detach().contiguous()
+        if rpm is None:
+            rpm = hover.reshape(1, n, 4).expand(T, n, 4)
+        else:
+            rpm = _tensor(rpm, "rpm", (T, E, D, 4), dev).reshape(T, n, 4)
+        out["rpm"] = rpm.detach().clone().contiguous()
+        if out["box"] is not None:                           # the guess projected into the box
+            lo, hi, per_tick = out["box"]
+            torch.minimum(torch.maximum(out["rpm"], lo), hi, out=out["rpm"])
+    out["planes0"], out["last_rpm"], out["rows"] = planes0, last_rpm, rows
+    out["graph"] = (targets, weights, ref, planes0, last_rpm, rows) if graph else None
+    return out
+
+
 class Problem:
     """The device buffers of one batched iLQR solve and its steps.  Arguments as BaseAviary.ilqr; `alphas` are the line
     search's step sizes (1 to 16).  `feedback = False` runs the line search and the commit with K = 0 (an open-loop line
@@ -84,78 +165,15 @@ class Problem:
                  phys=None, alphas=ALPHAS, rpm_bounds=None, graph=False):
         _refuse_downwash(env, "ilqr()", "Jacobian")
         E, D, n, dev = env._E, env._D, env._N, env.device
-        if not isinstance(target, dict) or "pos" not in target:
-            raise ValueError("target must be a dict with 'pos' ([3], [%d, %d, 3] or [T, %d, %d, 3]) and optionally quat, vel and "
-                             "rpy_rates" % (E, D, E, D))
-        bad = set(target) - {k for k, _ in STATE_KEYS}
-        if bad:
-            raise ValueError("unknown target keys %s (expected pos, quat, vel, rpy_rates)" % sorted(bad))
-        # T from num_steps, the target's time axis and rpm: every one that is given must agree
-        given = {}
-        if num_steps is not None:
-            given["num_steps"] = {int(num_steps)}
-        if _target_ticks(target):
-            given["target"] = _target_ticks(target)
-        if rpm is not None:
-            if not isinstance(rpm, torch.Tensor) or rpm.dim() != 4:
-                raise ValueError("rpm must be a [T, %d, %d, 4] float64 CUDA tensor" % (E, D))
-            given["rpm"] = {rpm.shape[0]}
-        if not given:
-            raise ValueError("ilqr() needs the horizon: num_steps, a target with a time axis [T, %d, %d, k] or rpm [T, %d, %d, 4]"
-                             % (E, D, E, D))
-        ticks = set().union(*given.values())
-        if len(ticks) != 1:
-            raise ValueError("ilqr(): the horizons of %s disagree (%s)" % (", ".join(sorted(given)), sorted(ticks)))
-        T = ticks.pop()
-        if T <= 0:
-            raise ValueError("ilqr(): the horizon T must be > 0, got %d" % T)
+        T = horizon(env, target, num_steps, rpm, "ilqr()")
         alphas = tuple(float(a) for a in alphas)
         if not 1 <= len(alphas) <= 16:
             raise ValueError("alphas must hold 1 to 16 step sizes")
-        with contextlib.nullcontext() if graph else torch.no_grad():
-            planes0, last_rpm, rows = _start_state(env, state, last_rpm, phys)
-            parts = [_per_drone(target[k], "target[%r]" % k, w, E, D, dev, T) if k in target
-                     else _per_drone(torch.tensor(HOVER_TARGET[k], dtype=torch.float64, device=dev), k, w, E, D, dev)
-                     for k, w in STATE_KEYS]
-            parts = [x if x.dim() == 3 else x.expand(T, n, x.shape[-1]) for x in parts]
-            targets = pack_traj(*parts)
-            self.targets = targets.detach().contiguous()
-            q = _weight(Q, "Q", DEFAULT_Q, E, dev)
-            qf = FINAL_SCALE * q if Q_final is None else _weight(Q_final, "Q_final", DEFAULT_Q, E, dev)
-            r = _weight(R, "R", DEFAULT_R, E, dev)
-            weights = torch.cat([q, qf, r], dim=1)                 # W_Q, W_Q_FINAL, W_R
-            self.weights = weights.detach().contiguous()
-            w_ok = torch.isfinite(self.weights).all() & (self.weights >= 0).all() & (r > 0).all()
-            max_rpm = rows[:, 13].reshape(E, 1, 1).expand(E, D, 4).reshape(n, 4)
-            box = _rpm_box(rpm_bounds, T, E, D, dev, max_rpm)
-            if box is None:
-                # the one synchronisation of a solve: the weights' values
-                if not bool(w_ok.item()):
-                    raise ValueError("ilqr(): Q and Q_final must be finite and >= 0, R finite and > 0")
-                self.box = None
-            else:
-                lo, hi, per_tick, b_ok = box
-                # the one synchronisation of a solve: the weights' and the bounds' values
-                w_ok, b_ok = torch.stack([w_ok, b_ok]).tolist()
-                if not w_ok:
-                    raise ValueError("ilqr(): Q and Q_final must be finite and >= 0, R finite and > 0")
-                if not b_ok:
-                    raise ValueError("ilqr(): rpm_bounds must not be NaN and must satisfy 0 <= lo <= hi <= MAX_RPM of each "
-                                     "drone's row")
-                self.box = (lo, hi, per_tick)                        # "motor": MAX_RPM is a constant
-            hover = rows[:, 12].reshape(E, 1, 1).expand(E, D, 4)
-            ref = hover.reshape(n, 4) if rpm_ref is None else _per_drone(rpm_ref, "rpm_ref", 4, E, D, dev)
-            self.rpm_ref = ref.detach().contiguous()
-            if rpm is None:
-                rpm = hover.reshape(1, n, 4).expand(T, n, 4)
-            else:
-                rpm = _tensor(rpm, "rpm", (T, E, D, 4), dev).reshape(T, n, 4)
-            self.rpm = rpm.detach().clone().contiguous()
-            if self.box is not None:                             # the guess projected into the box
-                lo, hi, per_tick = self.box
-                torch.minimum(torch.maximum(self.rpm, lo), hi, out=self.rpm)
+        pk = pack_inputs(env, target, T, rpm, Q, R, Q_final, rpm_ref, state, last_rpm, phys, rpm_bounds, "ilqr()", graph=graph)
+        self.targets, self.weights, self.rpm_ref, self.rpm, self.box = pk["targets"], pk["weights"], pk["rpm_ref"], pk["rpm"], pk["box"]
+        planes0, last_rpm, rows = pk["planes0"], pk["last_rpm"], pk["rows"]
         self.env_shape = (E, D)
-        self.graph = (targets, weights, ref, planes0, last_rpm, rows) if graph else None
+        self.graph = pk["graph"]
         self.planes0, self.last_rpm, self.rows = planes0.detach().contiguous(), last_rpm.detach().contiguous(), rows.detach().contiguous()
         self.cfg = dyn_cfg(env)
         self.T, self.n, self.dev = T, n, dev

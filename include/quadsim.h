@@ -1041,6 +1041,62 @@ int qs_dyn_lqr_traj(const QsParams* p, const QsDynLqrTrajIO* io, int n_envs, int
 int qs_dyn_lqr_traj_vjp(const QsParams* p, const QsDynLqrTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                         void* stream);
 
+/* MPPI (model predictive path integral) trajectory optimisation (DESIGN.md 4.5.2): the cost J of QsIlqrIO, minimised by
+ * importance-weighted averages of random perturbations of the nominal rpm.  The unit of a decision is the drone, or with
+ * downwash (effects & QS_EFFECT_DW) the aviary, whose J is the sum of its drones' J in drone order.  One iteration is
+ * qs_mppi_sample, qs_mppi_update and qs_mppi_commit; none of them reads anything back to the host.
+ * Noise: eps[k][s][i][r] = the normals of Philox4x32-10 with key (seed & 0xffffffff, seed >> 32) and counter
+ * (k, s, i, 2 iteration + h), whose words (w0, w1) and (w2, w3) give u = ((w << 32 | w') >> 11 + 0.5) 2^-53 and by Box-Muller
+ * rotors 2h and 2h + 1; eps = 0 for sample 0.  Sample s applies v_k = u_k + sig_i eps (sig_i = sigma[e] HOVER_RPM of the row),
+ * clamped to [rpm_lo, rpm_hi] with a box; its perturbation is delta = v - u with a box, sig_i eps without.  Nothing of size
+ * K T N is stored: the update regenerates eps from the counter. */
+typedef struct QsMppiIO {
+    int T;                          /* ticks, > 0 */
+    int K;                          /* samples, 2..1024; sample 0 is the nominal */
+    int iteration;                  /* >= 0: the noise's counter */
+    int per_tick;                   /* 0: rpm_lo / rpm_hi are [N][4]; 1: [T][N][4] */
+    unsigned long long seed;        /* the noise's key */
+    double temperature;             /* finite, > 0 (qs_mppi_update) */
+    const double* state0;           /* [13 N] the state before tick 0 */
+    const double* last_rpm;         /* [N][4] the clipped RPMs of the tick before tick 0 (drag); nullable = zeros */
+    const double* phys;             /* [n_envs][16] QsState.phys rows (16-byte aligned); nullable = the constants of QsParams */
+    const double* targets;          /* [T][13 N], as QsIlqrIO */
+    const double* weights;          /* [n_envs][30], as QsIlqrIO */
+    const double* rpm_ref;          /* [N][4], as QsIlqrIO */
+    const double* sigma;            /* [n_envs] the noise scale relative to HOVER_RPM, finite and > 0 (not checked here) */
+    const double* rpm_lo;           /* the box, nullable together with rpm_hi = none; as QsIlqrBoxIO, and the nominal lies in it */
+    const double* rpm_hi;
+    double* rpm;                    /* [T][N][4] the nominal raw commands: qs_mppi_commit in/out, the others in */
+    double* states;                 /* [T][13 N] the nominal's trajectory: qs_mppi_commit out */
+    double* J;                      /* [K][N] each drone's J of each sample: qs_mppi_sample out, update and commit in */
+    double* cand;                   /* [T][N][4] the candidate: qs_mppi_update out, qs_mppi_commit in (NULL: see commit) */
+    double* cost_out;               /* [N] each drone's J of the committed nominal: qs_mppi_commit out */
+    int* pick;                      /* qs_mppi_commit out, nullable: per unit, [N] by drone or with downwash [n_envs] by aviary;
+                                     * -1 the candidate was kept, else the sample taken */
+    double* noise;                  /* [K][T][N][4] qs_mppi_noise out */
+} QsMppiIO;
+int qs_sizeof_mppi_io(void);
+/* J[s][i] of every sample's rollout (qs_ilqr_line_search's ticks and stage cost with the sample's commands); no state is
+ * stored.  Without downwash one thread per (drone, sample); with downwash whole (aviary, sample) groups per 128-thread CTA, the
+ * positions shared every substep as qs_ctrl_rollout does.  Refusals, in this order: NULL params / io, NULL pointers, sizes
+ * (T, K in 2..1024, iteration >= 0, the grid), per_tick not 0 or 1, only one of rpm_lo and rpm_hi, effects (QS_ERR_ENUM;
+ * QS_ERR_UNSUPPORTED outside 0, GND, DRAG, GND|DRAG, DW, GND|DRAG|DW, or downwash with drones_per_env > 128), phys alignment.
+ * qs_mppi_update and qs_mppi_commit refuse the same, and a temperature that is not finite and > 0 (update). */
+int qs_mppi_sample(const QsParams* p, const QsMppiIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                   void* stream);
+/* One warp per unit: J_min, the mean over the finite J_s, lambda = temperature (mean - J_min), w_s = exp(-(J_s - J_min) /
+ * lambda) (1 when lambda = 0, 0 for a non-finite J_s), each sum in s order; cand = u + sum_s w_s delta_s / sum_s w_s with the
+ * noise regenerated per entry (the nominal when no J_s is finite). */
+int qs_mppi_update(const QsParams* p, const QsMppiIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                   void* stream);
+/* Rolls out the candidate (clamped to the box), then per unit keeps it when its J is <= the best sample's J (the lowest s
+ * with the least finite J), otherwise takes that sample's commands; writes rpm, states, cost_out and pick.  With cand NULL it
+ * rolls out the nominal itself into states and cost_out (J is not read): the trajectory before the first iteration. */
+int qs_mppi_commit(const QsParams* p, const QsMppiIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                   void* stream);
+/* noise[s][k][i][r] = eps of (T, K, seed, iteration) for every sample, tick, drone and rotor.  Refusals: NULL io / noise, sizes. */
+int qs_mppi_noise(const QsMppiIO* io, int n_envs, int drones_per_env, void* stream);
+
 /* Reset envs to their initial pose.  mask: [E] bytes, nullable = all envs.  Zeroes velocities, body rates,
  * last_rpm, step counter; with reset_pid != 0 also the PID state (the reference never does, SURVEY.md 3.3).
  * If obs != NULL also refreshes the kinematic part of the RL observation rows (obs_dim > 0) or the [N][20]
