@@ -148,7 +148,7 @@ __device__ double mppi_rollout_dw(const MppiArgs& a, bool live, long long i, int
                     const double dz = pos_s[3 * (b + q) + 2] - d.pz;
                     const double dx = pos_s[3 * (b + q)] - d.px, dy = pos_s[3 * (b + q) + 1] - d.py;
                     const double dxy2 = dx * dx + dy * dy;
-                    if (dz > 0.0 && dxy2 < 100.0) fz += qs::downwash_pair(a.P, dz, dxy2);
+                    if (qs::downwash_acts(dz, dxy2)) fz += qs::downwash_pair(a.P, dz, dxy2);
                 }
                 double rp[4];
 #pragma unroll

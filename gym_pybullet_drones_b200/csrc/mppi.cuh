@@ -8,7 +8,8 @@
 namespace qs {
 
 // eps[4]: the standard normals of drone `id` at tick k of sample s in iteration `it`; Philox4x32-10 with key (seed low, seed
-// high) and counter (k, s, id, 2 it + h) gives rotors 2h and 2h + 1.  Sample 0 is the nominal: eps = 0.
+// high) and counter (k, s, id, 2 it + h) gives rotors 2h and 2h + 1, the last word in unsigned arithmetic (every it in
+// [0, 2^31) has its own counter).  Sample 0 is the nominal: eps = 0.
 QS_HD void mppi_eps(unsigned long long seed, int k, int s, long long id, int it, double eps[4]) {
     if (s == 0) {
         eps[0] = eps[1] = eps[2] = eps[3] = 0.0;
@@ -17,7 +18,7 @@ QS_HD void mppi_eps(unsigned long long seed, int k, int s, long long id, int it,
     const uint32_t key[2] = {(uint32_t)(seed & 0xffffffffull), (uint32_t)(seed >> 32)};
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const uint32_t ctr[4] = {(uint32_t)k, (uint32_t)s, (uint32_t)id, (uint32_t)(2 * it + h)};
+        const uint32_t ctr[4] = {(uint32_t)k, (uint32_t)s, (uint32_t)id, 2u * (uint32_t)it + (uint32_t)h};   // no int overflow
         uint32_t w[4];
         philox4x32_10(ctr, key, w);
         box_muller(w, eps[2 * h], eps[2 * h + 1]);

@@ -489,8 +489,14 @@ QS_HD TaskTerms hover_terms(const QsParams& P, const Drone& d, const Derived& o,
 }
 
 // ---- downwash pair term (BaseAviary.py:798-803) ----------------------------------------------------
+// Whether the drone dz above and dxy2 = dx*dx + dy*dy away in xy acts on the one below: dz > 0 and |dxy| < 10, tested as the
+// reference's sqrt(dxy2) < 10.  Double sqrt is correctly rounded and monotone, and 99.99999999999999 (100 - 2^-46, one ulp below
+// 100) is the least double whose sqrt rounds to 10, so the compare below is exactly the reference's, without the sqrt;
+// `dxy2 < 100` would keep the pair at 100 - 2^-46, where the reference drops it (tests/test_core_host.py derives the constant).
+QS_HD bool downwash_acts(double dz, double dxy2) { return dz > 0.0 && dxy2 < 99.99999999999999; }
+
 QS_HD double downwash_pair(const QsParams& P, double dz, double dxy2) {
-    // caller guarantees dz > 0 and dxy2 < 100
+    // caller guarantees downwash_acts(dz, dxy2)
     const double rr = P.prop_radius / (4.0 * dz);
     const double alpha = P.dw_coeff[0] * (rr * rr);
     const double beta = P.dw_coeff[1] * dz + P.dw_coeff[2];

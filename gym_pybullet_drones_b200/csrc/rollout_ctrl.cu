@@ -220,7 +220,7 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
                         const double dz = pos_s[3 * (b + q) + 2] - d.pz;
                         const double dx = pos_s[3 * (b + q)] - d.px, dy = pos_s[3 * (b + q) + 1] - d.py;
                         const double dxy2 = dx * dx + dy * dy;
-                        if (dz > 0.0 && dxy2 < 100.0) fz += qs::downwash_pair(P, dz, dxy2);
+                        if (qs::downwash_acts(dz, dxy2)) fz += qs::downwash_pair(P, dz, dxy2);
                     }
                     // the previous RPMs selected element by element: a pointer chosen at run time between the two arrays puts
                     // both into local memory inside the substep loop; for the same reason the row of constants is re-read (L1)

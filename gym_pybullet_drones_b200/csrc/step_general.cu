@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
                     const double dz = pos_s[3 * (b + k) + 2] - d.pz;
                     const double dx = pos_s[3 * (b + k)] - d.px, dy = pos_s[3 * (b + k) + 1] - d.py;
                     const double dxy2 = dx * dx + dy * dy;
-                    if (dz > 0.0 && dxy2 < 100.0) fz += qs::downwash_pair(P, dz, dxy2);
+                    if (qs::downwash_acts(dz, dxy2)) fz += qs::downwash_pair(P, dz, dxy2);
                 }
                 if constexpr (PHYS) qs::dyn_tick_k<EFF>(P, ph, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);
                 else qs::dyn_tick<EFF>(P, d, rpm, s == 0 ? rpm_prev : rpm, fz, 1, R_last);

@@ -55,8 +55,9 @@ def upright(sarg, ra, rb):
     return (sarg > -0.99999) & (sarg < 0.99999) & ((rb > _UPRIGHT_T * ra.abs()) | ((rb == 0) & (ra == 0)))
 
 
-def substep(K, rows, x, u, ds, effects, exact_branch=False, gnd_clip_le=False):
+def substep(K, rows, x, u, ds, effects, exact_branch=False, gnd_clip_le=False, fz=None):
     """One _dynamics substep (BaseAviary.py:815-877) from x [B, 13] with clipped rpm u [B, 4] and drag sum ds [B].
+    fz [B]: a force along each drone's body z (the downwash sum), added after drag; None adds nothing.
     gnd_clip_le=True: the height clip as `hz <= clip`, which clips at equality -- a negative control only."""
     dt = K["dt"]
     p, q, v, w = x[:, 0:3], x[:, 3:7], x[:, 7:10], x[:, 10:13]
@@ -81,6 +82,8 @@ def substep(K, rows, x, u, ds, effects, exact_branch=False, gnd_clip_le=False):
     F = torch.stack([r02 * thrust, r12 * thrust, r22 * thrust - gravity], dim=1)
     if effects & EFFECT_DRAG:
         F = F - K["drag"] * ds[:, None] * v
+    if fz is not None:
+        F = F + torch.stack([r02, r12, r22], dim=1) * fz[:, None]
     vn = v + (dt * inv_m)[:, None] * F
     tt = torch.stack([tx, ty, tz], dim=1) - torch.cross(w, J * w, dim=1)
     wn = w + dt * J_inv * tt
@@ -95,7 +98,7 @@ def substep(K, rows, x, u, ds, effects, exact_branch=False, gnd_clip_le=False):
 def tick(K, rows, x, rpm, up, S, effects, renormalise=True, strict_clamp=False, **sub):
     """One control tick: clip(rpm, 0, MAX_RPM) for S substeps from x [B, 13]; up = the previous tick's clipped rpm (drag).
     strict_clamp=True: a clip whose gradient reaches rpm only strictly below MAX_RPM (at equality it goes to MAX_RPM) -- a
-    negative control only.  `sub`: substep's exact_branch and gnd_clip_le."""
+    negative control only.  `sub`: substep's exact_branch, gnd_clip_le and fz (the same body-z force in every substep)."""
     mx = rows[:, 13:14].expand_as(rpm)
     u = torch.clamp(rpm, min=torch.zeros_like(rpm), max=mx)
     if strict_clamp:

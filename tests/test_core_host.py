@@ -139,3 +139,27 @@ def test_half_angle_series_matches_libm():
         L.hh_half_angle(float(n * n), 1 / 240, C.byref(c), C.byref(s))
         th = n / 480
         assert abs(c.value - np.cos(th)) < 3e-16 and abs(s.value - np.sin(th) / n) < 3e-19 + 1e-15 * abs(np.sin(th) / n)
+
+
+def test_downwash_predicate_is_the_references_sqrt():
+    """qs::downwash_acts is BaseAviary._downwash's `dz > 0 and norm(dxy) < 10` as the oracle states it, sqrt(dx*dx + dy*dy) < 10
+    (oracle/dyn_oracle.py, downwash_body_z), at the boundary and on random pairs within a few ulps of 10 m apart"""
+    L = host_harness()
+    # the least double whose correctly rounded sqrt is 10: the kernels' constant, 100 - 2^-46 (dxy2 < 100 differs right there)
+    limit = next(x for x in (100.0 - k * 2.0 ** -46 for k in range(8)) if np.sqrt(np.nextafter(x, 0.0)) < 10.0)
+    assert limit == 99.99999999999999 and np.sqrt(limit) == 10.0
+    for dxy2 in (np.nextafter(limit, 0.0), limit, 100.0, np.nextafter(100.0, 200.0), 0.0, 25.0):
+        want = bool(np.sqrt(dxy2) < 10.0)
+        assert L.hh_downwash_acts(1.0, dxy2) == want, dxy2
+        assert L.hh_downwash_acts(0.0, dxy2) == 0 and L.hh_downwash_acts(-1.0, dxy2) == 0
+    assert L.hh_downwash_acts(1.0, limit) == 0 and limit < 100.0              # the pair `dxy2 < 100` would keep
+    rng = np.random.default_rng(0)
+    xy0 = rng.uniform(-5, 5, (20000, 2))
+    th = rng.uniform(0, 2 * np.pi, 20000)
+    xy1 = xy0 + (10.0 + rng.uniform(-4e-15, 4e-15, 20000))[:, None] * np.stack([np.cos(th), np.sin(th)], 1)
+    d = xy1 - xy0
+    dxy2 = d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]
+    want = np.sqrt(dxy2) < 10.0
+    got = np.array([L.hh_downwash_acts(1.0, float(x)) for x in dxy2], dtype=bool)
+    assert np.array_equal(got, want)
+    assert (want != (dxy2 < 100.0)).sum() > 100                               # the old compare disagrees on many of these

@@ -227,3 +227,96 @@ def test_abi_exports_struct_and_refusals():
     io.noise = a
     io.K = 1
     assert L.qs_mppi_noise(C.byref(io), 1, 1, None) == -3
+
+
+# ---- the float64 references of the GPU edge tests ------------------------------------------------------------------------------
+
+def test_eps_counter_past_2_to_the_30():
+    """the counter's fourth word is 2 it + h in unsigned arithmetic: every iteration in [0, 2^31) has its own noise, and the host
+    build agrees with the restatement on both sides of 2^30 (where 2 it no longer fits an int)"""
+    seed = 0x9e3779b97f4a7c15
+    got = {}
+    for it in (2 ** 30 - 1, 2 ** 30, 2 ** 31 - 1):
+        e = (C.c_double * 4)()
+        _h().mppi_eps_host(C.c_ulonglong(seed), 3, 7, C.c_longlong(11), it, e)
+        np.testing.assert_allclose(np.array(e), MR.eps(seed, 3, 7, 11, it), rtol=1e-14, atol=1e-15)
+        got[it] = tuple(e)
+    assert len(set(got.values())) == 3
+
+
+def test_vectorised_philox_matches_the_restatement():
+    rng = np.random.default_rng(7)
+    seed = 0x0123456789abcdef
+    k, s, i, it = (rng.integers(0, 48, 64), rng.integers(0, 1024, 64), rng.integers(0, 2 ** 31, 64), rng.integers(0, 2 ** 31, 64))
+    s[:4] = 0
+    got = MR.eps_vec(seed, k, s, i, it)
+    want = np.array([MR.eps(seed, *(int(x) for x in c)) for c in zip(k, s, i, it)])
+    assert np.array_equal(got[:4], np.zeros((4, 4)))
+    np.testing.assert_allclose(got, want, rtol=1e-14, atol=1e-15)
+
+
+def test_weights_sum_in_s_order():
+    """lambda's sum of the finite J runs in s order, as the kernel's scan: the restatement gives the host build's weights bit for
+    bit at K = 1024, where np.mean's pairwise partial sums round otherwise (the negative control); a finite sum that overflows
+    gives lambda = inf and every finite weight 1"""
+    rng = np.random.default_rng(8)
+    J = rng.uniform(0.0, 1.0, 1024) * 10.0 ** rng.integers(-3, 4, 1024)
+    J[5], J[77] = float("nan"), float("inf")
+    delta, u = np.zeros((1024, 1)), np.zeros(1)
+    w, _, best = _update(J, 1e-3, delta, u)
+    w_ref, best_ref = MR.weights(J, 1e-3)
+    assert best == best_ref and np.array_equal(w, w_ref)
+    assert not np.array_equal(w, MR.weights(J, 1e-3, order="numpy")[0])
+    big = np.array([1e308, 0.5, 1e308, 2.0])
+    w, _, best = _update(big, 0.1, np.zeros((4, 1)), u)
+    assert best == 1 and np.array_equal(w, np.ones(4)) and np.array_equal(MR.weights(big, 0.1)[0], w)
+    # the unit sum: drone order from 0.0, and the reverse order rounds otherwise
+    Jd = np.array([[1.0, 1e16, -1e16]])
+    assert MR.unit_sum(Jd, 3)[0, 0] == 0.0 and MR.unit_sum(Jd, 3, reverse=True)[0, 0] == 1.0
+
+
+def _stacked_states(rng, E, D, model):
+    from diff_testlib import quat_from_rpy
+    n = E * D
+    pos = np.zeros((E, D, 3))
+    pos[:, :, 2] = 0.06 + 1.5 * np.arange(D)                          # the lowest drone in ground effect
+    pos[:, :, :2] = rng.uniform(-0.05, 0.05, (E, D, 2))
+    pos[:, -1, 0] += 12.0                                             # the top drone beyond 10 m in xy: no pair with it
+    rpy = rng.uniform(-0.2, 0.2, (n, 3))
+    q = np.stack([quat_from_rpy(r) for r in rpy])
+    vel, w = rng.uniform(-0.5, 0.5, (n, 3)), rng.uniform(-2, 2, (n, 3))
+    return np.concatenate([pos.reshape(n, 3), q, vel, w], axis=1)
+
+
+@pytest.mark.parametrize("model", ["cf2x", "cf2p"])
+def test_downwash_reference_matches_oracle(model):
+    """mppi_ref.rollout_dw (GND|DRAG|DW, 240/48 Hz) against the NumPy oracle's downwash_body_z + dynamics_substep over four ticks
+    of stacked drones, drag's substep 0 reading the previous tick's rpm; a reference without the downwash is far off"""
+    import torch
+    import diff_ref as DR
+    from oracle import dyn_oracle as O
+    from test_diff_host import _nominal_rows
+    P, c = params_of(model, 240, 48)
+    OP = O.OracleParams(model, 240, 48)
+    rng = np.random.default_rng(3)
+    E, D, T, S = 3, 4, 4, 5
+    n = E * D
+    x0 = _stacked_states(rng, E, D, model)
+    v = float(c.HOVER_RPM) * (1 + 0.05 * rng.uniform(-1, 1, (T, n, 4)))
+    up0 = float(c.HOVER_RPM) * (1 + 0.05 * rng.uniform(-1, 1, (n, 4)))
+    got = MR.rollout_dw(DR.model_constants(P), P, _nominal_rows(model, n), torch.tensor(x0), torch.tensor(up0), torch.tensor(v), S, 7, D)
+    pos, quat, vel, w = x0[:, 0:3], x0[:, 3:7], x0[:, 7:10], x0[:, 10:13]
+    up, want, fz_seen = up0, [], 0.0
+    for k in range(T):
+        u = np.clip(v[k], 0, OP.MAX_RPM)
+        for s in range(S):
+            fz = O.downwash_body_z(OP, pos.reshape(E, D, 3)).reshape(n)
+            fz_seen = max(fz_seen, np.abs(fz).max())
+            pos, quat, vel, w, _ = O.dynamics_substep(OP, u, pos, quat, vel, w, 7, rpm_prev=up if s == 0 else u, dw_fz=fz)
+        up = u
+        want.append(np.concatenate([pos, quat, vel, w], axis=1))
+    want = np.stack(want)
+    err = np.max(np.abs(got.numpy() - want) / np.maximum(np.abs(want), 1.0))
+    assert fz_seen > 1e-3 and err <= 1e-12, (fz_seen, err)
+    none = DR.rollout(DR.model_constants(P), _nominal_rows(model, n), torch.tensor(x0), torch.tensor(v), torch.tensor(up0), S, 3)
+    assert np.max(np.abs(none.numpy() - want)) > 1e-6
