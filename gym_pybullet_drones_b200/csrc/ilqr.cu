@@ -9,7 +9,8 @@
 // The rollouts of the last two are ilqr_rollout, whose tick is dyn_traj_kernel's (clip_rpm, dyn_tick_k, round_to_planes), so a
 // committed trajectory is qs_dyn_traj's output for the committed rpm and the commit's J is the line search's J bit for bit.
 // BOX = true is the control-limited variant (qs_ilqr_box_*): the backward solves riccati.cuh's box QP per tick and writes the
-// held rotors, the rollouts clamp each command to [rpm_lo, rpm_hi] before the tick, the stage cost and the commit's store.
+// held rotors, the rollouts clamp each command to [rpm_lo, rpm_hi] (ld_box's row) before the tick, the stage cost and the
+// commit's store.
 #include <type_traits>
 #include "qs_common.cuh"
 #include "dyn_tangent.cuh"
@@ -39,13 +40,6 @@ struct IlqrBoxArgs : IlqrArgs {
 };
 template <bool BOX>
 using IlqrArgsOf = std::conditional_t<BOX, IlqrBoxArgs, IlqrArgs>;
-
-// the box [lo, hi] of the raw command of drone i at tick k
-__device__ __forceinline__ void box_at(const IlqrBoxArgs& a, int k, long long i, double lo[4], double hi[4]) {
-    const long long at = a.per_tick ? (long long)k * a.N + i : i;                    // lqr_law.cuh's box_row
-    ld4(a.lo, at, lo);
-    ld4(a.hi, at, hi);
-}
 
 // BOX: at least 3 CTAs (12 warps) per SM, as the unconstrained kernel runs.  Left free, the drag variant takes 196 registers
 // and 8 warps per SM, and its backward pass ran 37% longer than with the 24 spilled bytes this bound costs (DESIGN.md 4.5.1).
@@ -101,7 +95,7 @@ __global__ void __launch_bounds__(32 * kBwdWarps, BOX ? 3 : 0) ilqr_backward_ker
             std::conditional_t<BOX, qs::RicBoxGains, qs::RicGains> G;
             if constexpr (BOX) {
                 double lo[4], hi[4];                                  // the box of k: the command's box minus u_nom
-                box_at(a, k, i, lo, hi);
+                ld_box(a.lo, a.hi, a.per_tick, k, a.N, i, lo, hi);
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     lo[j] -= raw[j];
@@ -190,7 +184,7 @@ __device__ __forceinline__ double ilqr_rollout(const IlqrArgsOf<BOX>& a, long lo
         }
         if constexpr (BOX) {
             double lo[4], hi[4];
-            box_at(a, k, i, lo, hi);
+            ld_box(a.lo, a.hi, a.per_tick, k, a.N, i, lo, hi);
 #pragma unroll
             for (int j = 0; j < 4; ++j) u[j] = qs::clampd(u[j], lo[j], hi[j]);
         }

@@ -5,9 +5,10 @@
 //                                  (aviary, sample) groups per 128-thread CTA.
 //   mppi_update_kernel<DW, BOX>:   one warp per unit (drone, or aviary with downwash): the weights, then the candidate.
 //   mppi_commit_kernel<EFF, BOX>:  rolls out the candidate (per aviary with downwash) and commits it or the best sample.
-// Every rollout is ilqr_rollout's tick (clip_rpm, dyn_tick_k, round_to_planes) and stage cost, so sample 0's J is the nominal's
-// cost bit for bit; with downwash each substep is ctrl_rollout_kernel's (positions through shared memory, qs::downwash_pair in
-// drone order, one dyn_tick_k substep), so a committed trajectory is CtrlAviary.rollout()'s for the committed rpm.
+// Every rollout is mppi_rollout: ilqr_rollout's tick (clip_rpm, dyn_tick_k, round_to_planes) and stage cost, so sample 0's J is
+// the nominal's cost bit for bit; with downwash each substep is ctrl_rollout_kernel's (positions through shared memory,
+// qs::downwash_fz, one dyn_tick_k substep), so a committed trajectory is CtrlAviary.rollout()'s for the committed rpm.  The
+// checks and the launch over PlanEffects are traj_io.cuh's.
 #include "qs_common.cuh"
 #include "dyn_adjoint.cuh"
 #include "lqr_law.cuh"
@@ -22,8 +23,6 @@ constexpr int kMppiTPB = 128;         // sample and commit CTAs; with downwash w
 constexpr int kUpdWarps = 4;          // units (warps) per update CTA
 constexpr int kMaxSamples = 1024;
 
-using MppiEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_GND | QS_EFFECT_DRAG, QS_EFFECT_DW, 7>;
-
 struct MppiArgs {
     QsParams P;
     QsMppiIO io;
@@ -32,20 +31,13 @@ struct MppiArgs {
     int tpb;                        // downwash: the threads of a CTA that hold whole groups (D * (128 / D))
 };
 
-// the box of drone i at tick k
-__device__ __forceinline__ void mppi_box(const QsMppiIO& io, int k, long long N, long long i, double lo[4], double hi[4]) {
-    const long long at = box_row(io.per_tick, k, N, i);
-    ld4(io.rpm_lo, at, lo);
-    ld4(io.rpm_hi, at, hi);
-}
-
 // The commands of drone i at tick k: of sample s (s >= 0), or the candidate (s < 0) clamped into the box
 template <bool BOX>
 __device__ __forceinline__ void mppi_tick_command(const MppiArgs& a, double sig, long long i, int k, int s, double v[4]) {
     const QsMppiIO& io = a.io;
     const long long ki = (long long)k * a.N + i;
     double lo[4] = {0, 0, 0, 0}, hi[4] = {0, 0, 0, 0};
-    if constexpr (BOX) mppi_box(io, k, a.N, i, lo, hi);
+    if constexpr (BOX) ld_box(io.rpm_lo, io.rpm_hi, io.per_tick, k, a.N, i, lo, hi);
     if (s < 0) {
         ld4(io.cand, ki, v);
         if constexpr (BOX) {
@@ -84,40 +76,14 @@ __device__ __forceinline__ double mppi_tick_end(const MppiArgs& a, const double*
     return qs::stage_cost(x, ref, wt + qs::stage_weights(k, io.T), v, uref, Rt);
 }
 
-// J of drone i's rollout of sample s (s < 0: the candidate) without downwash.  With `store` the states and the commands are
-// written, each tick's commands over the nominal's after they are read.
+// J of drone i's rollout of sample s (s < 0: the candidate).  With `store` the states and the commands are written, each tick's
+// commands over the nominal's after they are read.  With downwash the rollout is one (aviary, sample) group's: thread t holds
+// drone i, its group's drones are the threads [b, b + D), every thread of the CTA runs the loop (the barriers) and `live` ones
+// compute; each substep is ctrl_rollout_kernel's.  Without downwash every caller is live.
 template <int EFF, bool BOX>
-__device__ double mppi_rollout(const MppiArgs& a, long long i, int s, bool store) {
+__device__ double mppi_rollout(const MppiArgs& a, bool live, long long i, int s, bool store, int t = 0, int b = 0,
+                               double* pos_s = nullptr) {
     const QsMppiIO& io = a.io;
-    const qs::PhysRow c = row_of(a, i);
-    const double* wt = io.weights + (long long)qs::kWeightsRow * (i / a.D);
-    double Rt[4], uref[4];
-    qs::rel_weights(wt, c, Rt);
-    ld4(io.rpm_ref, i, uref);
-    const double sig = mppi_sig(a, c, i);
-    qs::Drone d;
-    ld_state(io.state0, a.N, i, d);
-    double up[4] = {0, 0, 0, 0};
-    if ((EFF & QS_EFFECT_DRAG) && io.last_rpm) ld4(io.last_rpm, i, up);
-    double J = 0.0;
-    for (int k = 0; k < io.T; ++k) {
-        double v[4], uc[4], R_last[9];
-        mppi_tick_command<BOX>(a, sig, i, k, s, v);
-        clip_rpm(v, c.max_rpm, uc);
-        qs::dyn_tick_k<EFF>(a.P, c, d, uc, up, 0.0, a.substeps, R_last);
-        J += mppi_tick_end(a, wt, Rt, uref, i, k, v, d, store);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) up[j] = uc[j];
-    }
-    return J;
-}
-
-// The downwash rollout of one (aviary, sample) group: thread t holds drone i, its group's drones are the threads [b, b + D).
-// Every thread of the CTA runs the loop (the barriers); `live` ones compute.  Each substep is ctrl_rollout_kernel's.
-template <int EFF, bool BOX>
-__device__ double mppi_rollout_dw(const MppiArgs& a, bool live, long long i, int t, int b, int s, bool store, double* pos_s) {
-    const QsMppiIO& io = a.io;
-    const int D = a.D;
     qs::PhysRow c;
     const double* wt = io.weights;
     double Rt[4] = {0, 0, 0, 0}, uref[4] = {0, 0, 0, 0}, sig = 0.0;
@@ -125,7 +91,7 @@ __device__ double mppi_rollout_dw(const MppiArgs& a, bool live, long long i, int
     double up[4] = {0, 0, 0, 0};
     if (live) {
         c = row_of(a, i);
-        wt = io.weights + (long long)qs::kWeightsRow * (i / D);
+        wt = io.weights + (long long)qs::kWeightsRow * (i / a.D);
         qs::rel_weights(wt, c, Rt);
         ld4(io.rpm_ref, i, uref);
         sig = mppi_sig(a, c, i);
@@ -139,23 +105,21 @@ __device__ double mppi_rollout_dw(const MppiArgs& a, bool live, long long i, int
             mppi_tick_command<BOX>(a, sig, i, k, s, v);
             clip_rpm(v, c.max_rpm, uc);
         }
-        for (int ss = 0; ss < a.substeps; ++ss) {
-            if (live) { pos_s[3 * t] = d.px; pos_s[3 * t + 1] = d.py; pos_s[3 * t + 2] = d.pz; }
-            __syncthreads();
-            if (live) {
-                double fz = 0.0;
-                for (int q = 0; q < D; ++q) {                                 // BaseAviary.py:798-811
-                    const double dz = pos_s[3 * (b + q) + 2] - d.pz;
-                    const double dx = pos_s[3 * (b + q)] - d.px, dy = pos_s[3 * (b + q) + 1] - d.py;
-                    const double dxy2 = dx * dx + dy * dy;
-                    if (qs::downwash_acts(dz, dxy2)) fz += qs::downwash_pair(a.P, dz, dxy2);
-                }
-                double rp[4];
+        if constexpr (EFF & QS_EFFECT_DW) {
+            for (int ss = 0; ss < a.substeps; ++ss) {
+                if (live) { pos_s[3 * t] = d.px; pos_s[3 * t + 1] = d.py; pos_s[3 * t + 2] = d.pz; }
+                __syncthreads();
+                if (live) {
+                    const double fz = qs::downwash_fz(a.P, pos_s, b, a.D, d.px, d.py, d.pz);
+                    double rp[4];
 #pragma unroll
-                for (int j = 0; j < 4; ++j) rp[j] = ss == 0 ? up[j] : uc[j];
-                qs::dyn_tick_k<EFF>(a.P, c, d, uc, rp, fz, 1, R_last);
+                    for (int j = 0; j < 4; ++j) rp[j] = ss == 0 ? up[j] : uc[j];
+                    qs::dyn_tick_k<EFF>(a.P, c, d, uc, rp, fz, 1, R_last);
+                }
+                __syncthreads();
             }
-            __syncthreads();
+        } else if (live) {
+            qs::dyn_tick_k<EFF>(a.P, c, d, uc, up, 0.0, a.substeps, R_last);
         }
         if (live) {
             J += mppi_tick_end(a, wt, Rt, uref, i, k, v, d, store);
@@ -193,14 +157,14 @@ __global__ void __launch_bounds__(kMppiTPB) mppi_sample_kernel(const __grid_cons
         const long long e = sl.G / K;
         const int s = (int)(sl.G - e * K);
         const long long i = e * a.D + sl.q;
-        const double J = mppi_rollout_dw<EFF, BOX>(a, sl.live, i, threadIdx.x, sl.b, s, false, pos_s);
+        const double J = mppi_rollout<EFF, BOX>(a, sl.live, i, s, false, threadIdx.x, sl.b, pos_s);
         if (sl.live) io.J[(long long)s * a.N + i] = J;
     } else {
         const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
         if (g >= a.N * K) return;
         const long long i = g / K;
         const int s = (int)(g - i * K);
-        io.J[(long long)s * a.N + i] = mppi_rollout<EFF, BOX>(a, i, s, false);
+        io.J[(long long)s * a.N + i] = mppi_rollout<EFF, BOX>(a, true, i, s, false);
     }
 }
 
@@ -243,7 +207,7 @@ __global__ void __launch_bounds__(32 * kUpdWarps) mppi_update_kernel(const __gri
         const double sig = mppi_sig(a, c, i);
         double un[4], lo[4] = {0, 0, 0, 0}, hi[4] = {0, 0, 0, 0};
         ld4(io.rpm, ki, un);
-        if constexpr (BOX) mppi_box(io, k, a.N, i, lo, hi);
+        if constexpr (BOX) ld_box(io.rpm_lo, io.rpm_hi, io.per_tick, k, a.N, i, lo, hi);
         double num[4] = {0, 0, 0, 0};
         for (int s = 1; s < K; ++s) {                                 // delta_0 = 0; a zero weight adds nothing
             const double ws = w[s];
@@ -286,11 +250,11 @@ __global__ void __launch_bounds__(kMppiTPB) mppi_commit_kernel(const __grid_cons
         const long long e = sl.G, i = e * a.D + sl.q;
         const int t = threadIdx.x;
         if (!io.cand) {                                               // the nominal's own rollout (its rpm stored unchanged)
-            const double J = mppi_rollout_dw<EFF, BOX>(a, sl.live, i, t, sl.b, 0, true, pos_s);
+            const double J = mppi_rollout<EFF, BOX>(a, sl.live, i, 0, true, t, sl.b, pos_s);
             if (sl.live) io.cost_out[i] = J;
             return;
         }
-        const double jc = mppi_rollout_dw<EFF, BOX>(a, sl.live, i, t, sl.b, -1, false, pos_s);
+        const double jc = mppi_rollout<EFF, BOX>(a, sl.live, i, -1, false, t, sl.b, pos_s);
         if (sl.live) jc_s[t] = jc;
         __syncthreads();
         int pick = -1;
@@ -300,18 +264,18 @@ __global__ void __launch_bounds__(kMppiTPB) mppi_commit_kernel(const __grid_cons
             pick = commit_choice<true>(a, e, sum);
             if (io.pick && sl.q == 0) io.pick[e] = pick;
         }
-        const double J = mppi_rollout_dw<EFF, BOX>(a, sl.live, i, t, sl.b, pick, true, pos_s);
+        const double J = mppi_rollout<EFF, BOX>(a, sl.live, i, pick, true, t, sl.b, pos_s);
         if (sl.live) io.cost_out[i] = J;
     } else {
         const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
         if (i >= a.N) return;
         if (!io.cand) {
-            io.cost_out[i] = mppi_rollout<EFF, BOX>(a, i, 0, true);
+            io.cost_out[i] = mppi_rollout<EFF, BOX>(a, true, i, 0, true);
             return;
         }
-        const double jc = mppi_rollout<EFF, BOX>(a, i, -1, false);
+        const double jc = mppi_rollout<EFF, BOX>(a, true, i, -1, false);
         const int pick = commit_choice<false>(a, i, jc);
-        io.cost_out[i] = mppi_rollout<EFF, BOX>(a, i, pick, true);
+        io.cost_out[i] = mppi_rollout<EFF, BOX>(a, true, i, pick, true);
         if (io.pick) io.pick[i] = pick;
     }
 }
@@ -350,12 +314,9 @@ int launch_mppi(const QsParams* p, const QsMppiIO* io, int n_envs, int drones_pe
         return fail(QS_ERR_SIZE, what, "temperature must be finite and > 0");
     if (io->per_tick != 0 && io->per_tick != 1) return fail(QS_ERR_SIZE, what, "per_tick must be 0 or 1");
     if (!io->rpm_lo != !io->rpm_hi) return fail(QS_ERR_NULL, what, "rpm_lo and rpm_hi are both given or both NULL");
-    if (effects & ~7u) return fail(QS_ERR_ENUM, what, "bad effects");
-    if (!with_int(MppiEffects{}, (int)effects, [](auto) {}))
-        return fail(QS_ERR_UNSUPPORTED, what, "supports no DYN+ effect, GND, DRAG, GND|DRAG, DW or all three");
+    if (int rc = traj_check_effects(what, effects, io->phys, nullptr, true)) return rc;
     const bool dw = effects & QS_EFFECT_DW;
     if (dw && drones_per_env > kMppiTPB) return fail(QS_ERR_UNSUPPORTED, what, "downwash needs drones_per_env <= 128");
-    if (io->phys && !aligned16(io->phys)) return fail(QS_ERR_ALIGN, what, "phys rows must be 16-byte aligned");
     const long long N = (long long)n_envs * drones_per_env;
     MppiArgs a;
     memset(&a, 0, sizeof(a));
@@ -369,18 +330,13 @@ int launch_mppi(const QsParams* p, const QsMppiIO* io, int n_envs, int drones_pe
     if (blocks > 0x7fffffffLL) return fail(QS_ERR_SIZE, what, "the grid exceeds 2^31-1 CTAs");
     const size_t smem = WHICH == kUpdate ? (size_t)kUpdWarps * 2 * io->K * sizeof(double) : 0;
     const bool box = io->rpm_lo != nullptr;
-    cudaError_t e = cudaSuccess;
-    with_int(MppiEffects{}, (int)effects, [&](auto EFF) {
-        with_bool(box, [&](auto BOX) {
-            constexpr int EF = decltype(EFF)::value;
-            constexpr bool BX = decltype(BOX)::value;
-            auto* k = WHICH == kSample ? mppi_sample_kernel<EF, BX> : WHICH == kUpdate ? mppi_update_kernel<(EF & QS_EFFECT_DW) != 0, BX> : mppi_commit_kernel<EF, BX>;
-            if (smem > 48 * 1024) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e == cudaSuccess) k<<<(unsigned)blocks, WHICH == kUpdate ? 32 * kUpdWarps : kMppiTPB, smem, (cudaStream_t)stream>>>(a);
+    return traj_launch<PlanEffects>(what, effects, [box](auto EFF) {
+        return with_bool(box, [](auto BOX) {
+            constexpr int E = decltype(EFF)::value;
+            constexpr bool B = decltype(BOX)::value;
+            return WHICH == kSample ? mppi_sample_kernel<E, B> : WHICH == kUpdate ? mppi_update_kernel<(E & QS_EFFECT_DW) != 0, B> : mppi_commit_kernel<E, B>;
         });
-    });
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_fail(e, what);
+    }, (unsigned)blocks, WHICH == kUpdate ? 32 * kUpdWarps : kMppiTPB, smem, (cudaStream_t)stream, a);
 }
 
 }  // namespace

@@ -320,6 +320,7 @@ auto with_bool(bool b, F&& f) { return b ? f(std::true_type{}) : f(std::false_ty
 using AllEffects = IntList<0, 1, 2, 3, 4, 5, 6, 7>;                                                  // general step, action rollout
 using PolicyEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_DW, 7>;                    // policy and control rollouts
 using TrajEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_GND | QS_EFFECT_DRAG>;       // differentiable trajectories
+using PlanEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_GND | QS_EFFECT_DRAG, QS_EFFECT_DW, 7>;   // mppi
 inline bool policy_effects_supported(unsigned eff) { return with_int(PolicyEffects{}, (int)eff, [](auto) {}); }
 
 int check_state(const QsState* st, int need_tables);                      // quadsim.cu

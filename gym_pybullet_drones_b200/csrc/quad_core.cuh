@@ -504,4 +504,17 @@ QS_HD double downwash_pair(const QsParams& P, double dz, double dxy2) {
     return -alpha * exp(-0.5 * (u * u));
 }
 
+// The downwash force along body z on the drone at (px, py, pz) from the D drones of its aviary, whose positions are
+// pos[3 (b + q) + c]: downwash_pair summed over the pairs that act, in drone order q = 0..D-1 from 0.0 (BaseAviary.py:798-811)
+QS_HD double downwash_fz(const QsParams& P, const double* pos, int b, int D, double px, double py, double pz) {
+    double fz = 0.0;
+    for (int q = 0; q < D; ++q) {
+        const double dz = pos[3 * (b + q) + 2] - pz;
+        const double dx = pos[3 * (b + q)] - px, dy = pos[3 * (b + q) + 1] - py;
+        const double dxy2 = dx * dx + dy * dy;
+        if (downwash_acts(dz, dxy2)) fz += downwash_pair(P, dz, dxy2);
+    }
+    return fz;
+}
+
 }  // namespace qs

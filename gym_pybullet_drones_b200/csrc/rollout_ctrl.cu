@@ -214,14 +214,7 @@ ctrl_rollout_kernel(const __grid_constant__ typename CtrlArgsOf<MODE>::type a) {
                 if (live) { pos_s[3 * t] = d.px; pos_s[3 * t + 1] = d.py; pos_s[3 * t + 2] = d.pz; }
                 __syncthreads();
                 if (live) {
-                    double fz = 0.0;
-                    const int b = le * D;
-                    for (int q = 0; q < D; ++q) {                                 // BaseAviary.py:798-811
-                        const double dz = pos_s[3 * (b + q) + 2] - d.pz;
-                        const double dx = pos_s[3 * (b + q)] - d.px, dy = pos_s[3 * (b + q) + 1] - d.py;
-                        const double dxy2 = dx * dx + dy * dy;
-                        if (qs::downwash_acts(dz, dxy2)) fz += qs::downwash_pair(P, dz, dxy2);
-                    }
+                    const double fz = qs::downwash_fz(P, pos_s, le * D, D, d.px, d.py, d.pz);
                     // the previous RPMs selected element by element: a pointer chosen at run time between the two arrays puts
                     // both into local memory inside the substep loop; for the same reason the row of constants is re-read (L1)
                     // every substep rather than held across the barriers

@@ -609,14 +609,7 @@ rollout_kernel(const __grid_constant__ typename RolloutArgsOf<NET>::type a) {
                 if (live) { pos_s[3 * t] = d.px; pos_s[3 * t + 1] = d.py; pos_s[3 * t + 2] = d.pz; }
                 __syncthreads();
                 if (live && !pend) {                           // all drones of an aviary are pending together
-                    double fz = 0.0;
-                    const int b = le * D;
-                    for (int q = 0; q < D; ++q) {
-                        const double dz = pos_s[3 * (b + q) + 2] - d.pz;
-                        const double dx = pos_s[3 * (b + q)] - d.px, dy = pos_s[3 * (b + q) + 1] - d.py;
-                        const double dxy2 = dx * dx + dy * dy;
-                        if (qs::downwash_acts(dz, dxy2)) fz += qs::downwash_pair(P, dz, dxy2);
-                    }
+                    const double fz = qs::downwash_fz(P, pos_s, le * D, D, d.px, d.py, d.pz);
                     if constexpr (POLICY) {
                         // the same values selected element by element: a pointer chosen at run time between the two arrays
                         // puts both in local memory, inside the substep loop (the policy variants have no registers to spare);

@@ -195,6 +195,8 @@ __global__ void __launch_bounds__(kMaxTPB, 4) step_kernel(const __grid_constant_
             __syncthreads();
             double fz = 0.0;
             if (live && !pending) {
+                // quad_core.cuh's downwash_fz written out: through it the all-effects variants without phys rows took 16 and 32
+                // more bytes of stack at their 128-register cap
                 const int b = le * D;
                 for (int k = 0; k < D; ++k) {                                   // BaseAviary.py:798-811
                     const double dz = pos_s[3 * (b + k) + 2] - d.pz;

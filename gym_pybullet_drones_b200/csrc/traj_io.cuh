@@ -1,8 +1,10 @@
 // traj_io.cuh -- what the differentiable-trajectory translation units (dyn_traj.cu, dyn_ctrl_traj.cu, dyn_policy_traj.cu,
-// dyn_jvp.cu, dyn_ctrl_jvp.cu) share: device-side loads and stores of states in the planes layout, the substep record of the tick adjoint, the
-// per-drone inputs and outputs of a tick, and on the host the argument checks and the launch over TrajEffects.
+// dyn_jvp.cu, dyn_ctrl_jvp.cu) and the planners (ilqr.cu, mppi.cu) share: device-side loads and stores of states in the planes
+// layout, a box's row, the substep record of the tick adjoint, the per-drone inputs and outputs of a tick, and on the host the
+// argument checks and the launch over an effect list.
 #pragma once
 #include "qs_common.cuh"
+#include "lqr_law.cuh"
 
 namespace qsi {
 namespace {
@@ -39,6 +41,13 @@ __device__ __forceinline__ void add_state(const double* s, long long N, long lon
 }
 __device__ __forceinline__ void ld4(const double* p, long long i, double v[4]) {
     v[0] = p[4 * i]; v[1] = p[4 * i + 1]; v[2] = p[4 * i + 2]; v[3] = p[4 * i + 3];
+}
+// the box [lo, hi] of the raw command of drone i at tick k: row box_row(per_tick, k, N, i) of rpm_lo and rpm_hi
+__device__ __forceinline__ void ld_box(const double* rpm_lo, const double* rpm_hi, int per_tick, int k, long long N, long long i,
+                                       double lo[4], double hi[4]) {
+    const long long at = box_row(per_tick, k, N, i);
+    ld4(rpm_lo, at, lo);
+    ld4(rpm_hi, at, hi);
 }
 
 // The constants of drone i (a.D drones per aviary): its aviary's row of `phys`, or where `phys` is NULL what `fallback()` returns
@@ -135,20 +144,23 @@ inline int traj_check_sizes(const char* what, int n_envs, int drones_per_env, in
     if ((long long)n_envs * drones_per_env > 0x7fffffffLL) return fail(QS_ERR_SIZE, what, "n_envs * drones_per_env exceeds 2^31-1");
     return 0;
 }
-// leaves TrajEffects only: no bit above 7, no downwash
-inline int traj_check_effects(const char* what, unsigned effects, const double* phys, const double* t_phys) {
+// leaves TrajEffects only, or with `dw` PlanEffects: no bit above 7, downwash only where allowed and then only alone or with both
+inline int traj_check_effects(const char* what, unsigned effects, const double* phys, const double* t_phys, bool dw = false) {
     if (effects & ~7u) return fail(QS_ERR_ENUM, what, "bad effects");
-    if (effects & QS_EFFECT_DW) return fail(QS_ERR_UNSUPPORTED, what, "downwash couples the drones pairwise and has no derivative here");
+    if (!dw && (effects & QS_EFFECT_DW))
+        return fail(QS_ERR_UNSUPPORTED, what, "downwash couples the drones pairwise and has no derivative here");
+    if (dw && !with_int(PlanEffects{}, (int)effects, [](auto) {}))
+        return fail(QS_ERR_UNSUPPORTED, what, "supports no DYN+ effect, GND, DRAG, GND|DRAG, DW or all three");
     if (phys && !aligned16(phys)) return fail(QS_ERR_ALIGN, what, "phys rows must be 16-byte aligned");
     if (t_phys && !aligned16(t_phys)) return fail(QS_ERR_ALIGN, what, "t_phys rows must be 16-byte aligned");
     return 0;
 }
-// pick(EFF)<<<blocks, threads, smem, s>>>(a) for the checked effect set; above 48 KB of shared memory the kernel's limit is
-// raised first
-template <class Pick, class Args>
+// pick(EFF)<<<blocks, threads, smem, s>>>(a) for the checked effect set of the list Effects; above 48 KB of shared memory the
+// kernel's limit is raised first
+template <class Effects = TrajEffects, class Pick, class Args>
 int traj_launch(const char* what, unsigned effects, Pick pick, unsigned blocks, int threads, size_t smem, cudaStream_t s, const Args& a) {
     cudaError_t e = cudaSuccess;
-    with_int(TrajEffects{}, (int)effects, [&](auto EFF) {
+    with_int(Effects{}, (int)effects, [&](auto EFF) {
         auto* k = pick(EFF);
         if (smem > 48 * 1024) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e == cudaSuccess) k<<<blocks, threads, smem, s>>>(a);

@@ -72,6 +72,12 @@ def _weight(x, name, default, E, dev):
     return _tensor(x, name, (E, width), dev)
 
 
+def check_iters(iters):
+    """A planner's iteration count (ilqr(), differentiable_ilqr(), mppi()): an integer >= 0, else ValueError."""
+    if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
+        raise ValueError("iters must be an integer >= 0, got %r" % (iters,))
+
+
 def horizon(env, target, num_steps, rpm, what):
     """T of a planner's call (ilqr(), mppi()) from num_steps, the target's time axis and rpm, every one that is given agreeing,
     after checking the target's keys; anything else raises ValueError naming `what`."""
@@ -289,8 +295,7 @@ def solve(p, iters):
 def ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=20, state=None, last_rpm=None, phys=None,
          rpm_bounds=None):
     """BaseAviary.ilqr (see there)."""
-    if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
-        raise ValueError("iters must be an integer >= 0, got %r" % (iters,))
+    check_iters(iters)
     p = Problem(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, state=state, last_rpm=last_rpm,
                 phys=phys, rpm_bounds=rpm_bounds)
     return solve(p, iters)
@@ -405,8 +410,7 @@ def differentiable_ilqr(env, target, num_steps=None, rpm=None, Q=None, R=None, Q
                         last_rpm=None, phys=None, rpm_bounds=None):
     """BaseAviary.differentiable_ilqr (see there)."""
     _refuse_downwash(env, "differentiable_ilqr()", "Jacobian")
-    if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
-        raise ValueError("iters must be an integer >= 0, got %r" % (iters,))
+    check_iters(iters)
     if isinstance(rpm_bounds, (tuple, list)) and any(isinstance(b, torch.Tensor) and b.requires_grad for b in rpm_bounds):
         raise ValueError("differentiable_ilqr(): rpm_bounds are constants: a bound tensor must not require grad (detach it)")
     p = Problem(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, state=state, last_rpm=last_rpm,

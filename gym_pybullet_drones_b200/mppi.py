@@ -9,8 +9,8 @@ import numbers
 import torch
 
 from . import _native as N
-from .diff import _call, dyn_cfg, unpack_traj
-from .ilqr import horizon, pack_inputs
+from .diff import _call, _io, dyn_cfg, unpack_traj
+from .ilqr import check_iters, horizon, pack_inputs
 
 MAX_SAMPLES = 1024
 MAX_DW_DRONES = 128                  # downwash: whole aviaries per 128-thread CTA, as CtrlAviary.rollout()
@@ -29,9 +29,7 @@ def _sigma(sigma, E, dev):
     return s, torch.isfinite(s).all() & (s > 0).all()
 
 
-def _check_scalars(env, iters, samples, temperature, seed):
-    if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
-        raise ValueError("iters must be an integer >= 0, got %r" % (iters,))
+def _check_scalars(env, samples, temperature, seed):
     if isinstance(samples, bool) or not isinstance(samples, int) or not 2 <= samples <= MAX_SAMPLES:
         raise ValueError("mppi(): samples must be an integer in [2, %d], got %r" % (MAX_SAMPLES, samples))
     if isinstance(temperature, bool) or not isinstance(temperature, numbers.Real) or not (math.isfinite(temperature) and temperature > 0):
@@ -54,7 +52,7 @@ class Mppi:
 
     def __init__(self, env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, samples=64, sigma=0.02,
                  temperature=0.1, seed=0, state=None, last_rpm=None, phys=None, rpm_bounds=None):
-        _check_scalars(env, 0, samples, temperature, seed)
+        _check_scalars(env, samples, temperature, seed)
         E, D, n, dev = env._E, env._D, env._N, env.device
         T = horizon(env, target, num_steps, rpm, "mppi()")
         self.sigma, s_ok = _sigma(sigma, E, dev)
@@ -78,10 +76,8 @@ class Mppi:
                     rpm_ref=self.rpm_ref, sigma=self.sigma, rpm_lo=lo, rpm_hi=hi, rpm=self.rpm, states=self.states, J=self.J,
                     cand=self.cand, pick=self.pick)
         base.update(ptrs)
-        io = N.QsMppiIO(T=self.T, K=self.K, iteration=iteration, per_tick=int(per_tick), seed=self.seed, temperature=self.temperature)
-        for k, x in base.items():
-            setattr(io, k, None if x is None else x.data_ptr())
-        return io
+        return _io(N.QsMppiIO, self.T, base, K=self.K, iteration=iteration, per_tick=int(per_tick), seed=self.seed,
+                   temperature=self.temperature)
 
     def _launch(self, name, io):
         P, E, D, S, eff = self.cfg
@@ -107,9 +103,7 @@ class Mppi:
         """eps [K, T, N, 4] of iteration `it`"""
         out = torch.empty((self.K, self.T, self.n, 4), dtype=torch.float64, device=self.dev)
         E, D = self.env_shape
-        with torch.cuda.device(self.dev):
-            N.check(N.lib().qs_mppi_noise(C.byref(self.io(it, noise=out)), E, D, torch.cuda.current_stream().cuda_stream),
-                    "qs_mppi_noise")
+        _call("qs_mppi_noise", C.byref(self.io(it, noise=out)), E, D, device=self.dev)
         return out
 
     def result(self, cost):
@@ -136,7 +130,7 @@ def solve(m, iters):
 def mppi(env, target, num_steps=None, rpm=None, Q=None, R=None, Q_final=None, rpm_ref=None, iters=30, samples=64, sigma=0.02,
          temperature=0.1, seed=0, state=None, last_rpm=None, phys=None, rpm_bounds=None):
     """BaseAviary.mppi (see there)."""
-    _check_scalars(env, iters, samples, temperature, seed)
+    check_iters(iters)
     m = Mppi(env, target, num_steps=num_steps, rpm=rpm, Q=Q, R=R, Q_final=Q_final, rpm_ref=rpm_ref, samples=samples, sigma=sigma,
              temperature=temperature, seed=seed, state=state, last_rpm=last_rpm, phys=phys, rpm_bounds=rpm_bounds)
     return solve(m, iters)

@@ -106,5 +106,8 @@ void hh_hover_terms(const QsParams* P, const double* pos, const double* quat, co
 }
 double hh_downwash_pair(const QsParams* P, double dz, double dxy2) { return qs::downwash_pair(*P, dz, dxy2); }
 int hh_downwash_acts(double dz, double dxy2) { return qs::downwash_acts(dz, dxy2); }
+double hh_downwash_fz(const QsParams* P, const double* pos, int b, int D, double px, double py, double pz) {
+    return qs::downwash_fz(*P, pos, b, D, px, py, pz);
+}
 void hh_half_angle(double n2, double dt, double* c, double* s) { qs::half_angle_terms(n2, dt, *c, *s); }
 }

@@ -166,7 +166,7 @@ def dw_fz(P, pos, order=1, lt100=False):
 def rollout_dw(K_dyn, P, rows, x0, last_rpm, v, S, effects, D, order=1, drag_up0=True, lt100=False):
     """The states [T, B, 13] of commands v [T, B, 4] (after the box) with downwash, for B / D groups of D consecutive drones
     (an (aviary, sample) group each): every substep takes fz from that substep's start positions (dw_fz) and renormalises the
-    quaternion, as ctrl_rollout_kernel and mppi_rollout_dw run one dyn_tick_k substep at a time; drag reads the previous tick's
+    quaternion, as ctrl_rollout_kernel and mppi_rollout run one dyn_tick_k substep at a time; drag reads the previous tick's
     clipped rpm in substep 0 (last_rpm at tick 0).  Negative controls only: drag_up0=False reads the current rpm there;
     order and lt100 as dw_fz."""
     B = x0.shape[0]

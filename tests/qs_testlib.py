@@ -89,6 +89,8 @@ def host_harness():
     L.hh_downwash_pair.restype = C.c_double
     L.hh_downwash_pair.argtypes = [C.c_void_p, C.c_double, C.c_double]
     L.hh_downwash_acts.argtypes = [C.c_double, C.c_double]
+    L.hh_downwash_fz.restype = C.c_double
+    L.hh_downwash_fz.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double]
     L.hh_half_angle.argtypes = [C.c_double, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     L.hh_tick.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p]
     L.hh_pid.argtypes = [C.c_void_p] + [C.c_void_p, C.c_double] + [C.c_void_p] * 4 + [C.c_double] + [C.c_void_p] * 5

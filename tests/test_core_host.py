@@ -163,3 +163,33 @@ def test_downwash_predicate_is_the_references_sqrt():
     got = np.array([L.hh_downwash_acts(1.0, float(x)) for x in dxy2], dtype=bool)
     assert np.array_equal(got, want)
     assert (want != (dxy2 < 100.0)).sum() > 100                               # the old compare disagrees on many of these
+
+
+@pytest.mark.parametrize("D", [1, 3, 5, 32])
+def test_downwash_fz_is_the_pair_sum_in_drone_order(D):
+    """qs::downwash_fz, the in-CTA pair sum of every downwash kernel, against mppi_ref.dw_fz on random aviaries of D drones,
+    with drone 1 of aviary 0 above drone 0 at dx*dx + dy*dy = 100 - 2^-46: that pair does not act, and the reference that
+    tests dxy2 < 100 (a negative control) counts it"""
+    import torch
+    import mppi_ref as MR
+    L = host_harness()
+    P = fill_params(AviaryConstants(DroneModel.CF2X))
+    rng = np.random.default_rng(D)
+    G = 8
+    # drones within 0.3 m in xy, where the pair terms are large, and about half of them 12 m away in x, where pairs do not act
+    pos = np.concatenate([rng.uniform(-0.3, 0.3, (G, D, 2)), rng.uniform(0.1, 3, (G, D, 1))], axis=2)
+    pos[:, :, 0] += 12.0 * rng.integers(0, 2, (G, D))
+    if D > 1:
+        # above every other drone, so that only drone 1 could act on drone 0; 60 m apart in z, where a pair 10 m apart in xy
+        # has a term of -1.2e-5
+        x, y = 1.0402010050251256, 9.945751950915763
+        assert x * x + y * y == 99.99999999999999
+        pos[0, 0], pos[0, 1] = (0.0, 0.0, 100.0), (x, y, 160.0)
+    flat = np.ascontiguousarray(pos.reshape(-1))
+    got = np.array([[L.hh_downwash_fz(C.addressof(P), ptr(flat), g * D, D, *pos[g, j]) for j in range(D)] for g in range(G)])
+    want = MR.dw_fz(P, torch.from_numpy(pos)).numpy()
+    assert np.all(np.abs(got - want) <= 1e-14 * np.abs(want)), np.max(np.abs(got - want))
+    if D > 1:
+        assert (want < -1e-3).sum() >= want.size // 8                         # large sums, not only underflowed terms
+        lt100 = MR.dw_fz(P, torch.from_numpy(pos), lt100=True).numpy()
+        assert got[0, 0] == 0.0 and lt100[0, 0] < -1e-5
