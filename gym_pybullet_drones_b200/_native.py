@@ -14,7 +14,8 @@ LIB_PATH = os.environ.get("QS_LIBQUADSIM", os.path.join(_HERE, "libquadsim.so"))
 _CSRC = os.path.join(_HERE, "csrc")
 SOURCES = [os.path.join(_CSRC, f) for f in ("quadsim.cu", "step_fast.cu", "step_general.cu", "rollout.cu", "rollout_next.cu", "rollout_mlp.cu", "rollout_ctrl.cu",
                                              "formation.cu", "mrac.cu", "dyn_traj.cu", "dyn_ctrl_traj.cu", "dyn_policy_traj.cu", "dyn_jvp.cu",
-                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu", "ilqr_adjoint.cu", "mppi.cu")]
+                                             "dyn_ctrl_jvp.cu", "dyn_policy_jvp.cu", "ilqr.cu", "dyn_lqr_traj.cu", "ilqr_adjoint.cu", "mppi.cu",
+                                             "dyn_dw_traj.cu")]
 HEADERS = [os.path.join(_CSRC, "quad_core.cuh"), os.path.join(_CSRC, "mrac_core.cuh"), os.path.join(_CSRC, "dyn_adjoint.cuh"), os.path.join(_CSRC, "dyn_tangent.cuh"), os.path.join(_CSRC, "pid_adjoint.cuh"), os.path.join(_CSRC, "pid_tangent.cuh"), os.path.join(_CSRC, "ctrl_io.cuh"), os.path.join(_CSRC, "mlp_adjoint.cuh"), os.path.join(_CSRC, "mlp_tangent.cuh"), os.path.join(_CSRC, "policy_actor.cuh"), os.path.join(_CSRC, "traj_io.cuh"), os.path.join(_CSRC, "riccati.cuh"), os.path.join(_CSRC, "lqr_law.cuh"), os.path.join(_CSRC, "philox.cuh"), os.path.join(_CSRC, "mppi.cuh"), os.path.join(_CSRC, "qs_common.cuh"), os.path.join(_CSRC, "rollout_kernel.cuh"),
            os.path.join(_ROOT, "include", "quadsim.h")]
 OBJ_DIR = os.path.join(_ROOT, "build", "obj")
@@ -233,7 +234,8 @@ EXPORTS = ["qs_abi_version", "qs_last_error", "qs_sizeof_params", "qs_sizeof_sta
            "qs_ilqr_box_line_search", "qs_ilqr_box_commit", "qs_sizeof_ilqr_box_io", "qs_ctrl_rollout_lqr",
            "qs_sizeof_lqr_rollout_io", "qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp", "qs_sizeof_dyn_lqr_traj_io",
            "qs_ilqr_adjoint", "qs_ilqr_adjoint_rollout", "qs_sizeof_ilqr_adjoint_io", "qs_mppi_sample", "qs_mppi_update",
-           "qs_mppi_commit", "qs_mppi_noise", "qs_sizeof_mppi_io"]
+           "qs_mppi_commit", "qs_mppi_noise", "qs_sizeof_mppi_io", "qs_dyn_traj_dw", "qs_dyn_traj_dw_vjp", "qs_dyn_ctrl_traj_dw",
+           "qs_dyn_ctrl_traj_dw_vjp"]
 MAX_PEERS = 16
 
 
@@ -332,7 +334,7 @@ def lib():
     L.qs_ctrl_rollout_lqr.restype = C.c_int
     L.qs_ctrl_rollout_lqr.argtypes = [C.POINTER(QsParams), C.POINTER(QsState), C.POINTER(QsCtrlRolloutIO), C.POINTER(QsLqrRolloutIO),
                                       C.c_int, C.c_int, C.c_int, C.c_uint, C.c_uint, C.c_void_p]
-    for n in ("qs_dyn_traj", "qs_dyn_traj_vjp"):
+    for n in ("qs_dyn_traj", "qs_dyn_traj_vjp", "qs_dyn_traj_dw", "qs_dyn_traj_dw_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
     for n in ("qs_dyn_lqr_traj", "qs_dyn_lqr_traj_vjp"):
@@ -341,7 +343,7 @@ def lib():
     for n in ("qs_dyn_traj_jvp", "qs_dyn_tick_jac"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsDynTrajJvpIO), C.c_int, C.c_int, C.c_int, C.c_uint, C.c_void_p]
-    for n in ("qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp"):
+    for n in ("qs_dyn_ctrl_traj", "qs_dyn_ctrl_traj_vjp", "qs_dyn_ctrl_traj_dw", "qs_dyn_ctrl_traj_dw_vjp"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [C.POINTER(QsParams), C.POINTER(QsParams), C.POINTER(QsDynCtrlTrajIO), C.c_int, C.c_int, C.c_int,
                                   C.c_uint, C.c_void_p]

@@ -75,10 +75,11 @@ QS_HD void rpm_clip_vjp(const double raw[4], double max_rpm, const double L[4], 
 }
 
 // Adjoint of one substep of dyn_tick_k<EFF> from its start state x with (clipped) rpm u and drag sum ds.  L: in, the cotangent of
-// the substep's end state; out, of x.  Lu / Lds / G accumulate.
+// the substep's end state; out, of x.  Lu / Lds / G accumulate.  With QS_EFFECT_DW, fz is the substep's downwash force along body
+// z (held constant here) and *Lfz receives its cotangent, the cotangent of the thrust scalar.
 template <int EFF>
 QS_HD void substep_vjp(const QsParams& P, const PhysRow& c, const Drone& x, const double u[4], double ds, Drone& L, double Lu[4],
-                       double& Lds, PhysGrad& G) {
+                       double& Lds, PhysGrad& G, double fz = 0.0, double* Lfz = nullptr) {
     const double dt = P.dt, dt_m = dt * c.inv_m;
     const double X = x.qx, Y = x.qy, Z = x.qz, W = x.qw;
     // ---- forward values of the substep (unit quaternion: Bullet's s = 2) ----
@@ -111,6 +112,7 @@ QS_HD void substep_vjp(const QsParams& P, const PhysRow& c, const Drone& x, cons
     if (EFF & QS_EFFECT_DRAG) {
         F[0] += -P.drag_coeff[0] * ds * x.vx; F[1] += -P.drag_coeff[1] * ds * x.vy; F[2] += -P.drag_coeff[2] * ds * x.vz;
     }
+    if (EFF & QS_EFFECT_DW) { F[0] += r02 * fz; F[1] += r12 * fz; F[2] += r22 * fz; }
     const double g21 = c.j[2] - c.j[1], g02 = c.j[0] - c.j[2], g10 = c.j[1] - c.j[0];
     const double tt[3] = {tx - g21 * (x.wy * x.wz), ty - g02 * (x.wz * x.wx), tz - g10 * (x.wx * x.wy)};
     const double wn[3] = {x.wx + dt * c.j_inv[0] * tt[0], x.wy + dt * c.j_inv[1] * tt[1], x.wz + dt * c.j_inv[2] * tt[2]};
@@ -154,7 +156,9 @@ QS_HD void substep_vjp(const QsParams& P, const PhysRow& c, const Drone& x, cons
         Lv[0] -= P.drag_coeff[0] * ds * LF[0]; Lv[1] -= P.drag_coeff[1] * ds * LF[1]; Lv[2] -= P.drag_coeff[2] * ds * LF[2];
     }
     const double LT = r02 * LF[0] + r12 * LF[1] + r22 * LF[2];
-    double Lr02 = thrust * LF[0], Lr12 = thrust * LF[1], Lr22 = thrust * LF[2], Lr20 = 0.0, Lr21 = 0.0;
+    if (EFF & QS_EFFECT_DW) *Lfz = LT;                    // F = R[:,2] (T + fz) - g e_z: fz's cotangent is the thrust's
+    const double tf = (EFF & QS_EFFECT_DW) ? thrust + fz : thrust;
+    double Lr02 = tf * LF[0], Lr12 = tf * LF[1], Lr22 = tf * LF[2], Lr20 = 0.0, Lr21 = 0.0;
     // forces and torques
     G.g[4] += Ltt[0] * sxf; G.g[5] += Ltt[1] * syf;
 #pragma unroll
@@ -206,6 +210,13 @@ QS_HD void entry_normalise(Drone& d, double& inv) {
     d.qx *= inv; d.qy *= inv; d.qz *= inv; d.qw *= inv;
 }
 
+// The VJP of entry_normalise at its output xn (inv = 1 / |q|): q_hat = q / |q| gives L_q = (L_hat - q_hat (q_hat . L_hat)) / |q|
+QS_HD void entry_normalise_vjp(const Drone& xn, double inv, Drone& L) {
+    const double dot = xn.qx * L.qx + xn.qy * L.qy + xn.qz * L.qz + xn.qw * L.qw;
+    L.qx = (L.qx - xn.qx * dot) * inv; L.qy = (L.qy - xn.qy * dot) * inv;
+    L.qz = (L.qz - xn.qz * dot) * inv; L.qw = (L.qw - xn.qw * dot) * inv;
+}
+
 // drag's sum of the rotor speeds over four clipped RPMs (rad/s), as dyn_tick_k evaluates it
 QS_HD double drag_sum(const double r[4]) {
     const double kk = 2.0 * 3.14159265358979323846;
@@ -238,10 +249,63 @@ QS_HD void dyn_tick_vjp(const QsParams& P, const PhysRow& c, const Drone& d0, co
 #pragma unroll
         for (int i = 0; i < 4; ++i) { Lup[i] += (kk / 60.0) * Lds_prev; Lu[i] += (kk / 60.0) * Lds_cur; }
     }
-    // q_hat = q / |q|: L_q = (L_hat - q_hat (q_hat . L_hat)) / |q|
-    const double dot = x0.qx * L.qx + x0.qy * L.qy + x0.qz * L.qz + x0.qw * L.qw;
-    L.qx = (L.qx - x0.qx * dot) * inv; L.qy = (L.qy - x0.qy * dot) * inv;
-    L.qz = (L.qz - x0.qz * dot) * inv; L.qw = (L.qw - x0.qw * dot) * inv;
+    entry_normalise_vjp(x0, inv, L);
+}
+
+// ---- downwash (DESIGN.md 4.5, downwash adjoint) -------------------------------------------------------------------------------
+// An aviary tick with downwash runs its S substeps one dyn_tick_k<EFF>(., fz, 1, .) call at a time, fz = downwash_fz of the
+// substep's start positions, so each substep renormalises the quaternion on entry and every drone's substep depends on the
+// positions of its aviary.  The adjoint of substep s is two phases around a barrier: dw_substep_vjp (drone-local, fz held
+// constant) gives lambda, the cotangent of the drone's fz; downwash_pos_vjp then adds the pair terms to the positions' cotangents
+// from the lambdas of the whole aviary.
+
+// Adjoint of one downwash substep from x as recorded (before its entry renormalisation), with clipped rpm u, drag sum ds and
+// the pair force fz.  L: in, the cotangent of the end state; out, of x without the pair terms.  Lu / Lds / G accumulate.
+// Returns lambda.
+template <int EFF>
+QS_HD double dw_substep_vjp(const QsParams& P, const PhysRow& c, const Drone& x, const double u[4], double ds, double fz, Drone& L,
+                            double Lu[4], double& Lds, PhysGrad& G) {
+    Drone xn = x;
+    double inv, lam = 0.0;
+    entry_normalise(xn, inv);
+    substep_vjp<EFF>(P, c, xn, u, ds, L, Lu, Lds, G, fz, &lam);
+    entry_normalise_vjp(xn, inv, L);                     // touches the quaternion only: the pair terms below touch positions only
+    return lam;
+}
+
+// The pair terms of drone q's position cotangent: pos[3 (b + k) + c] are the positions of the aviary's D drones at the substep's
+// start and lam[b + k] the cotangents of their fz.  For a receiver i and a source k, fz_i += p(z_k - z_i, (x_k - x_i)^2 +
+// (y_k - y_i)^2) wherever downwash_acts holds (the forward's predicate and operands), so drone q gets -lam_q dp for the sources
+// over it (its receiver terms, summed in drone order) and then +lam_i dp for the receivers under it (its source terms, in drone
+// order).  No atomics: each drone sums its own terms.
+QS_HD void downwash_pos_vjp(const QsParams& P, const double* pos, const double* lam, int b, int D, int q, Drone& L) {
+    const double* pq = pos + 3 * (b + q);
+    const double lq = lam[b + q];
+    double gx = 0.0, gy = 0.0, gz = 0.0;
+    for (int k = 0; k < D; ++k) {                        // q the receiver, k the source
+        const double* pk = pos + 3 * (b + k);
+        const double dz = pk[2] - pq[2];
+        const double dx = pk[0] - pq[0], dy = pk[1] - pq[1];
+        const double dxy2 = dx * dx + dy * dy;
+        if (downwash_acts(dz, dxy2)) {
+            double g_dz, g_dxy2;
+            downwash_pair_grad(P, dz, dxy2, g_dz, g_dxy2);
+            gx -= lq * (2.0 * dx * g_dxy2); gy -= lq * (2.0 * dy * g_dxy2); gz -= lq * g_dz;
+        }
+    }
+    for (int k = 0; k < D; ++k) {                        // k the receiver, q the source
+        const double* pk = pos + 3 * (b + k);
+        const double dz = pq[2] - pk[2];
+        const double dx = pq[0] - pk[0], dy = pq[1] - pk[1];
+        const double dxy2 = dx * dx + dy * dy;
+        if (downwash_acts(dz, dxy2)) {
+            double g_dz, g_dxy2;
+            downwash_pair_grad(P, dz, dxy2, g_dz, g_dxy2);
+            const double lk = lam[b + k];
+            gx += lk * (2.0 * dx * g_dxy2); gy += lk * (2.0 * dy * g_dxy2); gz += lk * g_dz;
+        }
+    }
+    L.px += gx; L.py += gy; L.pz += gz;
 }
 
 // Lq += d rpy / d q ^T Lrpy for rpy = quat_to_euler<false>(q), on the forward's branch of the +-0.99999 gimbal guard

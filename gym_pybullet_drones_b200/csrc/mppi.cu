@@ -130,23 +130,6 @@ __device__ double mppi_rollout(const MppiArgs& a, bool live, long long i, int s,
     return J;
 }
 
-// The downwash CTA's group of thread t: the unit index G (aviary * K + sample for the sample kernel, aviary for the commit),
-// the first thread b of the group and whether t holds a drone of a live group
-struct DwSlot {
-    long long G;
-    int b, q;
-    bool live;
-};
-__device__ __forceinline__ DwSlot dw_slot(const MppiArgs& a, long long groups) {
-    const int t = threadIdx.x, g = t / a.D;
-    DwSlot sl;
-    sl.G = (long long)blockIdx.x * (a.tpb / a.D) + g;
-    sl.b = g * a.D;
-    sl.q = t - sl.b;
-    sl.live = t < a.tpb && sl.G < groups;
-    return sl;
-}
-
 template <int EFF, bool BOX>
 __global__ void __launch_bounds__(kMppiTPB) mppi_sample_kernel(const __grid_constant__ MppiArgs a) {
     const QsMppiIO& io = a.io;

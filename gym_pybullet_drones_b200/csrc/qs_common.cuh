@@ -321,6 +321,7 @@ using AllEffects = IntList<0, 1, 2, 3, 4, 5, 6, 7>;                             
 using PolicyEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_DW, 7>;                    // policy and control rollouts
 using TrajEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_GND | QS_EFFECT_DRAG>;       // differentiable trajectories
 using PlanEffects = IntList<0, QS_EFFECT_GND, QS_EFFECT_DRAG, QS_EFFECT_GND | QS_EFFECT_DRAG, QS_EFFECT_DW, 7>;   // mppi
+using DwTrajEffects = IntList<QS_EFFECT_DW, 7>;                                                      // downwash trajectories
 inline bool policy_effects_supported(unsigned eff) { return with_int(PolicyEffects{}, (int)eff, [](auto) {}); }
 
 int check_state(const QsState* st, int need_tables);                      // quadsim.cu

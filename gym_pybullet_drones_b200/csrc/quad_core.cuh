@@ -504,6 +504,22 @@ QS_HD double downwash_pair(const QsParams& P, double dz, double dxy2) {
     return -alpha * exp(-0.5 * (u * u));
 }
 
+// The derivatives of downwash_pair with respect to dz and dxy2 (the caller guarantees downwash_acts).  With p the pair term,
+// rr = R / (4 dz), alpha = c0 rr^2, beta = c1 dz + c2 and u = sqrt(dxy2) / beta: dp/d(dxy2) = -p / (2 beta^2) and
+// dp/d(dz) = p (c1 u^2 / beta - 2 / dz).  The sqrt is never differentiated, so stacked drones (dxy2 = 0) get finite derivatives;
+// where p is +-0 (exp underflow, or beta = 0 with dxy2 > 0) both are 0 rather than 0 * inf.
+QS_HD void downwash_pair_grad(const QsParams& P, double dz, double dxy2, double& g_dz, double& g_dxy2) {
+    const double p = downwash_pair(P, dz, dxy2);
+    if (p == 0.0) {
+        g_dz = g_dxy2 = 0.0;
+        return;
+    }
+    const double beta = P.dw_coeff[1] * dz + P.dw_coeff[2];
+    const double u = sqrt(dxy2) / beta;
+    g_dxy2 = -p / (2.0 * (beta * beta));
+    g_dz = p * (P.dw_coeff[1] * (u * u) / beta - 2.0 / dz);
+}
+
 // The downwash force along body z on the drone at (px, py, pz) from the D drones of its aviary, whose positions are
 // pos[3 (b + q) + c]: downwash_pair summed over the pairs that act, in drone order q = 0..D-1 from 0.0 (BaseAviary.py:798-811)
 QS_HD double downwash_fz(const QsParams& P, const double* pos, int b, int D, double px, double py, double pz) {

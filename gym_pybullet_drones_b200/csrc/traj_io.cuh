@@ -1,7 +1,7 @@
 // traj_io.cuh -- what the differentiable-trajectory translation units (dyn_traj.cu, dyn_ctrl_traj.cu, dyn_policy_traj.cu,
-// dyn_jvp.cu, dyn_ctrl_jvp.cu) and the planners (ilqr.cu, mppi.cu) share: device-side loads and stores of states in the planes
-// layout, a box's row, the substep record of the tick adjoint, the per-drone inputs and outputs of a tick, and on the host the
-// argument checks and the launch over an effect list.
+// dyn_jvp.cu, dyn_ctrl_jvp.cu, dyn_dw_traj.cu) and the planners (ilqr.cu, mppi.cu) share: device-side loads and stores of states
+// in the planes layout, a box's row, the substep record of the tick adjoint, the per-drone inputs and outputs of a tick, the
+// downwash CTA's groups, and on the host the argument checks and the launch over an effect list.
 #pragma once
 #include "qs_common.cuh"
 #include "lqr_law.cuh"
@@ -136,6 +136,25 @@ struct ScratchRec {
         d.vx = p[7 * N]; d.vy = p[8 * N]; d.vz = p[9 * N]; d.wx = p[10 * N]; d.wy = p[11 * N]; d.wz = p[12 * N];
     }
 };
+
+// The downwash CTA (whole groups of a.D drones in its first a.tpb threads) and thread t's group in it: the unit index G (aviary,
+// or aviary * K + sample for mppi's sample kernel), the first thread b of the group, the drone q of the group, and whether t holds
+// a drone of a live group
+struct DwSlot {
+    long long G;
+    int b, q;
+    bool live;
+};
+template <class Args>
+__device__ __forceinline__ DwSlot dw_slot(const Args& a, long long groups) {
+    const int t = threadIdx.x, g = t / a.D;
+    DwSlot sl;
+    sl.G = (long long)blockIdx.x * (a.tpb / a.D) + g;
+    sl.b = g * a.D;
+    sl.q = t - sl.b;
+    sl.live = t < a.tpb && sl.G < groups;
+    return sl;
+}
 
 // ---- host: the checks every entry point makes, in this order around its own, and the launch.  `what` is the entry point's name.
 inline int traj_check_sizes(const char* what, int n_envs, int drones_per_env, int substeps, int T) {

@@ -1,5 +1,6 @@
 """Differentiable trajectories of Physics.DYN: torch.autograd.Functions over qs_dyn_traj / qs_dyn_traj_vjp (raw RPMs),
-qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop), qs_dyn_lqr_traj / qs_dyn_lqr_traj_vjp (an iLQR plan's
+qs_dyn_ctrl_traj / qs_dyn_ctrl_traj_vjp (a DSLPIDControl in the loop), with downwash their aviary-unit twins qs_dyn_traj_dw /
+qs_dyn_traj_dw_vjp and qs_dyn_ctrl_traj_dw / qs_dyn_ctrl_traj_dw_vjp, qs_dyn_lqr_traj / qs_dyn_lqr_traj_vjp (an iLQR plan's
 LQR tracker in the loop) and qs_dyn_policy_traj / qs_dyn_policy_traj_vjp (an MlpPolicy in the loop) (include/quadsim.h, DESIGN.md 4.5), and their forward mode: the jvp of each Function (qs_dyn_traj_jvp,
 qs_dyn_ctrl_traj_jvp, qs_dyn_policy_traj_jvp) and the per-tick Jacobians of linearise (qs_dyn_tick_jac, qs_dyn_ctrl_tick_jac,
 qs_dyn_policy_tick_jac).
@@ -56,6 +57,20 @@ def _io(cls, T, ptrs, **scalars):
     return io
 
 
+def _entry(name, eff):
+    """The entry point `name` of the per-drone kernels, or its downwash twin (name + "_dw" before any "_vjp") for effects with
+    EFFECT_DW."""
+    if not eff & N.EFFECT_DW:
+        return name
+    return name[:-4] + "_dw_vjp" if name.endswith("_vjp") else name + "_dw"
+
+
+def _no_downwash_jvp(eff):
+    if eff & N.EFFECT_DW:
+        raise ValueError("differentiable_rollout(downwash=True) has reverse mode only: forward-mode (dual tensor) derivatives "
+                         "with downwash are not implemented (their Jacobians are per aviary)")
+
+
 def _no_double_backward():
     if torch.is_grad_enabled():
         raise ValueError("differentiable_rollout: double backward (create_graph=True) is not supported: the VJP kernel has no "
@@ -74,14 +89,15 @@ def _dyn_traj(cfg, rpm, planes0, last_rpm, rows):
     T, n = rpm.shape[0], E * D
     states = torch.empty((T, 13 * n), dtype=torch.float64, device=rpm.device)
     io = _io(N.QsDynTrajIO, T, _traj_ptrs(rpm, planes0, last_rpm, rows, states))
-    _call("qs_dyn_traj", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
+    _call(_entry("qs_dyn_traj", eff), C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
     return states
 
 
 class DynTrajectory(torch.autograd.Function):
     """states [T, 13 N] = the T ticks of qs_dyn_traj from planes0 [13 N] with rpm [T, N, 4], last_rpm [N, 4] and the per-aviary
     rows [E, 16]; backward = qs_dyn_traj_vjp, its per-drone row gradients summed over each aviary's drones (torch, deterministic);
-    jvp (torch.autograd.forward_ad) = qs_dyn_traj_jvp.  `cfg` = (QsParams, E, D, substeps, effects).  The inputs may have any
+    jvp (torch.autograd.forward_ad) = qs_dyn_traj_jvp.  `cfg` = (QsParams, E, D, substeps, effects); effects with EFFECT_DW run
+    qs_dyn_traj_dw and qs_dyn_traj_dw_vjp, and their jvp raises ValueError.  The inputs may have any
     strides (the kernels read dense buffers: they get contiguous copies).  Double backward and tangents that require grad raise
     ValueError."""
 
@@ -103,6 +119,7 @@ class DynTrajectory(torch.autograd.Function):
             raise ValueError("differentiable_rollout: a tangent that requires grad (reverse mode over forward mode) is not supported: "
                              "the JVP kernel has no derivative of its own")
         P, E, D, S, eff = ctx.cfg
+        _no_downwash_jvp(eff)
         states = ctx.saved_tensors[4]
         t_states = torch.empty_like(states)
         dense = [None if t is None else t.to(torch.float64).contiguous() for t in tangents]
@@ -131,7 +148,7 @@ def _dyn_traj_vjp(cfg, rpm, planes0, last_rpm, rows, states, g_states):
     ptrs = dict(_traj_ptrs(rpm, planes0, last_rpm, rows, states), g_states=g_states.to(torch.float64).contiguous(),
                 scratch=torch.empty((S, 13, n), **f64), **g)
     io = _io(N.QsDynTrajIO, T, ptrs)
-    _call("qs_dyn_traj_vjp", C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
+    _call(_entry("qs_dyn_traj_vjp", eff), C.byref(P), C.byref(io), E, D, S, eff, device=rpm.device)
     return g["g_rpm"], g["g_state0"], g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1)
 
 
@@ -146,7 +163,7 @@ def _dyn_ctrl_traj(cfg, ins):
     f64 = dict(dtype=torch.float64, device=tpos.device)
     outs = dict(states=torch.empty((T, 13 * n), **f64), rpm=torch.empty((T, n, 4), **f64), pid_states=torch.empty((T, 9, n), **f64))
     io = _io(N.QsDynCtrlTrajIO, T, dict(ins, **outs), control_timestep=dt)
-    _call("qs_dyn_ctrl_traj", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=tpos.device)
+    _call(_entry("qs_dyn_ctrl_traj", eff), C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=tpos.device)
     return outs
 
 
@@ -155,8 +172,8 @@ class DynCtrlTrajectory(torch.autograd.Function):
     [9, N], with target_pos [T, N, 3], target_vel / target_rpy / target_rpy_rates [N, 3], last_rpm [N, 4], the per-aviary rows
     [E, 16] and gain sets [E, 18]; backward = qs_dyn_ctrl_traj_vjp, its per-drone row and gain gradients summed over each
     aviary's drones (torch, deterministic); jvp (torch.autograd.forward_ad) = qs_dyn_ctrl_traj_jvp.  `cfg` = (env QsParams,
-    controller QsParams, control_timestep, E, D, substeps, effects).  The inputs may have any strides (the kernels get
-    contiguous copies).  Double backward and tangents that require grad raise ValueError."""
+    controller QsParams, control_timestep, E, D, substeps, effects); effects with EFFECT_DW run qs_dyn_ctrl_traj_dw and
+    qs_dyn_ctrl_traj_dw_vjp, and their jvp raises ValueError.  The inputs may have any strides (the kernels get contiguous copies).  Double backward and tangents that require grad raise ValueError."""
 
     @staticmethod
     def forward(ctx, planes0, pid0, tpos, tvel, trpy, trr, last_rpm, rows, gains, cfg):
@@ -177,6 +194,7 @@ class DynCtrlTrajectory(torch.autograd.Function):
                              "the JVP kernel has no derivative of its own")
         saved = ctx.saved_tensors
         P, CP, dt, E, D, S, eff = ctx.cfg
+        _no_downwash_jvp(eff)
         states = saved[9]
         dense = [None if t is None else t.to(torch.float64).contiguous() for t in tangents]
         if dense[7] is not None and dense[7].data_ptr() % 16:          # the kernel reads t_phys rows as 16-byte pairs
@@ -204,7 +222,7 @@ class DynCtrlTrajectory(torch.autograd.Function):
         outs.update(g_states=g_states.to(torch.float64).contiguous(), g_rpm_out=g_rpm.to(torch.float64).contiguous(),
                     scratch=torch.empty((S, 13, n), **f64))
         io = _io(N.QsDynCtrlTrajIO, T, dict(ins, **outs, **grads), control_timestep=dt)
-        _call("qs_dyn_ctrl_traj_vjp", C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=ins["target_pos"].device)
+        _call(_entry("qs_dyn_ctrl_traj_vjp", eff), C.byref(P), C.byref(CP), C.byref(io), E, D, S, eff, device=ins["target_pos"].device)
         g = grads
         return (g["g_state0"], g["g_pid0"], g["g_target_pos"], g["g_target_vel"], g["g_target_rpy"], g["g_target_rpy_rates"],
                 g["g_last_rpm"], g["g_phys"].view(E, D, 16).sum(dim=1), g["g_gains"].view(E, D, 18).sum(dim=1), None)
@@ -505,6 +523,24 @@ def _start_state(env, state, last_rpm, phys):
     return planes0, last_rpm, rows
 
 
+MAX_DW_DRONES = 128                  # downwash: whole aviaries per 128-thread CTA
+
+
+def _check_downwash(env, policy, controller):
+    """The refusals of differentiable_rollout(downwash=True)."""
+    from .ilqr import Tracker
+    if not env._effects & N.EFFECT_DW:
+        raise ValueError("differentiable_rollout(downwash=True): the env has no downwash to differentiate (use PYB_DW or "
+                         "PYB_GND_DRAG_DW, or leave downwash=False)")
+    if env._EXTERNAL_DOWNWASH:
+        raise ValueError("differentiable_rollout(downwash=True): the downwash of a formation sharded over devices is not available")
+    if env._D > MAX_DW_DRONES:
+        raise ValueError("differentiable_rollout(downwash=True): an aviary has at most %d drones, got %d" % (MAX_DW_DRONES, env._D))
+    if policy is not None or isinstance(controller, Tracker):
+        raise ValueError("differentiable_rollout(downwash=True) takes rpm= or controller=DSLPIDControl: the policy and tracker "
+                         "loops have no downwash adjoint")
+
+
 def _refuse_downwash(env, caller, derivative):
     if env._effects & N.EFFECT_DW or env._EXTERNAL_DOWNWASH:
         raise ValueError("%s does not support downwash: the pairwise term has no %s (use Physics.DYN, PYB, PYB_GND or PYB_DRAG)"
@@ -523,10 +559,13 @@ def _rpm_ticks(env, rpm):
 
 
 def differentiable_rollout(env, rpm=None, controller=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
-                           action_buffer=None, plan=None, **schedule):
+                           action_buffer=None, plan=None, downwash=False, **schedule):
     """BaseAviary.differentiable_rollout (see there)."""
     from .ilqr import Tracker
-    _refuse_downwash(env, "differentiable_rollout()", "adjoint")
+    if downwash:
+        _check_downwash(env, policy, controller)
+    else:
+        _refuse_downwash(env, "differentiable_rollout()", "adjoint")
     if (rpm is not None) + (controller is not None) + (policy is not None) != 1:
         raise ValueError("differentiable_rollout() takes exactly one of rpm [T, E, D, 4] (open loop), controller= (closed loop) or "
                          "policy= (an MlpPolicy in the loop)")

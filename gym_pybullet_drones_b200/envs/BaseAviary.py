@@ -556,7 +556,7 @@ class BaseAviary(Env):
     def differentiable_rollout(self, rpm=None, *, controller=None, waypoints=None, start=None, offset=None, target_rpy=None,
                                target_vel=None, target_rpy_rates=None, control_timestep=None, num_steps=None, gains=None,
                                pid_state=None, state=None, last_rpm=None, phys=None, policy=None, params=None, noise=None,
-                               action_buffer=None, plan=None):
+                               action_buffer=None, plan=None, downwash=False):
         """T control ticks of raw RPMs, of a DSLPIDControl tracking a waypoint schedule, or of an MlpPolicy acting on the
         aviary's observations, as a differentiable function (torch.autograd), without changing the env.  Pass exactly one of
         `rpm` (open loop), `controller` (closed loop) or `policy` (policy loop, at the end of this text).
@@ -575,8 +575,9 @@ class BaseAviary(Env):
         quaternion renormalisation on tick entry (the gradient w.r.t. state["quat"] has no radial part); the RPM clip as
         torch.clamp (the gradient passes for 0 <= rpm <= MAX_RPM and goes to MAX_RPM above); the ground-effect height clip with
         the forward's predicate; the upright switch as a constant.  Drag's first substep reads the previous tick's RPMs, so
-        their gradient flows to rpm[k-1], or to last_rpm for k = 0.  Physics.DYN, PYB, PYB_GND and PYB_DRAG; downwash, inputs
-        that are not float64 CUDA tensors of the right shape on the env's device, and double backward raise ValueError.
+        their gradient flows to rpm[k-1], or to last_rpm for k = 0.  Physics.DYN, PYB, PYB_GND and PYB_DRAG; downwash without
+        `downwash=True` (below), inputs that are not float64 CUDA tensors of the right shape on the env's device, and double
+        backward raise ValueError.
         Forward mode: torch.autograd.forward_ad dual tensors on rpm, state, last_rpm or phys give the tangents of the four
         outputs (one JVP kernel launch with the same derivative decisions; the primal outputs keep their bits); a tangent that
         itself requires grad raises ValueError.  linearise() gives the per-tick Jacobians.
@@ -639,10 +640,21 @@ class BaseAviary(Env):
         on any tensor of params, state, last_rpm, phys, action_buffer and noise give the tangents of the four state entries and
         `actions` (one batched forward-mode actor pass over the saved observations for the parameters' and the noise's part,
         then one JVP kernel launch with the same decisions; the primal outputs keep their bits; `obs` has no tangent).
-        linearise(policy=) gives the per-tick Jacobians of the policy loop."""
+        linearise(policy=) gives the per-tick Jacobians of the policy loop.
+
+        Downwash (PYB_DW, PYB_GND_DRAG_DW): `downwash=True` runs the open loop (rpm=) and the DSLPIDControl closed loop (with
+        all of its schedule, gains and pid_state arguments) on kernels whose unit is the aviary, and returns the same dict.  It
+        accepts their limits: at most 128 drones per aviary, and pair work of order D^2 per substep in the backward pass.  Each
+        substep takes the pair force from the aviary's positions at its start and renormalises the quaternion on entry, as
+        CtrlAviary.rollout() and step() do, so the forward is their bits.  The backward (DESIGN.md 4.5, downwash adjoint)
+        differentiates the pair term through both drones of every pair that acts, with the forward's predicate (no term at its
+        jump) and without differentiating the sqrt (stacked drones have finite derivatives), and each substep's renormalisation;
+        the downwash coefficients are constants.  An env without downwash, D > 128, a formation sharded over devices, policy= or
+        a Tracker, and forward mode (dual tensors: reverse mode only) raise ValueError.  linearise() refuses
+        downwash."""
         from ..diff import differentiable_rollout
         return differentiable_rollout(self, rpm, controller=controller, state=state, last_rpm=last_rpm, phys=phys, policy=policy,
-                                      params=params, noise=noise, action_buffer=action_buffer, waypoints=waypoints,
+                                      params=params, noise=noise, action_buffer=action_buffer, downwash=downwash, waypoints=waypoints,
                                       start=start, offset=offset, target_rpy=target_rpy, target_vel=target_vel,
                                       target_rpy_rates=target_rpy_rates, control_timestep=control_timestep, num_steps=num_steps,
                                       gains=gains, pid_state=pid_state, plan=plan)

@@ -9,11 +9,10 @@ import numbers
 import torch
 
 from . import _native as N
-from .diff import _call, _io, dyn_cfg, unpack_traj
+from .diff import MAX_DW_DRONES, _call, _io, dyn_cfg, unpack_traj
 from .ilqr import check_iters, horizon, pack_inputs
 
 MAX_SAMPLES = 1024
-MAX_DW_DRONES = 128                  # downwash: whole aviaries per 128-thread CTA, as CtrlAviary.rollout()
 
 
 def _sigma(sigma, E, dev):

@@ -662,6 +662,19 @@ int qs_dyn_traj(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones
 int qs_dyn_traj_vjp(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
                     void* stream);
 
+/* The raw-RPM trajectories of qs_dyn_traj with downwash, and their VJP (DESIGN.md 4.5, downwash adjoint): the same arguments and
+ * QsDynTrajIO, effects QS_EFFECT_DW or QS_EFFECT_GND | QS_EFFECT_DRAG | QS_EFFECT_DW only.  Each substep is qs_ctrl_rollout's:
+ * the pair force from the aviary's positions at the substep's start, then one substep that renormalises the quaternion on entry;
+ * so the forward is qs_ctrl_rollout's (QS_CTRL_RAW) bit for bit.  The VJP differentiates the pair term through both drones of
+ * every pair that acts (the forward's predicate, no term at its jump; at dxy2 = 0 the xy derivatives are 0) and each substep's
+ * entry renormalisation; the downwash coefficients and the propeller radius are constants.  One CTA of 128 threads holds whole
+ * aviaries, so the pair work is O(D^2) per substep.  Refusals in this order: NULL pointers and sizes as qs_dyn_traj, then
+ * QS_ERR_UNSUPPORTED for any other effect set and for drones_per_env > 128, QS_ERR_ALIGN for phys.  Deterministic (no atomics). */
+int qs_dyn_traj_dw(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                   void* stream);
+int qs_dyn_traj_dw_vjp(const QsParams* p, const QsDynTrajIO* io, int n_envs, int drones_per_env, int substeps, unsigned effects,
+                       void* stream);
+
 /* Forward mode of the raw-RPM trajectories of qs_dyn_traj (DESIGN.md 4.5): the tangent of the T states along given tangents of
  * the inputs (JVP), and the dense Jacobians of every tick.  Both read the forward's `states` and restart each tick from the
  * stored state k-1 (state0 for k = 0), so the trajectory is linearised at the forward's bits, and both take the derivative
@@ -735,6 +748,14 @@ int qs_dyn_ctrl_traj(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajI
                      unsigned effects, void* stream);
 int qs_dyn_ctrl_traj_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
                          int substeps, unsigned effects, void* stream);
+
+/* The closed-loop trajectories of qs_dyn_ctrl_traj with downwash, and their VJP: the same arguments and QsDynCtrlTrajIO, the
+ * effects, layout, refusals and derivative of qs_dyn_traj_dw around the controller of qs_dyn_ctrl_traj (called once per drone per
+ * tick before the substeps, as qs_ctrl_rollout's QS_CTRL_TRACK tick). */
+int qs_dyn_ctrl_traj_dw(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env, int substeps,
+                        unsigned effects, void* stream);
+int qs_dyn_ctrl_traj_dw_vjp(const QsParams* p, const QsParams* cp, const QsDynCtrlTrajIO* io, int n_envs, int drones_per_env,
+                            int substeps, unsigned effects, void* stream);
 
 /* Forward mode of the closed-loop trajectories of qs_dyn_ctrl_traj (DESIGN.md 4.5): the tangents of the T states and applied
  * RPMs along given tangents of the inputs (JVP), and the dense Jacobians of every closed-loop tick.  Both read the forward's
